@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- gradient-updates/s of the DQN hot path (BASELINE.json metric) on N B200s.
+"""bench.py -- gradient-updates/s of the DQN hot path (BASELINE.json metric) on N H100s.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b2rl|reference] [--workload dqn|per|c51|qr|ppo]
                   [--replay async|sync] [--repeats R] [--no-extras]
@@ -19,7 +19,7 @@ barrier + torch.cuda.synchronize() and timed with CUDA events on the launching s
   e2e_agent  the same update driven through the reference's own seam, ``DQNAgent.step()`` with ``config.cuda_graph``
              (actor env steps + host feed + one graph replay per step)
   roofline   the replay gather kernel (HBM): SURVEY 8d algorithmic bytes per launch / CUDA-event time per launch;
-             ``roofline_tensor``: the dominant tcgen05 kernel (conv1 forward) and the whole step against the bf16 peaks
+             ``roofline_tensor``: the dominant wgmma kernel (conv1 forward) and the whole step against the bf16 peaks
   extra_workloads   PER / C51 / QR-DQN / PPO (BASELINE configs[2..4]) measured in the same run
   cpu_baseline / --impl reference   the oracle port of the reference's CPU path (oracle/agents.py, torch-CPU) timed on the
              host cores with the reference's own ``set_one_thread()`` and with 32 threads (median of >= 20 updates where
@@ -133,7 +133,7 @@ def build_learner(rl, workload, device, rank, world, prefetch=True):
         kind = "qr"
     net, tgt = mk(), mk()
     tgt.load_state_dict(net.state_dict())
-    if rl.Config.DENSE_BACKEND != "tcgen05":               # cuDNN prefers channels_last weights; the tcgen05 path packs its own
+    if rl.Config.DENSE_BACKEND != "tcgen05":               # cuDNN prefers channels_last weights; the wgmma path packs its own
         net = net.to(memory_format=torch.channels_last)
         tgt = tgt.to(memory_format=torch.channels_last)
     opt = rl.ops.FlatOptimizer.from_torch(topt(net.parameters()))
@@ -217,8 +217,9 @@ def median(xs):
     return float(np.median(np.asarray(xs, dtype=np.float64)))
 
 
-def measure_learner(rl, workload, dev, rank, world, K, W, repeats, barrier, prefetch, full):
-    """Build + capture + time one workload.  ``full``: also the end-to-end (host buffers) figure."""
+def measure_learner(rl, workload, dev, rank, world, K, W, repeats, barrier, prefetch, full, dump=None):
+    """Build + capture + time one workload.  ``full``: also the end-to-end (host buffers) figure.  ``dump``: directory that
+    receives what the last timed update computed (see dump_outputs)."""
     import gc
     learner = build_learner(rl, workload, dev, rank, world, prefetch=prefetch)
     if world > 1:                                          # parameters identical on every rank
@@ -228,6 +229,8 @@ def measure_learner(rl, workload, dev, rank, world, K, W, repeats, barrier, pref
     for _ in range(W):
         learner.update()
     reg = timed_regions(learner.update, K, repeats, barrier, world, dev)
+    if dump and rank == 0:
+        dump_outputs(learner, dump)
     res = dict(value=round(world * K / (median(reg) * 1e-3), 1), ms_per_step=round(median(reg) / K, 4),
                repeat_ms=[round(x, 4) for x in reg], loss=float(learner.loss),
                replay="async_replay=True" if learner.prefetch else ("async_replay=False, K1 (conv1 reads the uint8 ring)" if learner.ring
@@ -255,6 +258,28 @@ def measure_learner(rl, workload, dev, rank, world, K, W, repeats, barrier, pref
                           d2h_bytes_per_step=4, ms_per_step=round(median(ereg) / K, 4), repeat_ms=[round(x, 4) for x in ereg])
         res["last_e2e_loss"] = last[0]
     return learner, res
+
+
+def dump_outputs(learner, out_dir):
+    """What the timed update hands its caller after the last timed step, as float32 .npy files: the parameter arena of the
+    online network (every weight and bias after the optimizer step, 6.7 MB for DQN) and the loss of that update."""
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "params.npy"), learner.opt.flat.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "loss.npy"), np.atleast_1d(learner.loss.detach().float().cpu().numpy()))
+
+
+def dump_ppo_outputs(ag, out_dir):
+    """What the last timed PPO iteration leaves its caller, as float32 .npy files: every network parameter in
+    ``named_parameters()`` order, and the state normaliser's running mean / variance."""
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    flat = torch.cat([p.detach().float().reshape(-1) for p in ag.network.parameters()])
+    np.save(os.path.join(out_dir, "params.npy"), flat.cpu().numpy())
+    rms = ag.config.state_normalizer.rms
+    f32 = lambda x: x.detach().float().cpu().numpy() if torch.is_tensor(x) else np.asarray(x, dtype=np.float32)
+    np.save(os.path.join(out_dir, "state_mean.npy"), f32(rms.mean))
+    np.save(os.path.join(out_dir, "state_var.npy"), f32(rms.var))
 
 
 def leave(world):
@@ -297,7 +322,7 @@ def time_kernel_graph(fn, iters=20, reps=5):
 
 
 def tensor_roofline(rl, learner, pk, value, world, workload):
-    """The dominant tcgen05 kernel family (conv1 forward: the largest share of the step's kernel time) timed alone, and the
+    """The dominant wgmma kernel family (conv1 forward: the largest share of the step's kernel time) timed alone, and the
     whole step's dense flops against the sustained bf16 peak."""
     from deeprl_b200.network import nature_tc
     dev = learner.dev
@@ -310,27 +335,16 @@ def tensor_roofline(rl, learner, pk, value, world, workload):
                                                        V=20, block_n=32)) * 1e3
     flops = 2.0 * B * 441 * 32 * 256
     ach = flops / (us * 1e-6) / 1e12
-    burst = pk.get("bf16_tflops", 1590.0)
-    sust = pk.get("bf16_tflops_sustained", 1400.0)
+    burst = pk.get("bf16_tflops", 989.0)
+    sust = pk.get("bf16_tflops_sustained", 989.0)
     step_flops = FLOPS_PER_UPDATE.get(workload)
-    return dict(bound="tensor", kernel="conv_slab_tcgen05_kernel<32> (conv1 forward, 2x2 taps x 64 channels, N = 32: "
-                                       "capped at ~30 % of the pipe by the 53-cycle tcgen05.mma issue floor at N <= 64)",
+    return dict(bound="tensor", kernel="conv_slab_wgmma_kernel<32> (conv1 forward, 2x2 taps x 64 channels, N = 32)",
                 achieved=round(ach, 1), peak=burst, unit="TFLOP/s", frac=round(ach / burst, 4), us_per_launch=round(us, 2),
                 flops_per_launch=flops, peak_source="MEASURED_PEAKS.json bf16_tflops (burst: kernel timed alone)" if "bf16_tflops" in pk
-                else "fallback 1590",
+                else "fallback 989 (H100 SXM data sheet, dense bf16)",
                 whole_step=(dict(flops_per_update=step_flops, achieved_tflops=round(step_flops * value / world / 1e12, 1),
                                  peak=sust, frac=round(step_flops * value / world / (sust * 1e12), 4),
                                  peak_source="bf16_tflops_sustained (kernels timed inside a long step)") if step_flops else None))
-
-
-def gather_traffic():
-    """dram__bytes_read + dram__bytes_write per launch of the gather kernel from this round's ncu --set full capture
-    (profiles/r02_gather_traffic.json, written by scripts/ncu_summary.py); None if the capture is not there."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "r02_gather_traffic.json")))
-        return int(d["dram_bytes_read"] + d["dram_bytes_write"]), d.get("source", "profiles/r02_gather_traffic.json")
-    except Exception:
-        return None, None
 
 
 def agent_e2e(rl, steps=48):
@@ -365,7 +379,7 @@ def agent_e2e(rl, steps=48):
     ag.close()
     return dict(value=round(steps / dt, 1), unit="updates/s", steps=steps, graph_path=bool(ok),
                 note="DQNAgent.step() through run_steps' seam: 4 host env steps, each with the actor's batch-1 forward as one captured "
-                     "launch sequence (GraphedQActor: pinned frame upload -> tcgen05 network -> pinned q download), + feed + one "
+                     "launch sequence (GraphedQActor: pinned frame upload -> wgmma network -> pinned q download), + feed + one "
                      "captured update per step; wall clock")
 
 
@@ -395,7 +409,8 @@ def run_b2rl(args):
         torch.cuda.synchronize()
 
     if args.quick:                                        # A/B runs: the resident-input number only
-        learner, res = measure_learner(rl, args.workload, dev, rank, world, K, W, 1, barrier, args.replay == "async", False)
+        learner, res = measure_learner(rl, args.workload, dev, rank, world, K, W, 1, barrier, args.replay == "async", False,
+                                       dump=args.dump_outputs)
         if rank == 0:
             print(json.dumps(dict(quick=True, value=res["value"], ms_per_step=res["ms_per_step"], loss=res["loss"],
                                   launches=res["gpu_launches_per_step"])), flush=True)
@@ -403,7 +418,8 @@ def run_b2rl(args):
         return
 
     with ClockSampler(local) as clocks:
-        learner, main = measure_learner(rl, args.workload, dev, rank, world, K, W, R, barrier, args.replay == "async", True)
+        learner, main = measure_learner(rl, args.workload, dev, rank, world, K, W, R, barrier, args.replay == "async", True,
+                                        dump=args.dump_outputs)
     # ---- the other replay mode (async_replay on / off), resident inputs
     pk = peaks()
     roof = roof_t = None
@@ -436,21 +452,16 @@ def run_b2rl(args):
         except Exception as e:                             # noqa: BLE001 -- an extra must never take the headline line down
             extras["ppo"] = dict(error=str(e).splitlines()[0][:200])
     # ---- roofline of the replay gather kernel, timed alone (burst peak applies)
-    hbm = pk.get("hbm_gbs", 6650.0)
+    hbm = pk.get("hbm_gbs", 3350.0)
     ach = B * ALGO_BYTES / (gt["bf16_s2d"] * 1e-3) / 1e9
     ach_u8 = B * ALGO_BYTES / (gt["u8"] * 1e-3) / 1e9
-    traffic, traffic_src = gather_traffic()
     roof = dict(bound="hbm", kernel="gather_cvt_kernel<bf16, space-to-depth> (replay sample: frame-stack gather -> exact u8->bf16 -> "
                                     "conv1 input layout; the kernel the step launches with async_replay)",
                 achieved=round(ach, 1), peak=hbm, unit="GB/s", frac=round(ach / hbm, 4),
-                peak_source="MEASURED_PEAKS.json hbm_gbs (burst: kernel timed alone)" if "hbm_gbs" in pk else "fallback 6650",
+                peak_source="MEASURED_PEAKS.json hbm_gbs (burst: kernel timed alone)" if "hbm_gbs" in pk else "fallback 3350 (H100 SXM data sheet)",
                 us_per_launch=round(gt["bf16_s2d"] * 1e3, 2), algorithmic_bytes_per_launch=B * ALGO_BYTES,
                 algorithmic_bytes_definition="SURVEY 8d: 512 samples x (5 unique frames read + 2 x 4 frames written) x 7056 B = 91 728 B "
                                              "per sample (this variant writes bf16, i.e. twice the write bytes, most of which stay in L2)",
-                traffic=traffic, traffic_source=traffic_src,
-                limited_by="not DRAM (traffic is below the algorithmic bytes: the bf16 batch stays in L2): 512 CTAs x 35 KB staging, "
-                           "u8->bf16 conversion and 16-byte stores through shared memory; the uint8 variant below moves exactly the "
-                           "SURVEY-8d bytes and is the HBM-bound form of the same gather",
                 raw_u8_variant=dict(kernel="gather_raw_tma_kernel (uint8 stacks: exactly the SURVEY 8d bytes; UniformReplay.sample())",
                                     achieved=round(ach_u8, 1), frac=round(ach_u8 / hbm, 4), us_per_launch=round(gt["u8"] * 1e3, 2)))
     ag = cpu = None
@@ -467,7 +478,7 @@ def run_b2rl(args):
         config=dict(workload=WORKLOADS[args.workload], batch=B, replay_capacity=CAP, replay_bytes=CAP * FRAME, actions=ACTIONS,
                     feeds_per_update=4, l2_policy="inputs larger than L2: 7.06 GB ring, fresh random indices every step",
                     parallelism="dp%d (rank-local replay shard, NCCL all-reduce of 6.7 MB fp32 gradients per step)" % world,
-                    dense=("tcgen05 GEMM kernels (csrc/gemm.cu): bf16 operands, fp32 accumulation in TMEM, fp32 master weights"
+                    dense=("wgmma GEMM kernels (csrc/gemm.cu): bf16 operands, fp32 accumulation in registers, fp32 master weights"
                            if rl.Config.DENSE_BACKEND == "tcgen05" else "cuDNN/cuBLAS bf16 (fp32 accumulate, fp32 master weights)"),
                     replay=main["replay"], cuda_graph=True, timing="median of %d regions of %d steps" % (R, K)),
         e2e=main["e2e"], e2e_agent=ag, gpu_launches=int(main["gpu_launches_per_step"] * K),
@@ -482,7 +493,7 @@ def run_b2rl(args):
     leave(world)
 
 
-WORKLOADS = {"dqn": "DQN synthetic 84x84x4 uint8 frames, 1M-transition uniform Replay, batch 512, NatureConvBody, 1 B200 (BASELINE configs[1])",
+WORKLOADS = {"dqn": "DQN synthetic 84x84x4 uint8 frames, 1M-transition uniform Replay, batch 512, NatureConvBody, 1 H100 (BASELINE configs[1])",
              "per": "Prioritized Dueling Double-DQN, 1M sum-tree PrioritizedReplay, batch 512 (BASELINE configs[2])",
              "c51": "C51 51 atoms, batch 512 (BASELINE configs[4])", "qr": "QR-DQN 200 quantiles, batch 512 (BASELINE configs[4])"}
 
@@ -521,7 +532,7 @@ def ppo_result(rl, args, quiet=False):
                 torch.cuda.synchronize()
                 sgd[0] += time.perf_counter() - t
             ag._graphed_epochs = timed_epochs
-        K, W = (1 if quiet else max(1, min(args.steps, 3))), 1
+        K, W = (1 if quiet else max(1, args.steps)), 1
         for _ in range(W):
             ag.step()
         torch.cuda.synchronize()
@@ -532,6 +543,8 @@ def ppo_result(rl, args, quiet=False):
             ag.step()
         torch.cuda.synchronize()
         dt = (time.perf_counter() - t0) / K
+        if not quiet and getattr(args, "dump_outputs", None):
+            dump_ppo_outputs(ag, args.dump_outputs)
         mb = c.optimization_epochs * (c.rollout_length * c.num_workers // c.mini_batch_size)
         res = dict(
             metric="PPO minibatch updates/sec (17-dim obs, 2048 x 16 rollout, GAE 0.95, 10 epochs x 64)", value=round(mb / dt, 1),
@@ -676,6 +689,8 @@ if __name__ == "__main__":
                          "mode is timed as well and reported under other_replay_mode")
     ap.add_argument("--quick", action="store_true", help="developer A/B runs: print the resident-input value only")
     ap.add_argument("--no-extras", action="store_true", help="skip the extra workloads (PER / C51 / QR / PPO)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed update computed (parameters, loss) as DIR/<name>.npy")
     a = ap.parse_args()
     if a.impl == "reference":
         run_reference(a)

@@ -1,4 +1,4 @@
-"""b2rl -- a B200-native RL training step behind the DeepRL (ShangtongZhang/DeepRL) API.
+"""b2rl -- an H100-native RL training step behind the DeepRL (ShangtongZhang/DeepRL) API.
 
 ``from deeprl_b200 import *`` mirrors ``from deep_rl import *`` (reference ``deep_rl/__init__.py:1-4``):
 agents, components, networks and utils are all re-exported, together with ``torch / np / nn / F`` which the

@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libb2rl.so")
 SOURCES = ["core.cu", "replay.cu", "sumtree.cu", "losses.cu", "onpolicy.cu", "optim.cu", "dense.cu", "gemm.cu", "pack.cu", "head.cu", "tail.cu", "disthead.cu", "actor.cu", "ppo_persistent.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 c_p, c_i32, c_i64, c_u64, c_f32, c_f64 = (ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_uint64,
@@ -100,7 +100,7 @@ class B2RLError(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile csrc/*.cu into csrc/libb2rl.so for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu into csrc/libb2rl.so for sm_90a (nvcc cross-compiles without a GPU)."""
     cmd = ["nvcc"] + NVCC_FLAGS + ["-o", LIB_PATH] + [os.path.join(CSRC, s) for s in SOURCES]
     if verbose:
         print(" ".join(cmd), file=sys.stderr)
@@ -125,7 +125,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise B2RLError("libb2rl.so is not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                            "(nvcc -gencode arch=compute_100a,code=sm_100a); there is no CPU fallback")
+                            "(nvcc -gencode arch=compute_90a,code=sm_90a); there is no CPU fallback")
         L = ctypes.CDLL(LIB_PATH)
         L.b2rl_version.restype = ctypes.c_int
         L.b2rl_last_error.restype = ctypes.c_char_p
@@ -191,6 +191,6 @@ def reset_launch_count():
 def require_cuda(device):
     device = torch.device(device)
     if device.type != "cuda":
-        raise B2RLError("the replay / loss kernels live in HBM and run on sm_100a: select a CUDA device "
+        raise B2RLError("the replay / loss kernels live in HBM and run on sm_90a: select a CUDA device "
                         "(select_device(0)); there is no CPU fallback")
     return device

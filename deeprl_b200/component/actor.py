@@ -139,7 +139,7 @@ class GraphedQActor:
     """The DQN-family actor's forward pass (DQN_agent.py:29-31: ``network(state_normalizer(stack(state)))`` at batch
     ``num_envs``, normally 1) as ONE CUDA-graph replay: pinned upload of the uint8 frame stacks -> frame-stack conversion to
     the exact-integer bf16 space-to-depth layout (``b2rl_replay_gather`` on the staging buffer; ImageNormalizer's 1/255 is
-    folded into conv1 like in the learner) -> the network on the tcgen05 kernels -> action values -> pinned download.  The
+    folded into conv1 like in the learner) -> the network on the wgmma kernels -> action values -> pinned download.  The
     epsilon-greedy draw stays on the host (``epsilon_greedy``: the reference's numpy stream, torch_utils.py:51-58).
 
     The eager form of the same step is ~40 kernel / memcpy launches of Python-driven work per env step; this is one launch and
@@ -213,7 +213,7 @@ class GraphedQActor:
 
 
 def q_actor_supported(config, network):
-    """``config.cuda_graph`` + synchronous actor + bf16 tcgen05 NatureConvBody on a CUDA device + ImageNormalizer-style rescale
+    """``config.cuda_graph`` + synchronous actor + bf16 wgmma NatureConvBody on a CUDA device + ImageNormalizer-style rescale
     of uint8 frames: the conditions under which the actor's forward is the captured device path."""
     from ..network.network_bodies import NatureConvBody
     from ..utils import Config

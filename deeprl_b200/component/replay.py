@@ -371,7 +371,7 @@ class UniformReplay:
         ``layout="s2d"``, as the space-to-depth(4) tensor [B, 16*history, H/4, W/4] (channels_last memory).
         ``scale=None`` emits the exact integers 0..255 (the consumer folds 1/255 into its first layer, see
         ``network.frame_scale``); otherwise ``float32(float64(v) * scale)`` rounded to ``out_dtype``.
-        ``layout="ring"`` (K1): nothing is gathered -- state / next_state are ``RingFrames`` (ring + indices) that the tcgen05
+        ``layout="ring"`` (K1): nothing is gathered -- state / next_state are ``RingFrames`` (ring + indices) that the wgmma
         ``NatureConvBody`` reads directly; they are valid until the ring rows are overwritten."""
         if channels_last is not None:
             layout = "nhwc" if channels_last else "nchw"

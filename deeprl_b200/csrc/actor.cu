@@ -9,7 +9,7 @@
 //       action = mean + std * z (z ~ N(0,1): Philox4x32-10 + Box-Muller, or supplied normals in parity mode),
 //       log_pi_a = sum_a Normal(mean, std).log_prob(action), entropy = sum_a Normal.entropy()
 //
-// One CTA (the batch is num_workers <= 64 rows; the MLPs are 17 -> 64 -> 64 -> 6 | 1): latency, not throughput.  sm_100a only.
+// One CTA (the batch is num_workers <= 64 rows; the MLPs are 17 -> 64 -> 64 -> 6 | 1): latency, not throughput.  sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {

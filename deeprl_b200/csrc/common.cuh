@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libb2rl.so (sm_100a only).
+// common.cuh -- shared helpers for libb2rl.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -25,7 +25,7 @@ inline int check_launch(const char* what) {
 // ---------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  Kernels on the per-update chain are launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs are scheduled, and run their prologue
-// (barrier init, TMEM allocation, tensor-map prefetch), while the previous kernel is still executing; they then block in
+// (barrier init, tensor-map prefetch), while the previous kernel is still executing; they then block in
 // pdl_wait() until the previous kernel has completed and its memory is visible.  Contract for every kernel launched
 // through launch_pdl(): (1) pdl_wait() is executed on EVERY path before the first global-memory access of any kind and
 // before any early return; (2) pdl_trigger() comes after pdl_wait(), so that the kernel after this one can only start once

@@ -2,7 +2,7 @@
 //   forward   y = relu(conv_or_linear(x) + bias)          -> b2rl_bias_act_bf16 (in place on the bf16 GEMM output)
 //   backward  g = gy * (y > 0);  dbias = sum_rows g       -> b2rl_act_bwd_bias_grad_bf16 (one pass, block partials + atomics)
 // Activations are bf16 [rows][C] (NHWC flattened: rows = batch x spatial), bias / dbias are fp32.
-// Both kernels are pure streaming passes (L2 / HBM bound): 16-byte vector loads, 8 channels per thread.  sm_100a only.
+// Both kernels are pure streaming passes (L2 / HBM bound): 16-byte vector loads, 8 channels per thread.  sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {
@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const __nv_bfloat16* __res
   __syncthreads();
   // block partial -> dbias with fp32 atomics (dbias is zeroed by the caller; the summation order over blocks is not
   // fixed, which perturbs the last bits of a bias gradient -- the deterministic single-block reduction it replaces was
-  // latency-bound at 15-25 us per layer)
+  // latency-bound)
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float s = 0.0f;
     for (int q = 0; q < rpb; ++q) s += sred[q * C + c];
@@ -135,7 +135,7 @@ extern "C" int b2rl_bias_act_bf16(uint16_t* y, const float* bias, int64_t rows, 
   B2RL_REQUIRE(reinterpret_cast<uintptr_t>(y) % 16 == 0, "y must be 16-byte aligned");
   const int64_t n8 = rows * C / 8;
   int blocks = (int)((n8 + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   launch_pdl(bias_act_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, reinterpret_cast<__nv_bfloat16*>(y), bias, n8, C / 8, relu);
   return check_launch("b2rl_bias_act_bf16");
 }
@@ -170,7 +170,7 @@ extern "C" int b2rl_bias_act_f32_to_bf16(const float* x, const float* bias, uint
   B2RL_REQUIRE(reinterpret_cast<uintptr_t>(x) % 16 == 0 && reinterpret_cast<uintptr_t>(y) % 16 == 0, "16-byte alignment");
   const int64_t n8 = rows * C / 8;
   int blocks = (int)((n8 + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   launch_pdl(bias_act_f32_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, x, bias, reinterpret_cast<__nv_bfloat16*>(y), n8, C / 8, relu);
   return check_launch("b2rl_bias_act_f32_to_bf16");
 }

@@ -1,12 +1,12 @@
 // disthead.cu -- the element-wise halves of the distributional heads (CategoricalNet / QuantileNet, network_heads.py:40-55, 89-102)
-// around the tcgen05 GEMMs of csrc/gemm.cu, so that the C51 / QR-DQN update runs no cuBLAS / ATen kernel:
+// around the wgmma GEMMs of csrc/gemm.cu, so that the C51 / QR-DQN update runs no cuBLAS / ATen kernel:
 //
 //   forward   logits [B][A*N] = phi W^T + b        b2rl_gemm_bf16 (bias in the epilogue, fp32 out)
 //             prob, log_prob = softmax / log_softmax over the N atoms of every (b, a)      dist_softmax_kernel   (C51)
 //   backward  dlogits = dlog_prob - prob * sum_n dlog_prob   (log_softmax backward; QR: dlogits = dquantile)
 //             -> bf16 GEMM operand g [B][ld] + bias gradient (column sums)                 dist_bwd_prep_kernel
 //             dW = g^T phi, dphi = relu_mask(g W)  b2rl_gemm_bf16 (MN-major operands) / b2rl_gemm_bwd_bf16
-// sm_100a only.
+// sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {

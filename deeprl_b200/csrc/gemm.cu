@@ -1,7 +1,7 @@
-// gemm.cu -- persistent tcgen05 / TMEM / TMA GEMM for the dense layers of the path: NatureConvBody convolutions as
-// shifted-row implicit GEMMs, fc4, heads (network_bodies.py:27-33, network_heads.py:18-21), forward, dgrad and wgrad.
+// gemm.cu -- persistent wgmma / TMA GEMM for the dense layers of the path: NatureConvBody convolutions as shifted-row
+// implicit GEMMs, fc4, heads (network_bodies.py:27-33, network_heads.py:18-21), forward, dgrad and wgrad.
 //
-//   D[M,N] (+)= A[M,K] * B[N,K]^T        bf16 operands, fp32 accumulation in tensor memory
+//   D[M,N] (+)= A[M,K] * B[N,K]^T        bf16 operands, fp32 accumulation in registers
 //
 // Operand storage is described per operand:
 //   K-major  (major = 0): row-major [rows = M or N][K], K contiguous            (activations x weights: y = x W^T)
@@ -16,25 +16,26 @@
 // kernel writes directly (the replay gather for conv1, conv1's epilogue for conv2).  dgrad is the same with negative
 // shifts; wgrad reads both operands MN-major with the tap shift applied to the B operand per output column block.
 //
-// One persistent CTA per SM loops over output tiles (128 x BN):
-//   warp 0    TMA producer   cp.async.bulk.tensor into a STAGES-deep 128B-swizzled smem ring (mbarrier full/empty)
-//   warp 1    MMA issuer     one ELECTED thread (elect.sync, see elect_one): tcgen05.mma.cta_group::1.kind::f16,
-//                            accumulators double-buffered in TMEM
-//   warps 2-5 epilogue of even tiles, warps 6-9 epilogue of odd tiles (one group per accumulator stage):
-//                            tcgen05.ld (32 lanes x 32 columns per warp) -> bias / ReLU -> bf16 | fp32 | atomic fp32,
-//                            overlapped with the next tile's MMAs; warp 2 also owns TMEM alloc / dealloc
-// Every kernel runs its prologue (barrier init, tensor-map prefetch, TMEM allocation) before pdl_sync(): under
-// programmatic dependent launch that part overlaps the tail of the previous kernel (common.cuh).
-// sm_100a only.
+// One persistent CTA per SM loops over output tiles (128 x BN), in three warpgroups:
+//   warpgroup 0      TMA producer: one ELECTED thread of warp 0 (elect.sync, see elect_one) issues cp.async.bulk.tensor
+//                    into a STAGES-deep 128B-swizzled smem ring (mbarrier full/empty); warps 1-3 idle
+//   warpgroups 1, 2  rows 0-63 / 64-127 of the tile: wgmma.mma_async m64nBNk16 (fp32 accumulators in registers), then the
+//                    epilogue: accumulators -> shared staging tile -> one row x 32 columns per thread -> bias / ReLU ->
+//                    bf16 | fp32 | atomic fp32
+// Every kernel runs its prologue (barrier init, tensor-map prefetch) before pdl_sync(): under programmatic dependent launch
+// that part overlaps the tail of the previous kernel (common.cuh).
+// sm_90a only.
 #include <cuda.h>
 #include <cstdlib>
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace b2rl {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;           // 64 bf16 = 128 bytes = one swizzle-128B atom row
-constexpr int GEMM_THREADS = 320;   // warp 0: TMA producer, warp 1: MMA issuer, warps 2-5 / 6-9: epilogue of even / odd tiles
+constexpr int GEMM_THREADS = 384;     // warpgroup 0: TMA producer, warpgroups 1 / 2: MMA + epilogue of rows 0-63 / 64-127
+constexpr int MMA_WARPS = 8;          // a shared-memory stage is free again once every MMA warp has arrived on its barrier
 
 __device__ __forceinline__ uint32_t s2u(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -48,7 +49,7 @@ __device__ __forceinline__ void mb_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s2u(bar)) : "memory");
 }
 // try_wait with a suspend-time hint: the waiting thread sleeps in hardware until the phase completes instead of polling
-// the barrier word -- eight epilogue warps spinning on shared memory measurably slow the tensor pipe's operand reads
+// the barrier word
 __device__ __forceinline__ void mb_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n"
@@ -68,9 +69,8 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "l"(map), "r"(s2u(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// One elected lane of a fully active warp.  Code guarded by this predicate (instead of `lane == 0`) lets the compiler issue
-// the uniform-datapath instructions (UTCHMMA, UTMALDG, UTCBAR) directly; behind a plain lane test it wraps every one
-// of them in an ELECT / BRA.U.ANY loop, which costs ~50 extra cycles per MMA on the issuing thread.
+// One elected lane of a fully active warp: the single-thread producer role is entered through elect.sync rather than a
+// plain `lane == 0` test, so that the compiler issues the TMA instructions without an ELECT / BRA.U.ANY loop around them.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -82,66 +82,53 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s2u(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// descriptor halves: the single MMA-issuing thread must stay lean (every instruction it executes is on the critical
-// path of the tensor pipe), so the 64-bit descriptors are kept as a constant high word and a low word that only
-// receives 32-bit adds.
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return ((smem_addr >> 4) & 0x3FFFu) | ((lbo_bytes >> 4) << 16);
-}
-constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);      // SBO = 1024 B, version 1, SWIZZLE_128B
-__device__ __forceinline__ void umma_f16_lh(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      ".reg .b64 da, db;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "mov.b64 da, {%1, %5};\n"
-      "mov.b64 db, {%2, %5};\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(DESC_HI)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// named barriers: 0 = __syncthreads, 1 = the 256 MMA threads, 2 / 3 = MMA warpgroup 1 / 2, 4 = uint8 converters
+__device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// wgmma shared-memory matrix descriptor, 128B swizzle (layout type 1 in bits 62-63):
+//   K-major : 8-row groups 1024 B apart (SBO), LBO unused
+//   MN-major: 64-element MN groups `lbo` bytes apart, 8-K-row groups 1024 B apart (SBO)
+// base_offset (bits 49-51) = (start address >> 7) & 7 for a start that is not aligned to the 1024-byte swizzle pattern;
+// 0 when the swizzle is taken from the address itself (see the slab kernel).
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t base_offset = 0) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)(base_offset & 7) << 49) | ((uint64_t)1 << 62);
 }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): 128B swizzle, version 1 (Blackwell)
-//   K-major : 8-row groups 1024 B apart (SBO), LBO = 1 (x16 B)
-//   MN-major: 64-element MN groups `lbo` bytes apart, 8-K-row groups 1024 B apart (SBO)
-// base_offset (bits 49-51) = (start address >> 7) & 7 when the start is not aligned to the 1024-byte swizzle pattern
-// (a window that begins s rows into a swizzled slab); 0 for pattern-aligned tiles.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                              uint32_t base_offset = 0) {
-  uint64_t d = 0;
-  d |= (uint64_t)(base_offset & 7) << 49;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;       // version
-  d |= (uint64_t)2 << 61;       // SWIZZLE_128B
-  return d;
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void acc_zero(float* d) {
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.0f;
+}
+// keeps the compiler from moving accumulator reads above wgmma.wait_group
+template <int N>
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// the four k16 steps of one 64-wide k-tile; a step advances K-major operands 32 bytes along the swizzled row, MN-major ones
+// 16 rows (2048 bytes) -- in 16-byte descriptor units 2 / 128
+template <int N, int TA, int TB>
+__device__ __forceinline__ void mma_ktile(float* d, uint64_t a, uint64_t b) {
+#pragma unroll
+  for (int k = 0; k < GEMM_BK / 16; ++k) {
+    if constexpr (N == 32) wgmma_n32<TA, TB>(d, a + k * (TA ? 128 : 2), b + k * (TB ? 128 : 2));
+    else if constexpr (N == 64) wgmma_n64<TA, TB>(d, a + k * (TA ? 128 : 2), b + k * (TB ? 128 : 2));
+    else wgmma_n128<TA, TB>(d, a + k * (TA ? 128 : 2), b + k * (TB ? 128 : 2));
+  }
+}
+// wgmma accumulator fragment of one warp (rows 16 wl .. 16 wl + 15 of the warpgroup's 64) -> rows of the staging tile `s`
+template <int N>
+__device__ __forceinline__ void stage_acc(const float* d, float* s, int ld, int wl, int lane) {
+  const int r = 16 * wl + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(s + r * ld + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(s + (r + 8) * ld + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
 
 struct GemmParams {
@@ -164,7 +151,7 @@ struct GemmParams {
   int dual;
   void* D2;
   const float* bias2;
-  // backward extras (see epilogue_tile): ReLU-gradient mask, bias-gradient accumulation, grid scatter maps 3 / 4
+  // backward extras (see epilogue_row): ReLU-gradient mask, bias-gradient accumulation, grid scatter maps 3 / 4
   const __nv_bfloat16* mask;
   int64_t mask_ld;
   float* dbias;
@@ -180,25 +167,8 @@ __device__ __forceinline__ int tap_shift(const GemmParams& p, int tap) {
   return p.shift_sign * ((tap / p.taps_x) * p.grid_w + tap % p.taps_x);
 }
 
-// Epilogue of one 128 x BN tile for one warp (TMEM lane quarter q): wait for the accumulator stage, read it 32 columns
-// at a time, hand the stage back to the MMA warp, apply bias / ReLU and store through the output row map.
-// The accumulator of a tile may be kept as ACC partial sums (the MMA issuer rotates over them, the epilogue adds them).
-// Optional in-kernel timeline (scripts/microbench/slab_trace.py builds a private copy of the library with -DB2RL_TRACE):
-// clock64 stamps per CTA / role / tile, never compiled into the shipped library.
-#ifdef B2RL_TRACE
-__device__ unsigned long long* g_trace_buf = nullptr;
-#define B2RL_TRACE_AT(role, it, slot)                                                                            \
-  do {                                                                                                           \
-    if (g_trace_buf && (it) < 16)                                                                                \
-      g_trace_buf[((((size_t)blockIdx.x * 4 + (role)) * 16 + (it)) * 4) + (slot)] = (unsigned long long)clock64(); \
-  } while (0)
-#else
-#define B2RL_TRACE_AT(role, it, slot)
-#endif
-
-// scripts/microbench/umma_rate.cu measured on B200: one issuing thread sustains one tcgen05.mma (M=128, K=16) every
-// max(53, N/2) cycles whatever the operand majors and whether consecutive MMAs hit the same accumulator or not, so
-// ACC = 1 is used; small-N tiles are bound by that 53-cycle issue floor, not by accumulator dependencies.
+// Epilogue of one row of a 128 x BN tile for one thread: `srow` is that row of the shared staging tile (fp32 accumulators),
+// the thread handles its 32-column chunks c0, c0 + 64, ...; the 32 lanes of a warp hold 32 consecutive rows.
 // Backward extras (dgrad GEMMs): `mask` is the saved forward activation in the GEMM's own output coordinates -- the ReLU
 // gradient is applied in the epilogue (v = mask > 0 ? v : 0); `dbias` receives the column sums of the masked tile (the bias
 // gradient of the layer below) through a per-CTA shared accumulator `s_dbias`, index = column % dbias_mod.  Output row maps
@@ -208,13 +178,9 @@ __device__ unsigned long long* g_trace_buf = nullptr;
 //   map 4: rows are images b, columns are V*V positions x sub_c channels
 //          -> grid row b*G*G + (pos / V)*G + pos % V, column = channel               (fc4's input gradient -> conv3's grid)
 // Grid rows that no tile covers keep whatever the destination holds: the caller keeps it zeroed (persistent buffer).
-template <int BN, int ACC, bool EXT>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, int m0, int n0, int q, int lane, uint32_t tmem_base,
-                                              uint32_t as, uint32_t parity, bool has_acc, uint64_t* tmem_full,
-                                              uint64_t* tmem_empty, float* s_dbias, uint32_t trace_it = 1u << 30) {
-  const bool tr = q == 0 && lane == 0;
-  if (tr) B2RL_TRACE_AT(2, trace_it, 0);
-  const int row = m0 + q * 32 + lane;
+template <int BN, bool EXT>
+__device__ __forceinline__ void epilogue_row(const GemmParams& p, int row, int n0, int lane, const float* srow, int c0,
+                                             float* s_dbias) {
   bool valid = row < p.M;
   int64_t drow = row;
   int dcol0 = 0;
@@ -239,44 +205,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, int m0, int n
   } else if (EXT && p.out_map == 4) {
     img = row;
   }
-  // backward extras: the ReLU mask of this thread's row (the saved forward activation) does not depend on the accumulator --
-  // all of it is requested BEFORE the wait for the MMAs, so that its latency is hidden behind them
-  int4 mk[EXT ? BN / 8 : 1];
-  if constexpr (EXT) {
-    if (p.mask && valid) {
-      const int4* mp = reinterpret_cast<const int4*>(p.mask + (int64_t)row * p.mask_ld + n0);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j)
-        if (n0 + 8 * j < p.N) mk[j] = __ldg(mp + j);
-    }
-  }
-  if (has_acc) {
-    mb_wait(&tmem_full[as], parity);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  }
-  if (tr) B2RL_TRACE_AT(2, trace_it, 1);
-#pragma unroll
-  for (int c = 0; c < BN; c += 32) {
+  for (int c = c0; c < BN; c += 64) {
     uint32_t r[32];
-    if (has_acc) {
-      const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + as * (ACC * BN) + c;
-      tmem_ld32(t0, r);
 #pragma unroll
-      for (int a = 1; a < ACC; ++a) {
-        uint32_t r2[32];
-        tmem_ld32(t0 + a * BN, r2);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) r[j] = 0;
-    }
-    if (c + 32 >= BN && has_acc) {
-      // all TMEM reads of this warp for this tile are done: hand the accumulator stage back to the MMA warp
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      if (lane == 0) mb_arrive(&tmem_empty[as]);
-      if (tr) B2RL_TRACE_AT(2, trace_it, 2);
+    for (int j = 0; j < 32; j += 4) {
+      const float4 v = *reinterpret_cast<const float4*>(srow + c + j);
+      r[j] = __float_as_uint(v.x); r[j + 1] = __float_as_uint(v.y); r[j + 2] = __float_as_uint(v.z); r[j + 3] = __float_as_uint(v.w);
     }
     const bool live = valid && n0 + c < p.N;
     if (live) {
@@ -303,9 +237,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, int m0, int n
       }
       if constexpr (EXT) {
         if (p.mask) {                                                   // ReLU gradient: zero where the forward output was <= 0
+          const int4* mp = reinterpret_cast<const int4*>(p.mask + (int64_t)row * p.mask_ld + n0 + c);
 #pragma unroll
           for (int j = 0; j < 32; j += 8) {
-            const int4 m4 = mk[(c >> 3) + (j >> 3)];
+            const int4 m4 = __ldg(mp + (j >> 3));
             const __nv_bfloat162* mh = reinterpret_cast<const __nv_bfloat162*>(&m4);
 #pragma unroll
             for (int t = 0; t < 4; ++t) {
@@ -390,63 +325,39 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, int m0, int n
       }
     }
   }
-  if (tr) B2RL_TRACE_AT(2, trace_it, 3);
 }
 
-// Epilogue of a split-K GEMM with in-kernel fix-up (out_mode 3; fc4 forward at batch 512: 32 output tiles cannot fill 148 SMs,
-// and the 196 dependent MMAs of one un-split tile take ~5 us at the 53-cycle issue floor).  Replaces zero-fill + atomic
-// split-K + bias/ReLU pass (three launches) by one launch.  Every CTA owns exactly ONE tile (the host sizes the grid so).
-// Warp group 0 (warps 2-5) drains the accumulator into the fp32 scratch; then all EIGHT epilogue warps of the CTA that arrived
-// last at the tile's counter add the `splits` partials -- each thread requests all its partials of a 32-column chunk before
-// adding them (in split order: deterministic), so the fix-up costs about one L2 round trip.
+// Epilogue of a split-K GEMM with in-kernel fix-up (out_mode 3; fc4 forward at batch 512: 32 output tiles cannot fill the
+// SMs).  Replaces zero-fill + atomic split-K + bias/ReLU pass (three launches) by one launch.  Every CTA owns exactly ONE tile
+// (the host sizes the grid so).  All 256 MMA threads store their rows of the staged partial tile to the fp32 scratch; the
+// CTA that arrived last at the tile's counter adds the `splits` partials -- each thread requests all its partials of a
+// 32-column chunk before adding them (in split order: deterministic), so the fix-up costs about one L2 round trip.
 template <int BN>
-__device__ __forceinline__ void epilogue_fixup(const GemmParams& p, int tile, int m0, int n0, int warp, int lane,
-                                               uint32_t tmem_base, bool has_acc, uint64_t* tmem_full, uint64_t* tmem_empty,
-                                               int* s_flag) {
-  const int q = warp & 3, grp = (warp - 2) >> 2;
-  const int row = m0 + q * 32 + lane;
+__device__ __forceinline__ void epilogue_fixup(const GemmParams& p, int tile, int m0, int n0, int rl, int c0, int ct,
+                                               const float* srow, int* s_flag) {
+  const int row = m0 + rl;
   const int splits = (int)gridDim.z;
-  if (grp == 0) {
-    if (has_acc) {
-      mb_wait(&tmem_full[0], 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    float* wrow = p.ws + ((int64_t)blockIdx.z * p.ws_rows + row) * p.ws_ld + n0;
+  float* wrow = p.ws + ((int64_t)blockIdx.z * p.ws_rows + row) * p.ws_ld + n0;
+  for (int c = c0; c < BN; c += 64) {
 #pragma unroll
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t r[32];
-      if (has_acc) {
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + c, r);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = 0;
-      }
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        __stcg(reinterpret_cast<float4*>(wrow + c + j), make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                                    __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3])));
-    }
-    if (has_acc) {
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      if (lane == 0) mb_arrive(&tmem_empty[0]);
-    }
-    __threadfence();
+    for (int j = 0; j < 32; j += 4) __stcg(reinterpret_cast<float4*>(wrow + c + j), *reinterpret_cast<const float4*>(srow + c + j));
   }
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  if (warp == 2 && lane == 0) *s_flag = atomicAdd(p.counters + tile, 1) == splits - 1;
-  asm volatile("bar.sync 1, 256;" ::: "memory");
+  __threadfence();
+  named_sync(1, 256);
+  if (ct == 0) *s_flag = atomicAdd(p.counters + tile, 1) == splits - 1;
+  named_sync(1, 256);
   if (!*s_flag) return;
   __threadfence();
-  if (warp == 2 && lane == 0) p.counters[tile] = 0;                       // re-armed for the next launch
+  if (ct == 0) p.counters[tile] = 0;                                       // re-armed for the next launch
   const bool valid = row < p.M;
-  for (int c = grp * 32; c < BN; c += 64) {                                // the two warp groups take alternate 32-column chunks
+  for (int c = c0; c < BN; c += 64) {
     float acc[32];
 #pragma unroll
     for (int j = 0; j < 32; ++j) acc[j] = 0.0f;
-    for (int sp0 = 0; sp0 < splits; sp0 += 4) {                            // 4 splits x 8 float4 requested before any is added
-      float4 v[4][8];
+    for (int sp0 = 0; sp0 < splits; sp0 += 2) {                            // 2 splits x 8 float4 requested before any is added
+      float4 v[2][8];                                                      // (more in flight spills beside the accumulators)
 #pragma unroll
-      for (int s4 = 0; s4 < 4; ++s4) {
+      for (int s4 = 0; s4 < 2; ++s4) {
         if (sp0 + s4 < splits) {
           const float4* src = reinterpret_cast<const float4*>(p.ws + ((int64_t)(sp0 + s4) * p.ws_rows + row) * p.ws_ld + n0 + c);
 #pragma unroll
@@ -454,7 +365,7 @@ __device__ __forceinline__ void epilogue_fixup(const GemmParams& p, int tile, in
         }
       }
 #pragma unroll
-      for (int s4 = 0; s4 < 4; ++s4) {
+      for (int s4 = 0; s4 < 2; ++s4) {
         if (sp0 + s4 < splits) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
@@ -491,12 +402,17 @@ __device__ __forceinline__ void epilogue_fixup(const GemmParams& p, int tile, in
   }
 }
 
+// accumulator staging tile of the epilogue: 128 rows x (BN + 4) fp32 (the 4-float pad keeps the row-per-lane reads free of
+// bank conflicts)
+__host__ __device__ constexpr int acc_ld(int bn) { return bn + 4; }
+__host__ __device__ constexpr size_t acc_stage_bytes(int bn) { return (size_t)GEMM_BM * acc_ld(bn) * 4; }
+
 template <int BN, int STAGES, bool EXT>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                       const __grid_constant__ CUtensorMap tmB,
-                                                                       const __grid_constant__ CUtensorMap tmA2,
-                                                                       const __grid_constant__ CUtensorMap tmB2,
-                                                                       const GemmParams p0) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                     const __grid_constant__ CUtensorMap tmB,
+                                                                     const __grid_constant__ CUtensorMap tmA2,
+                                                                     const __grid_constant__ CUtensorMap tmB2,
+                                                                     const GemmParams p0) {
   const int n_cta = p0.dual ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   const bool second = p0.dual && (int)blockIdx.x >= n_cta;
   const int cta = second ? (int)blockIdx.x - n_cta : (int)blockIdx.x;
@@ -505,17 +421,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tcgen05_kernel(const __g
   GemmParams p = p0;
   if (second) { p.D = p0.D2; p.bias = p0.bias2; }
   constexpr uint32_t A_BYTES = GEMM_BM * GEMM_BK * 2, B_BYTES = BN * GEMM_BK * 2;
-  constexpr int ACC = 1;     // partial accumulators per tile: measured, independent chains do not raise the MMA rate
-  constexpr uint32_t TMEM_COLS = 2 * ACC * BN < 32 ? 32 : 2 * ACC * BN;   // two accumulator stages
+  constexpr int ACC_LD = acc_ld(BN);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
+  float* sAcc = reinterpret_cast<float*>(sB + STAGES * B_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sAcc + GEMM_BM * ACC_LD);
   uint64_t* empty = full + STAGES;
-  uint64_t* tmem_full = empty + STAGES;      // [2]
-  uint64_t* tmem_empty = tmem_full + 2;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
   const int m_tiles = (p.M + GEMM_BM - 1) / GEMM_BM, n_tiles = (p.N + BN - 1) / BN;
@@ -529,21 +442,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tcgen05_kernel(const __g
   __shared__ int s_fix[2];                          // out_mode 3: "this CTA arrived last at the tile's counter"
   if (threadIdx.x < 128) s_dbias[threadIdx.x] = 0.0f;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mb_init(&tmem_full[s], 1); mb_init(&tmem_empty[s], 4); }
+    for (int s = 0; s < STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(mA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(mB) : "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s2u(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_sync();   // everything above (barriers, tensor-map prefetch, TMEM allocation) overlaps the previous kernel's tail
+  pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
 
   if (warp == 0 && n_kt > 0 && elect_one()) {
     // ---------------------------------------------------------------------- TMA producer
@@ -585,62 +490,45 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tcgen05_kernel(const __g
         }
       }
     }
-  } else if (warp == 1 && n_kt > 0 && elect_one()) {
-    // ---------------------------------------------------------------------- MMA issuer
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)p.a_mn << 15) | ((uint32_t)p.b_mn << 16) |
-                           ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(GEMM_BM >> 4) << 24);
-    const uint32_t a_lo0 = desc_lo(s2u(sA), p.a_mn ? 8192 : 16), b_lo0 = desc_lo(s2u(sB), p.b_mn ? 8192 : 16);
-    const uint32_t a_step = p.a_mn ? 128 : 2, b_step = p.b_mn ? 128 : 2;
-    uint32_t it = 0, tcount = 0;
-    for (int tile = cta; tile < tiles; tile += n_cta, ++tcount) {
-      const uint32_t as = tcount & 1;
-      mb_wait(&tmem_empty[as], ((tcount >> 1) & 1) ^ 1);     // epilogue drained this accumulator stage
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t acc = tmem_base + as * (ACC * BN);
+  } else if (warp >= 4) {
+    // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: rows 64 g .. 64 g + 63
+    // (K-major A: rows 64.. start 64 x 128 bytes into the stage; MN-major A: the second [64 k][64 m] box)
+    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
+    const int rl = g * 64 + (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;   // epilogue: tile row and first 32-column chunk
+    float* sAcc_g = sAcc + g * 64 * ACC_LD;
+    const uint64_t a0 = make_desc(s2u(sA) + g * 8192, 8192), b0 = make_desc(s2u(sB), 8192);
+    uint32_t it = 0;
+    for (int tile = cta; tile < tiles; tile += n_cta) {
+      const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
+      const int m0 = mt * GEMM_BM, n0 = nt * BN;
+      float d[BN / 2];
+      acc_zero<BN>(d);
       for (int i = 0; i < n_kt; ++i, ++it) {
         const int s = it % STAGES;
         mb_wait(&full[s], (it / STAGES) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // K-major: 16 k-elements = 32 bytes along the swizzled row; MN-major: 16 k-rows = 2048 bytes (in 16-byte units: 2 / 128)
-        uint32_t a_lo = a_lo0 + (uint32_t)s * (A_BYTES >> 4), b_lo = b_lo0 + (uint32_t)s * (B_BYTES >> 4);
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k) {
-          // k16 step k of every k-tile goes to partial accumulator k % ACC: ACC independent accumulation chains
-          umma_f16_lh(acc + (k % ACC) * BN, a_lo, b_lo, idesc, (i > 0 || k >= ACC) ? 1u : 0u);
-          a_lo += a_step;
-          b_lo += b_step;
+        const uint64_t a = a0 + (uint64_t)s * (A_BYTES >> 4), b = b0 + (uint64_t)s * (B_BYTES >> 4);
+        wg_fence();
+        if (!p.a_mn) {
+          if (!p.b_mn) mma_ktile<BN, 0, 0>(d, a, b);
+          else mma_ktile<BN, 0, 1>(d, a, b);
+        } else {
+          if (!p.b_mn) mma_ktile<BN, 1, 0>(d, a, b);
+          else mma_ktile<BN, 1, 1>(d, a, b);
         }
-        umma_commit(&empty[s]);                    // frees the smem stage when these MMAs retire
+        wg_commit();
+        wg_wait0();
+        acc_fence<BN>(d);
+        if (lane == 0) mb_arrive(&empty[s]);
       }
-      umma_commit(&tmem_full[as]);                 // accumulator of this tile complete
-    }
-  } else if (warp >= 2) {
-    // ---------------------------------------------------------------------- epilogue (warp%4 selects the TMEM lane quarter)
-    if (!EXT && p.out_mode == 3) {
-      // split-K with in-kernel fix-up: one tile per CTA, all eight epilogue warps take part in the fix-up
-      if (cta < tiles) {
-        const int mt = cta / n_tiles, nt = cta - mt * n_tiles;
-        epilogue_fixup<BN>(p, cta, mt * GEMM_BM, nt * BN, warp, lane, tmem_base, n_kt > 0, tmem_full, tmem_empty, s_fix);
-      }
-    } else {
-      // two groups of four warps, one per accumulator stage: the epilogue of tile t overlaps that of tile t+1
-      const int q = warp & 3;
-      const uint32_t grp = (uint32_t)(warp - 2) >> 2;
-      uint32_t tcount = 0;
-      for (int tile = cta; tile < tiles; tile += n_cta, ++tcount) {
-        if ((tcount & 1) != grp) continue;
-        const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-        const int m0 = mt * GEMM_BM, n0 = nt * BN;
-        epilogue_tile<BN, ACC, EXT>(p, m0, n0, q, lane, tmem_base, tcount & 1, (tcount >> 1) & 1, n_kt > 0, tmem_full, tmem_empty, s_dbias);
-      }
+      stage_acc<BN>(d, sAcc_g, ACC_LD, wl, lane);
+      named_sync(2 + g, 128);
+      if (!EXT && p.out_mode == 3) epilogue_fixup<BN>(p, tile, m0, n0, rl, c0, cw * 32 + lane, sAcc + rl * ACC_LD, s_fix);
+      else epilogue_row<BN, EXT>(p, m0 + rl, n0, lane, sAcc + rl * ACC_LD, c0, s_dbias);
+      named_sync(2 + g, 128);                        // staging tile read: the next tile may overwrite it
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
   if (EXT && p.dbias && p.dbias_mod > 0 && (int)threadIdx.x < p.dbias_mod) atomicAdd(p.dbias + threadIdx.x, s_dbias[threadIdx.x]);
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-  }
 }
 
 
@@ -648,11 +536,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tcgen05_kernel(const __g
 // Slab variant of the forward / dgrad convolution GEMM: the taps of a tile read overlapping row windows of the same
 // activation matrix, so the CTA loads ONE slab of 128 + max_shift rows per tile and issues every tap's MMAs on windows
 // that start `shift` rows (x 128 bytes) into that swizzled slab.  The 128-byte swizzle is a pure function of the shared
-// memory ADDRESS (bits 4-6 ^= bits 7-9), for TMA writes and UMMA reads alike, so a window may start at any row of a
-// 1024-byte-aligned slab with descriptor base_offset = 0 (measured on B200: base_offset = (start >> 7) & 7 gives wrong
-// results, 0 gives the right ones).  The weights (all taps) are loaded once per CTA and stay resident.  Activation traffic drops by the
-// number of taps (4x conv1/conv2, 9x conv3) and the weight traffic per tile to zero.
-// ---------------------------------------------------------------------------------------------------------------
+// memory ADDRESS (bits 4-6 ^= bits 7-9), for TMA writes and wgmma reads alike, so a window may start at any row of a
+// 1024-byte-aligned slab with descriptor base_offset = 0 (base_offset_mode 2; mode 1 sets (start >> 7) & 7 instead).  The
+// weights (all taps) are loaded once per CTA and stay resident.  Activation traffic drops by the number of taps (4x
+// conv1/conv2, 9x conv3) and the weight traffic per tile to zero.
 // ---------------------------------------------------------------------------------------------------------------
 // K1: fused replay gather -> exact u8->bf16 -> conv1 operand.  Instead of reading a materialised bf16 space-to-depth matrix
 // (57.8 MB per batch-512 stack, written by the gather kernel and re-read here), conv1's forward and weight-gradient kernels
@@ -696,7 +583,7 @@ __device__ __forceinline__ int4 cvt8_u8_bf16(uint32_t w0, uint32_t w1) {
 // (the 4 pixel rows of one grid row of one frame are 4 * frame_w contiguous bytes = frame_w words): the pixels a slab needs from
 // ONE image are the box [4 frames][slots grid rows][frame_w words] at (word 0, grid row q0 - b*G, ring row idx[b] + first) --
 // one tensor load per image the slab touches (at most two), instead of one bulk copy per (image, frame) whose fixed cost
-// (~0.2 us each, serialised per SM) made the kernel twice as slow as the bf16 version.  Grid rows past the end of the image are
+// is serialised per SM.  Grid rows past the end of the image are
 // zero-filled by the TMA and never read.
 //   staging layout of one tile: [image segment 0 | 1][frame f][slot = grid-row index q - qseg][4 * frame_w bytes]
 constexpr int U8_MAX_STAGES = 8;
@@ -743,7 +630,7 @@ __device__ __forceinline__ void u8_issue(const U8Src& u, const CUtensorMap* map,
 
 // explicit shared-space accesses: the staging / slab pointers are carved out of the dynamic shared memory through integer
 // arithmetic, so the compiler only sees GENERIC pointers -- generic loads of shared memory go through the L1 path with ~10x the
-// latency of LDS (measured: the converters took 4 000 cycles per tile with them, long_scoreboard-bound)
+// latency of LDS
 __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
@@ -778,7 +665,7 @@ __device__ __forceinline__ void u8_store_chunks(uint32_t stage, uint32_t slab, i
 // `slab_rows` rows x 64 channels whose first row is grid-matrix row R0; rows >= u.rows are zero (what the TMA's out-of-bounds
 // fill gave).  Thread t owns slab row t & 127 (consecutive threads -> consecutive pixels of the staging rows and the 8 distinct
 // swizzle positions of a 128-byte window: conflict-free both ways) and, with 256 threads, one half of its 8 chunks; rows beyond
-// 128 are shared out chunk-wise.  On return every thread's stores are fenced towards the async proxy (tcgen05.mma reads shared
+// 128 are shared out chunk-wise.  On return every thread's stores are fenced towards the async proxy (wgmma reads shared
 // memory through it) and all NT threads have arrived.
 template <int NT>
 __device__ __forceinline__ void u8_convert(const U8Src& u, const uint8_t* stage_p, uint8_t* slab_p, int R0, int slab_rows,
@@ -830,15 +717,13 @@ struct SlabParams {
   U8Src u8;                // U8 kernels: the activation slabs are built from the uint8 frame ring (K1), tmA is unused
 };
 
-// BN = 32 (conv1, 12 tiles per SM, 16 KB of weights) compiles for two resident CTAs per SM: with many tiles the work can be
-// split over 2 x 148 CTAs whose waits interleave (launch_slab uses a <= 110 KB shared-memory budget then).
-constexpr int SLAB_U8_THREADS = GEMM_THREADS + 128;   // K1: four converter warps (10-13) behind the ten of the TMA version
+constexpr int SLAB_U8_THREADS = GEMM_THREADS + 128;   // K1: a fourth warpgroup (warps 12-15) converts the uint8 pixels
 template <int BN, bool EXT, bool U8>
-__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, (BN == 32 && !U8) ? 2 : 1) conv_slab_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                            const __grid_constant__ CUtensorMap tmB,
-                                                                            const __grid_constant__ CUtensorMap tmA2,
-                                                                            const __grid_constant__ CUtensorMap tmB2,
-                                                                            const SlabParams sp) {
+__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_slab_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                          const __grid_constant__ CUtensorMap tmB,
+                                                                          const __grid_constant__ CUtensorMap tmA2,
+                                                                          const __grid_constant__ CUtensorMap tmB2,
+                                                                          const SlabParams sp) {
   const int n_cta = sp.g.dual ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   const bool second = sp.g.dual && (int)blockIdx.x >= n_cta;
   const int cta = second ? (int)blockIdx.x - n_cta : (int)blockIdx.x;
@@ -846,10 +731,8 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, (BN == 32
   const CUtensorMap* mB = second ? &tmB2 : &tmB;
   GemmParams p = sp.g;
   if (second) { p.D = sp.g.D2; p.bias = sp.g.bias2; }
-  if (threadIdx.x == 0) B2RL_TRACE_AT(3, 0, 0);
   constexpr uint32_t W_TILE = BN * 128;                               // one 64-wide k-tile of the weights
-  constexpr int ACC = 1;
-  constexpr uint32_t TMEM_COLS = 2 * ACC * BN < 32 ? 32 : 2 * ACC * BN;
+  constexpr int ACC_LD = acc_ld(BN);
   constexpr int MAX_STAGES = 6;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -858,16 +741,14 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, (BN == 32
   const uint32_t slab_bytes = slab_block * sp.col_blocks;
   uint8_t* sW = smem;
   uint8_t* sS = smem + (size_t)k_tiles * W_TILE;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sS + (size_t)sp.stages * slab_bytes);
+  float* sAcc = reinterpret_cast<float*>(sS + (size_t)sp.stages * slab_bytes);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sAcc + GEMM_BM * ACC_LD);
   uint64_t* empty = full + MAX_STAGES;
-  uint64_t* tmem_full = empty + MAX_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint64_t* w_full = tmem_empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_full + 1);
-  // U8 (K1): uint8 staging tiles + their full / empty barriers live behind the slab ring (launch_slab_t sizes the allocation)
+  uint64_t* w_full = empty + MAX_STAGES;
+  // U8 (K1): uint8 staging tiles + their full / empty barriers live behind the barriers (launch_slab_t sizes the allocation)
   const int u8_slots_ = U8 ? u8_slots(sp.slab_rows, sp.u8.G) : 0;
   const int u8_bytes = U8 ? u8_stage_bytes(sp.slab_rows, sp.u8.G, sp.u8.frame_w) : 0;
-  uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 127) & ~uintptr_t(127));
+  uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w_full + 2) + 127) & ~uintptr_t(127));
   const int U8_STAGES = U8 ? sp.u8.stages : 1;
   uint64_t* u8_full = reinterpret_cast<uint64_t*>(sU + (size_t)U8_STAGES * u8_bytes);
   uint64_t* u8_empty = u8_full + U8_MAX_STAGES;
@@ -878,8 +759,7 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, (BN == 32
   __shared__ float s_dbias[128];                    // per-CTA bias-gradient accumulator (backward extras)
   if (threadIdx.x < 128) s_dbias[threadIdx.x] = 0.0f;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mb_init(&tmem_full[s], 1); mb_init(&tmem_empty[s], 4); }
+    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS); }
     mb_init(w_full, 1);
     if (U8) {
       for (int s = 0; s < U8_STAGES; ++s) { mb_init(&u8_full[s], 1); mb_init(&u8_empty[s], 1); }
@@ -888,59 +768,45 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, (BN == 32
     asm volatile("prefetch.tensormap [%0];" ::"l"(mA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(mB) : "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s2u(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_sync();   // everything above (barriers, tensor-map prefetch, TMEM allocation) overlaps the previous kernel's tail
+  pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
 
   if (warp == 0 && elect_one()) {
-   if constexpr (U8) {
-    // ---------------------------------------------------------------------- K1 producer: weights, then the uint8 pixels of every
-    // tile (one tensor load per image the slab touches), up to sp.u8.stages tiles ahead; idx[] is requested one tile early
     mb_expect_tx(w_full, (uint32_t)k_tiles * W_TILE);
     for (int kt = 0; kt < k_tiles; ++kt) tma_load_2d(sW + (size_t)kt * W_TILE, mB, w_full, kt * GEMM_BK, 0);
-    const int nimg = sp.u8.rows / (sp.u8.G * sp.u8.G);
-    U8Plan pl = u8_plan(sp.u8, cta * GEMM_BM + sp.min_shift, sp.slab_rows);
-    long long i0 = 0, i1 = 0;
-    if (cta < tiles && pl.n0 > 0) { i0 = __ldg(sp.u8.idx + pl.b0); i1 = __ldg(sp.u8.idx + min(pl.b0 + 1, nimg - 1)); }
-    uint32_t it = 0;
-    for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
-      const U8Plan cur = pl;
-      const long long c0 = i0, c1 = i1;
-      if (tile + n_cta < tiles) {
-        pl = u8_plan(sp.u8, (tile + n_cta) * GEMM_BM + sp.min_shift, sp.slab_rows);
-        if (pl.n0 > 0) { i0 = __ldg(sp.u8.idx + pl.b0); i1 = __ldg(sp.u8.idx + min(pl.b0 + 1, nimg - 1)); }
+    if constexpr (U8) {
+      // -------------------------------------------------------------------- K1 producer: the uint8 pixels of every tile (one
+      // tensor load per image the slab touches), up to sp.u8.stages tiles ahead; idx[] is requested one tile early
+      const int nimg = sp.u8.rows / (sp.u8.G * sp.u8.G);
+      U8Plan pl = u8_plan(sp.u8, cta * GEMM_BM + sp.min_shift, sp.slab_rows);
+      long long i0 = 0, i1 = 0;
+      if (cta < tiles && pl.n0 > 0) { i0 = __ldg(sp.u8.idx + pl.b0); i1 = __ldg(sp.u8.idx + min(pl.b0 + 1, nimg - 1)); }
+      uint32_t it = 0;
+      for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
+        const U8Plan cur = pl;
+        const long long c0 = i0, c1 = i1;
+        if (tile + n_cta < tiles) {
+          pl = u8_plan(sp.u8, (tile + n_cta) * GEMM_BM + sp.min_shift, sp.slab_rows);
+          if (pl.n0 > 0) { i0 = __ldg(sp.u8.idx + pl.b0); i1 = __ldg(sp.u8.idx + min(pl.b0 + 1, nimg - 1)); }
+        }
+        const int us = it % U8_STAGES;
+        mb_wait(&u8_empty[us], ((it / U8_STAGES) & 1) ^ 1);
+        u8_issue(sp.u8, mA, cur, c0, c1, sU + (size_t)us * u8_bytes, &u8_full[us], u8_slots_);
       }
-      const int us = it % U8_STAGES;
-      mb_wait(&u8_empty[us], ((it / U8_STAGES) & 1) ^ 1);
-      u8_issue(sp.u8, mA, cur, c0, c1, sU + (size_t)us * u8_bytes, &u8_full[us], u8_slots_);
-    }
-   } else {
-    // ---------------------------------------------------------------------- TMA producer
-    B2RL_TRACE_AT(3, 0, 1);
-    mb_expect_tx(w_full, (uint32_t)k_tiles * W_TILE);
-    for (int kt = 0; kt < k_tiles; ++kt) tma_load_2d(sW + (size_t)kt * W_TILE, mB, w_full, kt * GEMM_BK, 0);
-    uint32_t it = 0;
-    if (!U8) {
+    } else {
+      // -------------------------------------------------------------------- TMA producer: one slab per tile
+      uint32_t it = 0;
       for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
         const int s = it % sp.stages;
-        B2RL_TRACE_AT(0, it, 0);
         mb_wait(&empty[s], ((it / sp.stages) & 1) ^ 1);
-        B2RL_TRACE_AT(0, it, 1);
         mb_expect_tx(&full[s], slab_bytes);
         for (int cb = 0; cb < sp.col_blocks; ++cb)
           tma_load_2d(sS + (size_t)s * slab_bytes + (size_t)cb * slab_block, mA, &full[s], cb * GEMM_BK,
                       tile * GEMM_BM + sp.min_shift);
       }
     }
-   }
-  } else if (U8 && warp >= 10) {
-    // ---------------------------------------------------------------------- K1 converters (warps 10-13): staged uint8 -> slab
+  } else if (U8 && warp >= 12) {
+    // ---------------------------------------------------------------------- K1 converters (warps 12-15): staged uint8 -> slab
     const int tid = (int)threadIdx.x - GEMM_THREADS;
     uint32_t it = 0;
     for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
@@ -948,78 +814,63 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, (BN == 32
       mb_wait(&empty[s], ((it / sp.stages) & 1) ^ 1);
       mb_wait(&u8_full[us], (it / U8_STAGES) & 1);
       u8_convert<128>(sp.u8, sU + (size_t)us * u8_bytes, sS + (size_t)s * slab_bytes, tile * GEMM_BM + sp.min_shift,
-                      sp.slab_rows, u8_slots_, tid, 2);
+                      sp.slab_rows, u8_slots_, tid, 4);
       if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
     }
-  } else if (warp == 1 && elect_one()) {
-    // ---------------------------------------------------------------------- MMA issuer
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(GEMM_BM >> 4) << 24);
-    mb_wait(w_full, 0);
-    B2RL_TRACE_AT(3, 0, 2);
-    const uint32_t slab_lo0 = desc_lo(s2u(sS), 16), w_lo0 = desc_lo(s2u(sW), 16);
+  } else if (warp >= 4 && warp < 12) {
+    // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: rows 64 g .. 64 g + 63
+    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
+    const int rl = g * 64 + (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;
+    float* sAcc_g = sAcc + g * 64 * ACC_LD;
+    const uint32_t slab0 = s2u(sS) + (uint32_t)g * 64 * 128, w0 = s2u(sW);
     const int taps_y = sp.taps / p.taps_x;
+    mb_wait(w_full, 0);
     uint32_t it = 0;
     for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
-      const uint32_t as = it & 1;
       const int s = it % sp.stages;
-      B2RL_TRACE_AT(1, it, 0);
-      mb_wait(&tmem_empty[as], ((it >> 1) & 1) ^ 1);
-      B2RL_TRACE_AT(1, it, 1);
       mb_wait(&full[s], (it / sp.stages) & 1);
-      B2RL_TRACE_AT(1, it, 2);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t acc = tmem_base + as * (ACC * BN);
-      const uint32_t slab_lo = slab_lo0 + (uint32_t)s * (slab_bytes >> 4);
-      uint32_t nmma = 0, b_lo = w_lo0;                                // nmma: MMAs issued for this tile (rotates the partials)
+      float d[BN / 2];
+      acc_zero<BN>(d);
+      const uint32_t slab = slab0 + (uint32_t)s * slab_bytes;
+      uint32_t kt = 0;
       // taps in (dy, dx) order; the window of tap (dy, dx) starts sign*(dy*grid_w + dx) - min_shift rows into the slab
       int row_dy = -sp.min_shift;                                   // rows, for dx = 0
       for (int dy = 0; dy < taps_y; ++dy, row_dy += p.shift_sign * p.grid_w) {
         int row = row_dy;
         for (int dx = 0; dx < p.taps_x; ++dx, row += p.shift_sign) {
-          uint32_t a_cb = slab_lo + (uint32_t)row * 8;              // 128 bytes per row = 8 x 16 B
-          for (int cb = 0; cb < sp.col_blocks; ++cb, a_cb += slab_block >> 4) {
-            uint32_t a_lo = a_cb;
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) {
-              umma_f16_lh(acc + (k % ACC) * BN, a_lo, b_lo, idesc, (nmma > 0 || k >= ACC) ? 1u : 0u);
-              a_lo += 2;
-              b_lo += 2;
-            }
-            nmma = 1;
-            b_lo += (W_TILE >> 4) - 8;                              // next 64-wide k-tile of the resident weights
+          for (int cb = 0; cb < sp.col_blocks; ++cb, ++kt) {
+            const uint32_t a_addr = slab + cb * slab_block + (uint32_t)row * 128;
+            const uint64_t a = make_desc(a_addr, 16, sp.base_offset_mode == 1 ? (a_addr >> 7) & 7 : 0);
+            // one commit group per k-tile: accumulator chains carried across the runtime tap loops without a wait make
+            // ptxas serialize every wgmma
+            wg_fence();
+            mma_ktile<BN, 0, 0>(d, a, make_desc(w0 + kt * W_TILE, 16));
+            wg_commit();
+            wg_wait0();
+            acc_fence<BN>(d);
           }
         }
       }
-      umma_commit(&empty[s]);
-      umma_commit(&tmem_full[as]);
-      B2RL_TRACE_AT(1, it, 3);
+      if (lane == 0) mb_arrive(&empty[s]);
+      stage_acc<BN>(d, sAcc_g, ACC_LD, wl, lane);
+      named_sync(2 + g, 128);
+      epilogue_row<BN, EXT>(p, tile * GEMM_BM + rl, 0, lane, sAcc + rl * ACC_LD, c0, s_dbias);
+      named_sync(2 + g, 128);
     }
-  } else if (warp >= 2 && warp < 10) {
-    const int q = warp & 3;
-    const uint32_t grp = (uint32_t)(warp - 2) >> 2;                    // accumulator stage this warp group drains
-    uint32_t it = 0;
-    for (int tile = cta; tile < tiles; tile += n_cta, ++it)
-      if ((it & 1) == grp)
-        epilogue_tile<BN, ACC, EXT>(p, tile * GEMM_BM, 0, q, lane, tmem_base, it & 1, (it >> 1) & 1, true, tmem_full, tmem_empty, s_dbias, it);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
   if (EXT && p.dbias && (int)threadIdx.x < p.dbias_mod) atomicAdd(p.dbias + threadIdx.x, s_dbias[threadIdx.x]);
-  if (threadIdx.x == 0) B2RL_TRACE_AT(3, 0, 3);
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-  }
 }
 
 
 // ---------------------------------------------------------------------------------------------------------------
 // Slab variant of the convolution weight gradient:  D[n, tap*C + c] += sum_r G[r, n] * X[r + shift(tap), c].
-// Both operands are read as stored (MN-major, K = rows).  A CTA owns a contiguous range of 64-row k-tiles; per k-tile it
-// loads the gradient rows ONCE and ONE slab of 64 + max_shift activation rows, and issues every tap's MMAs on windows of
-// that slab (a K-row shift is a 128-byte step in the MN-major swizzled layout, address-based swizzle as above) into one
-// TMEM accumulator per tap (taps x C fp32 columns, <= 512).  At the end each CTA stores its partial sums plainly at
-// D + blockIdx.x * partial_stride (the consumer sums them: deterministic), or adds them to D with fp32 vector atomics
-// when partial_stride == 0.
+// Both operands are read as stored (MN-major, K = rows).  A CTA owns a contiguous range of 64-row k-tiles (blockIdx.x) and
+// one group of taps (blockIdx.y: 128 output columns, two taps of 64 channels or one of 128); per k-tile it loads the
+// gradient rows ONCE and ONE slab of 64 + max_shift activation rows, and issues every tap's MMAs on windows of that slab (a
+// K-row shift is a 128-byte step in the MN-major swizzled layout, address-based swizzle as above) into register
+// accumulators.  At the end each CTA stores its partial sums plainly at D + blockIdx.x * partial_stride (the consumer sums
+// them: deterministic), or adds them to D with fp32 vector atomics when partial_stride == 0.
 // ---------------------------------------------------------------------------------------------------------------
 struct WgradParams {
   int rows, n_out, C, col_blocks;
@@ -1028,27 +879,23 @@ struct WgradParams {
   float* D;
   int ldd;
   int64_t partial_stride;   // 0: atomically accumulate into D; > 0: CTA i stores its partial sums at D + i*partial_stride
-  // MMAs of one k16 step, built on the host (launch_wgrad): with one 64-channel column block per tap (C == 64) the taps of
-  // one grid row (dx = 0..taps_x-1) are ONE MMA -- their windows start 1 row = 128 bytes apart in the slab, which is an
-  // MN-major B operand of N = run*64 columns whose 64-element groups are LBO = 128 bytes apart (the 128-byte swizzle is a
-  // function of the address, so overlapping groups read the right bytes) with adjacent TMEM accumulator columns.
+  // one window per tap, built on the host (launch_wgrad): slab window offset (16-byte units) and accumulator column
   int n_runs;
-  uint32_t run_off[9], run_acc[9], run_n[9];   // slab window offset (16-byte units), accumulator column, N of the MMA
-  // M-stacking (n_out <= 64): the A operand's second 64-row half holds the SAME gradient columns read `stack_delta` rows away
-  // (a second TMA box), so accumulator lanes 64-127 of a window at shift s hold the tap at shift s - stack_delta: with
-  // stack_delta = -grid_w the windows of tap row dy also produce tap row dy + 1 -- the last tap row costs no MMAs at all
-  // (conv2 / conv1: half the MMAs; conv3: 6 windows instead of 9 taps, 384 columns, ONE launch instead of two).
+  uint32_t run_off[9], run_acc[9];
+  // M-stacking (n_out <= 64): warpgroup 2's A operand holds the SAME gradient columns read `stack_delta` rows away (a second
+  // TMA box), so its accumulator rows of a window at shift s hold the tap at shift s - stack_delta: with stack_delta = -grid_w
+  // the windows of tap row dy also produce tap row dy + 1 -- the last tap row costs no MMAs at all (conv2 / conv1: half the
+  // MMAs; conv3: 6 windows instead of 9 taps).
   // run_low[j] = first output column of the lower half of run j, or -1 (a duplicate of an upper tap: dropped).
   int stack_delta, stack_rows;
   int run_low[9];
   U8Src u8;                                    // U8 kernels: the activation slabs come from the uint8 frame ring (K1)
 };
 
-template <int TMEM_COLS, bool U8>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) conv_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmG,
-                                                                             const __grid_constant__ CUtensorMap tmX,
-                                                                             const WgradParams w) {
-  if (threadIdx.x == 0) B2RL_TRACE_AT(3, 0, 0);
+template <bool U8>
+__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmG,
+                                                                                             const __grid_constant__ CUtensorMap tmX,
+                                                                                             const WgradParams w) {
   constexpr int MAX_STAGES = 6;
   constexpr uint32_t A_BYTES = 2 * 8192;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -1057,12 +904,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) conv_wgrad_tcgen05_kernel(con
   const uint32_t stage_bytes = A_BYTES + slab_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)w.stages * stage_bytes);
   uint64_t* empty = full + MAX_STAGES;
-  uint64_t* tmem_full = empty + MAX_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
   // U8 (K1): uint8 staging tiles + their full / empty barriers behind the operand ring (launch_wgrad sizes the allocation)
   const int u8_slots_ = U8 ? u8_slots(w.slab_rows, w.u8.G) : 0;
   const int u8_bytes = U8 ? u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w) : 0;
-  uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 127) & ~uintptr_t(127));
+  uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(empty + MAX_STAGES) + 127) & ~uintptr_t(127));
   const int U8_STAGES = U8 ? w.u8.stages : 1;
   uint64_t* u8_full = reinterpret_cast<uint64_t*>(sU + (size_t)U8_STAGES * u8_bytes);
   uint64_t* u8_empty = u8_full + U8_MAX_STAGES;
@@ -1072,8 +917,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) conv_wgrad_tcgen05_kernel(con
   const int n_kt = max(min(kt_total, kt_begin + w.k_tiles_per_cta) - kt_begin, 0);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], U8 ? 2 : 1); mb_init(&empty[s], 1); }   // U8: TMA + converters
-    mb_init(tmem_full, 1);
+    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], U8 ? 2 : 1); mb_init(&empty[s], MMA_WARPS); }   // U8: TMA + converters
     if (U8) {
       for (int s = 0; s < U8_STAGES; ++s) { mb_init(&u8_full[s], 1); mb_init(&u8_empty[s], 1); }
     }
@@ -1081,144 +925,115 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) conv_wgrad_tcgen05_kernel(con
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s2u(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_sync();   // everything above (barriers, tensor-map prefetch, TMEM allocation) overlaps the previous kernel's tail
+  pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
 
   if (warp == 0 && elect_one()) {
-   if constexpr (U8) {
-    // K1 producer: the uint8 pixels of every k-tile (one tensor load per image its slab touches, up to w.u8.stages k-tiles ahead,
-    // idx[] one k-tile early) and the gradient rows
-    const int nimg = w.u8.rows / (w.u8.G * w.u8.G);
-    U8Plan pl = u8_plan(w.u8, kt_begin * GEMM_BK, w.slab_rows);
-    long long i0 = 0, i1 = 0;
-    if (n_kt > 0 && pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
-    for (int i = 0; i < n_kt; ++i) {
-      const U8Plan cur = pl;
-      const long long c0 = i0, c1 = i1;
-      if (i + 1 < n_kt) {
-        pl = u8_plan(w.u8, (kt_begin + i + 1) * GEMM_BK, w.slab_rows);
-        if (pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
-      }
-      const int us = i % U8_STAGES, s = i % w.stages;
-      mb_wait(&u8_empty[us], ((i / U8_STAGES) & 1) ^ 1);
-      u8_issue(w.u8, &tmX, cur, c0, c1, sU + (size_t)us * u8_bytes, &u8_full[us], u8_slots_);
-      mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
-      mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192);
-      uint8_t* st = smem + (size_t)s * stage_bytes;
-      for (int g = 0; g < w.a_boxes; ++g)
-        tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, (kt_begin + i) * GEMM_BK + (g ? w.stack_delta : 0));
-    }
-   } else {
-    B2RL_TRACE_AT(3, 0, 1);
-    for (int i = 0; i < n_kt; ++i) {
-      const int s = i % w.stages;
-      B2RL_TRACE_AT(0, i, 0);
-      mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
-      B2RL_TRACE_AT(0, i, 1);
-      mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192 + (U8 ? 0u : slab_bytes));
-      uint8_t* st = smem + (size_t)s * stage_bytes;
-      const int k0 = (kt_begin + i) * GEMM_BK;
-      for (int g = 0; g < w.a_boxes; ++g)                                                                 // [64 k][64 n]
-        tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, k0 + (g ? w.stack_delta : 0));
-      if (!U8) {
-        for (int cb = 0; cb < w.col_blocks; ++cb)
-          tma_load_2d(st + A_BYTES + (size_t)cb * slab_block, &tmX, &full[s], cb * GEMM_BK, k0);         // [slab_rows][64 c]
-      }
-    }
-   }
-  } else if (warp == 1 && n_kt > 0 && elect_one()) {
-    const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(GEMM_BM >> 4) << 24);
-    const bool merge = w.C == 64;
-    const uint32_t a_lo0 = desc_lo(s2u(smem), 8192), b_lo0 = desc_lo(s2u(smem + A_BYTES), merge ? 128u : slab_block);
-    for (int i = 0; i < n_kt; ++i) {
-      const int s = i % w.stages;
-      B2RL_TRACE_AT(1, i, 0);
-      mb_wait(&full[s], (i / w.stages) & 1);
-      B2RL_TRACE_AT(1, i, 2);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a_st = a_lo0 + (uint32_t)s * (stage_bytes >> 4), b_st = b_lo0 + (uint32_t)s * (stage_bytes >> 4);
-      // runs outer (table in the constant bank, not unrolled), k16 steps inner: the issuing thread must stay lean --
-      // a fully unrolled predicated table cost ~190 cycles of bookkeeping per MMA
-      const uint32_t first = i > 0 ? 1u : 0u;
-#pragma unroll 1
-      for (int j = 0; j < w.n_runs; ++j) {
-        const uint32_t acc = tmem_base + w.run_acc[j], idesc = idesc0 | ((w.run_n[j] >> 3) << 17);
-        const uint32_t b_j = b_st + w.run_off[j];
-        umma_f16_lh(acc, a_st, b_j, idesc, first);
-#pragma unroll
-        for (int k = 1; k < GEMM_BK / 16; ++k) umma_f16_lh(acc, a_st + k * 128, b_j + k * 128, idesc, 1u);
-      }
-      umma_commit(&empty[s]);
-      B2RL_TRACE_AT(1, i, 3);
-    }
-    umma_commit(tmem_full);
-  } else if (warp >= 2 && n_kt > 0) {
-    if (U8) {
-      // K1 converters (all eight epilogue warps, idle until the accumulators are complete): the activation slab of every k-tile
-      // from the staged uint8 pixels
-      const int tid = (int)threadIdx.x - 2 * 32;
+    if constexpr (U8) {
+      // K1 producer: the uint8 pixels of every k-tile (one tensor load per image its slab touches, up to w.u8.stages k-tiles
+      // ahead, idx[] one k-tile early) and the gradient rows
+      const int nimg = w.u8.rows / (w.u8.G * w.u8.G);
+      U8Plan pl = u8_plan(w.u8, kt_begin * GEMM_BK, w.slab_rows);
+      long long i0 = 0, i1 = 0;
+      if (n_kt > 0 && pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
       for (int i = 0; i < n_kt; ++i) {
-        const int s = i % w.stages, us = i % U8_STAGES;
+        const U8Plan cur = pl;
+        const long long c0 = i0, c1 = i1;
+        if (i + 1 < n_kt) {
+          pl = u8_plan(w.u8, (kt_begin + i + 1) * GEMM_BK, w.slab_rows);
+          if (pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
+        }
+        const int us = i % U8_STAGES, s = i % w.stages;
+        mb_wait(&u8_empty[us], ((i / U8_STAGES) & 1) ^ 1);
+        u8_issue(w.u8, &tmX, cur, c0, c1, sU + (size_t)us * u8_bytes, &u8_full[us], u8_slots_);
         mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
-        mb_wait(&u8_full[us], (i / U8_STAGES) & 1);
-        u8_convert<256>(w.u8, sU + (size_t)us * u8_bytes, smem + (size_t)s * stage_bytes + A_BYTES, (kt_begin + i) * GEMM_BK,
-                        w.slab_rows, u8_slots_, tid, 2);
-        if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
+        mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192);
+        uint8_t* st = smem + (size_t)s * stage_bytes;
+        for (int g = 0; g < w.a_boxes; ++g)
+          tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, (kt_begin + i) * GEMM_BK + (g ? w.stack_delta : 0));
+      }
+    } else {
+      for (int i = 0; i < n_kt; ++i) {
+        const int s = i % w.stages;
+        mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
+        mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192 + slab_bytes);
+        uint8_t* st = smem + (size_t)s * stage_bytes;
+        const int k0 = (kt_begin + i) * GEMM_BK;
+        for (int g = 0; g < w.a_boxes; ++g)                                                                 // [64 k][64 n]
+          tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, k0 + (g ? w.stack_delta : 0));
+        for (int cb = 0; cb < w.col_blocks; ++cb)
+          tma_load_2d(st + A_BYTES + (size_t)cb * slab_block, &tmX, &full[s], cb * GEMM_BK, k0);           // [slab_rows][64 c]
       }
     }
-    const int q = warp & 3;
-    const int n = q * 32 + lane;
-    if (warp == 4 && lane == 0) B2RL_TRACE_AT(2, 0, 0);
-    mb_wait(tmem_full, 0);
-    if (warp == 4 && lane == 0) B2RL_TRACE_AT(2, 0, 1);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int cols = w.ntaps * w.C;
-    const bool low = w.stack_delta != 0 && q >= 2;                     // lanes 64-127: the stacked copy (warp-uniform)
-    const int nn = low ? n - 64 : n;
-    for (int c = ((warp - 2) >> 2) * 32; c < cols; c += 64) {         // the two warp groups take alternate 32-column chunks
-      int oc = w.tap0 * w.C + c;
-      if (low) {
-        int j = 0;
-        while (j + 1 < w.n_runs && (uint32_t)c >= w.run_acc[j + 1]) ++j;
-        if (w.run_low[j] < 0) continue;                                // duplicate of a tap the upper half already holds
-        oc = w.run_low[j] + (c - (int)w.run_acc[j]);
-      }
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + c, r);
-      if (nn < w.n_out) {
-        float* d = w.D + (int64_t)blockIdx.x * w.partial_stride + (int64_t)nn * w.ldd + oc;
-        if (w.partial_stride > 0) {
-          // split-K partials are stored plainly (coalesced 16-byte stores) and summed by the consumer
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(d + j) = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                            __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-        } else if ((reinterpret_cast<uintptr_t>(d) & 15) == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)       // 16-byte vector reductions (red.global.add.v4.f32)
-            atomicAdd(reinterpret_cast<float4*>(d + j), make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                                    __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3])));
+  } else if (U8 && warp >= 12) {
+    // K1 converters (warps 12-15): the activation slab of every k-tile from the staged uint8 pixels
+    const int tid = (int)threadIdx.x - GEMM_THREADS;
+    for (int i = 0; i < n_kt; ++i) {
+      const int s = i % w.stages, us = i % U8_STAGES;
+      mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
+      mb_wait(&u8_full[us], (i / U8_STAGES) & 1);
+      u8_convert<128>(w.u8, sU + (size_t)us * u8_bytes, smem + (size_t)s * stage_bytes + A_BYTES, (kt_begin + i) * GEMM_BK,
+                      w.slab_rows, u8_slots_, tid, 4);
+      if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
+    }
+  } else if (warp >= 4 && warp < 12 && n_kt > 0) {
+    // ---------------------------------------------------------------------- MMA, warpgroup g: accumulator rows (output
+    // channels) 64 g .. 64 g + 63 from A box g -- or, M-stacked, the same channels one tap row further down
+    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
+    const int j0 = blockIdx.y * (128 / w.C), nj = min(w.n_runs - j0, 128 / w.C);     // this CTA's taps
+    const bool busy = g < w.a_boxes;          // one A box (n_out <= 64, not stacked): warpgroup 2 only releases the stages
+    const uint64_t a0 = make_desc(s2u(smem) + g * 8192, 8192);
+    const uint32_t b_base = s2u(smem) + A_BYTES;
+    float d[64];
+    acc_zero<128>(d);
+    for (int i = 0; i < n_kt; ++i) {
+      const int s = i % w.stages;
+      mb_wait(&full[s], (i / w.stages) & 1);
+      const uint32_t st = (uint32_t)s * stage_bytes;
+      const uint64_t a = a0 + (st >> 4);
+      if (busy) {
+        wg_fence();
+        if (w.C == 128) {
+          mma_ktile<128, 1, 1>(d, a, make_desc(b_base + st + w.run_off[j0] * 16, slab_block));
         } else {
+          mma_ktile<64, 1, 1>(d, a, make_desc(b_base + st + w.run_off[j0] * 16, 8192));
+          if (nj > 1) mma_ktile<64, 1, 1>(d + 32, a, make_desc(b_base + st + w.run_off[j0 + 1] * 16, 8192));
+        }
+        wg_commit();
+        wg_wait0();
+        acc_fence<128>(d);
+      }
+      if (lane == 0) mb_arrive(&empty[s]);
+    }
+    // accumulator element d[32 sl + 4 jj + 2 h + e]: channel 16 wl + lane / 4 + 8 h, column 64 sl + 8 jj + 2 (lane % 4) + e
+    const bool low = w.stack_delta != 0 && g == 1;
+    float* base = w.D + (int64_t)blockIdx.x * w.partial_stride + 2 * (lane & 3);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) atomicAdd(d + j, __uint_as_float(r[j]));
+    for (int h = 0; h < 2; ++h) {
+      const int n = 16 * wl + (lane >> 2) + 8 * h;
+      const int nn = low ? n : g * 64 + n;
+      if (!busy || nn >= w.n_out) continue;
+#pragma unroll
+      for (int sl = 0; sl < 2; ++sl) {
+        if (sl >= nj) break;
+        const int j = j0 + sl;
+        int oc = w.tap0 * w.C + (int)w.run_acc[j];
+        if (low) {
+          if (w.run_low[j] < 0) continue;                              // duplicate of a tap the upper half already holds
+          oc = w.run_low[j];
+        }
+        float* dst = base + (int64_t)nn * w.ldd + oc;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          if (jj >= w.C / 8) break;
+          const float2 v = make_float2(d[32 * sl + 4 * jj + 2 * h], d[32 * sl + 4 * jj + 2 * h + 1]);
+          if (w.partial_stride > 0) *reinterpret_cast<float2*>(dst + 8 * jj) = v;   // split-K partials: summed by the consumer
+          else atomicAdd(reinterpret_cast<float2*>(dst + 8 * jj), v);
         }
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (warp == 4 && lane == 0) B2RL_TRACE_AT(2, 0, 3);
-  if (threadIdx.x == 0) B2RL_TRACE_AT(3, 0, 3);
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-  }
 }
 
 // ------------------------------------------------------------------------------------------------- host side
@@ -1258,9 +1073,28 @@ static int sm_count() {
   if (!n) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
+}
+
+// shared memory one CTA may use, static + dynamic (227 KB on sm_90)
+constexpr size_t SMEM_LIMIT = 227 * 1024;
+
+// dynamic shared memory kernel `k` may request: the per-CTA limit of the device minus the kernel's own static shared memory
+// (s_dbias, s_fix and the alignment of the extern region); 0 if the runtime cannot tell
+template <typename K>
+static size_t dyn_smem_limit(K k) {
+  static int optin = 0;
+  if (!optin) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess || optin <= 0)
+      optin = (int)SMEM_LIMIT;
+  }
+  cudaFuncAttributes a;
+  if (cudaFuncGetAttributes(&a, reinterpret_cast<const void*>(k)) != cudaSuccess || a.sharedSizeBytes >= (size_t)optin) return 0;
+  return (size_t)optin - a.sharedSizeBytes;
 }
 
 static bool has_ext(const GemmParams& p) { return p.mask || p.dbias || p.out_map >= 3; }
@@ -1268,8 +1102,14 @@ static bool has_ext(const GemmParams& p) { return p.mask || p.dbias || p.out_map
 template <int BN, int STAGES, bool EXT>
 static int launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ta2, const CUtensorMap& tb2,
                          const GemmParams& p, int splits, cudaStream_t st) {
-  constexpr size_t smem = 1024 + (size_t)STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + (2 * STAGES + 4) * 8 + 16;
-  auto k = gemm_tcgen05_kernel<BN, STAGES, EXT>;
+  constexpr size_t smem = 1024 + (size_t)STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + acc_stage_bytes(BN) + 2 * STAGES * 8;
+  static_assert(smem <= SMEM_LIMIT, "GEMM stages do not fit in shared memory");
+  auto k = gemm_wgmma_kernel<BN, STAGES, EXT>;
+  static const size_t limit = dyn_smem_limit(k);
+  if (smem > limit) {
+    set_error("b2rl_gemm_bf16: %zu bytes of shared memory per CTA exceed the %zu the device allows", smem, limit);
+    return B2RL_ERR_ARG;
+  }
   static bool attr_set = false;
   if (!attr_set) {
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1289,7 +1129,7 @@ static int launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
 }
 
 // the backward extras (mask / bias gradient / scatter maps) are compiled into their own instantiation: the forward and
-// weight-gradient kernels keep the lean epilogue (102 instead of 168 registers)
+// weight-gradient kernels keep the lean epilogue
 template <int BN, int STAGES>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ta2, const CUtensorMap& tb2,
                        const GemmParams& p, int splits, cudaStream_t st) {
@@ -1320,7 +1160,7 @@ static int gemm_dispatch(const uint16_t* A, int a_mn, int64_t lda, int64_t a_row
   }
   if (block_n == 32) return launch_gemm<32, 6>(ta, tb, ta2, tb2, p, splits, st);
   if (block_n == 64) return launch_gemm<64, 6>(ta, tb, ta2, tb2, p, splits, st);
-  return launch_gemm<128, 5>(ta, tb, ta2, tb2, p, splits, st);
+  return launch_gemm<128, 4>(ta, tb, ta2, tb2, p, splits, st);
 }
 
 template <int BN, bool EXT, bool U8>
@@ -1329,22 +1169,19 @@ static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   const size_t w_bytes = (size_t)sp.taps * sp.col_blocks * BN * 128;
   const size_t slab_bytes = (size_t)sp.slab_rows * 128 * sp.col_blocks;
   const int tiles = (sp.g.M + GEMM_BM - 1) / GEMM_BM;
-  static int two_cta = -1;                                           // B2RL_SLAB_2CTA=0 keeps one CTA per SM for BN = 32 too
-  if (two_cta < 0) {
-    const char* e = getenv("B2RL_SLAB_2CTA");
-    two_cta = (e && atoi(e) == 0) ? 0 : 1;
-  }
-  // two CTAs per SM when the kernel was compiled for it, the tiles are plentiful and both fit (<= 110 KB each, >= 3 stages)
-  const bool pair = BN == 32 && two_cta && !sp.g.dual && tiles >= 4 * sm_count() &&
-                    w_bytes + 3 * slab_bytes + 2048 + (U8 ? 3 * 16 * 1024 : 0) <= 110 * 1024;
+  // weights + slab ring + accumulator staging + barriers (+ uint8 staging) within the shared memory of one SM
+  const size_t fixed = 1024 + acc_stage_bytes(BN) + (2 * 6 + 2) * 8 + 128;
+  auto k = conv_slab_wgmma_kernel<BN, EXT, U8>;
+  static const size_t limit = dyn_smem_limit(k);
+  if (limit <= fixed) return 1;
   size_t u8_extra = 0;
-  size_t budget = pair ? 110 * 1024 - 2048 : 200 * 1024;
+  size_t budget = limit - fixed;
   if (U8) {
     // K1: three bf16 slabs are enough (shared -> shared conversion); everything else goes to uint8 staging tiles, each of which
     // is held for the copy latency plus the conversion
     const size_t ub = u8_stage_bytes(sp.slab_rows, sp.u8.G, sp.u8.frame_w);
-    if (w_bytes + 3 * slab_bytes + 2 * ub + 512 > budget) return 1;
-    int us = (int)((budget - w_bytes - 3 * slab_bytes - 512) / ub);
+    if (w_bytes + 3 * slab_bytes + 2 * ub + 2 * U8_MAX_STAGES * 8 > budget) return 1;
+    int us = (int)((budget - w_bytes - 3 * slab_bytes - 2 * U8_MAX_STAGES * 8) / ub);
     if (us > U8_MAX_STAGES) us = U8_MAX_STAGES;
     sp.u8.stages = us;
     u8_extra = (size_t)us * ub + 2 * U8_MAX_STAGES * 8;
@@ -1354,14 +1191,13 @@ static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   int stages = (int)((budget - w_bytes) / slab_bytes);
   if (stages > 6) stages = 6;
   sp.stages = stages;
-  const size_t smem = 1024 + w_bytes + stages * slab_bytes + (2 * 6 + 5) * 8 + 16 + 144 + u8_extra;
-  auto k = conv_slab_tcgen05_kernel<BN, EXT, U8>;
+  const size_t smem = fixed + w_bytes + stages * slab_bytes + u8_extra;
   static size_t attr = 0;
   if (attr < smem) {
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     attr = smem;
   }
-  int ctas = sp.g.dual ? sm_count() / 2 : (pair ? 2 * sm_count() : sm_count());   // per operand set
+  int ctas = sp.g.dual ? sm_count() / 2 : sm_count();                 // per operand set
   if (ctas > tiles) ctas = tiles;
   launch_pdl(k, dim3(sp.g.dual ? 2 * ctas : ctas), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, ta, tb, ta2, tb2, sp);
   return check_launch("b2rl_conv_gemm_bf16(slab)");
@@ -1381,16 +1217,20 @@ static int launch_slab(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
                        : launch_slab_t<BN, false, false>(ta, tb, ta2, tb2, sp, st);
 }
 
-template <int TMEM_COLS, bool U8 = false>
+template <bool U8 = false>
 static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParams w, cudaStream_t st, int* n_ctas = nullptr) {
   const size_t slab_bytes = (size_t)w.slab_rows * 128 * w.col_blocks, stage = 16384 + slab_bytes;
+  auto k = conv_wgrad_wgmma_kernel<U8>;
+  static const size_t limit = dyn_smem_limit(k);
+  const size_t fixed = 1024 + 2 * 6 * 8 + 16 + (U8 ? 2 * U8_MAX_STAGES * 8 + 144 : 0);
+  const size_t budget = limit > fixed + 200 * 1024 ? 200 * 1024 : (limit > fixed ? limit - fixed : 0);
   size_t u8_extra = 0;
-  int stages = (int)((200 * 1024) / stage);
+  int stages = (int)(budget / stage);
   if (U8) {                                                          // K1: four operand stages, the rest for uint8 staging tiles
     const size_t ub = u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w);
-    if (4 * stage + 2 * ub + 512 > 200 * 1024) return 1;
+    if (4 * stage + 2 * ub + 512 > budget) return 1;
     stages = 4;
-    int us = (int)((200 * 1024 - 4 * stage - 512) / ub);
+    int us = (int)((budget - 4 * stage - 512) / ub);
     if (us > U8_MAX_STAGES) us = U8_MAX_STAGES;
     w.u8.stages = us;
     u8_extra = (size_t)us * ub + 2 * U8_MAX_STAGES * 8 + 144;
@@ -1398,41 +1238,26 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   if (stages > 6) stages = 6;
   if (stages < 2) return 1;
   w.stages = stages;
-  const size_t smem = 1024 + stages * stage + (2 * 6 + 2) * 8 + 16 + u8_extra;
-  auto k = conv_wgrad_tcgen05_kernel<TMEM_COLS, U8>;
+  const size_t smem = 1024 + stages * stage + 2 * 6 * 8 + 16 + u8_extra;
   static size_t attr = 0;
   if (attr < smem) {
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     attr = smem;
   }
-  {
-    const bool merge = w.C == 64;
-    int tap = w.tap0, n = 0;
-    uint32_t acc = 0;
-    const int tap_end = w.tap0 + w.ntaps;
-    while (tap < tap_end && n < 9) {
-      const int dy = tap / w.taps_x, dx = tap - dy * w.taps_x;
-      int run = 1;
-      if (merge) {
-        run = w.taps_x - dx;
-        if (run > tap_end - tap) run = tap_end - tap;
-      }
-      w.run_off[n] = (uint32_t)(dy * w.grid_w + dx) * 8;
-      w.run_acc[n] = acc;
-      w.run_n[n] = (uint32_t)(run * w.C);
-      w.run_low[n] = (w.stack_delta && dy == w.stack_rows - 2) ? ((dy + 1) * w.taps_x + dx) * w.C : -1;
-      acc += run * w.C;
-      tap += run;
-      ++n;
-    }
-    if (tap < tap_end) return 1;
-    w.n_runs = n;
+  // one window per tap; a CTA accumulates the taps of one 128-column group (blockIdx.y)
+  if (w.ntaps > 9 || (w.C != 64 && w.C != 128)) return 1;
+  for (int n = 0; n < w.ntaps; ++n) {
+    const int tap = w.tap0 + n, dy = tap / w.taps_x, dx = tap - dy * w.taps_x;
+    w.run_off[n] = (uint32_t)(dy * w.grid_w + dx) * 8;
+    w.run_acc[n] = (uint32_t)(n * w.C);
+    w.run_low[n] = (w.stack_delta && dy == w.stack_rows - 2) ? ((dy + 1) * w.taps_x + dx) * w.C : -1;
   }
+  w.n_runs = w.ntaps;
+  const int groups = (w.ntaps * w.C + 127) / 128;
   const int kt_total = (w.rows + GEMM_BK - 1) / GEMM_BK;
-  // split-K over all SMs (the MMAs are shared-memory-read bound per SM, so the work must be spread); every CTA ends with
-  // n_out x cols / 4 vector reductions (red.global.add.v4.f32) into the same small D
+  // split-K over the SMs (groups x ctas CTAs); every CTA stores (or reduces) its n_out x 128 partial block
   int ctas = kt_total / 4;
-  if (ctas > sm_count()) ctas = sm_count();
+  if (ctas > sm_count() / groups) ctas = sm_count() / groups;
   static int cap = -1;                                               // tunable: B2RL_WGRAD_CTAS caps the split-K width
   if (cap < 0) {
     const char* e = getenv("B2RL_WGRAD_CTAS");
@@ -1443,17 +1268,11 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   w.k_tiles_per_cta = (kt_total + ctas - 1) / ctas;
   ctas = (kt_total + w.k_tiles_per_cta - 1) / w.k_tiles_per_cta;
   if (n_ctas) *n_ctas = ctas;
-  launch_pdl(k, dim3(ctas), dim3(GEMM_THREADS), smem, st, tg, tx, w);
+  launch_pdl(k, dim3(ctas, groups), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, tg, tx, w);
   return check_launch("b2rl_conv_gemm_bf16(wgrad slab)");
 }
 
 }  // namespace b2rl
-
-#ifdef B2RL_TRACE
-extern "C" int b2rl_debug_set_trace(unsigned long long* buf) {
-  return cudaMemcpyToSymbol(b2rl::g_trace_buf, &buf, sizeof(buf)) == cudaSuccess ? 0 : -1;
-}
-#endif
 
 using namespace b2rl;
 
@@ -1461,7 +1280,7 @@ static int g_wgrad_partials = 0;          // set by b2rl_conv_wgrad_partials for
 static float* g_partial_buf = nullptr;
 static int64_t g_partial_stride = 0;
 static int g_partial_count = 0;
-static int g_use_slab = 2;   // 2: shifted windows with base_offset 0 -- the 128B swizzle is a pure function of the smem address (verified on B200)
+static int g_use_slab = 2;   // 2: shifted windows with base_offset 0 -- the 128B swizzle is a pure function of the smem address
 extern "C" void b2rl_set_conv_slab(int32_t on) { g_use_slab = on; }
 
 static int check_common(const void* A, const void* B, const void* D, int64_t lda, int64_t ldb, int M, int N, int K,
@@ -1569,13 +1388,15 @@ static int conv_gemm_impl(int32_t mode, const uint16_t* X, int64_t rows, int32_t
   int rc = check_common(W_or_G, X, D, n_out, C, n_out, taps * C, (int)rows, out_mode, splits, block_n, 1, relu);
   if (rc) return rc;
   B2RL_REQUIRE(out_mode == 2, "wgrad accumulates with out_mode 2");
-  if (g_use_slab && C % 64 == 0 && C <= 128 && n_out <= 128 && shift_sign > 0) {
+  // (the slab kernel stores / reduces float2 pairs: D and its rows must be 8-byte aligned)
+  if (g_use_slab && C % 64 == 0 && C <= 128 && n_out <= 128 && shift_sign > 0 && ldd % 2 == 0 &&
+      reinterpret_cast<uintptr_t>(g_wgrad_partials ? g_partial_buf : D) % 8 == 0) {
     int max_shift = ((taps - 1) / taps_x) * grid_w + (taps - 1) % taps_x;
     WgradParams w = {};
     w.rows = (int)rows; w.n_out = n_out; w.C = C; w.col_blocks = C / 64; w.taps_x = taps_x; w.grid_w = grid_w;
     w.a_boxes = n_out > 64 ? 2 : 1;
     // M-stacking (see WgradParams): with at most 64 output channels the second half of the 128 accumulator lanes computes the
-    // last tap row from the windows of the row before it (B2RL_WGRAD_STACK=0: every tap its own window, as in round 1)
+    // last tap row from the windows of the row before it (B2RL_WGRAD_STACK=0: every tap its own window)
     static int stack_on = -1;
     if (stack_on < 0) {
       const char* e = getenv("B2RL_WGRAD_STACK");
@@ -1596,23 +1417,9 @@ static int conv_gemm_impl(int32_t mode, const uint16_t* X, int64_t rows, int32_t
     if (rc) return rc;
     rc = make_map(&tx, X, C, rows, C, w.slab_rows);                 // activation slab: box [slab_rows][64 c]
     if (rc) return rc;
-    const int per_launch = 512 / C;                                 // taps whose accumulators fit in TMEM together
-    if (w.stack_delta && win_taps > per_launch) {                   // (does not happen for the NatureConvBody shapes)
-      w.stack_delta = 0; w.stack_rows = 0; w.a_boxes = 1; win_taps = taps;
-      w.slab_rows = (GEMM_BK + ((taps - 1) / taps_x) * grid_w + (taps - 1) % taps_x + 7) / 8 * 8;
-      rc = make_map(&tx, X, C, rows, C, w.slab_rows);
-      if (rc) return rc;
-    }
-    int r2 = 0;
-    for (int t0 = 0; t0 < win_taps && r2 == 0; t0 += per_launch) {
-      w.tap0 = t0;
-      w.ntaps = win_taps - t0 < per_launch ? win_taps - t0 : per_launch;
-      const int cols = w.ntaps * C;
-      r2 = cols <= 64 ? launch_wgrad<64>(tg, tx, w, (cudaStream_t)stream, &g_partial_count)
-           : cols <= 128 ? launch_wgrad<128>(tg, tx, w, (cudaStream_t)stream, &g_partial_count)
-           : cols <= 256 ? launch_wgrad<256>(tg, tx, w, (cudaStream_t)stream, &g_partial_count)
-                         : launch_wgrad<512>(tg, tx, w, (cudaStream_t)stream, &g_partial_count);
-    }
+    w.tap0 = 0;
+    w.ntaps = win_taps;
+    const int r2 = launch_wgrad(tg, tx, w, (cudaStream_t)stream, &g_partial_count);
     if (r2 <= 0) return r2;
   }
   p.M = n_out; p.N = taps * C; p.K = (int)rows; p.a_mn = 1; p.b_mn = 1; p.b_tap_tiles = C / block_n;
@@ -1689,7 +1496,7 @@ extern "C" int b2rl_gemm_bwd_bf16(const uint16_t* A, int64_t lda, const uint16_t
   return gemm_dispatch(A, 0, lda, M, K, B, b_mn, ldb, b_mn ? K : N, b_mn ? N : K, p, 1, block_n, (cudaStream_t)stream);
 }
 
-// Weight gradient as split-K PARTIALS: partial i (one per CTA, n_partials_host of them, at most 148) is stored at
+// Weight gradient as split-K PARTIALS: partial i (one per CTA, n_partials_host of them, at most one per SM) is stored at
 // partials + i * n_out * taps * C; the consumer (b2rl_nature_unpack_grads) sums them.  Replaces ~1M fp32 atomics per
 // layer by coalesced stores.
 extern "C" int b2rl_conv_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out,
@@ -1809,6 +1616,7 @@ extern "C" int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capac
   int rc = u8_src(w.u8, frames, idx, first, row_bytes, frame_w, batch, history);
   if (rc) return rc;
   B2RL_REQUIRE(G_rows && partials && n_partials_host, "null pointer");
+  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(partials) % 8 == 0, "partials must be 8-byte aligned");
   B2RL_REQUIRE(n_out > 0 && n_out <= 64 && n_out % 8 == 0, "n_out <= 64, multiple of 8");
   B2RL_REQUIRE(reinterpret_cast<uintptr_t>(G_rows) % 16 == 0, "operands must be 16-byte aligned");
   const int G = w.u8.G, C = 64, taps = 4;
@@ -1826,7 +1634,7 @@ extern "C" int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capac
   rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(w.slab_rows, G));
   if (rc) return rc;
   int n = 0;
-  int r2 = launch_wgrad<128, true>(tg, tr, w, (cudaStream_t)stream, &n);
+  int r2 = launch_wgrad<true>(tg, tr, w, (cudaStream_t)stream, &n);
   if (r2 > 0) { set_error("b2rl_conv1_u8_wgrad_partials: the slab does not fit in shared memory"); return B2RL_ERR_ARG; }
   *n_partials_host = n;
   return r2;

@@ -4,7 +4,7 @@
 // backward counterparts).  Forward: q = phi W_a^T + b_a, or the dueling combine q = v + adv - mean(adv) with
 // v = phi W_v^T + b_v.  Backward: dphi = geff W, dW += geff^T phi, db += sum geff, where geff is dq mapped through the
 // dueling combine.  phi is the bf16 feature vector of the fused body; weights and gradients are fp32 (master).
-// sm_100a only.
+// sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {
@@ -238,7 +238,7 @@ __device__ __forceinline__ float head_per_raw_weight(float prob, int B, float be
 // the online head on s, the target head on s' [, the online head on s' for double-Q], the target / loss / PER block, and leaves
 // the effective output gradient of the row (through the dueling combine) in geff_out [B][HEAD_MAX_OUT + 1]; head_bwd_kernel then
 // reads geff directly.  The single-launch form below repeats the row dot products in every 64-column CTA of the backward grid,
-// which puts 4 dependent L2 round trips in front of the backward part of all 256 CTAs (measured 11 us slower per update).
+// which puts 4 dependent L2 round trips in front of the backward part of all 256 CTAs.
 template <int NB>
 __global__ void __launch_bounds__(128) dqn_head_loss_kernel(const DqnHeadArgs a, float* __restrict__ geff_out) {
   pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return

@@ -1,6 +1,6 @@
 // losses.cu -- fused target / loss / gradient kernels of the DQN family.
 // Reference: deep_rl/agent/DQN_agent.py:78-127, CategoricalDQN_agent.py:60-89,
-// QuantileRegressionDQN_agent.py:55-77, utils/torch_utils.py:47-48.  sm_100a only.
+// QuantileRegressionDQN_agent.py:55-77, utils/torch_utils.py:47-48.  sm_90a only.
 //
 // Each entry point replaces ~15-20 eager ATen launches with one kernel that produces the per-sample
 // loss tensor the reference's compute_loss returns, the PER priorities / importance weights

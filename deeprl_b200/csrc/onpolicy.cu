@@ -1,5 +1,5 @@
 // onpolicy.cu -- GAE backward recurrence, advantage normalisation, PPO clipped surrogate, A2C objective.
-// Reference: deep_rl/agent/A2C_agent.py:43-64, deep_rl/agent/PPO_agent.py:51-86.  sm_100a only.
+// Reference: deep_rl/agent/A2C_agent.py:43-64, deep_rl/agent/PPO_agent.py:51-86.  sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {

@@ -3,7 +3,7 @@
 // examples.py:67-68 (RMSprop lr 2.5e-4, alpha .95, eps .01, centered), :139,:204 (Adam).
 // Update rules are torch.optim's (RMSprop: _single_tensor_rmsprop, Adam: _single_tensor_adam),
 // clip rule is torch.nn.utils.clip_grad_norm_ (coef = max_norm / (total_norm + 1e-6), clamped to 1).
-// One arena => 2 launches instead of ~10 tensors x (norm + mul + ~8 optimizer ops).  sm_100a only.
+// One arena => 2 launches instead of ~10 tensors x (norm + mul + ~8 optimizer ops).  sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {
@@ -141,7 +141,7 @@ extern "C" int b2rl_clip_rmsprop(float* param, const float* grad, float* square_
   int rc = norm_pass(grad, n, grad_scale, max_norm, norm_scratch, st);
   if (rc) return rc;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   launch_pdl(rmsprop_kernel, dim3(blocks), dim3(256), 0, st, param, grad, square_avg, grad_avg, n, lr, alpha, eps, centered,
                                          reinterpret_cast<NormScratch*>(norm_scratch),
                                          reinterpret_cast<__nv_bfloat16*>(bf16_shadow));
@@ -160,7 +160,7 @@ static int clip_adam_impl(float* param, const float* grad, float* exp_avg, float
   rc = check_launch("adam/step");
   if (rc) return rc;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   launch_pdl(adam_kernel, dim3(blocks), dim3(256), 0, st, param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, step_dev,
              reinterpret_cast<NormScratch*>(norm_scratch), reinterpret_cast<__nv_bfloat16*>(bf16_shadow), gate, gate_max);
   return check_launch("b2rl_clip_adam");

@@ -2,7 +2,7 @@
 // conv [Cout,Cin,kh,kw], fc4 [512, (c,h,w)]) and the tap-major bf16 operands of the grid-GEMM convolution stack
 // (csrc/gemm.cu, network/nature_tc.py).  One launch packs all four layers (forward and dgrad orientations), one launch
 // maps the four fp32 weight gradients back and ACCUMULATES them (and the bias gradients) into the .grad arena.
-// sm_100a only.
+// sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {
@@ -153,7 +153,7 @@ extern "C" int b2rl_nature_pack_weights(const float* w1, const float* w2, const 
   a.w2d = reinterpret_cast<__nv_bfloat16*>(w2d); a.w3f = reinterpret_cast<__nv_bfloat16*>(w3f);
   a.w3d = reinterpret_cast<__nv_bfloat16*>(w3d); a.w4p = reinterpret_cast<__nv_bfloat16*>(w4p);
   a.c1 = c1; a.n4 = n4; a.scale = scale;
-  launch_pdl(pack_weights_kernel, dim3(148 * 8), dim3(256), 0, (cudaStream_t)stream, a);
+  launch_pdl(pack_weights_kernel, dim3(132 * 8), dim3(256), 0, (cudaStream_t)stream, a);
   return check_launch("b2rl_nature_pack_weights");
 }
 
@@ -169,6 +169,6 @@ extern "C" int b2rl_nature_unpack_grads(const float* g1f, const float* g2f, cons
   a.gw1 = gw1; a.gw2 = gw2; a.gw3 = gw3; a.gw4 = gw4; a.gb1 = gb1; a.gb2 = gb2; a.gb3 = gb3; a.gb4 = gb4;
   a.c1 = c1; a.n4 = n4; a.scale = scale;
   a.p1 = p1 < 1 ? 1 : p1; a.p2 = p2 < 1 ? 1 : p2; a.p3 = p3 < 1 ? 1 : p3;
-  launch_pdl(unpack_grads_kernel, dim3(148 * 8), dim3(256), 0, (cudaStream_t)stream, a);
+  launch_pdl(unpack_grads_kernel, dim3(132 * 8), dim3(256), 0, (cudaStream_t)stream, a);
   return check_launch("b2rl_nature_unpack_grads");
 }

@@ -3,12 +3,12 @@
 //
 // Why one block: an update is 2 M FMAs on an 11 k-parameter pair of MLPs over 64 rows -- a few microseconds of one SM -- and
 // every update depends on the parameters written by the one before it.  As separate launches (the CUDA-graph form,
-// learner.GraphedPPOLearner) it costs ~180 us, almost all of it launch / dependency latency of ~45 tiny kernels.  Here the
+// learner.GraphedPPOLearner) it is bound by the launch / dependency latency of ~45 tiny kernels.  Here the
 // weights live in shared memory for the whole iteration, the Adam moments in L2, the minibatch rows are fetched one update
 // ahead by the idle half of the block, and the only synchronisation is the block barrier between the nine phases of an
 // update (ppo_phases.h, ppo_sequence.inc: the same source is compiled for the host by tests/host_emul to check the arithmetic).
 // The actor and the critic are independent networks (non-shared representation): they run side by side on the two halves
-// of the block.  sm_100a only.
+// of the block.  sm_90a only.
 #include "common.cuh"
 #include "ppo_phases.h"
 

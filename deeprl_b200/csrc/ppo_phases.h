@@ -18,8 +18,7 @@
 #define PPO_FN __device__ __forceinline__
 #define PPO_HD __host__ __device__ inline
 // the dense building blocks are called from several phases: ONE copy each (the kernel runs as a single block, and with every
-// block inlined into every phase its code was 400 KB -- an order of magnitude beyond the 32 KB instruction cache; measured:
-// 52 us per update, 35 % of it in one phase).  Their pointer arguments are shared-memory addresses at every call site, which
+// block inlined into every phase its code was 400 KB -- an order of magnitude beyond the 32 KB instruction cache).  Their pointer arguments are shared-memory addresses at every call site, which
 // the compiler propagates into the one copy (LDS, not generic loads).
 #define PPO_SUB __device__ __noinline__
 #define PPO_LOOP _Pragma("unroll 1")
@@ -267,7 +266,7 @@ PPO_FN void wgrad_adam_tile(int t, const float* d, int ldd, const float* in, int
   // Adam.  The master copy `flat` is written once, when the kernel ends (ph_finish); the moments live in L2.  All moment
   // loads are issued before the arithmetic (independent round trips); rows of a weight whose K is a multiple of 4 are read
   // and written 128 bits at a time -- a warp then touches whole 32-byte sectors (the scalar form's 16-byte-strided stores
-  // kept the load/store unit busy long into the NEXT phase: 36 k cycles of a 6 k-cycle phase, measured with the phase clocks)
+  // kept the load/store unit busy long into the NEXT phase)
   float mo[4][4], vo[4][4];
   const bool vec = (K & 3) == 0;
   for (int r = 0; r < 4; ++r) {

@@ -1,5 +1,5 @@
 // replay.cu -- HBM-resident replay ring: feed, uniform index selection, frame-stack gather.
-// Reference semantics: deep_rl/component/replay.py:75-140 (UniformReplay).  sm_100a only.
+// Reference semantics: deep_rl/component/replay.py:75-140 (UniformReplay).  sm_90a only.
 //
 // Data layout (all in HBM, allocated by the caller):
 //   frames  uint8  [capacity][row_bytes]   one row per env step (newest 84x84 frame, DQN_agent.py:108)
@@ -479,7 +479,7 @@ static int launch_cvt1(dim3 grid, size_t smem, cudaStream_t st, const uint8_t* f
   auto k = gather_cvt_kernel<T, LAYOUT>;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   // plain stream order: with programmatic overlap the CTAs of back-to-back gathers are placed while the previous launch still
-  // holds its slots, the placement is skewed and the launch gets ~25 % slower (24.6 vs 19.2 us, profiles/r01_microbench.txt)
+  // holds its slots, the placement is skewed and the launch gets slower
   launch_ordered(k, dim3(grid), dim3(256), smem, st, frames, action, reward, mask, row_bytes, idx, hl, n, discount, lut, (T*)so, (T*)no, a, r, m,
                              use_tma, frame_w);
   return check_launch("b2rl_replay_gather");

@@ -1,5 +1,5 @@
 // sumtree.cu -- the prioritized-replay sum tree, resident in HBM, bit-identical to the reference.
-// Reference: deep_rl/utils/sum_tree.py:6-67, deep_rl/component/replay.py:152-196.  sm_100a only.
+// Reference: deep_rl/utils/sum_tree.py:6-67, deep_rl/component/replay.py:152-196.  sm_90a only.
 //
 // tree: float64 [2*cap-1] array heap (root 0, children 2i+1 / 2i+2, leaves [cap-1, 2cap-2]).
 // The reference NEVER recomputes an internal node from its children: update() adds the same float64

@@ -1,5 +1,5 @@
 // tail.cu -- the tail of one gradient update (DQN_agent.py:131-134: backward's last step, clip_grad_norm_, optimizer.step)
-// for a NatureConvBody network on the tcgen05 path, as TWO launches instead of five:
+// for a NatureConvBody network on the wgmma path, as TWO launches instead of five:
 //
 //   A  nature_grad_reduce_kernel : split-K partials of the three convolution weight gradients summed (deterministic order),
 //                                  all four weight gradients mapped from the GEMM layouts to the reference's parameter
@@ -12,12 +12,12 @@
 //                                  torch.nn.utils.clip_grad_norm_, applies RMSprop (plain / centered) or Adam exactly as
 //                                  csrc/optim.cu does, re-zeroes the gradient it consumed, and writes the updated weights
 //                                  straight into the bf16 tap-major GEMM operands (forward + dgrad orientations) that the next
-//                                  update's tcgen05 kernels read -- the separate pack launch disappears as well.
+//                                  update's wgmma kernels read -- the separate pack launch disappears as well.
 //
-// Replaces unpack_grads (29 us cold: it walked 46 MB of partials with strided gathers) + sumsq + rmsprop + pack_weights
+// Replaces unpack_grads (it walked the split-K partials with strided gathers) + sumsq + rmsprop + pack_weights
 // + the memset of the gradient arena.  Work is described by unit tables built once on the host (network/tail.py):
 // int32 x 4 per unit = {arena offset, length, kind, row | segment << 16}.
-// sm_100a only.
+// sm_90a only.
 #include "common.cuh"
 
 namespace b2rl {

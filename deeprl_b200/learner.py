@@ -83,9 +83,8 @@ class GraphedDQNLearner:
         # trains on the batch sampled during update k-1 while a third branch of the graph feeds + samples batch k+1
         # into the other buffer set.  Two graphs (one per buffer parity) are captured and replayed alternately.
         self.prefetch = bool(prefetch)
-        # dual: one launch per body layer for online(s) + target(s') (nature_tc.forward_dual).  Measured on B200 at B = 512:
-        # 27 instead of 33 launches per update, +1 % updates/s with synchronous replay, -2 % with the prefetch branch (the
-        # two-stream fork already hides the per-launch fixed cost), hence off by default.
+        # dual: one launch per body layer for online(s) + target(s') (nature_tc.forward_dual): 27 instead of 33 launches per
+        # update; off by default (the two-stream fork of the prefetch branch already hides the per-launch fixed cost).
         self.dual = bool(dual)
         self._batch = [None, None]
         self._parity = 0
@@ -103,7 +102,7 @@ class GraphedDQNLearner:
     # ------------------------------------------------------------------ fused tail / fused head (csrc/tail.cu, csrc/head.cu)
     def tail(self):
         """The two-launch update tail (gradient reduce + clip / optimizer / operand pack) when the online network has a
-        tcgen05 NatureConvBody and the backward epilogues are fused; None otherwise (generic unpack + FlatOptimizer.step)."""
+        wgmma NatureConvBody and the backward epilogues are fused; None otherwise (generic unpack + FlatOptimizer.step)."""
         if self._tail is None:
             from .network.tail import NatureTail
             body = getattr(self.net, "body", None)
@@ -126,8 +125,8 @@ class GraphedDQNLearner:
 
     def _heads(self):
         """(online head modules, target head modules) when the DQN head can run in the fused head + loss + backward kernel."""
-        # (off by default: measured on B200 at batch 512 the separate head_fwd | dqn_loss | head_bwd kernels -- the target head on
-        # the side branch -- give 224.7 us / update, the two-launch fused form 243.2 us, the one-launch form 252.9 us)
+        # (off by default: the separate head_fwd | dqn_loss | head_bwd kernels run the target head on the side branch, which the
+        # fused forms give up)
         if self.kind != "dqn" or self.tail() is None or os.environ.get("B2RL_FUSED_HEAD", "0") == "0":
             return None
         out = []
@@ -191,8 +190,7 @@ class GraphedDQNLearner:
                 self._packed_ev.record(side)
         # async replay: the batch of the NEXT update is fed + sampled on a parallel branch.  Uniform replay: that branch starts
         # after the backward pass, beside the (small-footprint, L2-bound) update tail -- started beside the forward pass its 512
-        # gather CTAs held the shared memory the convolution kernels need and delayed them by ~20 us (in-graph timeline,
-        # profiles/r02_timeline.txt).  Prioritized replay keeps the early start: the reference's replay worker draws the next
+        # gather CTAs would hold the shared memory the convolution kernels need and delay them.  Prioritized replay keeps the early start: the reference's replay worker draws the next
         # batch BEFORE this update's priorities arrive (replay.py:219-261), and the graph keeps that order.
         late = (self.prefetch and not self.per and getattr(self, "_one_graph", True)
                 and os.environ.get("B2RL_PREFETCH_LATE", "1") == "1")
@@ -270,8 +268,8 @@ class GraphedDQNLearner:
         fired = []
         if late and os.environ.get("B2RL_PREFETCH_AT", "end") == "dgrad":
             # option (B2RL_PREFETCH_AT=dgrad): fork the gather right after the last dgrad GEMM, beside the conv2 / conv1
-            # weight-gradient GEMMs.  Measured 227.6 us / update against 226.1 us for the fork after the backward pass (default):
-            # the gather slows the conv1 weight gradient and kernel A by as much as it gains
+            # weight-gradient GEMMs.  The default forks after the backward pass: beside the weight gradients the gather slows the
+            # conv1 weight gradient and kernel A
             nature_tc.AFTER_DGRAD = lambda: (self._prefetch_branch(parity, "gather"), fired.append(1))
         try:
             with nature_tc.wgrad_stream(None if side is cur else side), nature_tc.grad_sink(tail):   # weight-gradient GEMMs on the side branch
@@ -298,7 +296,7 @@ class GraphedDQNLearner:
                 nature_tc.mark("sampled")
 
     def _main_fused_head(self, t, per, heads, tail, fs):
-        """DQN with a VanillaNet / DuelingNet head: bodies on the tcgen05 kernels, then ONE launch for the online / target
+        """DQN with a VanillaNet / DuelingNet head: bodies on the wgmma kernels, then ONE launch for the online / target
         [/ double-Q] head forwards + target / loss / PER block + head backward (csrc/head.cu dqn_head_fused_kernel)."""
         cur, side = torch.cuda.current_stream(), self._side
         side.wait_stream(cur)
@@ -324,7 +322,7 @@ class GraphedDQNLearner:
         self.loss.copy_(r["loss"])
 
     def _repack(self, net, fs):
-        """tcgen05 backend: the learner owns the packed bf16 operands of both networks -- the online body is re-packed
+        """wgmma backend: the learner owns the packed bf16 operands of both networks -- the online body is re-packed
         once per update (one launch), the target body only when it is synchronised."""
         body = getattr(net, "body", None)
         if body is not None and hasattr(body, "repack") and self.dtype == torch.bfloat16:
@@ -363,7 +361,7 @@ class GraphedDQNLearner:
         return getattr(net, "fc_categorical", None) or getattr(net, "fc_quantiles", None)
 
     def _refresh_head_operands(self, online):
-        """Distributional heads (C51 / QR-DQN) on the tcgen05 GEMM: the online head reads its bf16 weight from the optimizer's
+        """Distributional heads (C51 / QR-DQN) on the wgmma GEMM: the online head reads its bf16 weight from the optimizer's
         arena-wide bf16 shadow (written by the fused optimizer kernel), the target head from a copy refreshed at target sync."""
         if self.kind not in ("c51", "qr") or self.tail() is None or os.environ.get("B2RL_DIST_HEAD", "1") == "0":
             return
@@ -389,7 +387,7 @@ class GraphedDQNLearner:
         # multi GPU, default: the collectives are captured INSIDE the update graph -- fc4's slice of the gradient arena (95 % of
         # the bytes) is all-reduced asynchronously right after its weight-gradient GEMM, beside the convolution backward, the
         # small remainder after the last GEMM.  B2RL_NCCL_IN_GRAPH=0: [sample..backward] graph | eager all-reduce of the whole
-        # arena | [clip + optimizer] graph (the round-1 form: +54 us per update at 2 and 4 GPUs, +85 us at 8).
+        # arena | [clip + optimizer] graph (the older form; it exposes the whole all-reduce).
         one_graph = self.world == 1 or os.environ.get("B2RL_NCCL_IN_GRAPH", "1") == "1"
         self._one_graph = one_graph      # (the late prefetch branch is joined after the optimizer kernels: one graph only)
         self._overlap = self.world > 1 and one_graph and self.tail() is not None
@@ -500,7 +498,7 @@ class GraphedPPOLearner:
     minibatch: row gather by a device-resident index matrix, network forward, ``b2rl_ppo_loss`` (clipped surrogate, value
     loss, approx-KL and their gradients in one launch), backward, KL-GATED actor Adam step (``b2rl_clip_adam_gated``: the
     reference's ``if approx_kl <= 1.5 * target_kl`` decided on the device) and the critic Adam step.  An iteration of
-    examples.py:496-522 is 5 120 such updates of an 11 k-parameter MLP: eager, each costs ~1.8 ms of Python and launch
+    examples.py:496-522 is 5 120 such updates of an 11 k-parameter MLP: eager, each is dominated by Python and launch
     latency; as a graph replay the host cost is one ``cudaGraphLaunch``.
 
     The rollout rows live in persistent device buffers (``load``); the minibatch index rows of ALL epochs are uploaded

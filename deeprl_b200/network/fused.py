@@ -171,7 +171,7 @@ class _NarrowHead(torch.autograd.Function):
             gwa, gba, gwv, gbv = z(wa), z(ba), z(wv), z(bv)
         from . import nature_tc
         if nature_tc.FUSED_BWD and phi.data_ptr() in nature_tc.RELU_FEATURES:
-            # phi = relu(fc4(.)) of a tcgen05 NatureConvBody: its ReLU backward and bias gradient ride along (the body's
+            # phi = relu(fc4(.)) of a wgmma NatureConvBody: its ReLU backward and bias gradient ride along (the body's
             # backward finds the column sums under the gradient's address and skips its own pass)
             sink = nature_tc.SINK               # persistent accumulator (re-zeroed by the tail's kernel A) or a fresh one
             colsum = sink.db4 if (sink is not None and sink.db4.numel() == K) else torch.zeros(K, dtype=torch.float32, device=phi.device)
@@ -203,7 +203,7 @@ def narrow_head_ok(phi, fc_action, fc_value=None):
 
 class _DistHead(torch.autograd.Function):
     """Distributional head (CategoricalNet / QuantileNet, network_heads.py:40-55, 89-102) on bf16 features with no cuBLAS / ATen
-    kernel: logits = phi W^T + b on the tcgen05 GEMM, softmax + log_softmax in one launch (csrc/disthead.cu), and in the backward
+    kernel: logits = phi W^T + b on the wgmma GEMM, softmax + log_softmax in one launch (csrc/disthead.cu), and in the backward
     pass the log_softmax gradient, the bf16 operand and the bias gradient in one launch followed by the two GEMMs
     (dW = g^T phi, dphi = relu_mask(g W) with fc4's bias gradient from the same epilogue)."""
 

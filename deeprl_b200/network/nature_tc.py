@@ -1,4 +1,4 @@
-"""NatureConvBody forward + backward entirely on the tcgen05 GEMM of ``csrc/gemm.cu`` (no cuDNN / cuBLAS).
+"""NatureConvBody forward + backward entirely on the wgmma GEMM of ``csrc/gemm.cu`` (no cuDNN / cuBLAS).
 
 Reference layer stack: ``network_bodies.py:10-33`` -- conv(4->32,k8,s4), conv(32->64,k4,s2), conv(64->64,k3,s1), fc(3136->512),
 ReLU after each.  Every layer is a GEMM over activations stored as [batch * G * G][C] grid matrices:
@@ -28,11 +28,11 @@ from .fused import act_bwd_bias_grad
 _bf16 = torch.bfloat16
 _f32 = torch.float32
 # fc4 forward at small batch: split-K factor (zero fill + split-K GEMM with fp32 atomics + bias/ReLU pass, 3 launches) or 1 =
-# one GEMM launch with the fused bias/ReLU epilogue (measured per network at B = 512: 10.1 us vs 10.0 us in isolation)
+# one GEMM launch with the fused bias/ReLU epilogue
 FC4_SPLITS = int(os.environ.get("B2RL_FC4_SPLITS", "4"))
 # split-K with the in-kernel fix-up (one launch) instead of zero fill + atomic split-K + bias/ReLU pass (three)
-# (measured on B200, batch 512: 234 us / update with the three launches vs 242 us with the fix-up -- the last-arriver's L2 round
-# trips are exposed, the three small launches overlap with the other network's chain -- so the fix-up is off by default)
+# (off by default: the last-arriver's L2 round trips are exposed, while the three small launches overlap with the other
+# network's chain)
 FC4_FIXUP = os.environ.get("B2RL_FC4_FIXUP", "0") == "1"
 # backward: ReLU mask + bias gradient + re-layout fused into the dgrad GEMM epilogues (b2rl_*_bwd_bf16) instead of three
 # b2rl_act_bwd_bias_grad_bf16 passes (B2RL_FUSED_BWD=0 restores them).
@@ -203,6 +203,11 @@ def _join():
         torch.cuda.current_stream().wait_stream(side)
 
 
+def _max_partials(device):
+    """The weight-gradient kernels write at most one split-K partial per SM."""
+    return torch.cuda.get_device_properties(device).multi_processor_count
+
+
 def wgrad_partials(X, G_rows, n_out, taps, taps_x, grid_w, stream=None):
     """Split-K partial weight gradients (one per CTA, no atomics): returns (partials [P_max, n_out, taps*C] fp32, P)."""
     rows, C = X.shape
@@ -210,7 +215,7 @@ def wgrad_partials(X, G_rows, n_out, taps, taps_x, grid_w, stream=None):
         out = torch.zeros((1, n_out, taps * C), dtype=_f32, device=X.device)
         conv_gemm(1, X, G_rows, n_out, taps, taps_x, grid_w, 1, out[0], splits=16, block_n=128 if C == 128 else 64)
         return out, 1
-    buf = torch.empty((148, n_out, taps * C), dtype=_f32, device=X.device)
+    buf = torch.empty((_max_partials(X.device), n_out, taps * C), dtype=_f32, device=X.device)
     n = ctypes.c_int32(0)
     _lib.call("b2rl_conv_wgrad_partials", _lib.ptr(X), int(rows), int(C), _lib.ptr(G_rows), int(n_out), int(taps), int(taps_x),
               int(grid_w), _lib.ptr(buf), ctypes.byref(n), stream if stream is not None else _lib.stream())
@@ -219,7 +224,7 @@ def wgrad_partials(X, G_rows, n_out, taps, taps_x, grid_w, stream=None):
 
 def wgrad_partials_ring(ring, G_rows, n_out, stream=None):
     """conv1's split-K partial weight gradients with the activations read from the uint8 ring (K1)."""
-    buf = torch.empty((148, n_out, 4 * 16 * ring.history), dtype=_f32, device=G_rows.device)
+    buf = torch.empty((_max_partials(G_rows.device), n_out, 4 * 16 * ring.history), dtype=_f32, device=G_rows.device)
     n = ctypes.c_int32(0)
     _lib.call("b2rl_conv1_u8_wgrad_partials", *ring.args(), _lib.ptr(G_rows), int(n_out), _lib.ptr(buf), ctypes.byref(n),
               stream if stream is not None else _lib.stream())
@@ -481,7 +486,8 @@ def nature_body(body, x0, scale):
 def repack(body, scale):
     pk = getattr(body, "_packed", None)
     if pk is None:
-        pk = body._packed = PackedWeights(body.conv1.in_channels, body.fc4.out_features, body.conv1.weight.device)
+        dev = _lib.require_cuda(body.conv1.weight.device)       # the pack kernel reads the parameters in device memory
+        pk = body._packed = PackedWeights(body.conv1.in_channels, body.fc4.out_features, dev)
     w = [m.weight.detach() for m in (body.conv1, body.conv2, body.conv3, body.fc4)]
     w = [t if t.is_contiguous() else t.contiguous() for t in w]
     pk.pack(w[0], w[1], w[2], w[3], scale)

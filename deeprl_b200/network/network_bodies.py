@@ -38,7 +38,7 @@ class NatureConvBody(nn.Module):
         if self.noisy_linear:
             self.fc4.reset_noise()
 
-    auto_repack = True        # tcgen05 backend: refresh the packed bf16 operands at every forward (safe default)
+    auto_repack = True        # wgmma backend: refresh the packed bf16 operands at every forward (safe default)
 
     def repack(self, scale=None):
         """Refresh the packed bf16 GEMM operands from the fp32 parameters (owners that set ``auto_repack = False``
@@ -72,7 +72,7 @@ class NatureConvBody(nn.Module):
         scale = fused.current_frame_scale()
         if (Config.DENSE_BACKEND == "tcgen05" and x.shape[1] == 16 * self.conv1.in_channels and x.shape[1] % 64 == 0
                 and tuple(x.shape[2:]) == (21, 21)):
-            from . import nature_tc                          # whole body on the tcgen05 GEMM (csrc/gemm.cu)
+            from . import nature_tc                          # whole body on the wgmma GEMM (csrc/gemm.cu)
             return nature_tc.nature_body(self, x, scale)
         w1 = self.conv1.weight
         if x.shape[1] == 16 * self.conv1.in_channels:                    # space-to-depth input

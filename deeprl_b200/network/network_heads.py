@@ -76,7 +76,7 @@ class CategoricalNet(nn.Module, BaseNet):
 
     def forward(self, x):
         phi = _phi(self.body, x)
-        if fused.dist_head_ok(phi, self.fc_categorical):           # tcgen05 GEMM + fused softmax / log_softmax (csrc/disthead.cu)
+        if fused.dist_head_ok(phi, self.fc_categorical):           # wgmma GEMM + fused softmax / log_softmax (csrc/disthead.cu)
             log_prob, prob = fused.dist_head(phi, self.fc_categorical, self.action_dim, self.num_atoms, True)
             return dict(prob=prob, log_prob=log_prob)
         with _autocast():
@@ -124,7 +124,7 @@ class QuantileNet(nn.Module, BaseNet):
 
     def forward(self, x):
         phi = _phi(self.body, x)
-        if fused.dist_head_ok(phi, self.fc_quantiles):             # tcgen05 GEMMs (csrc/disthead.cu for the backward operand)
+        if fused.dist_head_ok(phi, self.fc_quantiles):             # wgmma GEMMs (csrc/disthead.cu for the backward operand)
             q, _ = fused.dist_head(phi, self.fc_quantiles, self.action_dim, self.num_quantiles, False)
             return dict(quantile=q)
         with _autocast():

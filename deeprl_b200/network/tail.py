@@ -1,5 +1,5 @@
 """Host side of ``csrc/tail.cu``: the tail of one gradient update (``loss.backward()``'s last step, ``clip_grad_norm_``,
-``optimizer.step()`` -- DQN_agent.py:131-134) of a network with a tcgen05 ``NatureConvBody`` as TWO launches.
+``optimizer.step()`` -- DQN_agent.py:131-134) of a network with a wgmma ``NatureConvBody`` as TWO launches.
 
 ``NatureTail(opt, body, scale)`` binds a ``FlatOptimizer`` arena to the body's packed bf16 operands:
 

@@ -319,10 +319,10 @@ class FlatOptimizer:
         return self.scratch[0]
 
 
-# ------------------------------------------------------------------------------------------------- tcgen05 GEMM
+# ------------------------------------------------------------------------------------------------- wgmma GEMM
 def gemm_bf16(a, b, a_major="k", b_major="k", bias=None, relu=False, out_dtype=torch.bfloat16, out=None, splits=1,
               block_n=None, accumulate=False, stream=None):
-    """``D[M,N] (+)= A B^T`` on the 5th-generation tensor cores (csrc/gemm.cu: TMA -> tcgen05.mma -> TMEM).
+    """``D[M,N] (+)= A B^T`` on the tensor cores (csrc/gemm.cu: TMA -> wgmma -> register accumulators).
 
     ``a_major="k"``: ``a`` is [M, K] row-major; ``"mn"``: ``a`` is [K, M] row-major (its transpose is what is
     multiplied, without being materialised).  Same for ``b`` ([N, K] or [K, N]).  ``splits > 1`` or ``accumulate``

@@ -254,5 +254,5 @@ if __name__ == "__main__":
     mkdir("tf_log")
     set_one_thread()
     random_seed()
-    select_device(-1)                      # select_device(0) for the B200 path (required by the DQN family: HBM replay)
+    select_device(-1)                      # select_device(0) for the H100 path (required by the DQN family: HBM replay)
     a2c_feature(game="CartPole-v0", max_steps=int(2e4))

@@ -1,4 +1,4 @@
-/* b2rl.h -- C ABI of libb2rl.so: the sm_100a hot path behind the DeepRL (ShangtongZhang/DeepRL) API.
+/* b2rl.h -- C ABI of libb2rl.so: the sm_90a hot path behind the DeepRL (ShangtongZhang/DeepRL) API.
  *
  * The reference has NO FFI / plugin layer: its seams are duck-typed Python factories on Config
  * (SURVEY.md 8b).  This header is the boundary a maintainer binds with ctypes (INTEGRATION.md)
@@ -208,8 +208,8 @@ int b2rl_act_bwd_bias_grad_bf16(const uint16_t* gy, const uint16_t* y, int64_t r
                                 int32_t V, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * tcgen05 GEMM for the dense contractions (network_bodies.py:27-33, network_heads.py:18-21):
- *   D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 operands, fp32 accumulation in tensor memory (TMEM), TMA-fed.
+ * wgmma GEMM for the dense contractions (network_bodies.py:27-33, network_heads.py:18-21):
+ *   D[M,N] (+)= A[M,K] * B[N,K]^T, bf16 operands, fp32 accumulation in registers, TMA-fed.
  * a_mn / b_mn = 0: operand stored row-major [rows][K] (K-major); 1: stored row-major [K][rows] (MN-major) -- weight
  * gradients dW = g^T x read both operands as stored, nothing is transposed in memory.  lda/ldb/ldd: row strides in
  * elements (operands: multiples of 8).  out_mode 0: bf16 store, 1: fp32 store, 2: fp32 atomicAdd into D (required for
@@ -295,7 +295,7 @@ int b2rl_head_bwd(const float* gq, const uint16_t* phi, const float* Wa, const f
 int b2rl_head_bwd_relu(const float* gq, const uint16_t* phi, const float* Wa, const float* Wv, int32_t B, int32_t K, int32_t A,
                        uint16_t* gphi, float* gWa, float* gba, float* gWv, float* gbv, float* relu_colsum, void* stream);
 
-/* Convolution weight gradient as split-K partials (no atomics): partial i of *n_partials_host (<= 148, written on the
+/* Convolution weight gradient as split-K partials (no atomics): partial i of *n_partials_host (<= one per SM, written on the
  * HOST, deterministic for given shapes) is stored at partials + i * n_out*taps*C floats. */
 int b2rl_conv_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out, int32_t taps,
                              int32_t taps_x, int32_t grid_w, float* partials, int32_t* n_partials_host, void* stream);
@@ -325,7 +325,7 @@ int b2rl_gemm_splitk_bf16(const uint16_t* A, int64_t lda, const uint16_t* B, int
                           int32_t* counters, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Tail of one gradient update for a NatureConvBody network on the tcgen05 path (csrc/tail.cu):
+ * Tail of one gradient update for a NatureConvBody network on the wgmma path (csrc/tail.cu):
  * loss.backward()'s last step + clip_grad_norm_ + optimizer.step (DQN_agent.py:131-134) in two launches.
  * Work is described by unit tables (int32 x 4 per unit: arena offset, length, kind, row | segment << 16;
  * kinds 0 plain, 1-4 one output row (or 256-element segment of it) of conv1 / conv2 / conv3 / fc4 weights,
@@ -408,7 +408,7 @@ int b2rl_ppo_minibatch_updates(const float* state, const float* action, const fl
                                float kl_gate, float* stats, void* stream);
 
 /* Element-wise halves of the distributional heads (CategoricalNet / QuantileNet, network_heads.py:40-55, 89-102) around the
- * tcgen05 GEMMs: softmax + log_softmax over the N atoms of every (b, a) row (either output may be NULL), and the backward
+ * wgmma GEMMs: softmax + log_softmax over the N atoms of every (b, a) row (either output may be NULL), and the backward
  * preparation dlogits = dout - prob * sum_n dout (prob == NULL: dlogits = dout, QR-DQN) written as the bf16 GEMM operand
  * g [B][ld] (ld >= A*N, multiple of 8; padding zeroed) with its column sums ADDED to dbias [A*N] (the bias gradient). */
 int b2rl_dist_softmax(const float* logits, int32_t rows, int32_t N, float* prob, float* log_prob, void* stream);

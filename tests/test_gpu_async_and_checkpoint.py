@@ -116,7 +116,7 @@ def test_host_cursor_follows_feeds_captured_in_the_graph(rl, workload):
     then read the cursor from the device (replay.py:80-90 keeps it on the host; ours lives in ``ring_state``)."""
     import bench
     bench.CAP = 30_000
-    rl.Config.COMPUTE_DTYPE = torch.bfloat16             # (the learner bench.py builds: bf16 tcgen05 body)
+    rl.Config.COMPUTE_DTYPE = torch.bfloat16             # (the learner bench.py builds: bf16 wgmma body)
     try:
         lr = bench.build_learner(rl, workload, torch.device("cuda", 0), 0, 1, prefetch=False)
         rp = lr.replay

@@ -40,7 +40,7 @@ def test_conv1_from_ring_is_bit_identical(env, B, n_step):
     for a, b in ((mat.action, ring.action), (mat.reward, ring.reward), (mat.mask, ring.mask)):
         assert torch.equal(a, b)
     torch.manual_seed(0)
-    body = rl.NatureConvBody(in_channels=4)
+    body = rl.NatureConvBody(in_channels=4).to(dev)
     pk = nature_tc.repack(body, 1.0 / 255)
     b1 = body.conv1.bias.detach()
     for which, (m, r) in enumerate(((mat.state, ring.state), (mat.next_state, ring.next_state))):

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with ``-m gpu`` on the B200): every CUDA entry point of libb2rl.so, called through
+"""GPU parity tests (run with ``-m gpu`` on an H100): every CUDA entry point of libb2rl.so, called through
 the product's host mirror, against (a) the golden vectors generated from the reference itself and (b) the
 pinned CPU oracle on fresh seeded inputs.  Bars: bit-exact for indices, uint8 frames, float64 tree nodes and
 fp32 quantities whose operation order is fully specified; the tolerance written beside each check otherwise.
@@ -593,7 +593,7 @@ def test_conv_grid_gemm_vs_torch(rl, slab):
 
 
 def _conv_grid_gemm_vs_torch(rl):
-    """Shifted-row tcgen05 GEMMs of network/nature_tc.py against torch convolutions in fp32 on the same bf16 operands:
+    """Shifted-row wgmma GEMMs of network/nature_tc.py against torch convolutions in fp32 on the same bf16 operands:
     each layer's forward (with the space-to-depth / compaction epilogues), dgrad and wgrad, then the whole body."""
     import torch.nn.functional as F
     from deeprl_b200.network import nature_tc as tc
@@ -663,7 +663,7 @@ def _conv_grid_gemm_vs_torch(rl):
     tc.conv_gemm(1, x0m, g1, 32, 4, 2, 21, 1, gw1f, splits=32, block_n=64)
     g_un = tc.unpack_grads(gw1f, gw2f, gw3f, torch.zeros(512, 3136, device="cuda"), 1.0, 4)
     torch.testing.assert_close(g_un[0], w1l.grad, rtol=1e-3, atol=0.5)       # sums of 2400 products of magnitude ~100
-    # whole body through autograd: tcgen05 backend vs library backend (both bf16) on a NatureConvBody
+    # whole body through autograd: wgmma backend vs library backend (both bf16) on a NatureConvBody
     rl.Config.COMPUTE_DTYPE = torch.bfloat16
     try:
         torch.manual_seed(0)

@@ -1,4 +1,4 @@
-"""The assembled update that bench.py times (GraphedDQNLearner: bf16 tcgen05 body, K1 conv1 from the uint8 ring, fused loss,
+"""The assembled update that bench.py times (GraphedDQNLearner: bf16 wgmma body, K1 conv1 from the uint8 ring, fused loss,
 fused backward epilogues, two-launch tail) against the oracle's fp32 restatement of ``DQNAgent.step``'s update
 (DQN_agent.py:115-134; oracle/agents.py DQNFamilyOracle, pinned against the real reference by tests/test_oracle_golden.py)
 on the SAME batch (the indices the learner sampled), the same weights, target network and optimizer state, at batch 512.

@@ -183,7 +183,7 @@ def test_splitk_fixup_gemm_vs_torch(rl, M, N, K, splits, block_n):
 
 @pytest.mark.parametrize("kind,A,N", [("c51", 4, 51), ("qr", 4, 200), ("c51", 6, 51), ("qr", 18, 32)])
 def test_dist_head_vs_torch(rl, kind, A, N):
-    """Distributional head on the tcgen05 GEMM + csrc/disthead.cu (network/fused.py _DistHead) against fp32 torch on the same bf16
+    """Distributional head on the wgmma GEMM + csrc/disthead.cu (network/fused.py _DistHead) against fp32 torch on the same bf16
     operands: prob / log_prob (C51) or quantiles (QR-DQN), and the gradients w.r.t. the features, weight and bias."""
     from deeprl_b200.network import fused
     dev = torch.device("cuda", 0)
