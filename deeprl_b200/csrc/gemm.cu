@@ -82,8 +82,10 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// named barriers: 0 = __syncthreads, 1 = the 256 MMA threads, 2 / 3 = MMA warpgroup 1 / 2, 4 = uint8 converters
+// named barriers: 0 = __syncthreads, 1 = the 256 MMA threads, 2 / 3 = MMA warpgroup 1 / 2, 4 = uint8 converters,
+// 5 / 6 = "MMA turn" of warpgroup 1 / 2 (slab kernel)
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // wgmma shared-memory matrix descriptor, 128B swizzle (layout type 1 in bits 62-63):
 //   K-major : 8-row groups 1024 B apart (SBO), LBO unused
@@ -98,6 +100,7 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_b
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void acc_zero(float* d) {
 #pragma unroll
@@ -718,7 +721,13 @@ struct SlabParams {
 };
 
 constexpr int SLAB_U8_THREADS = GEMM_THREADS + 128;   // K1: a fourth warpgroup (warps 12-15) converts the uint8 pixels
-template <int BN, bool EXT, bool U8>
+// The tap grid (TX x TY taps) and the column blocks (CB = channels / 64) are template parameters: a tile's 2 x TX x TY x CB
+// k-tiles are then one unrolled chain of wgmmas in ONE commit group (a chain carried through runtime loops makes ptxas
+// serialize every wgmma).  The two MMA warpgroups ping-pong: warpgroup g takes every other tile of the CTA (the CTA's
+// i-th tile goes to warpgroup i % 2), whole 128-row tiles as two m64 accumulator halves, and "MMA turn" named barriers
+// let a warpgroup issue its tile's MMAs only after the other one has issued the previous tile's -- so one warpgroup's
+// epilogue runs while the other's MMAs keep the tensor cores busy.
+template <int BN, bool EXT, bool U8, int TX, int TY, int CB>
 __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_slab_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                           const __grid_constant__ CUtensorMap tmB,
                                                                           const __grid_constant__ CUtensorMap tmA2,
@@ -736,9 +745,9 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
   constexpr int MAX_STAGES = 6;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int k_tiles = sp.taps * sp.col_blocks;
+  constexpr int k_tiles = TX * TY * CB;
   const uint32_t slab_block = (uint32_t)sp.slab_rows * 128;          // one 64-channel column block of a slab
-  const uint32_t slab_bytes = slab_block * sp.col_blocks;
+  const uint32_t slab_bytes = slab_block * CB;
   uint8_t* sW = smem;
   uint8_t* sS = smem + (size_t)k_tiles * W_TILE;
   float* sAcc = reinterpret_cast<float*>(sS + (size_t)sp.stages * slab_bytes);
@@ -759,7 +768,7 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
   __shared__ float s_dbias[128];                    // per-CTA bias-gradient accumulator (backward extras)
   if (threadIdx.x < 128) s_dbias[threadIdx.x] = 0.0f;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS); }
+    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS / 2); }   // one warpgroup per slab
     mb_init(w_full, 1);
     if (U8) {
       for (int s = 0; s < U8_STAGES; ++s) { mb_init(&u8_full[s], 1); mb_init(&u8_empty[s], 1); }
@@ -770,8 +779,11 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
   }
   __syncthreads();
   pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
-
-  if (warp == 0 && elect_one()) {
+  // register file split of the 384-thread kernel (setmaxnreg): the producer warpgroup needs few, the MMA warpgroups hold two
+  // m64 x BN accumulator halves across the epilogue of the first (BN 128: 128 registers); 128 x 56 + 256 x 224 <= 64K
+  if (warp < 4) {
+    if constexpr (!U8) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+    if (warp == 0 && elect_one()) {
     mb_expect_tx(w_full, (uint32_t)k_tiles * W_TILE);
     for (int kt = 0; kt < k_tiles; ++kt) tma_load_2d(sW + (size_t)kt * W_TILE, mB, w_full, kt * GEMM_BK, 0);
     if constexpr (U8) {
@@ -800,10 +812,11 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
         const int s = it % sp.stages;
         mb_wait(&empty[s], ((it / sp.stages) & 1) ^ 1);
         mb_expect_tx(&full[s], slab_bytes);
-        for (int cb = 0; cb < sp.col_blocks; ++cb)
+        for (int cb = 0; cb < CB; ++cb)
           tma_load_2d(sS + (size_t)s * slab_bytes + (size_t)cb * slab_block, mA, &full[s], cb * GEMM_BK,
                       tile * GEMM_BM + sp.min_shift);
       }
+    }
     }
   } else if (U8 && warp >= 12) {
     // ---------------------------------------------------------------------- K1 converters (warps 12-15): staged uint8 -> slab
@@ -817,45 +830,59 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
                       sp.slab_rows, u8_slots_, tid, 4);
       if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
     }
-  } else if (warp >= 4 && warp < 12) {
-    // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: rows 64 g .. 64 g + 63
+  } else {
+    // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: tiles i = g, g + 2, ...
+    // of this CTA, rows 0-63 / 64-127 of a tile in accumulator halves d[0] / d[1]; the epilogue stages one half at a time
+    // through the warpgroup's own 64-row part of sAcc
+    if constexpr (!U8) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
     const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
-    const int rl = g * 64 + (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;
+    const int rl = (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;       // epilogue: row of the half, first 32-column chunk
     float* sAcc_g = sAcc + g * 64 * ACC_LD;
-    const uint32_t slab0 = s2u(sS) + (uint32_t)g * 64 * 128, w0 = s2u(sW);
-    const int taps_y = sp.taps / p.taps_x;
+    const uint32_t w0 = s2u(sW);
     mb_wait(w_full, 0);
-    uint32_t it = 0;
-    for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
+    uint32_t it = g;
+    for (int tile = cta + g * n_cta; tile < tiles; tile += 2 * n_cta, it += 2) {
       const int s = it % sp.stages;
+      if (it > 0) named_sync(5 + g, 256);                           // the other warpgroup has issued tile it - 1
       mb_wait(&full[s], (it / sp.stages) & 1);
-      float d[BN / 2];
-      acc_zero<BN>(d);
-      const uint32_t slab = slab0 + (uint32_t)s * slab_bytes;
-      uint32_t kt = 0;
-      // taps in (dy, dx) order; the window of tap (dy, dx) starts sign*(dy*grid_w + dx) - min_shift rows into the slab
-      int row_dy = -sp.min_shift;                                   // rows, for dx = 0
-      for (int dy = 0; dy < taps_y; ++dy, row_dy += p.shift_sign * p.grid_w) {
-        int row = row_dy;
-        for (int dx = 0; dx < p.taps_x; ++dx, row += p.shift_sign) {
-          for (int cb = 0; cb < sp.col_blocks; ++cb, ++kt) {
-            const uint32_t a_addr = slab + cb * slab_block + (uint32_t)row * 128;
-            const uint64_t a = make_desc(a_addr, 16, sp.base_offset_mode == 1 ? (a_addr >> 7) & 7 : 0);
-            // one commit group per k-tile: accumulator chains carried across the runtime tap loops without a wait make
-            // ptxas serialize every wgmma
-            wg_fence();
-            mma_ktile<BN, 0, 0>(d, a, make_desc(w0 + kt * W_TILE, 16));
-            wg_commit();
-            wg_wait0();
-            acc_fence<BN>(d);
+      float d[2][BN / 2];
+      acc_zero<BN>(d[0]);
+      acc_zero<BN>(d[1]);
+      acc_fence<BN>(d[0]);                                          // both halves zeroed before the chain: no wait inside it
+      acc_fence<BN>(d[1]);
+      const uint32_t slab = s2u(sS) + (uint32_t)s * slab_bytes;
+      wg_fence();
+      // taps in (dy, dx) order; the window of tap (dy, dx) of half h starts sign*(dy*grid_w + dx) - min_shift + 64 h rows
+      // into the slab
+#pragma unroll
+      for (int dy = 0; dy < TY; ++dy) {
+#pragma unroll
+        for (int dx = 0; dx < TX; ++dx) {
+#pragma unroll
+          for (int cb = 0; cb < CB; ++cb) {
+            const uint64_t b = make_desc(w0 + ((dy * TX + dx) * CB + cb) * W_TILE, 16);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = 64 * h - sp.min_shift + p.shift_sign * (dy * p.grid_w + dx);
+              const uint32_t a_addr = slab + cb * slab_block + (uint32_t)row * 128;
+              mma_ktile<BN, 0, 0>(d[h], make_desc(a_addr, 16, sp.base_offset_mode == 1 ? (a_addr >> 7) & 7 : 0), b);
+            }
           }
         }
       }
+      wg_commit();
+      if (tile + n_cta < tiles) named_arrive(5 + (g ^ 1), 256);      // MMA turn to the other warpgroup
+      wg_wait0();
+      acc_fence<BN>(d[0]);
+      acc_fence<BN>(d[1]);
       if (lane == 0) mb_arrive(&empty[s]);
-      stage_acc<BN>(d, sAcc_g, ACC_LD, wl, lane);
-      named_sync(2 + g, 128);
-      epilogue_row<BN, EXT>(p, tile * GEMM_BM + rl, 0, lane, sAcc + rl * ACC_LD, c0, s_dbias);
-      named_sync(2 + g, 128);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        stage_acc<BN>(d[h], sAcc_g, ACC_LD, wl, lane);
+        named_sync(2 + g, 128);
+        epilogue_row<BN, EXT>(p, tile * GEMM_BM + 64 * h + rl, 0, lane, sAcc_g + rl * ACC_LD, c0, s_dbias);
+        named_sync(2 + g, 128);
+      }
     }
   }
   __syncthreads();
@@ -881,6 +908,7 @@ struct WgradParams {
   int64_t partial_stride;   // 0: atomically accumulate into D; > 0: CTA i stores its partial sums at D + i*partial_stride
   // one window per tap, built on the host (launch_wgrad): slab window offset (16-byte units) and accumulator column
   int n_runs;
+  int win0;                 // window of blockIdx.y == 0 (the one-window instantiation serves the last of an odd count)
   uint32_t run_off[9], run_acc[9];
   // M-stacking (n_out <= 64): warpgroup 2's A operand holds the SAME gradient columns read `stack_delta` rows away (a second
   // TMA box), so its accumulator rows of a window at shift s hold the tap at shift s - stack_delta: with stack_delta = -grid_w
@@ -892,7 +920,12 @@ struct WgradParams {
   U8Src u8;                                    // U8 kernels: the activation slabs come from the uint8 frame ring (K1)
 };
 
-template <bool U8>
+// The windows of a CTA are a compile-time shape WIN: WGRAD_N128 (one n128 window, C = 128), WGRAD_2X64 (two n64 windows) or
+// WGRAD_1X64 (one n64 window: the last group of an odd window count).  With no runtime choice of MMA shape in the
+// accumulator chain, ptxas keeps the wgmmas asynchronous: every k-tile is one commit group, and the group of k-tile i - 1 is
+// retired (its stage released) only after k-tile i has been issued.
+constexpr int WGRAD_N128 = 0, WGRAD_2X64 = 1, WGRAD_1X64 = 2;
+template <bool U8, int WIN>
 __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmG,
                                                                                              const __grid_constant__ CUtensorMap tmX,
                                                                                              const WgradParams w) {
@@ -976,35 +1009,42 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
                       w.slab_rows, u8_slots_, tid, 4);
       if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
     }
+  } else if (warp >= 4 && warp < 12 && n_kt > 0 && (warp - 4) / 4 >= w.a_boxes) {
+    // one A box (n_out <= 64, not stacked): warpgroup 2 only releases the stages
+    for (int i = 0; i < n_kt; ++i) {
+      mb_wait(&full[i % w.stages], (i / w.stages) & 1);
+      if (lane == 0) mb_arrive(&empty[i % w.stages]);
+    }
   } else if (warp >= 4 && warp < 12 && n_kt > 0) {
     // ---------------------------------------------------------------------- MMA, warpgroup g: accumulator rows (output
     // channels) 64 g .. 64 g + 63 from A box g -- or, M-stacked, the same channels one tap row further down
+    constexpr int NJ = WIN == WGRAD_2X64 ? 2 : 1, WC = WIN == WGRAD_N128 ? 128 : 64;   // windows, columns per window
     const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
-    const int j0 = blockIdx.y * (128 / w.C), nj = min(w.n_runs - j0, 128 / w.C);     // this CTA's taps
-    const bool busy = g < w.a_boxes;          // one A box (n_out <= 64, not stacked): warpgroup 2 only releases the stages
+    const int j0 = w.win0 + (int)blockIdx.y * NJ;                                      // this CTA's first window
     const uint64_t a0 = make_desc(s2u(smem) + g * 8192, 8192);
-    const uint32_t b_base = s2u(smem) + A_BYTES;
-    float d[64];
-    acc_zero<128>(d);
+    const uint32_t b0 = s2u(smem) + A_BYTES + w.run_off[j0] * 16;
+    const uint32_t b1 = s2u(smem) + A_BYTES + w.run_off[NJ > 1 ? j0 + 1 : j0] * 16;
+    float d[NJ * WC / 2];
+    acc_zero<NJ * WC>(d);
     for (int i = 0; i < n_kt; ++i) {
       const int s = i % w.stages;
       mb_wait(&full[s], (i / w.stages) & 1);
       const uint32_t st = (uint32_t)s * stage_bytes;
       const uint64_t a = a0 + (st >> 4);
-      if (busy) {
-        wg_fence();
-        if (w.C == 128) {
-          mma_ktile<128, 1, 1>(d, a, make_desc(b_base + st + w.run_off[j0] * 16, slab_block));
-        } else {
-          mma_ktile<64, 1, 1>(d, a, make_desc(b_base + st + w.run_off[j0] * 16, 8192));
-          if (nj > 1) mma_ktile<64, 1, 1>(d + 32, a, make_desc(b_base + st + w.run_off[j0 + 1] * 16, 8192));
-        }
-        wg_commit();
-        wg_wait0();
-        acc_fence<128>(d);
+      wg_fence();
+      if constexpr (WIN == WGRAD_N128) {
+        mma_ktile<128, 1, 1>(d, a, make_desc(b0 + st, slab_block));
+      } else {
+        mma_ktile<64, 1, 1>(d, a, make_desc(b0 + st, 8192));
+        if constexpr (NJ > 1) mma_ktile<64, 1, 1>(d + 32, a, make_desc(b1 + st, 8192));
       }
-      if (lane == 0) mb_arrive(&empty[s]);
+      wg_commit();
+      wg_wait1();                                                      // k-tile i - 1 has retired: release its stage
+      if (i > 0 && lane == 0) mb_arrive(&empty[(i - 1) % w.stages]);
     }
+    wg_wait0();
+    acc_fence<NJ * WC>(d);
+    if (lane == 0) mb_arrive(&empty[(n_kt - 1) % w.stages]);
     // accumulator element d[32 sl + 4 jj + 2 h + e]: channel 16 wl + lane / 4 + 8 h, column 64 sl + 8 jj + 2 (lane % 4) + e
     const bool low = w.stack_delta != 0 && g == 1;
     float* base = w.D + (int64_t)blockIdx.x * w.partial_stride + 2 * (lane & 3);
@@ -1012,10 +1052,9 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
     for (int h = 0; h < 2; ++h) {
       const int n = 16 * wl + (lane >> 2) + 8 * h;
       const int nn = low ? n : g * 64 + n;
-      if (!busy || nn >= w.n_out) continue;
+      if (nn >= w.n_out) continue;
 #pragma unroll
-      for (int sl = 0; sl < 2; ++sl) {
-        if (sl >= nj) break;
+      for (int sl = 0; sl < NJ; ++sl) {
         const int j = j0 + sl;
         int oc = w.tap0 * w.C + (int)w.run_acc[j];
         if (low) {
@@ -1024,8 +1063,7 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
         }
         float* dst = base + (int64_t)nn * w.ldd + oc;
 #pragma unroll
-        for (int jj = 0; jj < 16; ++jj) {
-          if (jj >= w.C / 8) break;
+        for (int jj = 0; jj < WC / 8; ++jj) {
           const float2 v = make_float2(d[32 * sl + 4 * jj + 2 * h], d[32 * sl + 4 * jj + 2 * h + 1]);
           if (w.partial_stride > 0) *reinterpret_cast<float2*>(dst + 8 * jj) = v;   // split-K partials: summed by the consumer
           else atomicAdd(reinterpret_cast<float2*>(dst + 8 * jj), v);
@@ -1163,15 +1201,15 @@ static int gemm_dispatch(const uint16_t* A, int a_mn, int64_t lda, int64_t a_row
   return launch_gemm<128, 4>(ta, tb, ta2, tb2, p, splits, st);
 }
 
-template <int BN, bool EXT, bool U8>
+template <int BN, bool EXT, bool U8, int TX, int TY, int CB>
 static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ta2, const CUtensorMap& tb2,
                          SlabParams sp, cudaStream_t st) {
-  const size_t w_bytes = (size_t)sp.taps * sp.col_blocks * BN * 128;
-  const size_t slab_bytes = (size_t)sp.slab_rows * 128 * sp.col_blocks;
+  const size_t w_bytes = (size_t)TX * TY * CB * BN * 128;
+  const size_t slab_bytes = (size_t)sp.slab_rows * 128 * CB;
   const int tiles = (sp.g.M + GEMM_BM - 1) / GEMM_BM;
   // weights + slab ring + accumulator staging + barriers (+ uint8 staging) within the shared memory of one SM
   const size_t fixed = 1024 + acc_stage_bytes(BN) + (2 * 6 + 2) * 8 + 128;
-  auto k = conv_slab_wgmma_kernel<BN, EXT, U8>;
+  auto k = conv_slab_wgmma_kernel<BN, EXT, U8, TX, TY, CB>;
   static const size_t limit = dyn_smem_limit(k);
   if (limit <= fixed) return 1;
   size_t u8_extra = 0;
@@ -1203,25 +1241,57 @@ static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   return check_launch("b2rl_conv_gemm_bf16(slab)");
 }
 
+// the slab kernel is instantiated for the layer shapes of NatureConvBody (taps_x x taps_y taps, col_blocks 64-channel blocks):
+// conv1 forward (2x2, 1, block_n 32), conv2 forward (2x2, 2, 64), conv3 forward and dgrad (3x3, 1, 64), conv2 dgrad (2x2, 1,
+// 128); returns 1 for any other shape (the caller falls back to tap addressing)
+template <int BN, bool EXT>
+static int launch_slab_shape(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ta2, const CUtensorMap& tb2,
+                             const SlabParams& sp, cudaStream_t st) {
+  const int tx = sp.g.taps_x, ty = sp.taps / sp.g.taps_x, cb = sp.col_blocks;
+  if (tx * ty != sp.taps) return 1;
+  if constexpr (BN == 32) {
+    if (tx == 2 && ty == 2 && cb == 1) return launch_slab_t<32, EXT, false, 2, 2, 1>(ta, tb, ta2, tb2, sp, st);
+  } else if constexpr (BN == 64) {
+    if (tx == 2 && ty == 2 && cb == 2) return launch_slab_t<64, EXT, false, 2, 2, 2>(ta, tb, ta2, tb2, sp, st);
+    if (tx == 3 && ty == 3 && cb == 1) return launch_slab_t<64, EXT, false, 3, 3, 1>(ta, tb, ta2, tb2, sp, st);
+  } else {
+    if (tx == 2 && ty == 2 && cb == 1) return launch_slab_t<128, EXT, false, 2, 2, 1>(ta, tb, ta2, tb2, sp, st);
+  }
+  return 1;
+}
+
 template <int BN>
 static int launch_slab(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ta2, const CUtensorMap& tb2,
                        SlabParams sp, cudaStream_t st) {
   if (sp.u8.frames) {                                                // K1: conv1 forward straight from the uint8 ring
     if constexpr (BN == 32) {
-      if (!has_ext(sp.g) && !sp.g.dual && sp.col_blocks == 1) return launch_slab_t<32, false, true>(ta, tb, ta2, tb2, sp, st);
+      if (!has_ext(sp.g) && !sp.g.dual && sp.col_blocks == 1 && sp.taps == 4 && sp.g.taps_x == 2)
+        return launch_slab_t<32, false, true, 2, 2, 1>(ta, tb, ta2, tb2, sp, st);
     }
-    set_error("the uint8-ring producer serves block_n 32, 64 channels, no backward extras, no dual launch");
+    set_error("the uint8-ring producer serves block_n 32, 2x2 taps of 64 channels, no backward extras, no dual launch");
     return B2RL_ERR_ARG;
   }
-  return has_ext(sp.g) ? launch_slab_t<BN, true, false>(ta, tb, ta2, tb2, sp, st)
-                       : launch_slab_t<BN, false, false>(ta, tb, ta2, tb2, sp, st);
+  return has_ext(sp.g) ? launch_slab_shape<BN, true>(ta, tb, ta2, tb2, sp, st)
+                       : launch_slab_shape<BN, false>(ta, tb, ta2, tb2, sp, st);
+}
+
+// one launch of the weight-gradient instantiation for window shape WIN over `groups` tap groups from window w.win0 on
+template <bool U8, int WIN>
+static void launch_wgrad_k(const CUtensorMap& tg, const CUtensorMap& tx, const WgradParams& w, int ctas, int groups,
+                           size_t smem, cudaStream_t st) {
+  auto k = conv_wgrad_wgmma_kernel<U8, WIN>;
+  static size_t attr = 0;
+  if (attr < smem) {
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    attr = smem;
+  }
+  launch_pdl(k, dim3(ctas, groups), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, tg, tx, w);
 }
 
 template <bool U8 = false>
 static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParams w, cudaStream_t st, int* n_ctas = nullptr) {
   const size_t slab_bytes = (size_t)w.slab_rows * 128 * w.col_blocks, stage = 16384 + slab_bytes;
-  auto k = conv_wgrad_wgmma_kernel<U8>;
-  static const size_t limit = dyn_smem_limit(k);
+  static const size_t limit = dyn_smem_limit(conv_wgrad_wgmma_kernel<U8, WGRAD_2X64>);
   const size_t fixed = 1024 + 2 * 6 * 8 + 16 + (U8 ? 2 * U8_MAX_STAGES * 8 + 144 : 0);
   const size_t budget = limit > fixed + 200 * 1024 ? 200 * 1024 : (limit > fixed ? limit - fixed : 0);
   size_t u8_extra = 0;
@@ -1239,11 +1309,6 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   if (stages < 2) return 1;
   w.stages = stages;
   const size_t smem = 1024 + stages * stage + 2 * 6 * 8 + 16 + u8_extra;
-  static size_t attr = 0;
-  if (attr < smem) {
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    attr = smem;
-  }
   // one window per tap; a CTA accumulates the taps of one 128-column group (blockIdx.y)
   if (w.ntaps > 9 || (w.C != 64 && w.C != 128)) return 1;
   for (int n = 0; n < w.ntaps; ++n) {
@@ -1268,7 +1333,19 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   w.k_tiles_per_cta = (kt_total + ctas - 1) / ctas;
   ctas = (kt_total + w.k_tiles_per_cta - 1) / w.k_tiles_per_cta;
   if (n_ctas) *n_ctas = ctas;
-  launch_pdl(k, dim3(ctas, groups), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, tg, tx, w);
+  w.win0 = 0;
+  if constexpr (U8) {                                                // conv1 from the ring: two windows of 64 channels
+    if (w.C != 64 || w.ntaps != 2) return 1;
+    launch_wgrad_k<true, WGRAD_2X64>(tg, tx, w, ctas, 1, smem, st);
+  } else if (w.C == 128) {
+    launch_wgrad_k<false, WGRAD_N128>(tg, tx, w, ctas, groups, smem, st);
+  } else {                                                           // pairs of windows, then the odd one out on its own
+    if (w.ntaps >= 2) launch_wgrad_k<false, WGRAD_2X64>(tg, tx, w, ctas, w.ntaps / 2, smem, st);
+    if (w.ntaps % 2) {
+      w.win0 = w.ntaps - 1;
+      launch_wgrad_k<false, WGRAD_1X64>(tg, tx, w, ctas, 1, smem, st);
+    }
+  }
   return check_launch("b2rl_conv_gemm_bf16(wgrad slab)");
 }
 

@@ -1,0 +1,32 @@
+"""SASS-level guard: the convolution wgmma kernels keep their MMAs asynchronous.  When ptxas serializes wgmmas (C7511) every
+HGMMA is followed by a full drain (WARPGROUP.DEPBAR.LE gsb0, 0x0); a slab kernel that waits once per k-tile drains after
+every 4 HGMMAs.  The weight-gradient kernels retire k-tiles one behind (DEPBAR.LE gsb0, 0x1) and drain once, the slab
+kernels drain once per tile."""
+import subprocess
+
+import pytest
+
+from deeprl_b200 import _lib
+
+
+def test_conv_wgmma_kernels_do_not_drain_per_ktile():
+    import shutil
+    if shutil.which("cuobjdump") is None:
+        pytest.skip("cuobjdump not on PATH")
+    sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, timeout=300).stdout
+    counts = {}
+    name = None
+    for line in sass.splitlines():
+        if "Function :" in line:
+            name = line.split("Function :")[1].strip()
+            counts[name] = [0, 0, 0]
+        elif name is not None:
+            counts[name][0] += "HGMMA" in line
+            counts[name][1] += "WARPGROUP.DEPBAR" in line
+            counts[name][2] += "WARPGROUP.DEPBAR.LE gsb0, 0x0" in line
+    conv = {k: v for k, v in counts.items() if "conv_wgrad_wgmma_kernel" in k or "conv_slab_wgmma_kernel" in k}
+    assert sum("conv_wgrad" in k for k in conv) >= 4 and sum("conv_slab" in k for k in conv) >= 9, sorted(conv)
+    for k, (mma, waits, drains) in conv.items():
+        assert mma >= 12, (k, mma)
+        assert drains <= mma // 8, "%s: %d full drains for %d HGMMA" % (k, drains, mma)
+        assert waits <= mma // 4 + 1, "%s: %d waits for %d HGMMA" % (k, waits, mma)
