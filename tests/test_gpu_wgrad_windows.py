@@ -10,6 +10,8 @@ from deeprl_b200.network import nature_tc as tc
 @pytest.mark.gpu
 @pytest.mark.parametrize("n_out", [128, 96])
 def test_conv_wgrad_odd_window_count(n_out):
+    if not torch.cuda.is_available():
+        pytest.skip("needs a GPU")
     gen = torch.Generator(device="cuda").manual_seed(5)
     B, G, C, taps_x = 6, 10, 64, 3
     rows = B * G * G
