@@ -20,8 +20,8 @@
 //   warpgroup 0      TMA producer: one ELECTED thread of warp 0 (elect.sync, see elect_one) issues cp.async.bulk.tensor
 //                    into a STAGES-deep 128B-swizzled smem ring (mbarrier full/empty); warps 1-3 idle
 //   warpgroups 1, 2  rows 0-63 / 64-127 of the tile: wgmma.mma_async m64nBNk16 (fp32 accumulators in registers), then the
-//                    epilogue: accumulators -> shared staging tile -> one row x 32 columns per thread -> bias / ReLU ->
-//                    bf16 | fp32 | atomic fp32
+//                    epilogue: accumulators -> shared staging tile -> 8 columns x BN/16 rows per thread, whole rows
+//                    per warp instruction (epi_col / epi_row) -> bias / ReLU -> bf16 | fp32 | atomic fp32
 // Every kernel runs its prologue (barrier init, tensor-map prefetch) before pdl_sync(): under programmatic dependent launch
 // that part overlaps the tail of the previous kernel (common.cuh).
 // sm_90a only.
@@ -68,6 +68,10 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
           s2u(smem_dst)),
       "l"(map), "r"(s2u(bar)), "r"(c0), "r"(c1)
       : "memory");
+}
+// bulk prefetch of `bytes` (a multiple of 16, 16-byte aligned start) from global memory into L2
+__device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
 // One elected lane of a fully active warp: the single-thread producer role is entered through elect.sync rather than a
 // plain `lane == 0` test, so that the compiler issues the TMA instructions without an ELECT / BRA.U.ANY loop around them.
@@ -154,7 +158,7 @@ struct GemmParams {
   int dual;
   void* D2;
   const float* bias2;
-  // backward extras (see epilogue_row): ReLU-gradient mask, bias-gradient accumulation, grid scatter maps 3 / 4
+  // backward extras (see epilogue_half): ReLU-gradient mask, bias-gradient accumulation, grid scatter maps 3 / 4
   const __nv_bfloat16* mask;
   int64_t mask_ld;
   float* dbias;
@@ -170,164 +174,247 @@ __device__ __forceinline__ int tap_shift(const GemmParams& p, int tap) {
   return p.shift_sign * ((tap / p.taps_x) * p.grid_w + tap % p.taps_x);
 }
 
-// Epilogue of one row of a 128 x BN tile for one thread: `srow` is that row of the shared staging tile (fp32 accumulators),
-// the thread handles its 32-column chunks c0, c0 + 64, ...; the 32 lanes of a warp hold 32 consecutive rows.
+// accumulator staging tile of the epilogue: 128 rows x (BN + 8) fp32.  The 8-float pad puts consecutive rows 32 bytes apart
+// in the bank pattern: the float2 writes of stage_acc (4 rows x 32 bytes per half-warp) and the float4 reads of
+// epilogue_half (see there) are free of bank conflicts.  The split-K fix-up (epilogue_fixup, out_mode 3, off by default)
+// still reads one row per lane; its float4 reads see 2-way conflicts at this stride.
+__host__ __device__ constexpr int acc_ld(int bn) { return bn + 8; }
+__host__ __device__ constexpr size_t acc_stage_bytes(int bn) { return (size_t)GEMM_BM * acc_ld(bn) * 4; }
+
+// Epilogue thread mapping: in a 64-row half of a 128 x BN tile, thread t (0..127 of the warpgroup) owns the 8 columns
+// epi_col(t) .. + 7 of the rows epi_row(t, k), k = 0 .. BN/16 - 1.  BN/8 consecutive lanes cover one row, so one warp
+// instruction covers 32 / (BN/8) whole consecutive rows: every 16-byte store or mask load of a warp is part of a contiguous
+// run of BN * 2 bytes (bf16) per row -- or, for the scatter maps 3 / 4, of sub_c channels -- and a thread visits the same
+// columns in every row, which lets it keep the bias-gradient column sums of a half in registers (dbias_flush).
+template <int BN>
+__device__ __forceinline__ int epi_col(int t) { return 8 * (t % (BN / 8)); }
+template <int BN>
+__device__ __forceinline__ int epi_row(int t, int k) { return t / (BN / 8) + k * (1024 / BN); }
+
 // Backward extras (dgrad GEMMs): `mask` is the saved forward activation in the GEMM's own output coordinates -- the ReLU
 // gradient is applied in the epilogue (v = mask > 0 ? v : 0); `dbias` receives the column sums of the masked tile (the bias
-// gradient of the layer below) through a per-CTA shared accumulator `s_dbias`, index = column % dbias_mod.  Output row maps
-// 3 / 4 scatter the tile into the G x G grid matrix the next backward GEMMs read:
+// gradient of the layer below), index = column % dbias_mod (dbias_mod 0: the column).  Output row maps 3 / 4 scatter the
+// tile into the G x G grid matrix the next backward GEMMs read:
 //   map 3: rows are space-to-depth(2) positions [b][oy][ox] of an (V/2)^2 grid, columns are 4 sub-positions x sub_c channels
 //          -> grid row b*G*G + (2*oy + dy)*G + 2*ox + dx, column = channel           (conv2's input gradient -> conv1's grid)
 //   map 4: rows are images b, columns are V*V positions x sub_c channels
 //          -> grid row b*G*G + (pos / V)*G + pos % V, column = channel               (fc4's input gradient -> conv3's grid)
 // Grid rows that no tile covers keep whatever the destination holds: the caller keeps it zeroed (persistent buffer).
+//
+// The ReLU-gradient mask of one 64-row half (rows row0 ..), requested into registers ahead of its use so that its round
+// trip overlaps other work; the slab kernel's producer has prefetched it into L2 several tiles earlier.  A TMA ring of
+// 64-row mask boxes in shared memory fits beside the dgrad slab kernels only by giving up slab stages (conv2, BN 128: two
+// 16 KB boxes leave three of its five; conv3, BN 64: four 8 KB boxes leave four of six).  Built and measured that way, against the
+// old epilogue in the same session, it took conv2's dgrad from 59.5 to 52.7 us per update where these register loads take
+// it to 44.7 (from 60.1), and conv3's to 31.7 as these do to 31.1: the mask stays in global memory (DESIGN section 9).  fc4's dgrad, gemm_wgmma_kernel, has one tile per CTA.
+// 16-byte shared-memory load through an explicit shared-space address (a generic pointer would go through the L1 path
+// and hold a 64-bit address)
+__device__ __forceinline__ float4 lds128(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+// 16-byte read-only global load issued exactly where it is written: an asm volatile statement keeps its order with the
+// kernel's other asm volatile statements (barrier waits, wgmma), so the compiler cannot hoist it and its destination
+// registers above the MMAs
+__device__ __forceinline__ int4 ldg_v4_here(const void* ptr) {
+  int4 v;
+  asm volatile("ld.global.nc.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(ptr));
+  return v;
+}
 template <int BN, bool EXT>
-__device__ __forceinline__ void epilogue_row(const GemmParams& p, int row, int n0, int lane, const float* srow, int c0,
-                                             float* s_dbias) {
-  bool valid = row < p.M;
-  int64_t drow = row;
-  int dcol0 = 0;
-  int img = 0, sy = 0, sx = 0;                        // maps 3 / 4: image and source position of this row
-  if ((p.out_map == 1 || p.out_map == 2) && valid) {
+__device__ __forceinline__ void epi_mask_load(const GemmParams& p, int row0, int n0, int t, int4 (&m)[BN / 16]) {
+  if constexpr (EXT) {
+    const int n = n0 + epi_col<BN>(t);
+#pragma unroll
+    for (int k = 0; k < BN / 16; ++k) {
+      const int row = row0 + epi_row<BN>(t, k);
+      m[k] = make_int4(0, 0, 0, 0);
+      if (p.mask && row < p.M && n < p.N) m[k] = ldg_v4_here(p.mask + (int64_t)row * p.mask_ld + n);
+    }
+  }
+}
+
+// The bias-gradient sums a thread has kept for its 8 columns n0 + epi_col(t) .. + 7 -> added up over the lanes of the warp
+// that share those columns, then one shared-memory atomic per column and warp (BN / 32 instructions) into the per-CTA
+// accumulator s_dbias (index column % dbias_mod, or the column itself for dbias_mod 0), which the kernel adds to global
+// memory once at its end (dbias_slots).  dbias_mod 0 columns past 128 (plain GEMMs only) go to global memory directly.
+// All 32 lanes take part.
+template <int BN>
+__device__ __forceinline__ void dbias_flush(const GemmParams& p, int n0, int t, float (&dsum)[8], float* s_dbias) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+#pragma unroll
+    for (int s = BN / 8; s < 32; s <<= 1) dsum[j] += __shfl_xor_sync(0xffffffffu, dsum[j], s);
+  }
+  // lanes 0 .. BN/8 - 1 now hold the warp's sums of columns 8 lane .. + 7; spread them one column per lane, so that each
+  // shared-memory atomic instruction covers 32 distinct columns
+  const int lane = t & 31;
+#pragma unroll
+  for (int r = 0; r < BN / 32; ++r) {
+    const int v = 32 * r + lane;
+    float x = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float y = __shfl_sync(0xffffffffu, dsum[j], v >> 3);
+      if (j == (v & 7)) x = y;
+    }
+    const int col = n0 + v;
+    if (col < p.N) {
+      const int i = p.dbias_mod > 0 ? col % p.dbias_mod : col;
+      if (i < 128) atomicAdd(s_dbias + i, x);
+      else atomicAdd(p.dbias + col, x);
+    }
+  }
+}
+// entries of s_dbias a CTA adds to global memory at its end
+__device__ __forceinline__ int dbias_slots(const GemmParams& p) { return p.dbias_mod > 0 ? p.dbias_mod : min(p.N, 128); }
+
+// Row part of a destination offset (element index of the row's column 0 in D), or -1 for a row that is not stored: rows
+// past M, grid positions outside the valid V x V (maps 1 / 2)
+template <bool EXT>
+__device__ __forceinline__ int64_t epi_row_base(const GemmParams& p, int row) {
+  if (row >= p.M) return -1;
+  if (p.out_map == 1 || p.out_map == 2) {
     const int gg = p.G * p.G;
-    const int b = row / gg, rem = row - b * gg;
+    const int bi = row / gg, rem = row - bi * gg;
     const int oy = rem / p.G, ox = rem - oy * p.G;
-    valid = oy < p.V && ox < p.V;
-    if (p.out_map == 1) {
-      const int h = p.V >> 1;
-      drow = (int64_t)b * h * h + (oy >> 1) * h + (ox >> 1);
-      dcol0 = (((oy & 1) << 1) | (ox & 1)) * p.N;
-    } else {
-      drow = (int64_t)b * p.V * p.V + oy * p.V + ox;
-    }
-  } else if (EXT && p.out_map == 3 && valid) {
+    if (oy >= p.V || ox >= p.V) return -1;
+    if (p.out_map == 2) return ((int64_t)bi * p.V * p.V + oy * p.V + ox) * p.ldd;
+    const int h = p.V >> 1;
+    return ((int64_t)bi * h * h + (oy >> 1) * h + (ox >> 1)) * p.ldd + (((oy & 1) << 1) | (ox & 1)) * p.N;
+  }
+  if (EXT && p.out_map == 3) {
     const int h = p.V >> 1, hh = h * h;
-    img = row / hh;
-    const int rem = row - img * hh;
-    sy = rem / h, sx = rem - sy * h;
-  } else if (EXT && p.out_map == 4) {
-    img = row;
+    const int img = row / hh, rem = row - img * hh;
+    const int sy = rem / h, sx = rem - sy * h;
+    return ((int64_t)img * p.G * p.G + 2 * sy * p.G + 2 * sx) * p.ldd;
   }
-  for (int c = c0; c < BN; c += 64) {
-    uint32_t r[32];
+  if (EXT && p.out_map == 4) return (int64_t)row * p.G * p.G * p.ldd;
+  return (int64_t)row * p.ldd;
+}
+// Column part of a destination offset for column n (maps 3 / 4: sub_c is a multiple of 32, so 8 columns share one sub-position)
+template <bool EXT>
+__device__ __forceinline__ int64_t epi_col_off(const GemmParams& p, int n) {
+  if (EXT && p.out_map == 3) {
+    const int sub = n / p.sub_c, cc = n - sub * p.sub_c;
+    return (int64_t)((sub >> 1) * p.G + (sub & 1)) * p.ldd + cc;
+  }
+  if (EXT && p.out_map == 4) {
+    const int pos = n / p.sub_c, cc = n - pos * p.sub_c;
+    return (int64_t)((pos / p.V) * p.G + pos % p.V) * p.ldd + cc;
+  }
+  return n;
+}
+
+// Epilogue of one 64-row half of a 128 x BN tile (first row row0, first column n0) for warpgroup thread t: `s` is the
+// half's fp32 staging tile, `m` its mask (epi_mask_load).  The bias-gradient column sums of the half stay in registers
+// (dsum: the thread's 8 columns over its BN/16 rows) until one dbias_flush at the end.
+template <int BN, bool EXT>
+__device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int n0, int t, const float* s,
+                                              const int4 (&m)[BN / 16], float* s_dbias) {
+  constexpr int ACC_LD = acc_ld(BN);
+  float dsum[8] = {};
+  const int c = epi_col<BN>(t), n = n0 + c;
+  const bool cols = n < p.N, full = n + 8 <= p.N;
+  const bool add_bias = p.bias && blockIdx.z == 0 && cols;
+  float b[8];
+  if (add_bias) {
+    const float* bp = p.bias + n;
+    if (full && (reinterpret_cast<uintptr_t>(bp) & 15) == 0) {
+      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bp)), b1 = __ldg(reinterpret_cast<const float4*>(bp + 4));
+      b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+    } else {
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      const float4 v = *reinterpret_cast<const float4*>(srow + c + j);
-      r[j] = __float_as_uint(v.x); r[j + 1] = __float_as_uint(v.y); r[j + 2] = __float_as_uint(v.z); r[j + 3] = __float_as_uint(v.w);
-    }
-    const bool live = valid && n0 + c < p.N;
-    if (live) {
-      if (p.bias && blockIdx.z == 0) {
-        const float* bp = p.bias + n0 + c;
-        if (n0 + c + 32 <= p.N && (reinterpret_cast<uintptr_t>(bp) & 15) == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {                             // 8 broadcast 16-byte loads instead of 32 scalar ones
-            const float4 b4 = __ldg(reinterpret_cast<const float4*>(bp + j));
-            r[j] = __float_as_uint(__uint_as_float(r[j]) + b4.x);
-            r[j + 1] = __float_as_uint(__uint_as_float(r[j + 1]) + b4.y);
-            r[j + 2] = __float_as_uint(__uint_as_float(r[j + 2]) + b4.z);
-            r[j + 3] = __float_as_uint(__uint_as_float(r[j + 3]) + b4.w);
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (n0 + c + j < p.N) r[j] = __float_as_uint(__uint_as_float(r[j]) + __ldg(bp + j));
-        }
-      }
-      if (p.relu) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(fmaxf(__uint_as_float(r[j]), 0.0f));
-      }
-      if constexpr (EXT) {
-        if (p.mask) {                                                   // ReLU gradient: zero where the forward output was <= 0
-          const int4* mp = reinterpret_cast<const int4*>(p.mask + (int64_t)row * p.mask_ld + n0 + c);
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            const int4 m4 = __ldg(mp + (j >> 3));
-            const __nv_bfloat162* mh = reinterpret_cast<const __nv_bfloat162*>(&m4);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const float2 mf = __bfloat1622float2(mh[t]);
-              if (!(mf.x > 0.0f)) r[j + 2 * t] = 0;
-              if (!(mf.y > 0.0f)) r[j + 2 * t + 1] = 0;
-            }
-          }
-        }
-      }
-    }
-    if (EXT && p.dbias) {
-      // column sums over the 32 rows of this warp: 5-step register transpose-reduce (31 shuffles), lane l ends up with the
-      // total of column l; rows that are not live contribute zeros.  All 32 lanes take part.
-      float v[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = live ? __uint_as_float(r[j]) : 0.0f;
-#pragma unroll
-      for (int s = 16; s >= 1; s >>= 1) {
-        const bool hi = (lane & s) != 0;
-#pragma unroll
-        for (int j = 0; j < s; ++j) {
-          const float send = hi ? v[j] : v[j + s];
-          const float keep = hi ? v[j + s] : v[j];
-          v[j] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-        }
-      }
-      if (n0 + c + lane < p.N) {
-        if (p.dbias_mod > 0) atomicAdd(s_dbias + (n0 + c + lane) % p.dbias_mod, v[0]);
-        else atomicAdd(p.dbias + n0 + c + lane, v[0]);             // dbias_mod 0: one bias per output column, straight to global
-      }
-    }
-    if (live) {
-      int64_t off;
-      if (EXT && p.out_map == 3) {
-        const int sub = (n0 + c) / p.sub_c, cc = (n0 + c) - sub * p.sub_c;
-        off = ((int64_t)img * p.G * p.G + (2 * sy + (sub >> 1)) * p.G + 2 * sx + (sub & 1)) * p.ldd + cc;
-      } else if (EXT && p.out_map == 4) {
-        const int pos = (n0 + c) / p.sub_c, cc = (n0 + c) - pos * p.sub_c;
-        off = ((int64_t)img * p.G * p.G + (pos / p.V) * p.G + pos % p.V) * p.ldd + cc;
-      } else {
-        off = drow * p.ldd + dcol0 + n0 + c;
-      }
-      if (p.out_mode == 0) {
-        __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(p.D) + off;
-        if (n0 + c + 32 <= p.N && (off % 8 == 0)) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            int4 v;
-            __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&v);
-#pragma unroll
-            for (int t = 0; t < 4; ++t)
-              h[t] = __floats2bfloat162_rn(__uint_as_float(r[j + 2 * t]), __uint_as_float(r[j + 2 * t + 1]));
-            *reinterpret_cast<int4*>(d + j) = v;
-          }
-        } else {
-          for (int j = 0; j < 32; ++j)
-            if (n0 + c + j < p.N) d[j] = __float2bfloat16_rn(__uint_as_float(r[j]));
-        }
-      } else if (p.out_mode == 1) {
-        float* d = reinterpret_cast<float*>(p.D) + off;
-        if (n0 + c + 32 <= p.N && (off % 4 == 0)) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(d + j) = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                            __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-        } else {
-          for (int j = 0; j < 32; ++j)
-            if (n0 + c + j < p.N) d[j] = __uint_as_float(r[j]);
-        }
-      } else {
-        float* d = reinterpret_cast<float*>(p.D) + off;
-        if (n0 + c + 32 <= p.N && (reinterpret_cast<uintptr_t>(d) & 15) == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            atomicAdd(reinterpret_cast<float4*>(d + j), make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                                    __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3])));
-        } else {
-          for (int j = 0; j < 32; ++j)
-            if (n0 + c + j < p.N) atomicAdd(d + j, __uint_as_float(r[j]));
-        }
-      }
+      for (int j = 0; j < 8; ++j) b[j] = n + j < p.N ? __ldg(bp + j) : 0.0f;
     }
   }
+  // the 8 lanes of a 128-bit shared-memory access phase read distinct banks when the half of the 8 columns a lane reads
+  // first alternates with column group (BN 64 / 128: 8 lanes on one row) and with the row (BN 32: 4 lanes on each of two
+  // rows 32 bytes apart in the bank pattern); the rows of one thread all have the same parity
+  const int h0 = ((c >> 5) ^ epi_row<BN>(t, 0)) & 1;
+  const uint32_t s_base = s2u(s);
+  // destination offset = row part + column part: the column part is the same in every row of the thread; the row part
+  // (integer divisions for the maps) is computed once per row of the warp, by lane q for the warp's q-th row (pass
+  // q / (32 / (BN/8)), row q % (32 / (BN/8)) of the pass), and handed to the lanes of that row by a shuffle
+  const int64_t coff = epi_col_off<EXT>(p, n);
+  int64_t rbase = -1;
+  if ((t & 31) < 16) {
+    constexpr int RPW = 256 / BN;                                     // rows per warp instruction
+    const int q = t & 31;
+    rbase = epi_row_base<EXT>(p, row0 + (t >> 5) * RPW + q % RPW + (q / RPW) * 4 * RPW);
+  }
+#pragma unroll
+  for (int k = 0; k < BN / 16; ++k) {
+    const int rl = epi_row<BN>(t, k);
+    const uint32_t sp = s_base + (uint32_t)(rl * ACC_LD + c) * 4;
+    const float4 x = lds128(sp + 16 * h0), y = lds128(sp + 16 * (h0 ^ 1));
+    const float4 lo = h0 ? y : x, hi = h0 ? x : y;
+    float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    const int64_t base = __shfl_sync(0xffffffffu, rbase, k * (256 / BN) + (t & 31) / (BN / 8));
+    const int64_t off = base + coff;
+    if (!(base >= 0 && cols)) continue;
+    if (add_bias) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (full || n + j < p.N) v[j] += b[j];
+    }
+    if (p.relu) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.0f);
+    }
+    if constexpr (EXT) {
+      if (p.mask) {                                                     // ReLU gradient: zero where the forward output was <= 0
+        const __nv_bfloat162* mh = reinterpret_cast<const __nv_bfloat162*>(&m[k]);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 mf = __bfloat1622float2(mh[q]);
+          if (!(mf.x > 0.0f)) v[2 * q] = 0.0f;
+          if (!(mf.y > 0.0f)) v[2 * q + 1] = 0.0f;
+        }
+      }
+      if (p.dbias) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (full || n + j < p.N) dsum[j] += v[j];
+      }
+    }
+    if (p.out_mode == 0) {
+      __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(p.D) + off;
+      if (full && off % 8 == 0) {
+        int4 o;
+        __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
+        *reinterpret_cast<int4*>(d) = o;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (n + j < p.N) d[j] = __float2bfloat16_rn(v[j]);
+      }
+    } else if (p.out_mode == 1) {
+      float* d = reinterpret_cast<float*>(p.D) + off;
+      if (full && off % 4 == 0) {
+        *reinterpret_cast<float4*>(d) = make_float4(v[0], v[1], v[2], v[3]);
+        *reinterpret_cast<float4*>(d + 4) = make_float4(v[4], v[5], v[6], v[7]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (n + j < p.N) d[j] = v[j];
+      }
+    } else {
+      float* d = reinterpret_cast<float*>(p.D) + off;
+      if (full && (reinterpret_cast<uintptr_t>(d) & 15) == 0) {
+        atomicAdd(reinterpret_cast<float4*>(d), make_float4(v[0], v[1], v[2], v[3]));
+        atomicAdd(reinterpret_cast<float4*>(d + 4), make_float4(v[4], v[5], v[6], v[7]));
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (n + j < p.N) atomicAdd(d + j, v[j]);
+      }
+    }
+  }
+  if (EXT && p.dbias) dbias_flush<BN>(p, n0, t, dsum, s_dbias);
 }
 
 // Epilogue of a split-K GEMM with in-kernel fix-up (out_mode 3; fc4 forward at batch 512: 32 output tiles cannot fill the
@@ -404,11 +491,6 @@ __device__ __forceinline__ void epilogue_fixup(const GemmParams& p, int tile, in
     }
   }
 }
-
-// accumulator staging tile of the epilogue: 128 rows x (BN + 4) fp32 (the 4-float pad keeps the row-per-lane reads free of
-// bank conflicts)
-__host__ __device__ constexpr int acc_ld(int bn) { return bn + 4; }
-__host__ __device__ constexpr size_t acc_stage_bytes(int bn) { return (size_t)GEMM_BM * acc_ld(bn) * 4; }
 
 template <int BN, int STAGES, bool EXT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
@@ -497,7 +579,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: rows 64 g .. 64 g + 63
     // (K-major A: rows 64.. start 64 x 128 bytes into the stage; MN-major A: the second [64 k][64 m] box)
     const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
-    const int rl = g * 64 + (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;   // epilogue: tile row and first 32-column chunk
+    const int rl = g * 64 + (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;   // split-K fix-up: tile row and first 32-column chunk
+    const int t = wl * 32 + lane;                                          // epilogue_half's thread index in the warpgroup
     float* sAcc_g = sAcc + g * 64 * ACC_LD;
     const uint64_t a0 = make_desc(s2u(sA) + g * 8192, 8192), b0 = make_desc(s2u(sB), 8192);
     uint32_t it = 0;
@@ -523,15 +606,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
         acc_fence<BN>(d);
         if (lane == 0) mb_arrive(&empty[s]);
       }
+      int4 mk[BN / 16];
+      epi_mask_load<BN, EXT>(p, m0 + 64 * g, n0, t, mk);     // in flight during the staging (fc4 dgrad: one tile per CTA)
       stage_acc<BN>(d, sAcc_g, ACC_LD, wl, lane);
       named_sync(2 + g, 128);
       if (!EXT && p.out_mode == 3) epilogue_fixup<BN>(p, tile, m0, n0, rl, c0, cw * 32 + lane, sAcc + rl * ACC_LD, s_fix);
-      else epilogue_row<BN, EXT>(p, m0 + rl, n0, lane, sAcc + rl * ACC_LD, c0, s_dbias);
+      else epilogue_half<BN, EXT>(p, m0 + 64 * g, n0, t, sAcc_g, mk, s_dbias);
       named_sync(2 + g, 128);                        // staging tile read: the next tile may overwrite it
     }
   }
   __syncthreads();
-  if (EXT && p.dbias && p.dbias_mod > 0 && (int)threadIdx.x < p.dbias_mod) atomicAdd(p.dbias + threadIdx.x, s_dbias[threadIdx.x]);
+  if (EXT && p0.dbias && (int)threadIdx.x < dbias_slots(p0)) atomicAdd(p0.dbias + threadIdx.x, s_dbias[threadIdx.x]);
 }
 
 
@@ -815,6 +900,12 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
         for (int cb = 0; cb < CB; ++cb)
           tma_load_2d(sS + (size_t)s * slab_bytes + (size_t)cb * slab_block, mA, &full[s], cb * GEMM_BK,
                       tile * GEMM_BM + sp.min_shift);
+        if (EXT && p.mask) {
+          // the tile's ReLU-gradient mask rows into L2, as many tiles ahead as the slab ring: the epilogue's register loads
+          // of them (epi_mask_load) then wait for an L2 hit, not for HBM
+          const int r0 = tile * GEMM_BM, nr = min(GEMM_BM, p.M - r0);
+          prefetch_l2_bulk(p.mask + (int64_t)r0 * p.mask_ld, (uint32_t)(((int64_t)(nr - 1) * p.mask_ld + p.N) * 2));
+        }
       }
     }
     }
@@ -836,7 +927,7 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
     // through the warpgroup's own 64-row part of sAcc
     if constexpr (!U8) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
     const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
-    const int rl = (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;       // epilogue: row of the half, first 32-column chunk
+    const int t = wl * 32 + lane;                                   // epilogue_half's thread index in the warpgroup
     float* sAcc_g = sAcc + g * 64 * ACC_LD;
     const uint32_t w0 = s2u(sW);
     mb_wait(w_full, 0);
@@ -872,21 +963,28 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
       }
       wg_commit();
       if (tile + n_cta < tiles) named_arrive(5 + (g ^ 1), 256);      // MMA turn to the other warpgroup
+      // first half's mask: in flight while the MMAs run, the second half's during the first half's epilogue -- at BN 128
+      // each only once the registers it needs are free (128 accumulator and 32 mask registers together spill)
+      int4 mk[2][BN / 16];
+      if constexpr (BN <= 64) epi_mask_load<BN, EXT>(p, tile * GEMM_BM, 0, t, mk[0]);
       wg_wait0();
       acc_fence<BN>(d[0]);
       acc_fence<BN>(d[1]);
       if (lane == 0) mb_arrive(&empty[s]);
+      if constexpr (BN > 64) epi_mask_load<BN, EXT>(p, tile * GEMM_BM, 0, t, mk[0]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
+        if (BN > 64 && h == 1) epi_mask_load<BN, EXT>(p, tile * GEMM_BM + 64, 0, t, mk[1]);
         stage_acc<BN>(d[h], sAcc_g, ACC_LD, wl, lane);
         named_sync(2 + g, 128);
-        epilogue_row<BN, EXT>(p, tile * GEMM_BM + 64 * h + rl, 0, lane, sAcc_g + rl * ACC_LD, c0, s_dbias);
+        if (BN <= 64 && h == 0) epi_mask_load<BN, EXT>(p, tile * GEMM_BM + 64, 0, t, mk[1]);   // in flight during the first half
+        epilogue_half<BN, EXT>(p, tile * GEMM_BM + 64 * h, 0, t, sAcc_g, mk[h], s_dbias);
         named_sync(2 + g, 128);
       }
     }
   }
   __syncthreads();
-  if (EXT && p.dbias && (int)threadIdx.x < p.dbias_mod) atomicAdd(p.dbias + threadIdx.x, s_dbias[threadIdx.x]);
+  if (EXT && sp.g.dbias && (int)threadIdx.x < dbias_slots(sp.g)) atomicAdd(sp.g.dbias + threadIdx.x, s_dbias[threadIdx.x]);
 }
 
 
