@@ -70,6 +70,14 @@ SIGNATURES = {
     "b2rl_gaussian_actor_step": [c_p, c_p, c_p, c_p, c_i32, c_f64, c_f64] + [c_p] * 13 + [c_i32] * 5 + [c_p, c_u64, c_p, c_p] + [c_p] * 6 + [c_p],
     "b2rl_ppo_set_phase_clocks": [c_p],
     "b2rl_ppo_minibatch_updates": [c_p] * 5 + [c_i32] * 5 + [c_p, c_i32] + [c_p] * 10 + [c_f32] * 11 + [c_p, c_p],
+    "b2rl_ppo_minibatch_updates_dp": ([c_p] * 5 + [c_i32] * 5 + [c_p, c_i32] + [c_p] * 10 + [c_f32] * 11 + [c_p]
+                                      + [c_i32] * 5 + [c_p, c_i64, c_i64, c_p, c_i32, c_p]),
+    "b2rl_ipc_alloc": [c_i64, c_p],
+    "b2rl_ipc_get_handle": [c_p, c_p],
+    "b2rl_ipc_open_handle": [c_p, c_p],
+    "b2rl_ipc_close": [c_p],
+    "b2rl_ipc_free": [c_p],
+    "b2rl_peer_access_ok": [c_i32, c_i32, c_p],
     "b2rl_dist_softmax": [c_p, c_i32, c_i32, c_p, c_p, c_p],
     "b2rl_dist_head_bwd_prep": [c_p, c_p, c_i32, c_i32, c_i32, c_p, c_i32, c_p, c_p],
     "b2rl_grad_norm": [c_p, c_i64, c_f32, c_f32, c_p, c_p],
@@ -132,6 +140,8 @@ def lib():
         L.b2rl_launch_count.restype = ctypes.c_int64
         L.b2rl_ppo_minibatch_smem_bytes.restype = ctypes.c_int64
         L.b2rl_ppo_minibatch_smem_bytes.argtypes = [ctypes.c_int32] * 5
+        L.b2rl_ppo_dp_region_bytes.restype = ctypes.c_int64
+        L.b2rl_ppo_dp_region_bytes.argtypes = [ctypes.c_int32] * 2
         L.b2rl_reset_launch_count.restype = None
         for name, args in SIGNATURES.items():
             fn = getattr(L, name)          # AttributeError here = header / library mismatch: fail loudly

@@ -36,6 +36,18 @@ class PPOAgent(BaseAgent):
             self.lr_scheduler = torch.optim.lr_scheduler.LambdaLR(self.opt, lambda step: 1 - step / config.max_steps)
         self.gae_exact = True
         self.last_stats = None
+        # data parallel under torchrun (parallel.init(), world > 1): rank-local rollout / GAE / advantage normalisation /
+        # permutations / state normaliser; every minibatch update is one step on the union of the ranks' minibatches, with the
+        # gradients exchanged inside the persistent PPO kernel.  Parameters start as rank 0's.
+        import torch.distributed as dist
+        self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        if self.world > 1:
+            if config.shared_repr or not getattr(config, "graph_minibatch", False):
+                raise NotImplementedError("data-parallel PPO (world size %d) runs on the persistent PPO kernel only: it needs "
+                                          "config.shared_repr = False and config.graph_minibatch = True" % self.world)
+            with torch.no_grad():
+                for p in self.network.parameters():
+                    dist.broadcast(p.data, 0)
 
     def eval_step(self, state):
         with torch.no_grad():
@@ -204,6 +216,9 @@ class PPOAgent(BaseAgent):
                 and rows % config.mini_batch_size == 0 and not shared_phi and entries.action.dim() == 2):
             self._graphed_epochs(entries)                  # same updates, one CUDA-graph replay each (learner.py)
             return
+        if self.world > 1:
+            raise NotImplementedError("data-parallel PPO needs CUDA rollouts, continuous actions, no shared phi_body and "
+                                      "rollout rows divisible by mini_batch_size (the persistent PPO kernel)")
         for _ in range(config.optimization_epochs):
             for batch_indices in random_sample(np.arange(rows), config.mini_batch_size):
                 self._minibatch(entries, batch_indices)
@@ -223,9 +238,16 @@ class PPOAgent(BaseAgent):
             persistent = (getattr(config, "persistent_minibatch", True) and a.kind == "adam" and c.kind == "adam"
                           and PersistentPPOLearner.supported(self.network, mb))
             cls = PersistentPPOLearner if persistent else GraphedPPOLearner
+            kw = {}
+            if self.world > 1:
+                if not persistent:
+                    raise NotImplementedError("data-parallel PPO runs on the persistent PPO kernel: Adam for actor and critic "
+                                              "and a network PersistentPPOLearner.supported() accepts")
+                import torch.distributed as dist
+                kw = dict(world=self.world, rank=dist.get_rank())
             self._graph = cls(self.network, a, c, rows, entries.state.shape[1], entries.action.shape[1], mb,
                               config.ppo_ratio_clip, config.entropy_weight, config.target_kl,
-                              config.optimization_epochs * (rows // mb))
+                              config.optimization_epochs * (rows // mb), **kw)
             self._graph.load(entries)
             self._graph.capture()
         g = self._graph

@@ -27,6 +27,7 @@
 #define PPO_HD static inline
 #define PPO_SUB static
 #define PPO_LOOP
+#include <chrono>
 #endif
 
 namespace b2rl_ppo {
@@ -235,8 +236,11 @@ PPO_FN int wgrad_tiles(int J, int K) { return ((J + 3) / 4) * ((K + 3) / 4); }
 // tile `t` of: g[j][k] = sum_n d[n][j] * in[n][k], then Adam on element j*K + k of the tensor at arena offset `off`
 // (shared-memory copy W[j*ldw + k]; moments m / v [off + j*K + k]).  tile = rows 4tj..4tj+3 x columns 4tk..4tk+3 of the
 // weight: one 128-bit load of d and one of `in` per sample (rows 16-byte aligned; ldd = 1, the value head, takes scalars)
+// DP (data-parallel kernel): the same sums are stored to gout[off + j*K + k] (this rank's exchange slot) instead, and Adam
+// runs after the exchange (ph_dp_reduce_adam)
+template <bool DP = false>
 PPO_FN void wgrad_adam_tile(int t, const float* d, int ldd, const float* in, int ldin, float* W, int ldw, int M, int J, int K,
-                            float* m, float* v, int off, const AdamCoef& ac) {
+                            float* m, float* v, int off, const AdamCoef& ac, float* gout = nullptr) {
   const int tkn = (K + 3) / 4;
   const int tj = t / tkn, tk = t - tj * tkn;
   float acc[4][4];
@@ -262,6 +266,19 @@ PPO_FN void wgrad_adam_tile(int t, const float* d, int ldd, const float* in, int
         acc[r][2] = fmaf(dq, xv.z, acc[r][2]); acc[r][3] = fmaf(dq, xv.w, acc[r][3]);
       }
     }
+  }
+  if constexpr (DP) {
+    for (int r = 0; r < 4; ++r) {
+      const int e = off + (4 * tj + r) * K + 4 * tk;
+      if (4 * tj + r < J && (K & 3) == 0) {
+        ppo_f4 g;
+        g.x = acc[r][0]; g.y = acc[r][1]; g.z = acc[r][2]; g.w = acc[r][3]; ppo_st4(gout + e, g);
+      } else if (4 * tj + r < J) {
+        for (int c = 0; c < 4; ++c)
+          if (4 * tk + c < K) gout[e + c] = acc[r][c];
+      }
+    }
+    return;
   }
   // Adam.  The master copy `flat` is written once, when the kernel ends (ph_finish); the moments live in L2.  All moment
   // loads are issued before the arithmetic (independent round trips); rows of a weight whose K is a multiple of 4 are read
@@ -311,8 +328,10 @@ PPO_FN void wgrad_adam_tile(int t, const float* d, int ldd, const float* in, int
   }
 }
 
-// element j of: g[j] = sum_n d[n][j], then Adam (bias vectors, the std parameter)
-PPO_FN void bias_adam_elem(int j, const float* d, int ldd, float* Bv, int M, float* m, float* v, int off, const AdamCoef& ac) {
+// element j of: g[j] = sum_n d[n][j], then Adam (bias vectors, the std parameter); DP: g stored to gout[off + j] instead
+template <bool DP = false>
+PPO_FN void bias_adam_elem(int j, const float* d, int ldd, float* Bv, int M, float* m, float* v, int off, const AdamCoef& ac,
+                           float* gout = nullptr) {
   float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
   int n = 0;
   for (; n + 3 < M; n += 4) {
@@ -320,16 +339,18 @@ PPO_FN void bias_adam_elem(int j, const float* d, int ldd, float* Bv, int M, flo
     s2 += d[(size_t)(n + 2) * ldd + j]; s3 += d[(size_t)(n + 3) * ldd + j];
   }
   for (; n < M; ++n) s0 += d[(size_t)n * ldd + j];
-  Bv[j] = adam_elem(Bv[j], (s0 + s1) + (s2 + s3), m, v, off + j, ac);
+  if constexpr (DP) gout[off + j] = (s0 + s1) + (s2 + s3);
+  else Bv[j] = adam_elem(Bv[j], (s0 + s1) + (s2 + s3), m, v, off + j, ac);
 }
 
 // all parameter gradients + Adam of one three-layer network, spread over the block as ONE index space:
 //   [W2 tiles | W1 tiles | W3 tiles | b1 | b2 | b3 | extra (std)]
-// d1 / d2 / d3: pre-activation gradients of the three layers; x / h1 / h2: their inputs
+// d1 / d2 / d3: pre-activation gradients of the three layers; x / h1 / h2: their inputs.  DP: gradients only, into gout
+template <bool DP = false>
 PPO_FN void net_wgrad_adam(const float* x, int ldx, const float* h1, const float* h2, int ldh, const float* d1, const float* d2,
                            const float* d3, int ld3, int M, int D, int H1, int H2, int O, float* w1, int ld1, float* b1,
                            float* w2, float* b2, float* w3, float* b3, float* extra, const float* dextra, float* m, float* v,
-                           const int* off, const AdamCoef& ac, int tid, int NT) {
+                           const int* off, const AdamCoef& ac, int tid, int NT, float* gout = nullptr) {
   const int t2 = wgrad_tiles(H2, H1), t1 = wgrad_tiles(H1, D), t3 = wgrad_tiles(O, H2);
   const int nt = t2 + t1 + t3, nb = H1 + H2 + O + (extra ? O : 0);
   PPO_LOOP
@@ -341,7 +362,7 @@ PPO_FN void net_wgrad_adam(const float* x, int ldx, const float* h1, const float
       if (u < t2) { d = d2; ldd = ldh; in = h1; ldin = ldh; W = w2; ldw = ldh; J = H2; K = H1; o = off[2]; }
       else if (u < t2 + t1) { u -= t2; d = d1; ldd = ldh; in = x; ldin = ldx; W = w1; ldw = ld1; J = H1; K = D; o = off[0]; }
       else { u -= t2 + t1; d = d3; ldd = ld3; in = h2; ldin = ldh; W = w3; ldw = ldh; J = O; K = H2; o = off[4]; }
-      wgrad_adam_tile(u, d, ldd, in, ldin, W, ldw, M, J, K, m, v, o, ac);
+      wgrad_adam_tile<DP>(u, d, ldd, in, ldin, W, ldw, M, J, K, m, v, o, ac, gout);
     } else {                                               // an element of a bias vector / the std parameter
       const float* d;
       float* Bv;
@@ -350,7 +371,7 @@ PPO_FN void net_wgrad_adam(const float* x, int ldx, const float* h1, const float
       else if (u < H1 + H2) { u -= H1; d = d2; ldd = ldh; Bv = b2; o = off[3]; }
       else if (u < H1 + H2 + O) { u -= H1 + H2; d = d3; ldd = ld3; Bv = b3; o = off[5]; }
       else { u -= H1 + H2 + O; d = dextra; ldd = ld3; Bv = extra; o = off[6]; }
-      bias_adam_elem(u, d, ldd, Bv, M, m, v, o, ac);
+      bias_adam_elem<DP>(u, d, ldd, Bv, M, m, v, o, ac, gout);
     }
   }
 }
@@ -488,7 +509,10 @@ PPO_FN void ph4_loss(PpoShared& S, const PpoArgs& a, int b, int tid, int NT) {
   }
 }
 // P5: actor: the reference's `if approx_kl <= 1.5 * target_kl` (PPO_agent.py:94), decided once for the block;
-//     critic: back into layer 1
+//     critic: back into layer 1.
+//     DP: the gate is decided on the MEAN kl over ranks, after the exchange (ph_dp_wait); here this rank's kl and policy loss
+//     are only recorded and the actor backward is switched on unconditionally (its gradient goes into the exchange slot)
+template <bool DP = false>
 PPO_FN void ph5_gate(PpoShared& S, const PpoArgs& a, int b, int tid, int NT) {
   const int h = NT / 2;
   if (tid >= h) {
@@ -500,6 +524,12 @@ PPO_FN void ph5_gate(PpoShared& S, const PpoArgs& a, int b, int tid, int NT) {
   const float kl = sum_strided4(S.red + a.mb, a.mb) * invM;
   float ent = 0.0f;
   for (int j = 0; j < a.A; ++j) ent += 0.5f + 0.91893853320467274178f + S.lsd[j];    // Normal.entropy, summed over actions
+  if constexpr (DP) {
+    S.flag[0] = 1.0f;
+    S.flag[2] = -(sum_strided4(S.red, a.mb) * invM) - a.ent_w * ent;
+    S.flag[3] = kl;
+    return;
+  }
   const bool gate = kl <= a.gate_max;
   S.flag[0] = gate ? 1.0f : 0.0f;
   S.flag[2] = -(sum_strided4(S.red, a.mb) * invM) - a.ent_w * ent;
@@ -529,15 +559,17 @@ PPO_FN void ph6_head_bwd(PpoShared& S, const PpoArgs& a, int b, int tid, int NT)
   }
 }
 // P7: actor (gate): back into layer 2; critic: all its parameter gradients + Adam (PPO_agent.py:97-99)
-PPO_FN void ph7_critic_update(PpoShared& S, const PpoArgs& a, int b, int tid, int NT) {
+//     (DP: the critic's gradients into its part of the exchange slot, `gout`)
+template <bool DP = false>
+PPO_FN void ph7_critic_update(PpoShared& S, const PpoArgs& a, int b, int tid, int NT, float* gout = nullptr) {
   const int h = NT / 2;
   if (tid < h) {
     if (S.flag[0] != 0.0f) dense_bwd_data(S.dmu, S.lda, S.aw3, S.ldh, S.ah2, S.ldh, S.ad2, S.ldh, a.mb, a.A, a.H2, tid, h);
     return;
   }
-  const AdamCoef ac = adam_coef(a.c_lr, a.c_b1, a.c_b2, a.c_eps, S.steps[1]);
-  net_wgrad_adam((S.xb + (b & 1) * S.x_stride), S.ld1, S.ch1, S.ch2, S.ldh, S.cd1, S.cd2, S.dv, 1, a.mb, a.D, a.H1, a.H2, 1, S.cw1, S.ld1, S.cb1,
-                 S.cw2, S.cb2, S.cw3, S.cb3, nullptr, nullptr, a.c_m, a.c_v, a.c_off, ac, tid - h, h);
+  const AdamCoef ac = DP ? AdamCoef{} : adam_coef(a.c_lr, a.c_b1, a.c_b2, a.c_eps, S.steps[1]);
+  net_wgrad_adam<DP>((S.xb + (b & 1) * S.x_stride), S.ld1, S.ch1, S.ch2, S.ldh, S.cd1, S.cd2, S.dv, 1, a.mb, a.D, a.H1, a.H2, 1, S.cw1, S.ld1, S.cb1,
+                     S.cw2, S.cb2, S.cw3, S.cb3, nullptr, nullptr, a.c_m, a.c_v, a.c_off, ac, tid - h, h, gout);
 }
 // P8: actor (gate): back into layer 1
 PPO_FN void ph8_actor_bwd1(PpoShared& S, const PpoArgs& a, int b, int tid, int NT) {
@@ -545,11 +577,20 @@ PPO_FN void ph8_actor_bwd1(PpoShared& S, const PpoArgs& a, int b, int tid, int N
   dense_bwd_data(S.ad2, S.ldh, S.aw2, S.ldh, S.ah1, S.ldh, S.ad1, S.ldh, a.mb, a.H2, a.H1, tid, NT);
 }
 // P9: actor (gate): all its parameter gradients + Adam (PPO_agent.py:94-96), the whole block
-PPO_FN void ph9_actor_update(PpoShared& S, const PpoArgs& a, int b, int tid, int NT) {
+//     (DP: the actor's gradients into the start of the exchange slot `gout`, and this rank's loss / kl values after them)
+template <bool DP = false>
+PPO_FN void ph9_actor_update(PpoShared& S, const PpoArgs& a, int b, int tid, int NT, float* gout = nullptr, int stat_at = 0) {
   if (S.flag[0] == 0.0f) return;
-  const AdamCoef ac = adam_coef(a.a_lr, a.a_b1, a.a_b2, a.a_eps, S.steps[0]);
-  net_wgrad_adam((S.xb + (b & 1) * S.x_stride), S.ld1, S.ah1, S.ah2, S.ldh, S.ad1, S.ad2, S.dmu, S.lda, a.mb, a.D, a.H1, a.H2, a.A, S.aw1, S.ld1,
-                 S.ab1, S.aw2, S.ab2, S.aw3, S.ab3, S.sdp, S.dsd, a.a_m, a.a_v, a.a_off, ac, tid, NT);
+  const AdamCoef ac = DP ? AdamCoef{} : adam_coef(a.a_lr, a.a_b1, a.a_b2, a.a_eps, S.steps[0]);
+  net_wgrad_adam<DP>((S.xb + (b & 1) * S.x_stride), S.ld1, S.ah1, S.ah2, S.ldh, S.ad1, S.ad2, S.dmu, S.lda, a.mb, a.D, a.H1, a.H2, a.A, S.aw1, S.ld1,
+                     S.ab1, S.aw2, S.ab2, S.aw3, S.ab3, S.sdp, S.dsd, a.a_m, a.a_v, a.a_off, ac, tid, NT, gout);
+  if constexpr (DP) {
+    if (tid == NT - 1) {
+      gout[stat_at + 0] = S.flag[2];
+      gout[stat_at + 1] = S.flag[3];
+      gout[stat_at + 2] = S.flag[4];
+    }
+  }
 }
 
 PPO_FN void copy_rows_out(float* dst, const float* src, int ld, int rows, int cols, int tid, int NT) {
@@ -581,6 +622,187 @@ PPO_FN void ph_finish(PpoShared& S, const PpoArgs& a, int tid, int NT) {
   a.stats[1] = S.flag[4];
   a.stats[2] = S.flag[3];
   a.stats[3] = S.flag[1];
+}
+
+// ------------------------------------------------------------------------------------------------ data parallel (ppo_dp_sequence.inc)
+// W ranks, each with its own rollout rows and minibatch permutation; update b of every rank is ONE step of PPO_agent.py:68-99
+// on the union of the ranks' b-th minibatches.  Every loss term is a mean over rows, so the union's gradients / losses / kl are
+// the means over ranks of the per-rank values: each rank publishes its gradients and loss values in an exchange slot, waits for
+// every peer's, sums them over ranks 0..W-1 in that order, scales by 1/W (exact for W = 1) and applies the same Adam
+// arithmetic -- parameters, moments and step counts stay bit-identical on every rank.
+//
+// Exchange region of one rank (allocated by that rank, mapped into every peer):
+//   int64 flag[8] (128-byte header) | slot 0 | slot 1          slot = [actor gradients | critic gradients | policy loss, kl, value loss]
+// flag[p] of rank r's region = the last update rank p has published (written by rank p: flags are pushed, each rank polls
+// only its own region).  Update b of a launch has the global sequence number seq = seq_base + b + 1 (monotonic across launches,
+// never reset) and uses slot seq & 1.
+constexpr int PPO_DP_MAX_WORLD = 8;
+constexpr int PPO_DP_HEADER_FLOATS = 32;
+
+struct PpoDp {
+  float* region[PPO_DP_MAX_WORLD];   // exchange region of rank p, as seen from this rank
+  int world, rank;
+  int slot_floats, c_base, stat_at;  // floats per slot; slot offsets of the critic gradients and of the three loss values
+  long long seq_base;                // updates exchanged before this launch
+  long long timeout_ns;              // bound on the wait for one update's peers (%globaltimer)
+  long long* status;                 // 0, or after a timeout 1 + peer + 16 * update (update index within the launch)
+};
+
+PPO_HD int ppo_dp_slot_floats(int a_n, int c_n, int* c_base, int* stat_at) {
+  const int cb = (a_n + 3) / 4 * 4, sa = cb + (c_n + 3) / 4 * 4;
+  if (c_base) *c_base = cb;
+  if (stat_at) *stat_at = sa;
+  return sa + 4;
+}
+PPO_HD long long* dp_flags(float* region) { return reinterpret_cast<long long*>(region); }
+PPO_HD float* dp_slot(float* region, long long seq, int slot_floats) {
+  return region + PPO_DP_HEADER_FLOATS + (int)(seq & 1) * slot_floats;
+}
+
+#ifdef __CUDACC__
+PPO_FN void ppo_fence_sys() { asm volatile("fence.acq_rel.sys;" ::: "memory"); }
+PPO_FN void ppo_st_release_sys(long long* p, long long v) {
+  asm volatile("st.release.sys.global.b64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+PPO_FN long long ppo_ld_acquire_sys(const long long* p) {
+  long long v;
+  asm volatile("ld.acquire.sys.global.b64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+PPO_FN float ppo_ld_peer(const float* p) { return __ldcg(p); }      // L2 / NVLink, never a (possibly stale) L1 line
+PPO_FN unsigned long long ppo_now_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+PPO_FN void ppo_backoff(unsigned ns) { __nanosleep(ns); }
+#else
+PPO_FN void ppo_fence_sys() { __atomic_thread_fence(__ATOMIC_ACQ_REL); }
+PPO_FN void ppo_st_release_sys(long long* p, long long v) { __atomic_store_n(p, v, __ATOMIC_RELEASE); }
+PPO_FN long long ppo_ld_acquire_sys(const long long* p) { return __atomic_load_n(p, __ATOMIC_ACQUIRE); }
+PPO_FN float ppo_ld_peer(const float* p) { return *p; }
+PPO_FN unsigned long long ppo_now_ns() {
+  return (unsigned long long)std::chrono::duration_cast<std::chrono::nanoseconds>(
+      std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+PPO_FN void ppo_backoff(unsigned) {}
+#endif
+
+// Publish update b: this rank's slot was written in P7 / P9 and the block barrier after P9 orders those writes before this
+// phase; thread 0 makes them visible at system scope and pushes seq into flag[rank] of every rank's region (release).
+PPO_FN void ph_dp_publish(const PpoDp& d, int b, int tid) {
+  if (tid != 0) return;
+  const long long seq = d.seq_base + b + 1;
+  ppo_fence_sys();
+  for (int p = 0; p < d.world; ++p) ppo_st_release_sys(dp_flags(d.region[p]) + d.rank, seq);
+}
+
+// Wait for update b of every peer (thread 0, acquire loads of this rank's own flags, bounded by d.timeout_ns), then decide
+// the KL gate on the MEAN kl over ranks (PPO_agent.py:94 on the union minibatch) and keep the mean losses as the statistics.
+// On a timeout: status word, S.flag[6] = 1, and the sequence skips the remaining updates.
+//
+// Slot reuse: update b writes slot seq & 1, which update seq - 2 used.  This rank got here for seq - 1 only after it saw every
+// peer's flag for seq - 1, and a peer publishes seq - 1 only after its reduce of seq - 2 (the last read of that slot) has
+// finished: nobody still reads the slot this rank overwrites.  The barrier after this phase orders every thread's slot reads
+// (ld.global.cg, which bypasses L1: a slot is reused, so an L1 line could be stale) after the acquire.
+PPO_FN void ph_dp_wait(PpoShared& S, const PpoArgs& a, const PpoDp& d, int b, int tid) {
+  if (tid != 0) return;
+  const long long seq = d.seq_base + b + 1;
+  const long long* fl = dp_flags(d.region[d.rank]);
+  const unsigned long long t0 = ppo_now_ns();
+  for (int p = 0; p < d.world; ++p) {
+    unsigned ns = 32;
+    while (ppo_ld_acquire_sys(fl + p) < seq) {
+      if ((long long)(ppo_now_ns() - t0) > d.timeout_ns) {
+        *d.status = 1 + p + 16LL * b;
+        S.flag[6] = 1.0f;
+        return;
+      }
+      ppo_backoff(ns);
+      if (ns < 1024) ns *= 2;
+    }
+  }
+  float v[3];
+  for (int i = 0; i < 3; ++i) {
+    v[i] = ppo_ld_peer(dp_slot(d.region[0], seq, d.slot_floats) + d.stat_at + i);
+    for (int p = 1; p < d.world; ++p) v[i] += ppo_ld_peer(dp_slot(d.region[p], seq, d.slot_floats) + d.stat_at + i);
+    v[i] *= 1.0f / (float)d.world;
+  }
+  const bool gate = v[1] <= a.gate_max;
+  S.flag[0] = gate ? 1.0f : 0.0f;
+  S.flag[2] = v[0];
+  S.flag[3] = v[1];
+  S.flag[4] = v[2];
+  if (gate) {
+    S.steps[0] += 1;
+    S.flag[1] += 1.0f;
+  }
+}
+
+// element e of the index space [critic tensors | actor tensors] (no arena padding): its shared-memory copy and arena offset
+PPO_FN float* dp_param(PpoShared& S, const PpoArgs& a, int e, int nc, bool& actor, int& off) {
+  actor = e >= nc;
+  int u = actor ? e - nc : e;
+#define PPO_DP_T(ptr, rows, cols, ld, o)                       \
+  if (u < (rows) * (cols)) {                                   \
+    const int j = u / (cols);                                  \
+    off = (o) + u;                                             \
+    return (ptr) + j * (ld) + (u - j * (cols));                \
+  }                                                            \
+  u -= (rows) * (cols);
+  if (!actor) {
+    PPO_DP_T(S.cw1, a.H1, a.D, S.ld1, a.c_off[0]) PPO_DP_T(S.cb1, 1, a.H1, 0, a.c_off[1])
+    PPO_DP_T(S.cw2, a.H2, a.H1, S.ldh, a.c_off[2]) PPO_DP_T(S.cb2, 1, a.H2, 0, a.c_off[3])
+    PPO_DP_T(S.cw3, 1, a.H2, 0, a.c_off[4])
+    off = a.c_off[5];
+    return S.cb3;
+  }
+  PPO_DP_T(S.aw1, a.H1, a.D, S.ld1, a.a_off[0]) PPO_DP_T(S.ab1, 1, a.H1, 0, a.a_off[1])
+  PPO_DP_T(S.aw2, a.H2, a.H1, S.ldh, a.a_off[2]) PPO_DP_T(S.ab2, 1, a.H2, 0, a.a_off[3])
+  PPO_DP_T(S.aw3, a.A, a.H2, S.ldh, a.a_off[4]) PPO_DP_T(S.ab3, 1, a.A, 0, a.a_off[5])
+  off = a.a_off[6] + u;
+  return S.sdp + u;
+#undef PPO_DP_T
+}
+
+// Reduce + Adam: every element's gradient summed over ranks 0..W-1 in order, times 1/W, then adam_elem (the arithmetic of
+// wgrad_adam_tile / bias_adam_elem).  Critic always (PPO_agent.py:97-99); actor iff the mean-kl gate is open (:94-96).
+PPO_FN void ph_dp_reduce_adam(PpoShared& S, const PpoArgs& a, const PpoDp& d, int b, int tid, int NT) {
+  const long long seq = d.seq_base + b + 1;
+  const int nc = a.H1 * a.D + a.H1 + a.H2 * a.H1 + a.H2 + a.H2 + 1;
+  const int na = a.H1 * a.D + a.H1 + a.H2 * a.H1 + a.H2 + a.A * a.H2 + 2 * a.A;
+  const int n = nc + (S.flag[0] != 0.0f ? na : 0);
+  const float invW = 1.0f / (float)d.world;
+  const AdamCoef cc = adam_coef(a.c_lr, a.c_b1, a.c_b2, a.c_eps, S.steps[1]);
+  const AdamCoef ca = adam_coef(a.a_lr, a.a_b1, a.a_b2, a.a_eps, S.steps[0]);
+  PPO_LOOP
+  for (int e0 = tid; e0 < n; e0 += 4 * NT) {                // four elements per thread in flight: 4 loads per peer round trip
+    float* w[4];
+    int so[4], off[4];
+    bool act[4];
+    float g[4];
+    for (int q = 0; q < 4; ++q) {
+      const int e = e0 + q * NT;
+      so[q] = -1;
+      if (e < n) {
+        w[q] = dp_param(S, a, e, nc, act[q], off[q]);
+        so[q] = (act[q] ? 0 : d.c_base) + off[q];
+      }
+    }
+    const float* s0 = dp_slot(d.region[0], seq, d.slot_floats);
+    for (int q = 0; q < 4; ++q) g[q] = so[q] >= 0 ? ppo_ld_peer(s0 + so[q]) : 0.0f;
+    PPO_LOOP
+    for (int p = 1; p < d.world; ++p) {
+      const float* sp = dp_slot(d.region[p], seq, d.slot_floats);
+      for (int q = 0; q < 4; ++q)
+        if (so[q] >= 0) g[q] += ppo_ld_peer(sp + so[q]);
+    }
+    for (int q = 0; q < 4; ++q) {
+      if (so[q] < 0) continue;
+      *w[q] = act[q] ? adam_elem(*w[q], g[q] * invW, a.a_m, a.a_v, off[q], ca)
+                     : adam_elem(*w[q], g[q] * invW, a.c_m, a.c_v, off[q], cc);
+    }
+  }
 }
 
 }  // namespace b2rl_ppo

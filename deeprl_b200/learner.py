@@ -617,9 +617,10 @@ class PersistentPPOLearner:
         return int(_lib.lib().b2rl_ppo_minibatch_smem_bytes(D, A, H1, H2, int(mini_batch_size))) <= 227 * 1024
 
     def __init__(self, network, actor_opt, critic_opt, rows, state_dim, action_dim, mini_batch_size, ppo_ratio_clip,
-                 entropy_weight, target_kl, max_batches):
+                 entropy_weight, target_kl, max_batches, world=1, rank=0, exchange_timeout_s=5.0):
         self.net, self.actor_opt, self.critic_opt = network, actor_opt, critic_opt
         self.mb, self.clip, self.ent_w, self.target_kl = int(mini_batch_size), ppo_ratio_clip, entropy_weight, target_kl
+        self.world, self.rank, self.rows = int(world), int(rank), int(rows)
         if actor_opt.kind != "adam" or critic_opt.kind != "adam":
             raise NotImplementedError("the persistent PPO kernel implements Adam (examples.py:508-509)")
         dev = actor_opt.flat.device
@@ -637,6 +638,22 @@ class PersistentPPOLearner:
         self.A = network.fc_action.out_features
         self.launches_per_update = 0.0
         self.n = 0
+        if self.world > 1:
+            # data parallel (one process per GPU): every update exchanges the ranks' gradients inside the kernel, through
+            # exchange regions mapped into every peer (parallel.ExchangeRegions); seq = updates exchanged so far
+            a_n, c_n = actor_opt.flat.numel(), critic_opt.flat.numel()
+            self.exchange = parallel.ExchangeRegions(int(_lib.lib().b2rl_ppo_dp_region_bytes(a_n, c_n)), dev)
+            self.status = torch.zeros(1, dtype=torch.int64, device=dev)
+            self.seq = 0
+            self.timeout_ns = int(exchange_timeout_s * 1e9)
+
+    def check_exchange(self):
+        """Raise if a data-parallel launch gave up waiting for a peer (synchronises with the device)."""
+        if self.world > 1:
+            code = int(self.status[0])
+            if code:
+                peer, k = (code - 1) % 16, (code - 1) // 16
+                raise _lib.B2RLError("PPO data-parallel exchange: rank %d did not publish update %d" % (peer, self.seq_last + k))
 
     @staticmethod
     def _offsets(opt, params):
@@ -665,6 +682,21 @@ class PersistentPPOLearner:
 
     def run(self, n_batches):
         a, c, b = self.actor_opt, self.critic_opt, self.buf
+        if self.world > 1:
+            self.check_exchange()                      # (the previous iteration's launch)
+            n_batches = parallel.agree(n_batches, self.dev, "PPO minibatches per iteration")
+            _lib.call("b2rl_ppo_minibatch_updates_dp", _lib.ptr(b["state"]), _lib.ptr(b["action"]), _lib.ptr(b["log_pi_a"]),
+                      _lib.ptr(b["ret"]), _lib.ptr(b["advantage"]), self.D, self.A, self.H1, self.H2, self.mb,
+                      _lib.ptr(self.perm), int(n_batches), _lib.ptr(a.flat), _lib.ptr(a.s1), _lib.ptr(a.s2),
+                      _lib.ptr(a.step_dev), _lib.ptr(self.a_off), _lib.ptr(c.flat), _lib.ptr(c.s1), _lib.ptr(c.s2),
+                      _lib.ptr(c.step_dev), _lib.ptr(self.c_off), float(a.lr), float(a.betas[0]), float(a.betas[1]), float(a.eps),
+                      float(c.lr), float(c.betas[0]), float(c.betas[1]), float(c.eps), float(self.clip), float(self.ent_w),
+                      float(1.5 * self.target_kl), _lib.ptr(self.stats), self.rows, a.flat.numel(), c.flat.numel(), self.world,
+                      self.rank, self.exchange.table, self.seq, self.timeout_ns, _lib.ptr(self.status), 1, _lib.stream())
+            self.seq_last = self.seq
+            self.seq += int(n_batches)
+            self.n = int(n_batches)
+            return
         _lib.call("b2rl_ppo_minibatch_updates", _lib.ptr(b["state"]), _lib.ptr(b["action"]), _lib.ptr(b["log_pi_a"]),
                   _lib.ptr(b["ret"]), _lib.ptr(b["advantage"]), self.D, self.A, self.H1, self.H2, self.mb, _lib.ptr(self.perm),
                   int(n_batches), _lib.ptr(a.flat), _lib.ptr(a.s1), _lib.ptr(a.s2), _lib.ptr(a.step_dev), _lib.ptr(self.a_off),

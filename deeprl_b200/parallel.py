@@ -68,6 +68,61 @@ def max_over_ranks(value, device):
     return float(t)
 
 
+def agree(value, device, what):
+    """The same integer on every rank, or a B2RLError naming the disagreement (one all-reduce of [v, -v] with MAX)."""
+    t = torch.tensor([int(value), -int(value)], dtype=torch.int64, device=device)
+    if dist.is_initialized() and dist.get_world_size() > 1:
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    hi, lo = int(t[0]), -int(t[1])
+    if hi != lo:
+        from ._lib import B2RLError
+        raise B2RLError("%s differs between ranks (%d .. %d)" % (what, lo, hi))
+    return hi
+
+
+class ExchangeRegions:
+    """The device memory the data-parallel PPO kernel exchanges gradients through (csrc/ppo_phases.h, "data parallel"): this
+    rank's region (cudaMalloc'd and zero-filled once) and every peer's, mapped into this process with CUDA IPC.
+    ``table`` holds the device addresses in rank order (``table[rank]`` is this rank's own region)."""
+
+    def __init__(self, nbytes, device):
+        import ctypes
+        from . import _lib
+        world, rank = dist.get_world_size(), dist.get_rank()
+        dev = torch.device(device).index
+        self.own = ctypes.c_void_p()
+        _lib.call("b2rl_ipc_alloc", int(nbytes), ctypes.addressof(self.own))
+        handle = ctypes.create_string_buffer(64)
+        _lib.call("b2rl_ipc_get_handle", self.own, handle)
+        infos = [None] * world
+        dist.all_gather_object(infos, (dev, bytes(handle.raw)))
+        self.opened, table = [], []
+        for p, (pdev, raw) in enumerate(infos):
+            if p == rank:
+                table.append(self.own.value)
+                continue
+            ok = ctypes.c_int32(0)
+            _lib.call("b2rl_peer_access_ok", dev, pdev, ctypes.addressof(ok))
+            if not ok.value:
+                raise _lib.B2RLError("PPO data-parallel exchange: device %d (rank %d) has no peer access to device %d (rank %d)"
+                                     % (dev, rank, pdev, p))
+            ptr = ctypes.c_void_p()
+            _lib.call("b2rl_ipc_open_handle", ctypes.create_string_buffer(raw, 64), ctypes.addressof(ptr))
+            self.opened.append(ptr)
+            table.append(ptr.value)
+        self.table = (ctypes.c_void_p * world)(*table)
+        dist.barrier()                 # every peer has mapped every region before any rank publishes into one
+
+    def close(self):
+        from . import _lib
+        for ptr in self.opened:
+            _lib.call("b2rl_ipc_close", ptr)
+        self.opened = []
+        if self.own:
+            _lib.call("b2rl_ipc_free", self.own)
+            self.own = None
+
+
 def rank_seed(base_seed):
     """Rank-local RNG stream for the replay shard / envs."""
     _, rank, _ = env_world()

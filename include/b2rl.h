@@ -393,7 +393,8 @@ int b2rl_gaussian_actor_step(const float* obs, double* rm_mean, double* rm_var, 
  * for critic_body.* and fc_critic.*.  stats float32 [4] = policy loss, value loss, approx_kl of the LAST minibatch and the
  * number of actor steps taken.  Limits: D <= 256, A <= 32, hidden <= 128, mini batch <= 128 and a multiple of 4. */
 /* Profiling hook of b2rl_ppo_minibatch_updates: install (NULL: remove) a device buffer int64 [2 + 9 * n_batches] that the next
- * launches fill with clock64() of thread 0 after every phase barrier (scripts/ppo_phase_clocks.py). */
+ * launches fill with clock64() of thread 0 after every phase barrier (scripts/ppo_phase_clocks.py).  The data-parallel form
+ * fills [2 + 12 * n_batches] (rank 0 of the launch; scripts/ppo_dp_scaling.py). */
 int b2rl_ppo_set_phase_clocks(int64_t* clocks);
 
 /* Dynamic shared memory (bytes) b2rl_ppo_minibatch_updates needs for these sizes; it must fit the 227 KB of one SM. */
@@ -406,6 +407,39 @@ int b2rl_ppo_minibatch_updates(const float* state, const float* action, const fl
                                int64_t* c_step, const int32_t* c_off, float a_lr, float a_beta1, float a_beta2, float a_eps,
                                float c_lr, float c_beta1, float c_beta2, float c_eps, float ratio_clip, float entropy_weight,
                                float kl_gate, float* stats, void* stream);
+
+/* Data-parallel form of b2rl_ppo_minibatch_updates: `world` ranks, each with its own rollout rows, advantage normalisation and
+ * minibatch permutation; update k of every rank is ONE step on the union of the ranks' k-th minibatches.  Each rank writes
+ * its gradients and loss values into its exchange region, pushes the update's sequence number into every peer's flags, waits
+ * for every peer, sums the gradients over ranks 0..world-1 in order, scales them by 1/world and applies Adam (critic always,
+ * actor iff the MEAN approx_kl over ranks <= kl_gate): parameters, moments and step counts stay bit-identical on every rank.
+ * regions: host array [world] of device pointers to every rank's exchange region of b2rl_ppo_dp_region_bytes(a_n, c_n) bytes,
+ * zero-filled once (regions[rank] is this rank's own).  a_n / c_n: arena lengths (elements).  seq_base: updates exchanged
+ * before this launch (monotonic across launches; the flags are never reset).  timeout_ns: bound on the wait for one update's
+ * peers; on expiry status (int64, device) gets 1 + peer + 16 * update and the launch skips its remaining updates.
+ * ranks_in_launch: 1 = one process per GPU (regions mapped by b2rl_ipc_open_handle); world = all ranks as the blocks of ONE
+ * cooperative launch on one device (pass rank 0): every per-rank array then holds world consecutive copies (rows rows each
+ * for the rollout arrays, n_batches x mb for perm, a_n / c_n for the arenas, 1 per step count and status word, 4 per stats). */
+int64_t b2rl_ppo_dp_region_bytes(int32_t a_n, int32_t c_n);
+int b2rl_ppo_minibatch_updates_dp(const float* state, const float* action, const float* old_log_pi_a, const float* ret,
+                                  const float* advantage, int32_t D, int32_t A, int32_t H1, int32_t H2, int32_t mb,
+                                  const int64_t* perm, int32_t n_batches, float* a_flat, float* a_exp_avg, float* a_exp_avg_sq,
+                                  int64_t* a_step, const int32_t* a_off, float* c_flat, float* c_exp_avg, float* c_exp_avg_sq,
+                                  int64_t* c_step, const int32_t* c_off, float a_lr, float a_beta1, float a_beta2, float a_eps,
+                                  float c_lr, float c_beta1, float c_beta2, float c_eps, float ratio_clip, float entropy_weight,
+                                  float kl_gate, float* stats, int32_t rows, int32_t a_n, int32_t c_n, int32_t world,
+                                  int32_t rank, void* const* regions, int64_t seq_base, int64_t timeout_ns, int64_t* status,
+                                  int32_t ranks_in_launch, void* stream);
+
+/* Device memory shared between processes (CUDA IPC; setup only, never on the update path): allocate + zero-fill, export a
+ * 64-byte handle, map a peer's handle (peer access enabled lazily), unmap, free; peer_access_ok: *ok = 1 when device dev_a can
+ * address device dev_b's memory (or dev_a == dev_b). */
+int b2rl_ipc_alloc(int64_t bytes, void** out);
+int b2rl_ipc_get_handle(void* ptr, void* handle_out);
+int b2rl_ipc_open_handle(const void* handle, void** out);
+int b2rl_ipc_close(void* ptr);
+int b2rl_ipc_free(void* ptr);
+int b2rl_peer_access_ok(int32_t dev_a, int32_t dev_b, int32_t* ok);
 
 /* Element-wise halves of the distributional heads (CategoricalNet / QuantileNet, network_heads.py:40-55, 89-102) around the
  * wgmma GEMMs: softmax + log_softmax over the N atoms of every (b, a) row (either output may be NULL), and the backward
