@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libb2rl.so")
-SOURCES = ["core.cu", "replay.cu", "sumtree.cu", "losses.cu", "onpolicy.cu", "optim.cu", "dense.cu", "gemm.cu", "pack.cu", "head.cu", "tail.cu", "disthead.cu", "actor.cu", "ppo_persistent.cu"]
+SOURCES = ["core.cu", "replay.cu", "sumtree.cu", "losses.cu", "onpolicy.cu", "optim.cu", "dense.cu", "gemm.cu", "pack.cu", "head.cu", "tail.cu", "disthead.cu", "actor.cu", "ppo_persistent.cu", "a2c.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
@@ -72,6 +72,10 @@ SIGNATURES = {
     "b2rl_ppo_minibatch_updates": [c_p] * 5 + [c_i32] * 5 + [c_p, c_i32] + [c_p] * 10 + [c_f32] * 11 + [c_p, c_p],
     "b2rl_ppo_minibatch_updates_dp": ([c_p] * 5 + [c_i32] * 5 + [c_p, c_i32] + [c_p] * 10 + [c_f32] * 11 + [c_p]
                                       + [c_i32] * 5 + [c_p, c_i64, c_i64, c_p, c_i32, c_p]),
+    "b2rl_a2c_smem_bytes": [c_i32] * 8,
+    "b2rl_a2c_actor_step": [c_i32, c_i32, c_i32, c_p, c_f64, c_p, c_p] + [c_i32] * 5 + [c_p, c_p, c_p, c_u64, c_p, c_p],
+    "b2rl_a2c_update": [c_i32, c_i32, c_i32] + [c_p] * 4 + [c_i32] * 6 + [c_p] * 5 + [c_f32] * 3 + [c_i32] + [c_f32] * 2
+                       + [c_i32] + [c_f32] * 3 + [c_p, c_p],
     "b2rl_ipc_alloc": [c_i64, c_p],
     "b2rl_ipc_get_handle": [c_p, c_p],
     "b2rl_ipc_open_handle": [c_p, c_p],
@@ -147,6 +151,7 @@ def lib():
             fn = getattr(L, name)          # AttributeError here = header / library mismatch: fail loudly
             fn.argtypes = args
             fn.restype = ctypes.c_int
+        L.b2rl_a2c_smem_bytes.restype = ctypes.c_int64       # (a size, not a status)
         _lib = L
     return _lib
 

@@ -5,6 +5,11 @@ stores tensors with grad, A2C_agent.py:31) and does ONE backward.  On a CUDA dev
 objective (+ its gradient with respect to log-prob / entropy / value) are the kernels of ``csrc/onpolicy.cu``; on
 ``select_device(-1)`` -- BASELINE configs[0], "a2c_feature CartPole, 8 workers, CPU only, plumbing" -- the same
 statements run as torch expressions, which is the reference's own path, not a fallback for a missing library.
+
+``config.device_a2c = True`` (off by default) runs the whole step on the device for the feature launchers' networks: one
+``b2rl_a2c_actor_step`` launch per env step and one ``b2rl_a2c_update`` launch per rollout (csrc/a2c.cu, component/actor.py
+``DeviceA2C``).  The actions are then drawn from the device's Philox stream, not from torch's generator.  Configurations the
+kernels do not cover raise ``NotImplementedError`` naming the unmet condition.
 """
 import numpy as np
 import torch
@@ -56,6 +61,12 @@ class A2CAgent(BaseAgent):
         self.total_steps = 0
         self.states = self.task.reset()
         self.last_loss = None
+        self.device_a2c = None
+        if getattr(config, "device_a2c", False):
+            from ..component.actor import DeviceA2C
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
+            self.device_a2c = DeviceA2C(self.network, self.optimizer, config, seed)
+            self.optimizer = self.device_a2c.opt
 
     def eval_step(self, state):
         with torch.no_grad():
@@ -63,6 +74,8 @@ class A2CAgent(BaseAgent):
         return to_np(prediction["action"])
 
     def step(self):
+        if self.device_a2c is not None:
+            return self._step_device()
         config = self.config
         storage = Storage(config.rollout_length)
         states = self.states
@@ -100,3 +113,20 @@ class A2CAgent(BaseAgent):
             self.last_loss = loss.detach()
         nn.utils.clip_grad_norm_(self.network.parameters(), config.gradient_clip)
         self.optimizer.step()
+
+    def _step_device(self):
+        """``step()`` with ``config.device_a2c``: T actor launches, each followed by ``task.step`` on the host; rewards and masks
+        stay in host arrays until the rollout ends; then the final observations, one upload, and one update launch."""
+        config, dev = self.config, self.device_a2c
+        dev.begin_rollout()
+        states = self.states
+        for t in range(config.rollout_length):
+            action = dev.act(t, states)
+            next_states, rewards, terminals, info = self.task.step(action)
+            self.record_online_return(info)
+            dev.rewards[t] = np.asarray(config.reward_normalizer(rewards), dtype=np.float32)   # tensor(): float32
+            dev.masks[t] = np.asarray(1 - terminals, dtype=np.float32)
+            states = next_states
+            self.total_steps += config.num_workers
+        self.states = states
+        self.last_loss = dev.update(config.state_normalizer(np.asarray([np.asarray(s) for s in states])))

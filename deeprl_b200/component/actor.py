@@ -224,3 +224,157 @@ def q_actor_supported(config, network):
                 and body.conv1.in_channels == 4
                 and Config.COMPUTE_DTYPE == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
                 and isinstance(config.state_normalizer, RescaleNormalizer))
+
+
+# ------------------------------------------------------------------------------------------------ A2C on the device
+def a2c_unsupported(network, optimizer, config):
+    """``None`` when ``config.device_a2c``'s kernels (csrc/a2c.cu) cover this agent, else the unmet condition."""
+    import torch.nn.functional as F
+
+    from ..network.network_heads import CategoricalActorCriticNet, GaussianActorCriticNet
+    from ..utils.normalizer import RescaleNormalizer
+    fc2 = lambda b: isinstance(b, FCBody) and len(b.layers) == 2 and not b.noisy_linear
+    if isinstance(network, CategoricalActorCriticNet):
+        if not (fc2(network.phi_body) and isinstance(network.actor_body, DummyBody)
+                and isinstance(network.critic_body, DummyBody)):
+            return ("a CategoricalActorCriticNet needs a two-layer FCBody phi_body and DummyBody actor / critic bodies "
+                    "(got %s / %s / %s)" % tuple(type(b).__name__ for b in (network.phi_body, network.actor_body,
+                                                                              network.critic_body)))
+        trunks = [network.phi_body]
+    elif isinstance(network, GaussianActorCriticNet):
+        if not (isinstance(network.phi_body, DummyBody) and fc2(network.actor_body) and fc2(network.critic_body)):
+            return ("a GaussianActorCriticNet needs a DummyBody phi_body and two-layer FCBody actor / critic bodies "
+                    "(got %s / %s / %s)" % tuple(type(b).__name__ for b in (network.phi_body, network.actor_body,
+                                                                              network.critic_body)))
+        trunks = [network.actor_body, network.critic_body]
+    else:
+        return "the network is a %s, not a CategoricalActorCriticNet or GaussianActorCriticNet" % type(network).__name__
+    widths = [(b.layers[0].in_features, b.layers[0].out_features, b.layers[1].out_features) for b in trunks]
+    if len(set(widths)) != 1 or len(set(id(b.gate) for b in trunks)) != 1:
+        return "the actor and critic bodies must have the same widths and gate"
+    D, H1, H2 = widths[0]
+    A = network.fc_action.out_features
+    if trunks[0].gate not in (torch.tanh, F.relu):
+        return "the FCBody gate must be torch.tanh or F.relu"
+    if not network.fc_action.weight.is_cuda:
+        return "the network is not on a CUDA device (select_device(0))"
+    if D > 256 or H1 > 128 or H2 > 128 or A > 32:
+        return "sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, actions %d <= 32" % (D, H1, H2, A)
+    if not isinstance(optimizer, torch.optim.RMSprop):
+        return "the optimizer is %s; the device update implements RMSprop" % type(optimizer).__name__
+    if type(config.state_normalizer) is not RescaleNormalizer:
+        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
+    head = 0 if isinstance(network, CategoricalActorCriticNet) else 1
+    smem = _lib.lib().b2rl_a2c_smem_bytes(head, int(head == 0), D, H1, H2, A, config.num_workers, config.rollout_length)
+    if not 0 < smem <= 227 * 1024:
+        return ("a rollout of %d x %d rows needs %d bytes of shared memory, more than one SM has (b2rl_a2c_smem_bytes)"
+                % (config.rollout_length + 1, config.num_workers, smem))
+    return None
+
+
+class DeviceA2C:
+    """``A2CAgent.step()`` on the device (``config.device_a2c``): the rollout arenas, the pinned upload / download buffers,
+    the Philox counter and the arguments of ``b2rl_a2c_actor_step`` (one launch per env step) and ``b2rl_a2c_update`` (one
+    launch per rollout).  The torch RMSprop built by ``config.optimizer_fn`` is replaced by a ``FlatOptimizer`` with the same
+    hyper-parameters: the module's parameters become views into its arena, so ``state_dict()`` is always current.
+
+    ``forced``: test hook -- a callable returning the actions of the next env step, which the actor step then writes through
+    unchanged instead of drawing (parity mode)."""
+
+    def __init__(self, network, optimizer, config, seed):
+        import torch.nn.functional as F
+
+        from .. import ops
+        from ..network.network_heads import CategoricalActorCriticNet
+        why = a2c_unsupported(network, optimizer, config)
+        if why is not None:
+            raise NotImplementedError("config.device_a2c: " + why)
+        n = network
+        self.net, self.cfg = n, config
+        self.head = 0 if isinstance(n, CategoricalActorCriticNet) else 1
+        self.shared = int(self.head == 0)
+        trunks = [n.phi_body] if self.shared else [n.actor_body, n.critic_body]
+        self.gate = 0 if trunks[0].gate is torch.tanh else 1
+        assert trunks[0].gate in (torch.tanh, F.relu)
+        self.tensors = [t for b in trunks for m in b.layers for t in (m.weight, m.bias)]
+        self.tensors += [n.fc_action.weight, n.fc_action.bias, n.fc_critic.weight, n.fc_critic.bias]
+        if self.head == 1:
+            self.tensors.append(n.std)
+        self.opt = ops.FlatOptimizer.from_torch(optimizer, list(n.parameters()))
+        self.dev = self.opt.flat.device
+        self.N, self.T = int(config.num_workers), int(config.rollout_length)
+        self.D, self.H1, self.H2 = trunks[0].layers[0].in_features, trunks[0].layers[0].out_features, trunks[0].layers[1].out_features
+        self.A = n.fc_action.out_features
+        self.acols = 1 if self.head == 0 else self.A
+        N, T, D = self.N, self.T, self.D
+        self.states = torch.zeros((T + 1, N, D), dtype=_f32, device=self.dev)
+        self.actions = torch.zeros((T, N, self.acols), dtype=_f32, device=self.dev)
+        self.rm = torch.zeros((2, T, N), dtype=_f32, device=self.dev)                 # rewards, masks
+        self.h_rm = torch.zeros((2, T, N), dtype=_f32, pin_memory=True)
+        self.h_obs = [torch.zeros((N, D), dtype=_f64, pin_memory=True) for _ in range(2)]
+        self.d_obs = [torch.zeros((N, D), dtype=_f64, device=self.dev) for _ in range(2)]
+        self.h_last = torch.zeros((N, D), dtype=_f32, pin_memory=True)
+        self.h_action = torch.zeros((N, self.acols), dtype=_f32, pin_memory=True)
+        self.h_given = torch.zeros((N, self.acols), dtype=_f32, pin_memory=True)
+        self.d_given = torch.zeros((N, self.acols), dtype=_f32, device=self.dev)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self.seed = int(seed)
+        self.off = torch.zeros(len(self.tensors), dtype=torch.int32)
+        self.slot = 0
+        self.forced = None
+        self.rewards, self.masks = self.h_rm[0].numpy(), self.h_rm[1].numpy()
+
+    def begin_rollout(self):
+        """Arena offsets of the parameters, read once per rollout (and checked: a parameter re-pointed out of the arena would
+        otherwise be trained in a copy nobody reads)."""
+        base, n = self.opt.flat.data_ptr(), self.opt.n
+        for i, t in enumerate(self.tensors):
+            o = (t.data_ptr() - base) // 4
+            if not (0 <= o and o + t.numel() <= n and t.is_contiguous()):
+                raise _lib.B2RLError("DeviceA2C: a parameter no longer lives in the optimizer's arena")
+            self.off[i] = o
+        o = self.off
+        self._net = (self.head, self.shared, self.gate)
+        self._dims = (self.D, self.H1, self.H2, self.A)
+        self._flat = _lib.ptr(self.opt.flat)
+        self._off = _lib.ptr(o)
+        self._obs = [_lib.ptr(t) for t in self.d_obs]
+        self._np_obs = [t.numpy() for t in self.h_obs]
+        self._row = self.N * self.D * 4, self.N * self.acols * 4
+        self._scale = float(self.cfg.state_normalizer.coef)
+
+    def act(self, t, raw_obs):
+        """Env step ``t`` of the rollout: rescale + forward + draw in one launch; returns the actions for ``task.step``."""
+        k = self.slot
+        self.slot = 1 - k
+        self._np_obs[k][...] = np.asarray([np.asarray(s) for s in raw_obs], dtype=np.float64).reshape(self.N, self.D)
+        self.d_obs[k].copy_(self.h_obs[k], non_blocking=True)
+        given = None
+        if self.forced is not None:
+            self.h_given.numpy()[...] = np.asarray(self.forced(), dtype=np.float32).reshape(self.N, self.acols)
+            self.d_given.copy_(self.h_given, non_blocking=True)
+            given = _lib.ptr(self.d_given)
+        _lib.call("b2rl_a2c_actor_step", *self._net, self._obs[k], self._scale, self._flat, self._off, *self._dims, self.N,
+                  ctypes.c_void_p(self.states.data_ptr() + t * self._row[0]),
+                  ctypes.c_void_p(self.actions.data_ptr() + t * self._row[1]), given, self.seed, _lib.ptr(self.counter),
+                  _lib.stream())
+        self.h_action.copy_(self.actions[t], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        a = self.h_action.numpy()
+        return a[:, 0].astype(np.int64) if self.head == 0 else a.copy()
+
+    def update(self, last_states):
+        """The final (normalised) observations into row T, rewards / masks (``self.rewards`` / ``self.masks``, filled by the
+        caller) up in one copy, then the update launch.  Returns the objective as a 0-dim device tensor."""
+        c = self.cfg
+        self.h_last.numpy()[...] = np.asarray(last_states, dtype=np.float32).reshape(self.N, self.D)
+        self.states[self.T].copy_(self.h_last, non_blocking=True)
+        self.rm.copy_(self.h_rm, non_blocking=True)
+        loss = torch.empty((), dtype=_f32, device=self.dev)
+        o = self.opt
+        _lib.call("b2rl_a2c_update", *self._net, _lib.ptr(self.states), _lib.ptr(self.actions), _lib.ptr(self.rm[0]),
+                  _lib.ptr(self.rm[1]), self.T, self.N, *self._dims, self._flat, _lib.ptr(o.s1), _lib.ptr(o.s2),
+                  _lib.ptr(o.step_dev), self._off, float(o.lr), float(o.alpha), float(o.eps), int(o.centered),
+                  float(c.discount), float(c.gae_tau), int(bool(c.use_gae)), float(c.entropy_weight),
+                  float(c.value_loss_weight), float(c.gradient_clip), _lib.ptr(loss), _lib.stream())
+        return loss

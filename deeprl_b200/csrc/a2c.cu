@@ -1,0 +1,207 @@
+// a2c.cu -- A2CAgent.step() (A2C_agent.py:22-64) on the device for the feature launchers (a2c_feature, a2c_continuous):
+//
+//   b2rl_a2c_actor_step   ONE launch per env step: RescaleNormalizer of the raw observations (float64 product, rounded once to
+//                         float32 like tensor()), the actor's forward (a2c_phases.h) and the action draw -- categorical: inverse
+//                         CDF of the softmax on one Philox uniform; Gaussian: mean + softplus(std) z with Box-Muller normals.
+//                         The state goes to row t of the rollout arena, the action to row t of the action arena.  No log-prob,
+//                         entropy or value: the parameters do not change during a rollout, so the update recomputes them from
+//                         the same weights.
+//   b2rl_a2c_update       the rest of step() as ONE launch of one block: forward of all (T + 1) N rows, GAE, the objective,
+//                         backward, clip_grad_norm_, RMSprop on the FlatOptimizer arena (a2c_sequence.inc).  The network is
+//                         5-12 k parameters over 25-100 rows: the eager form is several hundred launches of a few microseconds.
+//
+// sm_90a only.
+#include "common.cuh"
+#include "a2c_phases.h"
+
+namespace b2rl {
+
+constexpr int A2C_NT = 512, A2C_ACT_NT = 256;
+constexpr uint64_t A2C_PHILOX_STREAM = 13;
+
+template <int HEAD, bool SHARED, int GATE>
+__global__ void __launch_bounds__(A2C_NT, 1) a2c_update_kernel(const __grid_constant__ b2rl_a2c::A2cArgs a) {
+  using namespace b2rl_a2c;
+  pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return
+  extern __shared__ __align__(16) float a2c_smem[];
+  A2cShared S;
+  a2c_carve<HEAD, SHARED>(S, a2c_smem, a.net.D, a.net.H1, a.net.H2, a.net.A, (a.T + 1) * a.N, a.T * a.N);
+  const int NT = A2C_NT;
+#define A2C_PHASE(...) { const int tid = threadIdx.x; __VA_ARGS__; } __syncthreads();
+#include "a2c_sequence.inc"
+#undef A2C_PHASE
+}
+
+struct A2cActorArgs {
+  b2rl_a2c::A2cNet net;
+  const double* obs;          // raw observations [N][D]
+  double scale;               // RescaleNormalizer coefficient
+  int N;
+  float* state_out;           // row t of the rollout arena [N][D]
+  float* action_out;          // row t of the action arena [N][acols]
+  const float* given;         // parity mode: these actions are written through, nothing is drawn
+  uint64_t seed;
+  int64_t* counter;           // Philox position, advanced by the number of draws
+};
+
+template <int HEAD, bool SHARED, int GATE>
+__global__ void __launch_bounds__(A2C_ACT_NT, 1) a2c_actor_kernel(const __grid_constant__ A2cActorArgs a) {
+  using namespace b2rl_a2c;
+  pdl_sync();
+  extern __shared__ __align__(16) float a2c_smem[];
+  A2cShared S;
+  a2c_carve<HEAD, SHARED>(S, a2c_smem, a.net.D, a.net.H1, a.net.H2, a.net.A, a.N, 0);
+  const int tid = threadIdx.x, NT = A2C_ACT_NT, D = a.net.D, A = a.net.A;
+  const int64_t ctr0 = *a.counter;               // read by every thread before the barriers; thread 0 writes it at the end
+  ph_load_weights<HEAD, SHARED>(S, a.net, true, tid, NT);
+  for (int e = tid; e < a.N * D; e += NT) {
+    const int n = e / D, k = e - n * D;
+    const float x = (float)(a.scale * a.obs[e]);
+    S.x[n * S.ldx + k] = x;
+    a.state_out[e] = x;
+  }
+  __syncthreads();
+  ph_fwd1<HEAD, SHARED, GATE>(S, a.net, true, tid, NT);
+  __syncthreads();
+  ph_fwd2<HEAD, SHARED, GATE>(S, a.net, true, tid, NT);
+  __syncthreads();
+  ph_heads<HEAD, SHARED>(S, a.net, true, tid, NT);
+  __syncthreads();
+  if (HEAD == CAT) {
+    for (int n = tid; n < a.N; n += NT) {
+      if (a.given) {
+        a.action_out[n] = a.given[n];
+        continue;
+      }
+      const float* z = S.z + n * S.lda;
+      float mx = z[0];
+      for (int j = 1; j < A; ++j) mx = fmaxf(mx, z[j]);
+      float s = 0.0f;
+      for (int j = 0; j < A; ++j) s += expf(z[j] - mx);
+      const float target = Philox::u24(a.seed, (uint64_t)(ctr0 + n), A2C_PHILOX_STREAM) * s;
+      int pick = A - 1;                           // (rounding may leave the target above the last partial sum)
+      float c = 0.0f;
+      for (int j = 0; j < A; ++j) {
+        c += expf(z[j] - mx);
+        if (target < c) { pick = j; break; }
+      }
+      a.action_out[n] = (float)pick;
+    }
+  } else {
+    for (int e = tid; e < a.N * A; e += NT) {
+      const int n = e / A, j = e - n * A;
+      a.action_out[e] = a.given ? a.given[e]
+                                : S.z[n * S.lda + j] + S.sdv[j] * Philox::normal(a.seed, (uint64_t)(ctr0 + e), A2C_PHILOX_STREAM);
+    }
+  }
+  if (tid == 0 && !a.given) *a.counter = ctr0 + (int64_t)a.N * (HEAD == CAT ? 1 : A);
+}
+
+// the instantiated configurations: (CAT, shared trunk) and (GAUSS, separate trunks), each with a tanh or ReLU gate
+template <template <int, bool, int> class F, typename... Args>
+static bool a2c_dispatch(int head, int shared, int gate, Args&&... args) {
+  using namespace b2rl_a2c;
+  if (head == CAT && shared && gate == TANH) return F<CAT, true, TANH>::run(args...), true;
+  if (head == CAT && shared && gate == RELU) return F<CAT, true, RELU>::run(args...), true;
+  if (head == GAUSS && !shared && gate == TANH) return F<GAUSS, false, TANH>::run(args...), true;
+  if (head == GAUSS && !shared && gate == RELU) return F<GAUSS, false, RELU>::run(args...), true;
+  return false;
+}
+
+template <int HEAD, bool SHARED, int GATE> struct UpdateLaunch {
+  static void run(const b2rl_a2c::A2cArgs& a, size_t smem, cudaStream_t st) {
+    static size_t attr = 0;
+    if (smem > attr) {
+      cudaFuncSetAttribute(a2c_update_kernel<HEAD, SHARED, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      attr = smem;
+    }
+    launch_pdl(a2c_update_kernel<HEAD, SHARED, GATE>, dim3(1), dim3(A2C_NT), smem, st, a);
+  }
+};
+
+template <int HEAD, bool SHARED, int GATE> struct ActorLaunch {
+  static void run(const A2cActorArgs& a, size_t smem, cudaStream_t st) {
+    static size_t attr = 0;
+    if (smem > attr) {
+      cudaFuncSetAttribute(a2c_actor_kernel<HEAD, SHARED, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      attr = smem;
+    }
+    launch_pdl(a2c_actor_kernel<HEAD, SHARED, GATE>, dim3(1), dim3(A2C_ACT_NT), smem, st, a);
+  }
+};
+
+static size_t a2c_bytes(int head, int shared, int D, int H1, int H2, int A, int R, int M) {
+  using namespace b2rl_a2c;
+  A2cShared probe;
+  float* dummy = reinterpret_cast<float*>(uintptr_t(4096));
+  if (head == CAT && shared) return a2c_carve<CAT, true>(probe, dummy, D, H1, H2, A, R, M) * sizeof(float);
+  if (head == GAUSS && !shared) return a2c_carve<GAUSS, false>(probe, dummy, D, H1, H2, A, R, M) * sizeof(float);
+  return 0;
+}
+
+}  // namespace b2rl
+
+using namespace b2rl;
+
+#define A2C_CHECK_NET()                                                                                                      \
+  B2RL_REQUIRE(flat && off, "null pointer");                                                                                 \
+  B2RL_REQUIRE((head == 0 && shared == 1) || (head == 1 && shared == 0),                                                     \
+               "instantiated: categorical head on a shared trunk, Gaussian head on separate trunks");                        \
+  B2RL_REQUIRE(gate == 0 || gate == 1, "gate must be 0 (tanh) or 1 (relu)");                                                 \
+  B2RL_REQUIRE(D > 0 && D <= 256 && H1 > 0 && H1 <= 128 && H2 > 0 && H2 <= 128 && A > 0 && A <= 32,                          \
+               "shape limits: D <= 256, hidden <= 128, A <= 32");                                                            \
+  B2RL_REQUIRE(head == 1 || A >= 2, "a categorical head needs at least two actions")
+
+static b2rl_a2c::A2cNet a2c_net(float* flat, const int32_t* off, int head, int shared, int D, int H1, int H2, int A) {
+  b2rl_a2c::A2cNet net;
+  net.flat = flat;
+  const int nt = 4 * (shared ? 1 : 2) + 4 + (head == 1 ? 1 : 0);
+  for (int i = 0; i < b2rl_a2c::A2C_MAX_TENSORS; ++i) net.off[i] = i < nt ? off[i] : 0;
+  net.D = D; net.H1 = H1; net.H2 = H2; net.A = A;
+  return net;
+}
+
+// dynamic shared memory of the update kernel for these sizes (the caller checks it against the 227 KB of one SM)
+extern "C" int64_t b2rl_a2c_smem_bytes(int32_t head, int32_t shared, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N,
+                                       int32_t T) {
+  if (D <= 0 || H1 <= 0 || H2 <= 0 || A <= 0 || N <= 0 || T <= 0) return 0;
+  return (int64_t)a2c_bytes(head, shared, D, H1, H2, A, (T + 1) * N, T * N);
+}
+
+extern "C" int b2rl_a2c_actor_step(int32_t head, int32_t shared, int32_t gate, const double* obs, double obs_scale,
+                                   const float* flat, const int32_t* off, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N,
+                                   float* state_out, float* action_out, const float* given_action, uint64_t seed,
+                                   int64_t* counter, void* stream) {
+  A2C_CHECK_NET();
+  B2RL_REQUIRE(obs && state_out && action_out && counter, "null pointer");
+  B2RL_REQUIRE(N > 0 && N <= 1024, "N must be in [1, 1024]");
+  A2cActorArgs a;
+  a.net = a2c_net(const_cast<float*>(flat), off, head, shared, D, H1, H2, A);
+  a.obs = obs; a.scale = obs_scale; a.N = N; a.state_out = state_out; a.action_out = action_out; a.given = given_action;
+  a.seed = seed; a.counter = counter;
+  const size_t smem = a2c_bytes(head, shared, D, H1, H2, A, N, 0);
+  B2RL_REQUIRE(smem <= 227 * 1024, "network / worker count too large for the shared memory of one SM");
+  a2c_dispatch<ActorLaunch>(head, shared, gate, a, smem, (cudaStream_t)stream);
+  return check_launch("b2rl_a2c_actor_step");
+}
+
+extern "C" int b2rl_a2c_update(int32_t head, int32_t shared, int32_t gate, const float* states, const float* actions,
+                               const float* reward, const float* mask, int32_t T, int32_t N, int32_t D, int32_t H1, int32_t H2,
+                               int32_t A, float* flat, float* square_avg, float* grad_avg, int64_t* step, const int32_t* off,
+                               float lr, float alpha, float eps, int32_t centered, float discount, float tau, int32_t use_gae,
+                               float entropy_weight, float value_loss_weight, float max_norm, float* loss, void* stream) {
+  A2C_CHECK_NET();
+  B2RL_REQUIRE(states && actions && reward && mask && square_avg && step && loss && (grad_avg || !centered), "null pointer");
+  B2RL_REQUIRE(T > 0 && N > 0, "bad T / N");
+  b2rl_a2c::A2cArgs a;
+  a.net = a2c_net(flat, off, head, shared, D, H1, H2, A);
+  a.state = states; a.action = actions; a.reward = reward; a.mask = mask; a.T = T; a.N = N;
+  a.sq = square_avg; a.ga = grad_avg; a.step = step;
+  a.lr = lr; a.alpha = alpha; a.eps = eps; a.centered = centered;
+  a.discount = discount; a.tau = tau; a.use_gae = use_gae;
+  a.ent_w = entropy_weight; a.vw = value_loss_weight; a.max_norm = max_norm; a.loss = loss;
+  const size_t smem = (size_t)b2rl_a2c_smem_bytes(head, shared, D, H1, H2, A, N, T);
+  B2RL_REQUIRE(smem > 0 && smem <= 227 * 1024, "rollout / network too large for the shared memory of one SM (b2rl_a2c_smem_bytes)");
+  a2c_dispatch<UpdateLaunch>(head, shared, gate, a, smem, (cudaStream_t)stream);
+  return check_launch("b2rl_a2c_update");
+}

@@ -126,9 +126,7 @@ __global__ void __launch_bounds__(256) gaussian_actor_step_kernel(const ActorArg
         if (a.z) {
           zz = a.z[n * A + j];
         } else {                                           // Box-Muller on two 24-bit uniforms of one Philox draw
-          const uint4 r = Philox::gen(a.seed, (uint64_t)(ctr0 + n * A + j), 7);
-          const float u1 = ((r.x >> 8) + 1) * (1.0f / 16777216.0f), u2 = (r.y >> 8) * (1.0f / 16777216.0f);
-          zz = sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
+          zz = Philox::normal(a.seed, (uint64_t)(ctr0 + n * A + j), 7);
         }
         act = m + sd * zz;
       }

@@ -101,6 +101,16 @@ struct Philox {
     uint64_t x = ((uint64_t)r.x << 32) | r.y;
     return __umul64hi(x, n);
   }
+  // uniform float in [0, 1) with 24 random bits
+  __device__ static inline float u24(uint64_t seed, uint64_t ctr, uint64_t stream) {
+    return (gen(seed, ctr, stream).x >> 8) * (1.0f / 16777216.0f);
+  }
+  // standard normal: Box-Muller on two 24-bit uniforms of one draw (u1 in (0, 1], so the log is finite)
+  __device__ static inline float normal(uint64_t seed, uint64_t ctr, uint64_t stream) {
+    const uint4 r = gen(seed, ctr, stream);
+    const float u1 = ((r.x >> 8) + 1) * (1.0f / 16777216.0f), u2 = (r.y >> 8) * (1.0f / 16777216.0f);
+    return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
+  }
 };
 
 // ---------------------------------------------------------------------------------------------

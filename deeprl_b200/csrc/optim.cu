@@ -5,6 +5,7 @@
 // clip rule is torch.nn.utils.clip_grad_norm_ (coef = max_norm / (total_norm + 1e-6), clamped to 1).
 // One arena => 2 launches instead of ~10 tensors x (norm + mul + ~8 optimizer ops).  sm_90a only.
 #include "common.cuh"
+#include "optim_elem.h"
 
 namespace b2rl {
 
@@ -59,18 +60,7 @@ __global__ void __launch_bounds__(256) rmsprop_kernel(float* __restrict__ p, con
   const float coef = sc->coef;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float gr = g[i] * coef;
-    float s = alpha * sq[i] + (1.0f - alpha) * gr * gr;          // square_avg.mul_(alpha).addcmul_(g, g, 1-alpha)
-    sq[i] = s;
-    float avg;
-    if (centered) {
-      float a = ga[i];
-      a = a + (1.0f - alpha) * (gr - a);                          // grad_avg.lerp_(grad, 1 - alpha)
-      ga[i] = a;
-      avg = sqrtf(s - a * a) + eps;                               // addcmul(grad_avg, grad_avg, -1).sqrt_().add_(eps)
-    } else {
-      avg = sqrtf(s) + eps;
-    }
-    const float np_ = p[i] - lr * (gr / avg);                     // param.addcdiv_(grad, avg, value=-lr)
+    const float np_ = b2rl_elem::rmsprop_elem(p[i], gr, sq, ga, i, lr, alpha, eps, centered);
     p[i] = np_;
     if (shadow) shadow[i] = __float2bfloat16_rn(np_);
   }

@@ -434,6 +434,29 @@ int b2rl_ppo_minibatch_updates_dp(const float* state, const float* action, const
 /* Device memory shared between processes (CUDA IPC; setup only, never on the update path): allocate + zero-fill, export a
  * 64-byte handle, map a peer's handle (peer access enabled lazily), unmap, free; peer_access_ok: *ok = 1 when device dev_a can
  * address device dev_b's memory (or dev_a == dev_b). */
+/* A2CAgent.step() (A2C_agent.py:22-64) on the device for FCBody actor-critic networks: head 0 = CategoricalActorCriticNet on a
+ * shared two-layer phi_body (shared 1), head 1 = GaussianActorCriticNet on separate two-layer actor / critic bodies (shared 0);
+ * gate 0 = tanh, 1 = ReLU.  flat: the FlatOptimizer arena; off (host, int32): arena offset of every tensor in the order
+ * trunk 0 (w1 b1 w2 b2), [trunk 1 (w1 b1 w2 b2)], fc_action (w b), fc_critic (w b), [std].
+ * smem_bytes: dynamic shared memory of the update for a rollout of T steps of N workers (0: not an instantiated configuration);
+ *   it must fit the 227 KB of one SM.
+ * actor_step: one env step in one launch -- state_out[n][d] = (float)(obs_scale * obs[n][d]) (RescaleNormalizer; obs is the
+ *   float64 raw observation [N][D]), the actor's forward and the draw: categorical inverse CDF of the softmax on one Philox
+ *   uniform, Gaussian mean + softplus(std) * N(0, 1) (Box-Muller); action_out [N][1] (the category as a float) or [N][A].
+ *   *counter (device) advances by the number of draws (N or N * A).  given_action != NULL: written through, nothing drawn.
+ * update: forward of states [T + 1][N][D], GAE (discount, tau, use_gae; the reference's order and association), objective
+ *   -mean(log pi(a) adv) - entropy_weight mean(entropy) + value_loss_weight 0.5 mean((ret - v)^2) into *loss (device), its
+ *   gradient, clip_grad_norm_(max_norm) and RMSprop (lr, alpha, eps, centered) on flat / square_avg / grad_avg; *step += 1. */
+int64_t b2rl_a2c_smem_bytes(int32_t head, int32_t shared, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, int32_t T);
+int b2rl_a2c_actor_step(int32_t head, int32_t shared, int32_t gate, const double* obs, double obs_scale, const float* flat,
+                        const int32_t* off, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, float* state_out,
+                        float* action_out, const float* given_action, uint64_t seed, int64_t* counter, void* stream);
+int b2rl_a2c_update(int32_t head, int32_t shared, int32_t gate, const float* states, const float* actions, const float* reward,
+                    const float* mask, int32_t T, int32_t N, int32_t D, int32_t H1, int32_t H2, int32_t A, float* flat,
+                    float* square_avg, float* grad_avg, int64_t* step, const int32_t* off, float lr, float alpha, float eps,
+                    int32_t centered, float discount, float tau, int32_t use_gae, float entropy_weight,
+                    float value_loss_weight, float max_norm, float* loss, void* stream);
+
 int b2rl_ipc_alloc(int64_t bytes, void** out);
 int b2rl_ipc_get_handle(void* ptr, void* handle_out);
 int b2rl_ipc_open_handle(const void* handle, void** out);

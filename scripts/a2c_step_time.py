@@ -1,0 +1,110 @@
+"""A2C steps per second of the two feature launchers' configurations, eager (the torch path of A2CAgent.step) against
+``config.device_a2c`` (one actor-step launch per env step, one update launch per rollout: csrc/a2c.cu), in one process on one
+card, the two alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
+left to the learner is visible.  Prints the card's name and power limit with the numbers.
+
+    python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--out DIR]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+CONFIGS = [("a2c_feature", "CartPole-v0"), ("a2c_continuous", "SyntheticCheetah-v0")]
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:                                  # noqa: BLE001
+        q = "nvidia-smi unavailable (%s)" % e
+    return "%s | nvidia-smi: %s" % (torch.cuda.get_device_name(0), q)
+
+
+def make_agent(name, game, device_a2c):
+    import examples
+    got = []
+    run_steps = examples.run_steps
+    examples.run_steps = got.append
+    try:
+        getattr(examples, name)(game=game, device_a2c=device_a2c)
+    finally:
+        examples.run_steps = run_steps
+    return got[0]
+
+
+def timed(agent, steps):
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(steps):
+        agent.step()
+    torch.cuda.synchronize()
+    return steps / (time.perf_counter() - t0)
+
+
+def env_only(agent, steps):
+    """task.step alone, T * steps times, with the actions of one draw (what the host envs cost per A2C step)."""
+    from deeprl_b200 import CategoricalActorCriticNet
+    c = agent.config
+    a = (np.zeros(c.num_workers, dtype=np.int64) if isinstance(agent.network, CategoricalActorCriticNet)
+         else np.zeros((c.num_workers, c.action_dim), dtype=np.float32))
+    t0 = time.perf_counter()
+    for _ in range(steps * c.rollout_length):
+        agent.task.step(a)
+    return steps / (time.perf_counter() - t0)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=300)
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("a2c_step_time.py measures on a CUDA device; none is visible")
+    import deeprl_b200 as rl
+    rl.select_device(0)
+    rl.random_seed(0)
+    result = dict(card=card(), steps_per_round=args.steps, rounds=args.rounds, configs={})
+    print(result["card"])
+    for name, game in CONFIGS:
+        agents = {"eager": make_agent(name, game, False), "device_a2c": make_agent(name, game, True)}
+        for ag in agents.values():
+            timed(ag, args.warmup)
+        rates = {k: [] for k in agents}
+        for _ in range(args.rounds):                        # alternated: both see the same host / card conditions
+            for k, ag in agents.items():
+                rates[k].append(timed(ag, args.steps))
+        env = env_only(agents["eager"], args.steps)
+        c = agents["eager"].config
+        med = {k: float(np.median(v)) for k, v in rates.items()}
+        learner_ms = {k: 1e3 / med[k] - 1e3 / env for k in med}
+        row = dict(game=game, num_workers=c.num_workers, rollout_length=c.rollout_length, a2c_steps_per_s=rates,
+                   median_a2c_steps_per_s=med, speedup=med["device_a2c"] / med["eager"], env_only_a2c_steps_per_s=env,
+                   ms_per_step_besides_envs=learner_ms)
+        result["configs"][name] = row
+        print("%-15s %-20s N=%d T=%d  eager %8.1f steps/s  device_a2c %8.1f steps/s  (x%.2f)  envs alone %8.1f steps/s;  "
+              "ms per step besides the envs: eager %.3f, device_a2c %.3f"
+              % (name, game, c.num_workers, c.rollout_length, med["eager"], med["device_a2c"], row["speedup"], env,
+                 learner_ms["eager"], learner_ms["device_a2c"]))
+        for ag in agents.values():
+            ag.close()
+    print(json.dumps(result))
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, "a2c_step_time.json"), "w") as f:
+            json.dump(result, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
