@@ -76,6 +76,10 @@ SIGNATURES = {
     "b2rl_a2c_actor_step": [c_i32, c_i32, c_i32, c_p, c_f64, c_p, c_p] + [c_i32] * 5 + [c_p, c_p, c_p, c_u64, c_p, c_p],
     "b2rl_a2c_update": [c_i32, c_i32, c_i32] + [c_p] * 4 + [c_i32] * 6 + [c_p] * 5 + [c_f32] * 3 + [c_i32] + [c_f32] * 2
                        + [c_i32] + [c_f32] * 3 + [c_p, c_p],
+    "b2rl_nstep_dqn_smem_bytes": [c_i32] * 6,
+    "b2rl_nstep_dqn_actor_step": [c_i32, c_p, c_f64, c_p, c_p] + [c_i32] * 5 + [c_f32, c_p, c_p, c_p, c_u64, c_p, c_p],
+    "b2rl_nstep_dqn_update": ([c_i32] + [c_p] * 4 + [c_i32] * 6 + [c_p, c_p, c_i32] + [c_p] * 4 + [c_f32] * 3 + [c_i32]
+                              + [c_f32] * 2 + [c_p, c_p]),
     "b2rl_ipc_alloc": [c_i64, c_p],
     "b2rl_ipc_get_handle": [c_p, c_p],
     "b2rl_ipc_open_handle": [c_p, c_p],
@@ -152,6 +156,7 @@ def lib():
             fn.argtypes = args
             fn.restype = ctypes.c_int
         L.b2rl_a2c_smem_bytes.restype = ctypes.c_int64       # (a size, not a status)
+        L.b2rl_nstep_dqn_smem_bytes.restype = ctypes.c_int64
         _lib = L
     return _lib
 

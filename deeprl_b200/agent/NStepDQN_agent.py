@@ -8,6 +8,12 @@
 On a CUDA device the return scan is the K7 scan kernel (``ops.gae``: its ``ret`` output is this recurrence; csrc/onpolicy.cu) and
 the loss and its gradient are the fused DQN kernel (``ops.dqn_loss_fused`` with the n-step return as the target: reward = ret, mask = 0;
 csrc/losses.cu).  On ``select_device(-1)`` the same statements run as torch expressions -- the reference's own CPU path.
+
+``config.device_nstep_dqn = True`` (off by default) runs the whole step on the device for a VanillaNet on a two-layer FCBody
+(``n_step_dqn_feature``): one ``b2rl_nstep_dqn_actor_step`` launch per env step and one ``b2rl_nstep_dqn_update`` launch per
+rollout, the target sync included (csrc/a2c.cu, component/actor.py ``DeviceNStepDQN``).  The epsilon-greedy draws then come from
+the device's Philox stream, not from numpy's.  Configurations the kernels do not cover raise ``NotImplementedError`` naming the
+unmet condition.
 """
 import numpy as np
 import torch
@@ -31,6 +37,12 @@ class NStepDQNAgent(BaseAgent):
         self.total_steps = 0
         self.states = self.task.reset()
         self.last_loss = None
+        self.device_nstep_dqn = None
+        if getattr(config, "device_nstep_dqn", False):
+            from ..component.actor import DeviceNStepDQN
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
+            self.device_nstep_dqn = DeviceNStepDQN(self.network, self.target_network, self.optimizer, config, seed)
+            self.optimizer = self.device_nstep_dqn.opt
 
     def eval_step(self, state):
         """(the reference defines none for this agent; greedy action, as DQNAgent.eval_step DQN_agent.py:69-75)"""
@@ -42,6 +54,8 @@ class NStepDQNAgent(BaseAgent):
         return self.config.state_normalizer(np.asarray([np.asarray(s) for s in states]))
 
     def step(self):
+        if self.device_nstep_dqn is not None:
+            return self._step_device()
         config = self.config
         T = config.rollout_length
         storage = Storage(T)
@@ -88,3 +102,23 @@ class NStepDQNAgent(BaseAgent):
         self.last_loss = loss.detach()
         nn.utils.clip_grad_norm_(self.network.parameters(), config.gradient_clip)
         self.optimizer.step()
+
+    def _step_device(self):
+        """``step()`` with ``config.device_nstep_dqn``: T actor launches, each followed by ``task.step`` on the host; rewards and
+        masks stay in host arrays until the rollout ends; then the final observations, one upload, and one update launch, which
+        also does the target sync when an env step of this rollout reached its schedule (:48-50)."""
+        config, dev = self.config, self.device_nstep_dqn
+        dev.begin_rollout()
+        states = self.states
+        sync = False
+        for t in range(config.rollout_length):
+            action = dev.act(t, states, config.random_action_prob(config.num_workers))
+            next_states, rewards, terminals, info = self.task.step(action)
+            self.record_online_return(info)
+            dev.rewards[t] = np.asarray(config.reward_normalizer(rewards), dtype=np.float32)   # tensor(): float32
+            dev.masks[t] = np.asarray(1 - np.asarray(terminals), dtype=np.float32)
+            states = next_states
+            self.total_steps += config.num_workers
+            sync = sync or self.total_steps // config.num_workers % config.target_network_update_freq == 0
+        self.states = states
+        self.last_loss = dev.update(self._obs(states), sync)

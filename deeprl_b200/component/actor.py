@@ -272,7 +272,80 @@ def a2c_unsupported(network, optimizer, config):
     return None
 
 
-class DeviceA2C:
+class _DeviceRollout:
+    """What ``DeviceA2C`` and ``DeviceNStepDQN`` share: the rollout arenas, the pinned double-buffered float64 observation
+    upload, rewards / masks (uploaded once per rollout), the action download, the parity-mode actions, the Philox counter and
+    the check that the parameters still live in the optimizer's arena.  The subclass sets ``opt``, ``dev``, ``tensors`` (kernel
+    order), ``cfg``, ``N``, ``T``, ``D`` and ``acols`` first."""
+
+    def _buffers(self, seed):
+        N, T, D, acols = self.N, self.T, self.D, self.acols
+        self.states = torch.zeros((T + 1, N, D), dtype=_f32, device=self.dev)
+        self.actions = torch.zeros((T, N, acols), dtype=_f32, device=self.dev)
+        self.rm = torch.zeros((2, T, N), dtype=_f32, device=self.dev)                 # rewards, masks
+        self.h_rm = torch.zeros((2, T, N), dtype=_f32, pin_memory=True)
+        self.h_obs = [torch.zeros((N, D), dtype=_f64, pin_memory=True) for _ in range(2)]
+        self.d_obs = [torch.zeros((N, D), dtype=_f64, device=self.dev) for _ in range(2)]
+        self.h_last = torch.zeros((N, D), dtype=_f32, pin_memory=True)
+        self.h_action = torch.zeros((N, acols), dtype=_f32, pin_memory=True)
+        self.h_given = torch.zeros((N, acols), dtype=_f32, pin_memory=True)
+        self.d_given = torch.zeros((N, acols), dtype=_f32, device=self.dev)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self.seed = int(seed)
+        self.off = torch.zeros(len(self.tensors), dtype=torch.int32)
+        self.slot = 0
+        self.forced = None
+        self.rewards, self.masks = self.h_rm[0].numpy(), self.h_rm[1].numpy()
+
+    def _arena_offsets(self):
+        """Arena offsets of the parameters, read once per rollout (and checked: a parameter re-pointed out of the arena would
+        otherwise be trained in a copy nobody reads), and the launch arguments that follow from them."""
+        base, n = self.opt.flat.data_ptr(), self.opt.n
+        for i, t in enumerate(self.tensors):
+            o = (t.data_ptr() - base) // 4
+            if not (0 <= o and o + t.numel() <= n and t.is_contiguous()):
+                raise _lib.B2RLError("%s: a parameter no longer lives in the optimizer's arena" % type(self).__name__)
+            self.off[i] = o
+        self._flat = _lib.ptr(self.opt.flat)
+        self._off = _lib.ptr(self.off)
+        self._obs = [_lib.ptr(t) for t in self.d_obs]
+        self._np_obs = [t.numpy() for t in self.h_obs]
+        self._row = self.N * self.D * 4, self.N * self.acols * 4
+        self._scale = float(self.cfg.state_normalizer.coef)
+
+    def _stage(self, raw_obs):
+        """The env step's raw observations up (pinned, double-buffered) and, in parity mode, the given actions; returns the
+        device addresses of both (None: draw)."""
+        k = self.slot
+        self.slot = 1 - k
+        self._np_obs[k][...] = np.asarray([np.asarray(s) for s in raw_obs], dtype=np.float64).reshape(self.N, self.D)
+        self.d_obs[k].copy_(self.h_obs[k], non_blocking=True)
+        given = None
+        if self.forced is not None:
+            self.h_given.numpy()[...] = np.asarray(self.forced(), dtype=np.float32).reshape(self.N, self.acols)
+            self.d_given.copy_(self.h_given, non_blocking=True)
+            given = _lib.ptr(self.d_given)
+        return self._obs[k], given
+
+    def _row_ptrs(self, t):
+        return (ctypes.c_void_p(self.states.data_ptr() + t * self._row[0]),
+                ctypes.c_void_p(self.actions.data_ptr() + t * self._row[1]))
+
+    def _fetch(self, t):
+        """Row t of the action arena down to the host (pinned copy + one stream synchronise)."""
+        self.h_action.copy_(self.actions[t], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return self.h_action.numpy()
+
+    def _stage_last(self, last_states):
+        """The final (normalised) observations into row T; rewards / masks (``self.rewards`` / ``self.masks``, filled by the
+        caller) up in one copy."""
+        self.h_last.numpy()[...] = np.asarray(last_states, dtype=np.float32).reshape(self.N, self.D)
+        self.states[self.T].copy_(self.h_last, non_blocking=True)
+        self.rm.copy_(self.h_rm, non_blocking=True)
+
+
+class DeviceA2C(_DeviceRollout):
     """``A2CAgent.step()`` on the device (``config.device_a2c``): the rollout arenas, the pinned upload / download buffers,
     the Philox counter and the arguments of ``b2rl_a2c_actor_step`` (one launch per env step) and ``b2rl_a2c_update`` (one
     launch per rollout).  The torch RMSprop built by ``config.optimizer_fn`` is replaced by a ``FlatOptimizer`` with the same
@@ -306,70 +379,26 @@ class DeviceA2C:
         self.D, self.H1, self.H2 = trunks[0].layers[0].in_features, trunks[0].layers[0].out_features, trunks[0].layers[1].out_features
         self.A = n.fc_action.out_features
         self.acols = 1 if self.head == 0 else self.A
-        N, T, D = self.N, self.T, self.D
-        self.states = torch.zeros((T + 1, N, D), dtype=_f32, device=self.dev)
-        self.actions = torch.zeros((T, N, self.acols), dtype=_f32, device=self.dev)
-        self.rm = torch.zeros((2, T, N), dtype=_f32, device=self.dev)                 # rewards, masks
-        self.h_rm = torch.zeros((2, T, N), dtype=_f32, pin_memory=True)
-        self.h_obs = [torch.zeros((N, D), dtype=_f64, pin_memory=True) for _ in range(2)]
-        self.d_obs = [torch.zeros((N, D), dtype=_f64, device=self.dev) for _ in range(2)]
-        self.h_last = torch.zeros((N, D), dtype=_f32, pin_memory=True)
-        self.h_action = torch.zeros((N, self.acols), dtype=_f32, pin_memory=True)
-        self.h_given = torch.zeros((N, self.acols), dtype=_f32, pin_memory=True)
-        self.d_given = torch.zeros((N, self.acols), dtype=_f32, device=self.dev)
-        self.counter = torch.zeros(1, dtype=torch.int64, device=self.dev)
-        self.seed = int(seed)
-        self.off = torch.zeros(len(self.tensors), dtype=torch.int32)
-        self.slot = 0
-        self.forced = None
-        self.rewards, self.masks = self.h_rm[0].numpy(), self.h_rm[1].numpy()
+        self._buffers(seed)
 
     def begin_rollout(self):
-        """Arena offsets of the parameters, read once per rollout (and checked: a parameter re-pointed out of the arena would
-        otherwise be trained in a copy nobody reads)."""
-        base, n = self.opt.flat.data_ptr(), self.opt.n
-        for i, t in enumerate(self.tensors):
-            o = (t.data_ptr() - base) // 4
-            if not (0 <= o and o + t.numel() <= n and t.is_contiguous()):
-                raise _lib.B2RLError("DeviceA2C: a parameter no longer lives in the optimizer's arena")
-            self.off[i] = o
-        o = self.off
+        self._arena_offsets()
         self._net = (self.head, self.shared, self.gate)
         self._dims = (self.D, self.H1, self.H2, self.A)
-        self._flat = _lib.ptr(self.opt.flat)
-        self._off = _lib.ptr(o)
-        self._obs = [_lib.ptr(t) for t in self.d_obs]
-        self._np_obs = [t.numpy() for t in self.h_obs]
-        self._row = self.N * self.D * 4, self.N * self.acols * 4
-        self._scale = float(self.cfg.state_normalizer.coef)
 
     def act(self, t, raw_obs):
         """Env step ``t`` of the rollout: rescale + forward + draw in one launch; returns the actions for ``task.step``."""
-        k = self.slot
-        self.slot = 1 - k
-        self._np_obs[k][...] = np.asarray([np.asarray(s) for s in raw_obs], dtype=np.float64).reshape(self.N, self.D)
-        self.d_obs[k].copy_(self.h_obs[k], non_blocking=True)
-        given = None
-        if self.forced is not None:
-            self.h_given.numpy()[...] = np.asarray(self.forced(), dtype=np.float32).reshape(self.N, self.acols)
-            self.d_given.copy_(self.h_given, non_blocking=True)
-            given = _lib.ptr(self.d_given)
-        _lib.call("b2rl_a2c_actor_step", *self._net, self._obs[k], self._scale, self._flat, self._off, *self._dims, self.N,
-                  ctypes.c_void_p(self.states.data_ptr() + t * self._row[0]),
-                  ctypes.c_void_p(self.actions.data_ptr() + t * self._row[1]), given, self.seed, _lib.ptr(self.counter),
-                  _lib.stream())
-        self.h_action.copy_(self.actions[t], non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        a = self.h_action.numpy()
+        obs, given = self._stage(raw_obs)
+        _lib.call("b2rl_a2c_actor_step", *self._net, obs, self._scale, self._flat, self._off, *self._dims, self.N,
+                  *self._row_ptrs(t), given, self.seed, _lib.ptr(self.counter), _lib.stream())
+        a = self._fetch(t)
         return a[:, 0].astype(np.int64) if self.head == 0 else a.copy()
 
     def update(self, last_states):
-        """The final (normalised) observations into row T, rewards / masks (``self.rewards`` / ``self.masks``, filled by the
-        caller) up in one copy, then the update launch.  Returns the objective as a 0-dim device tensor."""
+        """The final observations and the rollout's rewards / masks up, then the update launch.  Returns the objective as a
+        0-dim device tensor."""
         c = self.cfg
-        self.h_last.numpy()[...] = np.asarray(last_states, dtype=np.float32).reshape(self.N, self.D)
-        self.states[self.T].copy_(self.h_last, non_blocking=True)
-        self.rm.copy_(self.h_rm, non_blocking=True)
+        self._stage_last(last_states)
         loss = torch.empty((), dtype=_f32, device=self.dev)
         o = self.opt
         _lib.call("b2rl_a2c_update", *self._net, _lib.ptr(self.states), _lib.ptr(self.actions), _lib.ptr(self.rm[0]),
@@ -377,4 +406,106 @@ class DeviceA2C:
                   _lib.ptr(o.step_dev), self._off, float(o.lr), float(o.alpha), float(o.eps), int(o.centered),
                   float(c.discount), float(c.gae_tau), int(bool(c.use_gae)), float(c.entropy_weight),
                   float(c.value_loss_weight), float(c.gradient_clip), _lib.ptr(loss), _lib.stream())
+        return loss
+
+
+# ------------------------------------------------------------------------------------------------ n-step Q on the device
+def nstep_dqn_unsupported(network, optimizer, config):
+    """``None`` when ``config.device_nstep_dqn``'s kernels (csrc/a2c.cu, b2rl_nstep_dqn_*) cover this agent, else the unmet
+    condition."""
+    import torch.nn.functional as F
+
+    from ..network.network_heads import VanillaNet
+    from ..utils.normalizer import RescaleNormalizer
+    if not isinstance(network, VanillaNet):
+        return "the network is a %s, not a VanillaNet" % type(network).__name__
+    body = network.body
+    if not isinstance(body, FCBody):
+        return "a VanillaNet needs an FCBody body (got %s)" % type(body).__name__
+    if body.noisy_linear:
+        return "the FCBody has NoisyLinear layers; the device kernels implement nn.Linear"
+    if len(body.layers) != 2:
+        return "the device kernels implement a two-layer FCBody (got %d layers)" % len(body.layers)
+    if body.gate not in (torch.tanh, F.relu):
+        return "the FCBody gate must be torch.tanh or F.relu"
+    if not network.fc_head.weight.is_cuda:
+        return "the network is not on a CUDA device (select_device(0))"
+    D, H1, H2, A = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features, network.fc_head.out_features
+    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32:
+        return "sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32" % (D, H1, H2, A)
+    if not isinstance(optimizer, torch.optim.RMSprop):
+        return "the optimizer is %s; the device update implements RMSprop" % type(optimizer).__name__
+    if type(config.state_normalizer) is not RescaleNormalizer:
+        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
+    smem = _lib.lib().b2rl_nstep_dqn_smem_bytes(D, H1, H2, A, config.num_workers, config.rollout_length)
+    if not 0 < smem <= 227 * 1024:
+        return ("a rollout of %d x %d rows needs %d bytes of shared memory, more than one SM has (b2rl_nstep_dqn_smem_bytes)"
+                % (config.rollout_length + 1, config.num_workers, smem))
+    return None
+
+
+class DeviceNStepDQN(_DeviceRollout):
+    """``NStepDQNAgent.step()`` on the device (``config.device_nstep_dqn``): one ``b2rl_nstep_dqn_actor_step`` launch per env
+    step (epsilon-greedy on the device's Philox stream) and one ``b2rl_nstep_dqn_update`` launch per rollout, which also does the
+    rollout's target sync.  The torch RMSprop built by ``config.optimizer_fn`` is replaced by a ``FlatOptimizer`` with the same
+    hyper-parameters, and the target network's parameters become views into a second arena of the same layout (``target``), so
+    both modules' ``state_dict()`` are always current.
+
+    ``forced``: test hook -- a callable returning the actions of the next env step, which the actor step then writes through
+    unchanged instead of drawing (parity mode)."""
+
+    def __init__(self, network, target_network, optimizer, config, seed):
+        from .. import ops
+        why = nstep_dqn_unsupported(network, optimizer, config)
+        if why is not None:
+            raise NotImplementedError("config.device_nstep_dqn: " + why)
+        self.net, self.target_net, self.cfg = network, target_network, config
+        body = network.body
+        self.gate = 0 if body.gate is torch.tanh else 1
+        self.tensors = self.kernel_order(network)
+        self.opt = ops.FlatOptimizer.from_torch(optimizer, list(network.parameters()))
+        self.dev = self.opt.flat.device
+        self.target = torch.zeros_like(self.opt.flat)
+        with torch.no_grad():
+            for p, o in zip(target_network.parameters(), self.opt.offsets):
+                k = p.numel()
+                self.target[o:o + k].copy_(p.detach().reshape(-1))
+                p.data = self.target[o:o + k].view_as(p)
+        self.N, self.T = int(config.num_workers), int(config.rollout_length)
+        self.D, self.H1, self.H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
+        self.A = network.fc_head.out_features
+        self.acols = 1
+        self._buffers(seed)
+
+    @staticmethod
+    def kernel_order(net):
+        """A VanillaNet's parameters in the kernels' tensor order: w1 b1 w2 b2 fc_head.w fc_head.b."""
+        return [t for m in net.body.layers for t in (m.weight, m.bias)] + [net.fc_head.weight, net.fc_head.bias]
+
+    def begin_rollout(self):
+        self._arena_offsets()
+        base = self.target.data_ptr()
+        for t, o in zip(self.kernel_order(self.target_net), self.off.tolist()):
+            if t.data_ptr() != base + 4 * o:
+                raise _lib.B2RLError("DeviceNStepDQN: a target parameter no longer lives in the target arena")
+        self._dims = (self.D, self.H1, self.H2, self.A)
+
+    def act(self, t, raw_obs, epsilon):
+        """Env step ``t`` of the rollout: rescale + forward + epsilon-greedy in one launch; returns the actions for
+        ``task.step``."""
+        obs, given = self._stage(raw_obs)
+        _lib.call("b2rl_nstep_dqn_actor_step", self.gate, obs, self._scale, self._flat, self._off, *self._dims, self.N,
+                  float(epsilon), *self._row_ptrs(t), given, self.seed, _lib.ptr(self.counter), _lib.stream())
+        return self._fetch(t)[:, 0].astype(np.int64)
+
+    def update(self, last_states, sync_target):
+        """The final observations and the rollout's rewards / masks up, then the update launch; ``sync_target``: an env step of
+        this rollout reached the target sync schedule.  Returns the objective as a 0-dim device tensor."""
+        c, o = self.cfg, self.opt
+        self._stage_last(last_states)
+        loss = torch.empty((), dtype=_f32, device=self.dev)
+        _lib.call("b2rl_nstep_dqn_update", self.gate, _lib.ptr(self.states), _lib.ptr(self.actions), _lib.ptr(self.rm[0]),
+                  _lib.ptr(self.rm[1]), self.T, self.N, *self._dims, self._flat, _lib.ptr(self.target), int(bool(sync_target)),
+                  _lib.ptr(o.s1), _lib.ptr(o.s2), _lib.ptr(o.step_dev), self._off, float(o.lr), float(o.alpha), float(o.eps),
+                  int(o.centered), float(c.discount), float(c.gradient_clip), _lib.ptr(loss), _lib.stream())
         return loss

@@ -9,6 +9,9 @@
 //   b2rl_a2c_update       the rest of step() as ONE launch of one block: forward of all (T + 1) N rows, GAE, the objective,
 //                         backward, clip_grad_norm_, RMSprop on the FlatOptimizer arena (a2c_sequence.inc).  The network is
 //                         5-12 k parameters over 25-100 rows: the eager form is several hundred launches of a few microseconds.
+//   b2rl_nstep_dqn_*      NStepDQNAgent.step() (NStepDQN_agent.py:26-67) for a VanillaNet on a two-layer FCBody the same way: an
+//                         actor step with epsilon-greedy on Philox uniforms, and one update launch (nstep_sequence.inc) that also
+//                         does the rollout's target sync.
 //
 // sm_90a only.
 #include "common.cuh"
@@ -97,6 +100,89 @@ __global__ void __launch_bounds__(A2C_ACT_NT, 1) a2c_actor_kernel(const __grid_c
   if (tid == 0 && !a.given) *a.counter = ctr0 + (int64_t)a.N * (HEAD == CAT ? 1 : A);
 }
 
+// ------------------------------------------------------------------------------------------------ n-step Q (NStepDQN_agent.py)
+constexpr uint64_t NSTEP_PHILOX_STREAM = 17;
+
+template <int GATE>
+__global__ void __launch_bounds__(A2C_NT, 1) nstep_dqn_update_kernel(const __grid_constant__ b2rl_a2c::NStepArgs q) {
+  using namespace b2rl_a2c;
+  pdl_sync();
+  extern __shared__ __align__(16) float a2c_smem[];
+  const A2cArgs& a = q.a;
+  A2cShared S;
+  a2c_carve<Q, true>(S, a2c_smem, a.net.D, a.net.H1, a.net.H2, a.net.A, (a.T + 1) * a.N, a.T * a.N);
+  const int NT = A2C_NT;
+#define A2C_PHASE(...) { const int tid = threadIdx.x; __VA_ARGS__; } __syncthreads();
+#include "nstep_sequence.inc"
+#undef A2C_PHASE
+}
+
+// epsilon-greedy on the actor step's q (torch_utils.py:51-58 with the device's Philox stream): per row two uniforms, the dice
+// u0 < epsilon and the random action min(floor(u1 A), A - 1); otherwise the first index of the maximum, as np.argmax
+template <int GATE>
+__global__ void __launch_bounds__(A2C_ACT_NT, 1) nstep_dqn_actor_kernel(const __grid_constant__ A2cActorArgs a, float epsilon) {
+  using namespace b2rl_a2c;
+  pdl_sync();
+  extern __shared__ __align__(16) float a2c_smem[];
+  A2cShared S;
+  a2c_carve<Q, true>(S, a2c_smem, a.net.D, a.net.H1, a.net.H2, a.net.A, a.N, 0);
+  const int tid = threadIdx.x, NT = A2C_ACT_NT, D = a.net.D, A = a.net.A;
+  const int64_t ctr0 = *a.counter;
+  // the forward of a2c_actor_kernel (not shared through a helper: that changes the A2C kernels' instruction schedule)
+  ph_load_weights<Q, true>(S, a.net, true, tid, NT);
+  for (int e = tid; e < a.N * D; e += NT) {
+    const int n = e / D, k = e - n * D;
+    const float x = (float)(a.scale * a.obs[e]);
+    S.x[n * S.ldx + k] = x;
+    a.state_out[e] = x;
+  }
+  __syncthreads();
+  ph_fwd1<Q, true, GATE>(S, a.net, true, tid, NT);
+  __syncthreads();
+  ph_fwd2<Q, true, GATE>(S, a.net, true, tid, NT);
+  __syncthreads();
+  ph_heads<Q, true>(S, a.net, true, tid, NT);
+  __syncthreads();
+  for (int n = tid; n < a.N; n += NT) {
+    if (a.given) {
+      a.action_out[n] = a.given[n];
+      continue;
+    }
+    const uint64_t c = (uint64_t)(ctr0 + 2 * (int64_t)n);
+    int pick;
+    if (Philox::u24(a.seed, c, NSTEP_PHILOX_STREAM) < epsilon) {
+      pick = min((int)(Philox::u24(a.seed, c + 1, NSTEP_PHILOX_STREAM) * (float)A), A - 1);
+    } else {
+      const float* z = S.z + n * S.lda;
+      pick = 0;
+      for (int j = 1; j < A; ++j)
+        if (z[j] > z[pick]) pick = j;
+    }
+    a.action_out[n] = (float)pick;
+  }
+  if (tid == 0 && !a.given) *a.counter = ctr0 + 2 * (int64_t)a.N;
+}
+
+template <int GATE>
+static void nstep_update_launch(const b2rl_a2c::NStepArgs& q, size_t smem, cudaStream_t st) {
+  static size_t attr = 0;
+  if (smem > attr) {
+    cudaFuncSetAttribute(nstep_dqn_update_kernel<GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    attr = smem;
+  }
+  launch_pdl(nstep_dqn_update_kernel<GATE>, dim3(1), dim3(A2C_NT), smem, st, q);
+}
+
+template <int GATE>
+static void nstep_actor_launch(const A2cActorArgs& a, float epsilon, size_t smem, cudaStream_t st) {
+  static size_t attr = 0;
+  if (smem > attr) {
+    cudaFuncSetAttribute(nstep_dqn_actor_kernel<GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    attr = smem;
+  }
+  launch_pdl(nstep_dqn_actor_kernel<GATE>, dim3(1), dim3(A2C_ACT_NT), smem, st, a, epsilon);
+}
+
 // the instantiated configurations: (CAT, shared trunk) and (GAUSS, separate trunks), each with a tanh or ReLU gate
 template <template <int, bool, int> class F, typename... Args>
 static bool a2c_dispatch(int head, int shared, int gate, Args&&... args) {
@@ -155,7 +241,7 @@ using namespace b2rl;
 static b2rl_a2c::A2cNet a2c_net(float* flat, const int32_t* off, int head, int shared, int D, int H1, int H2, int A) {
   b2rl_a2c::A2cNet net;
   net.flat = flat;
-  const int nt = 4 * (shared ? 1 : 2) + 4 + (head == 1 ? 1 : 0);
+  const int nt = head == b2rl_a2c::Q ? b2rl_a2c::A2cKind<b2rl_a2c::Q, true>::ntensors : 4 * (shared ? 1 : 2) + 4 + (head == 1 ? 1 : 0);
   for (int i = 0; i < b2rl_a2c::A2C_MAX_TENSORS; ++i) net.off[i] = i < nt ? off[i] : 0;
   net.D = D; net.H1 = H1; net.H2 = H2; net.A = A;
   return net;
@@ -204,4 +290,66 @@ extern "C" int b2rl_a2c_update(int32_t head, int32_t shared, int32_t gate, const
   B2RL_REQUIRE(smem > 0 && smem <= 227 * 1024, "rollout / network too large for the shared memory of one SM (b2rl_a2c_smem_bytes)");
   a2c_dispatch<UpdateLaunch>(head, shared, gate, a, smem, (cudaStream_t)stream);
   return check_launch("b2rl_a2c_update");
+}
+
+// ------------------------------------------------------------------------------------------------ n-step Q entry points
+#define NSTEP_CHECK_NET()                                                                                                    \
+  B2RL_REQUIRE(flat && off, "null pointer");                                                                                 \
+  B2RL_REQUIRE(gate == 0 || gate == 1, "gate must be 0 (tanh) or 1 (relu)");                                                 \
+  B2RL_REQUIRE(D > 0 && D <= 256 && H1 > 0 && H1 <= 128 && H2 > 0 && H2 <= 128 && A >= 2 && A <= 32,                         \
+               "shape limits: D <= 256, hidden <= 128, 2 <= A <= 32")
+
+static size_t nstep_bytes(int D, int H1, int H2, int A, int R, int M) {
+  b2rl_a2c::A2cShared probe;
+  return b2rl_a2c::a2c_carve<b2rl_a2c::Q, true>(probe, reinterpret_cast<float*>(uintptr_t(4096)), D, H1, H2, A, R, M) *
+         sizeof(float);
+}
+
+// dynamic shared memory of the n-step Q update for these sizes (the caller checks it against the 227 KB of one SM)
+extern "C" int64_t b2rl_nstep_dqn_smem_bytes(int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, int32_t T) {
+  if (D <= 0 || H1 <= 0 || H2 <= 0 || A <= 0 || N <= 0 || T <= 0) return 0;
+  return (int64_t)nstep_bytes(D, H1, H2, A, (T + 1) * N, T * N);
+}
+
+extern "C" int b2rl_nstep_dqn_actor_step(int32_t gate, const double* obs, double obs_scale, const float* flat, const int32_t* off,
+                                         int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, float epsilon,
+                                         float* state_out, float* action_out, const float* given_action, uint64_t seed,
+                                         int64_t* counter, void* stream) {
+  NSTEP_CHECK_NET();
+  B2RL_REQUIRE(obs && state_out && action_out && counter, "null pointer");
+  B2RL_REQUIRE(N > 0 && N <= 1024, "N must be in [1, 1024]");
+  A2cActorArgs a;
+  a.net = a2c_net(const_cast<float*>(flat), off, b2rl_a2c::Q, 1, D, H1, H2, A);
+  a.obs = obs; a.scale = obs_scale; a.N = N; a.state_out = state_out; a.action_out = action_out; a.given = given_action;
+  a.seed = seed; a.counter = counter;
+  const size_t smem = nstep_bytes(D, H1, H2, A, N, 0);
+  B2RL_REQUIRE(smem <= 227 * 1024, "network / worker count too large for the shared memory of one SM");
+  if (gate == b2rl_a2c::TANH) nstep_actor_launch<b2rl_a2c::TANH>(a, epsilon, smem, (cudaStream_t)stream);
+  else nstep_actor_launch<b2rl_a2c::RELU>(a, epsilon, smem, (cudaStream_t)stream);
+  return check_launch("b2rl_nstep_dqn_actor_step");
+}
+
+extern "C" int b2rl_nstep_dqn_update(int32_t gate, const float* states, const float* actions, const float* reward,
+                                     const float* mask, int32_t T, int32_t N, int32_t D, int32_t H1, int32_t H2, int32_t A,
+                                     float* flat, float* target, int32_t sync_target, float* square_avg, float* grad_avg,
+                                     int64_t* step, const int32_t* off, float lr, float alpha, float eps, int32_t centered,
+                                     float discount, float max_norm, float* loss, void* stream) {
+  NSTEP_CHECK_NET();
+  B2RL_REQUIRE(states && actions && reward && mask && target && square_avg && step && loss && (grad_avg || !centered),
+               "null pointer");
+  B2RL_REQUIRE(T > 0 && N > 0, "bad T / N");
+  b2rl_a2c::NStepArgs q = {};
+  b2rl_a2c::A2cArgs& a = q.a;
+  a.net = a2c_net(flat, off, b2rl_a2c::Q, 1, D, H1, H2, A);
+  a.state = states; a.action = actions; a.reward = reward; a.mask = mask; a.T = T; a.N = N;
+  a.sq = square_avg; a.ga = grad_avg; a.step = step;
+  a.lr = lr; a.alpha = alpha; a.eps = eps; a.centered = centered;
+  a.discount = discount; a.max_norm = max_norm; a.loss = loss;
+  q.target = target; q.sync = sync_target != 0;
+  const size_t smem = (size_t)b2rl_nstep_dqn_smem_bytes(D, H1, H2, A, N, T);
+  B2RL_REQUIRE(smem > 0 && smem <= 227 * 1024,
+               "rollout / network too large for the shared memory of one SM (b2rl_nstep_dqn_smem_bytes)");
+  if (gate == b2rl_a2c::TANH) nstep_update_launch<b2rl_a2c::TANH>(q, smem, (cudaStream_t)stream);
+  else nstep_update_launch<b2rl_a2c::RELU>(q, smem, (cudaStream_t)stream);
+  return check_launch("b2rl_nstep_dqn_update");
 }

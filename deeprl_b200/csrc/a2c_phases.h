@@ -12,10 +12,13 @@
 //             HEAD = GAUSS: GaussianActorCriticNet with DummyBody phi, FCBody actor / critic bodies (separate trunks):
 //                           mean = tanh(fc_action(actor_body(x))), v = fc_critic(critic_body(x)),
 //                           std = softplus(std_param)                                                  (network_heads.py:173-214)
+//             HEAD = Q:     VanillaNet on an FCBody (SHARED trunk), no critic: q = fc_head(phi)    (network_heads.py:11-21)
 //             trunks: two Linear layers, each followed by GATE (tanh or ReLU)
 //   update    forward of all (T + 1) N rows (row block T: the bootstrap value, A2C_agent.py:38-41); GAE (:43-53, the arithmetic of
 //             gae_seq_kernel mode 0); -mean(log pi * adv) - w_ent mean(entropy) + w_v 0.5 mean((ret - v)^2) (:55-62); backward;
 //             clip_grad_norm_ (:63); RMSprop on the FlatOptimizer arena (:64)
+//   n-step Q  (NStepDQN_agent.py:26-67, nstep_sequence.inc) forward of the T N rollout rows, the target network on row block T
+//             and its max over actions (:56-57), the return scan (:58-60), 0.5 mean((q[a] - ret)^2) (:63), backward, clip, RMSprop
 #pragma once
 #include <math.h>
 #include <stddef.h>
@@ -39,7 +42,7 @@
 
 namespace b2rl_a2c {
 
-enum { CAT = 0, GAUSS = 1 };             // head kind
+enum { CAT = 0, GAUSS = 1, Q = 2 };      // head kind
 enum { TANH = 0, RELU = 1, LINEAR = 2 }; // gate of a layer
 constexpr int A2C_MAX_TENSORS = 13;      // two trunks x (w1 b1 w2 b2) + fc_action w b + fc_critic w b + std
 constexpr int A2C_CHUNK = 64;            // gradient elements per partial sum of the global norm
@@ -64,13 +67,20 @@ struct A2cArgs {
   float* loss;                           // device scalar: the objective
 };
 
+// the n-step Q update's arguments besides A2cArgs (whose tau, use_gae, ent_w and vw it does not read)
+struct NStepArgs {
+  A2cArgs a;
+  float* target;                         // the target network's arena: the layout of a.net.flat, the same offsets
+  int sync;                              // copy the online arena into it first, and bootstrap from the online weights
+};
+
 // ------------------------------------------------------------------------------------------------ layout
-// Tensor order: trunk t (t < ntr) w1 b1 w2 b2 at 4t..4t+3, then fc_action w b, fc_critic w b, std (GAUSS only).  The trunk
-// serving the actor head is trunk 0, the critic's is trunk ntr - 1.
+// Tensor order: trunk t (t < ntr) w1 b1 w2 b2 at 4t..4t+3, then fc_action w b (Q: fc_head w b), fc_critic w b (not Q), std
+// (GAUSS only).  The trunk serving the actor head is trunk 0, the critic's is trunk ntr - 1.
 template <int HEAD, bool SHARED> struct A2cKind {
   static constexpr int ntr = SHARED ? 1 : 2;
   static constexpr int fa = 4 * ntr, ba = fa + 1, fc = fa + 2, bc = fa + 3, sd = fa + 4;
-  static constexpr int ntensors = 4 * ntr + 4 + (HEAD == GAUSS ? 1 : 0);
+  static constexpr int ntensors = HEAD == Q ? 4 * ntr + 2 : 4 * ntr + 4 + (HEAD == GAUSS ? 1 : 0);
   static constexpr int critic_trunk = ntr - 1;
 };
 
@@ -112,7 +122,8 @@ struct A2cShared {
   float* x;                              // [R][ldx] states
   float* h;                              // trunk t, layer l output at h + (2t + l) * hstride, [R][ldh]; the backward overwrites
                                          // them in place with the pre-activation gradients
-  float *z, *dz;                         // [R][lda] logits (CAT) / mean (GAUSS); gradient w.r.t. the logits / pre-tanh mean
+  float *z, *dz;                         // [R][lda] logits (CAT) / mean (GAUSS) / q (Q); gradient w.r.t. the logits /
+                                         // pre-tanh mean / q
   float *v, *dv, *adv, *ret, *logp, *ent, *lse;   // [R]
   float* red;                            // [3][M] per-row loss terms
   float* part;                           // [nchunks] sums of squares of the gradient
@@ -122,11 +133,12 @@ struct A2cShared {
 };
 
 // carve the shared block for R forward rows and M = T N loss rows (M = 0: actor step, no gradients); returns the floats used.
-// base may be a dummy when only the size is wanted.
+// The Q update's online forward covers only the M rollout rows (S.R = M): rows M..R-1 of h and z hold the target network's
+// forward of the bootstrap states.  base may be a dummy when only the size is wanted.
 template <int HEAD, bool SHARED>
 A2C_HD size_t a2c_carve(A2cShared& S, float* base, int D, int H1, int H2, int A, int R, int M) {
   using K = A2cKind<HEAD, SHARED>;
-  const bool upd = M > 0;
+  const bool upd = M > 0, critic = HEAD != Q;
   const TensorDesc last = a2c_tensor(K::ntensors - 1, K::ntr, D, H1, H2, A);
   const size_t wsize = (size_t)last.woff + (size_t)last.rows * last.ld;
   int nchunks = 0;
@@ -138,28 +150,28 @@ A2C_HD size_t a2c_carve(A2cShared& S, float* base, int D, int H1, int H2, int A,
   S.ldh = a2c_odd(H1 > H2 ? H1 : H2);
   S.lda = a2c_odd(A);
   S.hstride = R * S.ldh;
-  S.R = R;
+  S.R = critic || !upd ? R : M;
   S.M = M;
   S.nchunks = nchunks;
   size_t off = 0;
 #define A2C_TAKE(n) (base + (off += ((size_t)(n) + 3) / 4 * 4) - ((size_t)(n) + 3) / 4 * 4)
   S.W = A2C_TAKE(wsize);
   S.G = upd ? A2C_TAKE(wsize) : nullptr;
-  S.x = A2C_TAKE((size_t)R * S.ldx);
+  S.x = A2C_TAKE((size_t)S.R * S.ldx);
   S.h = A2C_TAKE((size_t)2 * K::ntr * S.hstride);
   S.z = A2C_TAKE((size_t)R * S.lda);
   S.dz = upd ? A2C_TAKE((size_t)M * S.lda) : nullptr;
-  S.v = A2C_TAKE(R);
-  S.dv = upd ? A2C_TAKE(M) : nullptr;
-  S.adv = upd ? A2C_TAKE(M) : nullptr;
+  S.v = critic ? A2C_TAKE(R) : nullptr;
+  S.dv = upd && critic ? A2C_TAKE(M) : nullptr;
+  S.adv = upd && critic ? A2C_TAKE(M) : nullptr;
   S.ret = upd ? A2C_TAKE(M) : nullptr;
-  S.logp = upd ? A2C_TAKE(M) : nullptr;
-  S.ent = upd ? A2C_TAKE(M) : nullptr;
-  S.lse = upd ? A2C_TAKE(M) : nullptr;
-  S.red = upd ? A2C_TAKE((size_t)3 * M) : nullptr;
+  S.logp = upd && critic ? A2C_TAKE(M) : nullptr;
+  S.ent = upd && critic ? A2C_TAKE(M) : nullptr;
+  S.lse = upd && critic ? A2C_TAKE(M) : nullptr;
+  S.red = upd ? A2C_TAKE((size_t)(critic ? 3 : 1) * M) : nullptr;
   S.part = upd ? A2C_TAKE(nchunks) : nullptr;
-  S.sdv = A2C_TAKE(A);
-  S.lsd = A2C_TAKE(A);
+  S.sdv = critic ? A2C_TAKE(A) : nullptr;
+  S.lsd = critic ? A2C_TAKE(A) : nullptr;
   S.scal = A2C_TAKE(4);
 #undef A2C_TAKE
   return off;
@@ -291,7 +303,7 @@ A2C_FN void ph_fwd2(A2cShared& S, const A2cNet& net, bool actor_only, int tid, i
   }
 }
 
-// heads: logits / mean = tanh(fc_action(.)), v = fc_critic(.) (not in the actor step), softplus(std) (GAUSS)
+// heads: logits / mean = tanh(fc_action(.)) / q = fc_head(.), v = fc_critic(.) (not in the actor step), softplus(std) (GAUSS)
 template <int HEAD, bool SHARED>
 A2C_FN void ph_heads(A2cShared& S, const A2cNet& net, bool actor_only, int tid, int NT) {
   using K = A2cKind<HEAD, SHARED>;
@@ -299,7 +311,7 @@ A2C_FN void ph_heads(A2cShared& S, const A2cNet& net, bool actor_only, int tid, 
   const TensorDesc ba = a2c_tensor(K::ba, K::ntr, net.D, net.H1, net.H2, net.A);
   dense_fwd<HEAD == GAUSS ? TANH : LINEAR>(a2c_h(S, 0, 1), S.ldh, S.W + fa.woff, fa.ld, S.W + ba.woff, S.z, S.lda, S.R, net.H2,
                                            net.A, tid, NT);
-  if (!actor_only) {
+  if (!actor_only && HEAD != Q) {
     const TensorDesc fc = a2c_tensor(K::fc, K::ntr, net.D, net.H1, net.H2, net.A);
     const TensorDesc bc = a2c_tensor(K::bc, K::ntr, net.D, net.H1, net.H2, net.A);
     dense_fwd<LINEAR>(a2c_h(S, K::critic_trunk, 1), S.ldh, S.W + fc.woff, fc.ld, S.W + bc.woff, S.v, 1, S.R, net.H2, 1, tid, NT);
@@ -398,7 +410,7 @@ A2C_FN void ph_loss_grad(A2cShared& S, const A2cArgs& a, int tid, int NT) {
   }
 }
 
-// the heads' parameter gradients (fc_action, fc_critic, std) and the objective (one thread)
+// the heads' parameter gradients (fc_action / fc_head, fc_critic, std) and the objective (one thread)
 template <int HEAD, bool SHARED>
 A2C_FN void ph_head_wgrad(A2cShared& S, const A2cArgs& a, int tid, int NT) {
   using K = A2cKind<HEAD, SHARED>;
@@ -409,6 +421,10 @@ A2C_FN void ph_head_wgrad(A2cShared& S, const A2cArgs& a, int tid, int NT) {
   const TensorDesc fc = a2c_tensor(K::fc, K::ntr, net.D, net.H1, net.H2, A);
   const TensorDesc bc = a2c_tensor(K::bc, K::ntr, net.D, net.H1, net.H2, A);
   dense_wgrad(S.dz, S.lda, a2c_h(S, 0, 1), S.ldh, S.G + fa.woff, fa.ld, S.G + ba.woff, M, A, net.H2, tid, NT);
+  if (HEAD == Q) {
+    if (tid == NT - 1) S.scal[0] = 0.5f * (sum4(S.red, M) * (1.0f / (float)M));   // NStepDQN_agent.py:63
+    return;
+  }
   dense_wgrad(S.dv, 1, a2c_h(S, K::critic_trunk, 1), S.ldh, S.G + fc.woff, fc.ld, S.G + bc.woff, M, 1, net.H2, tid, NT);
   if (HEAD == GAUSS) {                                  // d / d std_param: summed over rows, then through softplus
     const TensorDesc sd = a2c_tensor(K::sd, K::ntr, net.D, net.H1, net.H2, A);
@@ -439,7 +455,9 @@ A2C_FN void ph_bwd2(A2cShared& S, const A2cArgs& a, int tid, int NT) {
   const TensorDesc fa = a2c_tensor(K::fa, K::ntr, net.D, net.H1, net.H2, net.A);
   const TensorDesc fc = a2c_tensor(K::fc, K::ntr, net.D, net.H1, net.H2, net.A);
   float* h0 = a2c_h(S, 0, 1);
-  if (SHARED) {
+  if (HEAD == Q) {
+    dense_bwd<GATE>(S.dz, S.lda, S.W + fa.woff, fa.ld, net.A, nullptr, 0, nullptr, 0, 0, h0, h0, S.ldh, S.M, net.H2, tid, NT);
+  } else if (SHARED) {
     dense_bwd<GATE>(S.dz, S.lda, S.W + fa.woff, fa.ld, net.A, S.dv, 1, S.W + fc.woff, fc.ld, 1, h0, h0, S.ldh, S.M, net.H2, tid, NT);
   } else {
     float* h1 = a2c_h(S, 1, 1);
@@ -528,6 +546,69 @@ A2C_FN void ph_rmsprop(A2cShared& S, const A2cArgs& a, int tid, int NT) {
   if (tid == 0) {
     *a.step += 1;
     *a.loss = S.scal[0];
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ phases (n-step Q)
+// P0: ph_load, and the target sync (NStepDQN_agent.py:48-50): the online parameters do not change during a rollout, so a sync at
+// any of its env steps is a copy of the arena as it is before this update
+A2C_FN void ph_nstep_load(A2cShared& S, const NStepArgs& q, int tid, int NT) {
+  using K = A2cKind<Q, true>;
+  ph_load<Q, true>(S, q.a, tid, NT);
+  if (!q.sync) return;
+  const A2cNet& net = q.a.net;
+  for (int i = 0; i < K::ntensors; ++i) {
+    const TensorDesc d = a2c_tensor(i, K::ntr, net.D, net.H1, net.H2, net.A);
+    for (int e = tid; e < d.rows * d.cols; e += NT) q.target[net.off[i] + e] = net.flat[net.off[i] + e];
+  }
+}
+
+// layer l (0, 1: the trunk, 2: fc_head) of the target network on the N bootstrap states (row block T), into rows M.. of h / z.
+// Its weights are read from the arena in global memory (rows of `cols` floats); after a sync they are the online ones, which
+// the arena still holds until the last phase.  Runs in the same phase as the online forward's layer l (disjoint rows).
+template <int GATE>
+A2C_FN void ph_boot(A2cShared& S, const NStepArgs& q, int l, int tid, int NT) {
+  using K = A2cKind<Q, true>;
+  const A2cNet& net = q.a.net;
+  const float* w = q.sync ? net.flat : q.target;
+  const int N = q.a.N;
+  const size_t rh = (size_t)S.M * S.ldh;
+  if (l == 0)
+    dense_fwd<GATE>(q.a.state + (size_t)S.M * net.D, net.D, w + net.off[0], net.D, w + net.off[1], a2c_h(S, 0, 0) + rh, S.ldh,
+                    N, net.D, net.H1, tid, NT);
+  else if (l == 1)
+    dense_fwd<GATE>(a2c_h(S, 0, 0) + rh, S.ldh, w + net.off[2], net.H1, w + net.off[3], a2c_h(S, 0, 1) + rh, S.ldh, N, net.H1,
+                    net.H2, tid, NT);
+  else
+    dense_fwd<LINEAR>(a2c_h(S, 0, 1) + rh, S.ldh, w + net.off[K::fa], net.H2, w + net.off[K::ba], S.z + (size_t)S.M * S.lda,
+                      S.lda, N, net.H2, net.A, tid, NT);
+}
+
+// per worker (one thread each): the bootstrap max_a q_target(s_T) (:56-57) and the return scan ret = r + (discount mask) ret
+// (:58-60), the arithmetic of ph_rows' ret (gae_seq_kernel mode 0)
+A2C_FN void ph_nstep_returns(A2cShared& S, const A2cArgs& a, int tid, int NT) {
+  const int N = a.N, T = a.T, A = a.net.A;
+  for (int i = tid; i < N; i += NT) {
+    const float* zb = S.z + (size_t)(S.M + i) * S.lda;
+    float ret = zb[0];
+    for (int j = 1; j < A; ++j) ret = fmaxf(ret, zb[j]);
+    for (int t = T - 1; t >= 0; --t) {
+      const int o = t * N + i;
+      ret = A2C_ADD(a.reward[o], A2C_MUL(A2C_MUL(a.discount, a.mask[o]), ret));
+      S.ret[o] = ret;
+    }
+  }
+}
+
+// e_n = q[n][a_n] - ret_n, e_n^2 for the objective, and d(0.5 mean(e^2)) / dq[n][j] = (j == a_n) e_n / M
+A2C_FN void ph_nstep_loss_grad(A2cShared& S, const A2cArgs& a, int tid, int NT) {
+  const int M = S.M, A = a.net.A;
+  const float invM = 1.0f / (float)M;
+  for (int e = tid; e < M * A; e += NT) {
+    const int n = e / A, j = e - n * A, an = (int)a.action[n];
+    const float err = A2C_SUB(S.z[(size_t)n * S.lda + an], S.ret[n]);
+    S.dz[(size_t)n * S.lda + j] = j == an ? A2C_MUL(err, invM) : 0.0f;
+    if (j == 0) S.red[n] = A2C_MUL(err, err);
   }
 }
 

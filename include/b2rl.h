@@ -457,6 +457,25 @@ int b2rl_a2c_update(int32_t head, int32_t shared, int32_t gate, const float* sta
                     int32_t centered, float discount, float tau, int32_t use_gae, float entropy_weight,
                     float value_loss_weight, float max_norm, float* loss, void* stream);
 
+/* NStepDQNAgent.step() (NStepDQN_agent.py:26-67) on the device for a VanillaNet on a two-layer FCBody (gate 0 = tanh, 1 = ReLU).
+ * flat: the FlatOptimizer arena; off (host, int32): arena offset of w1 b1 w2 b2 fc_head.w fc_head.b.
+ * smem_bytes: dynamic shared memory of the update for a rollout of T steps of N workers; it must fit the 227 KB of one SM.
+ * actor_step: state_out = (float)(obs_scale * obs) (RescaleNormalizer), q = net(state) and per row epsilon-greedy on two Philox
+ *   uniforms: u0 < epsilon draws min(floor(u1 * A), A - 1), otherwise the first index of the largest q; action_out [N] (as a
+ *   float).  *counter (device) advances by 2 N.  given_action != NULL: written through, nothing drawn, counter unchanged.
+ * update: forward of states [T][N][D], bootstrap max_a q_target(states[T]), ret = r + discount * mask * ret backwards over T,
+ *   0.5 mean((q[a] - ret)^2) into *loss (device), its gradient, clip_grad_norm_(max_norm) and RMSprop on flat / square_avg /
+ *   grad_avg; *step += 1.  target: the target network's arena (same offsets).  sync_target != 0: target = flat (before the
+ *   RMSprop step) first, and the bootstrap uses those weights. */
+int64_t b2rl_nstep_dqn_smem_bytes(int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, int32_t T);
+int b2rl_nstep_dqn_actor_step(int32_t gate, const double* obs, double obs_scale, const float* flat, const int32_t* off, int32_t D,
+                              int32_t H1, int32_t H2, int32_t A, int32_t N, float epsilon, float* state_out, float* action_out,
+                              const float* given_action, uint64_t seed, int64_t* counter, void* stream);
+int b2rl_nstep_dqn_update(int32_t gate, const float* states, const float* actions, const float* reward, const float* mask,
+                          int32_t T, int32_t N, int32_t D, int32_t H1, int32_t H2, int32_t A, float* flat, float* target,
+                          int32_t sync_target, float* square_avg, float* grad_avg, int64_t* step, const int32_t* off, float lr,
+                          float alpha, float eps, int32_t centered, float discount, float max_norm, float* loss, void* stream);
+
 int b2rl_ipc_alloc(int64_t bytes, void** out);
 int b2rl_ipc_get_handle(void* ptr, void* handle_out);
 int b2rl_ipc_open_handle(const void* handle, void** out);

@@ -1,6 +1,7 @@
-"""A2C steps per second of the two feature launchers' configurations, eager (the torch path of A2CAgent.step) against
-``config.device_a2c`` (one actor-step launch per env step, one update launch per rollout: csrc/a2c.cu), in one process on one
-card, the two alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
+"""Agent steps per second of the rollout launchers' configurations, eager (the torch path of ``step()``) against the launcher's
+device flag (one actor-step launch per env step, one update launch per rollout: csrc/a2c.cu) -- ``config.device_a2c`` for
+A2CAgent (a2c_feature, a2c_continuous), ``config.device_nstep_dqn`` for NStepDQNAgent (n_step_dqn_feature) -- in one process on
+one card, the two alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
 left to the learner is visible.  Prints the card's name and power limit with the numbers.
 
     python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--out DIR]
@@ -18,7 +19,9 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CONFIGS = [("a2c_feature", "CartPole-v0"), ("a2c_continuous", "SyntheticCheetah-v0")]
+# (launcher, game, its device flag, the agent's name in the output keys)
+CONFIGS = [("a2c_feature", "CartPole-v0", "device_a2c", "a2c"), ("a2c_continuous", "SyntheticCheetah-v0", "device_a2c", "a2c"),
+           ("n_step_dqn_feature", "CartPole-v0", "device_nstep_dqn", "nstep_dqn")]
 
 
 def card():
@@ -30,13 +33,13 @@ def card():
     return "%s | nvidia-smi: %s" % (torch.cuda.get_device_name(0), q)
 
 
-def make_agent(name, game, device_a2c):
+def make_agent(name, game, flag, on):
     import examples
     got = []
     run_steps = examples.run_steps
     examples.run_steps = got.append
     try:
-        getattr(examples, name)(game=game, device_a2c=device_a2c)
+        getattr(examples, name)(game=game, **{flag: on})
     finally:
         examples.run_steps = run_steps
     return got[0]
@@ -52,10 +55,10 @@ def timed(agent, steps):
 
 
 def env_only(agent, steps):
-    """task.step alone, T * steps times, with the actions of one draw (what the host envs cost per A2C step)."""
-    from deeprl_b200 import CategoricalActorCriticNet
+    """task.step alone, T * steps times, with the actions of one draw (what the host envs cost per agent step)."""
+    from deeprl_b200 import CategoricalActorCriticNet, VanillaNet
     c = agent.config
-    a = (np.zeros(c.num_workers, dtype=np.int64) if isinstance(agent.network, CategoricalActorCriticNet)
+    a = (np.zeros(c.num_workers, dtype=np.int64) if isinstance(agent.network, (CategoricalActorCriticNet, VanillaNet))
          else np.zeros((c.num_workers, c.action_dim), dtype=np.float32))
     t0 = time.perf_counter()
     for _ in range(steps * c.rollout_length):
@@ -77,8 +80,8 @@ def main():
     rl.random_seed(0)
     result = dict(card=card(), steps_per_round=args.steps, rounds=args.rounds, configs={})
     print(result["card"])
-    for name, game in CONFIGS:
-        agents = {"eager": make_agent(name, game, False), "device_a2c": make_agent(name, game, True)}
+    for name, game, flag, unit in CONFIGS:
+        agents = {"eager": make_agent(name, game, flag, False), flag: make_agent(name, game, flag, True)}
         for ag in agents.values():
             timed(ag, args.warmup)
         rates = {k: [] for k in agents}
@@ -89,14 +92,14 @@ def main():
         c = agents["eager"].config
         med = {k: float(np.median(v)) for k, v in rates.items()}
         learner_ms = {k: 1e3 / med[k] - 1e3 / env for k in med}
-        row = dict(game=game, num_workers=c.num_workers, rollout_length=c.rollout_length, a2c_steps_per_s=rates,
-                   median_a2c_steps_per_s=med, speedup=med["device_a2c"] / med["eager"], env_only_a2c_steps_per_s=env,
-                   ms_per_step_besides_envs=learner_ms)
+        row = {"game": game, "num_workers": c.num_workers, "rollout_length": c.rollout_length, unit + "_steps_per_s": rates,
+               "median_%s_steps_per_s" % unit: med, "speedup": med[flag] / med["eager"], "env_only_%s_steps_per_s" % unit: env,
+               "ms_per_step_besides_envs": learner_ms}
         result["configs"][name] = row
-        print("%-15s %-20s N=%d T=%d  eager %8.1f steps/s  device_a2c %8.1f steps/s  (x%.2f)  envs alone %8.1f steps/s;  "
-              "ms per step besides the envs: eager %.3f, device_a2c %.3f"
-              % (name, game, c.num_workers, c.rollout_length, med["eager"], med["device_a2c"], row["speedup"], env,
-                 learner_ms["eager"], learner_ms["device_a2c"]))
+        print("%-18s %-20s N=%d T=%d  eager %8.1f steps/s  %s %8.1f steps/s  (x%.2f)  envs alone %8.1f steps/s;  "
+              "ms per step besides the envs: eager %.3f, %s %.3f"
+              % (name, game, c.num_workers, c.rollout_length, med["eager"], flag, med[flag], row["speedup"], env,
+                 learner_ms["eager"], flag, learner_ms[flag]))
         for ag in agents.values():
             ag.close()
     print(json.dumps(result))
