@@ -316,7 +316,7 @@ class GraphedDQNLearner:
             self.replay.update_priorities((t.idx, r["priority"]))
         gphi = r["gphi"]
         nature_tc.mark("head")
-        nature_tc.PREMASKED[gphi.data_ptr()] = tail.db4  # already masked by relu(fc4); its column sums are in the tail's db4
+        nature_tc.premask(gphi, tail.db4)                # already masked by relu(fc4); its column sums are in the tail's db4
         with nature_tc.wgrad_stream(side), nature_tc.grad_sink(tail):
             phi.backward(gphi)
         self.loss.copy_(r["loss"])

@@ -138,6 +138,13 @@ def space_to_depth_weight(weight, block=4):
     return w.permute(0, 1, 3, 5, 2, 4).reshape(co, ci * block * block, 2, 2)
 
 
+def _fc4_relu_features(phi):
+    """True if ``phi`` is the live output of a wgmma NatureConvBody's fc4 ReLU (network/nature_tc.py): the head's backward
+    then applies that ReLU's mask and bias gradient itself.  Decided in the forward pass, while the features are alive."""
+    from . import nature_tc
+    return nature_tc.FUSED_BWD and nature_tc.is_relu_features(phi)
+
+
 class _NarrowHead(torch.autograd.Function):
     """VanillaNet / DuelingNet head on bf16 features (csrc/head.cu): 2 launches per update instead of ~12."""
 
@@ -151,6 +158,7 @@ class _NarrowHead(torch.autograd.Function):
                   _lib.ptr(q), _lib.stream())
         ctx.save_for_backward(phi)
         ctx.params = (wa, ba, wv, bv)
+        ctx.relu = _fc4_relu_features(phi)
         return q
 
     @staticmethod
@@ -170,7 +178,7 @@ class _NarrowHead(torch.autograd.Function):
             z = lambda p: None if p is None else torch.zeros_like(p, dtype=torch.float32)
             gwa, gba, gwv, gbv = z(wa), z(ba), z(wv), z(bv)
         from . import nature_tc
-        if nature_tc.FUSED_BWD and phi.data_ptr() in nature_tc.RELU_FEATURES:
+        if ctx.relu:
             # phi = relu(fc4(.)) of a wgmma NatureConvBody: its ReLU backward and bias gradient ride along (the body's
             # backward finds the column sums under the gradient's address and skips its own pass)
             sink = nature_tc.SINK               # persistent accumulator (re-zeroed by the tail's kernel A) or a fresh one
@@ -178,7 +186,7 @@ class _NarrowHead(torch.autograd.Function):
             _lib.call("b2rl_head_bwd_relu", _lib.ptr(gq), _lib.ptr(phi), _lib.ptr(wa.detach()),
                       _lib.ptr(None if wv is None else wv.detach()), B, K, A, _lib.ptr(gphi), _lib.ptr(gwa), _lib.ptr(gba),
                       _lib.ptr(gwv), _lib.ptr(gbv), _lib.ptr(colsum), _lib.stream())
-            nature_tc.PREMASKED[gphi.data_ptr()] = colsum
+            nature_tc.premask(gphi, colsum)
             nature_tc.mark("head_bwd")
         else:
             _lib.call("b2rl_head_bwd", _lib.ptr(gq), _lib.ptr(phi), _lib.ptr(wa.detach()),
@@ -215,6 +223,7 @@ class _DistHead(torch.autograd.Function):
         logits = gemm_bf16(phi, w16, bias=bias.detach(), out_dtype=torch.float32, block_n=64)
         ctx.dims = (A, N, bool(softmax))
         ctx.params = (weight, bias)
+        ctx.relu = _fc4_relu_features(phi)
         if softmax:
             prob = torch.empty((B, A, N), dtype=torch.float32, device=phi.device)
             logp = torch.empty((B, A, N), dtype=torch.float32, device=phi.device)
@@ -252,13 +261,12 @@ class _DistHead(torch.autograd.Function):
         # dphi = (g W) masked by relu(fc4) with fc4's bias gradient from the same epilogue
         gphi = torch.empty_like(phi)
         sink = nature_tc.SINK
-        relu = nature_tc.FUSED_BWD and phi.data_ptr() in nature_tc.RELU_FEATURES
-        if relu:
+        if ctx.relu:
             colsum = sink.db4 if (sink is not None and sink.db4.numel() == K) else torch.zeros(K, dtype=torch.float32, device=phi.device)
             e = _lib.bwd_epilogue(phi, colsum, 0, 0)               # dbias_mod 0: one bias gradient per feature column
             _lib.call("b2rl_gemm_bwd_bf16", _lib.ptr(gv), gv.stride(0), _lib.ptr(w16), 1, w16.stride(0), _lib.ptr(gphi), gphi.stride(0),
                       B, K, AN, 0, 0, 0, ctypes.byref(e), 128, _lib.stream())
-            nature_tc.PREMASKED[gphi.data_ptr()] = colsum
+            nature_tc.premask(gphi, colsum)
         else:
             gemm_bf16(gv, w16, a_major="k", b_major="mn", out=gphi, block_n=128)
         if inplace:

@@ -18,6 +18,7 @@ layout ([Cout, Cin, kh, kw], (c, h, w)-ordered fc4 columns) to the tap-major bf1
 import contextlib
 import ctypes
 import os
+import weakref
 
 import torch
 
@@ -49,8 +50,40 @@ def mark(name, stream=None):
 AFTER_DGRAD = None         # callable run once, on the current stream, right after the last dgrad GEMM of the backward pass was
                            # launched (the learner forks its late prefetch branch there: beside the weight-gradient tail)
 SINK = None                # network/tail.py NatureTail while ``grad_sink`` is active: backward hands it the GEMM-layout gradients
-RELU_FEATURES = set()      # data_ptr of feature tensors y4 = relu(fc4(.)) produced by nature_body (for head_bwd_relu)
-PREMASKED = {}             # data_ptr of a feature gradient already masked by head_bwd_relu -> its column sums (= db4)
+RELU_FEATURES = {}         # data_ptr -> weak reference to the feature tensor y4 = relu(fc4(.)) nature_body produced there
+PREMASKED = {}             # data_ptr of a feature gradient already masked by head_bwd_relu -> (that gradient, its column sums = db4)
+
+
+def mark_relu_features(y4):
+    """Record ``y4`` as the output of fc4's ReLU, so that a head on it may fold the ReLU backward into its own."""
+    if len(RELU_FEATURES) > 256:
+        for k in [k for k, r in RELU_FEATURES.items() if r() is None]:
+            del RELU_FEATURES[k]
+    RELU_FEATURES[y4.data_ptr()] = weakref.ref(y4)
+
+
+def is_relu_features(phi):
+    """True if ``phi`` lies at the address of a y4 that is still alive.  A live y4 keeps its memory, so ``phi`` is that
+    y4 (or a view of it); once y4 is freed, the allocator may hand its address to any other tensor."""
+    r = RELU_FEATURES.get(phi.data_ptr())
+    return r is not None and r() is not None
+
+
+def premask(gphi, db4):
+    """Record that ``gphi`` is already masked by relu(fc4) with its column sums in ``db4``: the body's backward then skips
+    its own mask / bias-gradient pass.  The entry holds ``gphi`` itself, so its address cannot be reused by another
+    gradient, and autograd cannot accumulate into it in place, before the body's backward takes the entry."""
+    if len(PREMASKED) >= 16:                    # entries nobody took (e.g. the gradient was summed with another one)
+        PREMASKED.pop(next(iter(PREMASKED)))
+    PREMASKED[gphi.data_ptr()] = (gphi, db4)
+
+
+def take_premasked(gy4):
+    """The column sums recorded by ``premask`` for this very gradient, or None (the entry is removed)."""
+    if gy4.dtype != _bf16 or not gy4.is_contiguous():
+        return None
+    e = PREMASKED.pop(gy4.data_ptr(), None)
+    return e[1] if e is not None and e[0].shape == gy4.shape else None
 
 
 class RingFrames:
@@ -116,7 +149,7 @@ def _backward_fused(ctx, gy4):
     x0m, x1, y2, y3, y4, w2d, w3d, w4p = ctx.saved_tensors
     B, dev = y4.shape[0], y4.device
     sink = _sink_for(ctx.params)
-    db4 = PREMASKED.pop(gy4.data_ptr(), None) if gy4.dtype == _bf16 and gy4.is_contiguous() else None
+    db4 = take_premasked(gy4)
     if db4 is not None:
         g4 = gy4                                                                        # masked + summed by b2rl_head_bwd_relu
     else:
@@ -477,9 +510,7 @@ def nature_body(body, x0, scale):
     y4 = _NatureBody.apply(x0, c1.weight, c1.bias, c2.weight, c2.bias, c3.weight, c3.bias, f4.weight, f4.bias,
                            float(scale), pk, companion)
     if FUSED_BWD:
-        if len(RELU_FEATURES) > 256:
-            RELU_FEATURES.clear()
-        RELU_FEATURES.add(y4.data_ptr())
+        mark_relu_features(y4)
     return y4
 
 
