@@ -7,9 +7,11 @@
 //                                  there too (and their atomic accumulators re-zeroed), and the sum of squares of every
 //                                  gradient element -- including the head's, which head_bwd already put in the arena --
 //                                  left as one partial per work unit.
-//   B  nature_fused_opt_kernel   : every CTA adds the unit partials in the same fixed order (the same bits in every CTA:
-//                                  no grid barrier, no second launch), derives the clip coefficient of
-//                                  torch.nn.utils.clip_grad_norm_, applies RMSprop (plain / centered) or Adam exactly as
+//   B  nature_fused_opt_kernel   : takes the clip coefficient of torch.nn.utils.clip_grad_norm_ from the norm scratch
+//                                  (what NatureTail.step does: kernel A's last CTA left it there, or b2rl_grad_norm after
+//                                  a multi-GPU all-reduce) or, given the unit partials, has every CTA add them in the same
+//                                  fixed order and derive it itself (the same bits in every CTA and as kernel A's: no grid
+//                                  barrier, no second launch), applies RMSprop (plain / centered) or Adam exactly as
 //                                  csrc/optim.cu does, re-zeroes the gradient it consumed, and writes the updated weights
 //                                  straight into the bf16 tap-major GEMM operands (forward + dgrad orientations) that the next
 //                                  update's wgmma kernels read -- the separate pack launch disappears as well.
