@@ -287,6 +287,23 @@ __global__ void __launch_bounds__(256) qr_loss_kernel(const float* __restrict__ 
   }
 }
 
+// Shape limits of the C51 / QR entry points.  Their dynamic shared memory is (3N + A) floats: 64 KiB at the limits, past the
+// 48 KiB a launch gets by default and well inside the 227 KiB per block of sm_90.  A request over 48 KiB raises the kernel's
+// limit to the largest accepted request (always the same value, so no call lowers it under a launch a captured graph holds).
+constexpr int DIST_MAX_N = 4096, DIST_MAX_A = 4096;
+constexpr size_t DIST_MAX_SMEM = (size_t)(3 * DIST_MAX_N + DIST_MAX_A) * sizeof(float);
+static_assert(DIST_MAX_SMEM + 1024 <= 227 * 1024, "C51 / QR shared memory at the shape limits exceeds sm_90's per-block limit");
+
+template <typename K>
+static int raise_dyn_smem(K kernel, size_t smem, const char* what) {
+  if (smem <= 48 * 1024) return B2RL_OK;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DIST_MAX_SMEM) != cudaSuccess) {
+    set_error("%s: cannot raise the dynamic shared-memory limit to %zu bytes", what, DIST_MAX_SMEM);
+    return B2RL_ERR_CUDA;
+  }
+  return B2RL_OK;
+}
+
 }  // namespace b2rl
 
 using namespace b2rl;
@@ -310,10 +327,11 @@ extern "C" int b2rl_c51_loss(const float* log_prob, const float* prob_next_targe
                              float alpha, float* kl_out, float* priority_out, float* loss_out, float* dlogp_out,
                              float* target_prob_out, int32_t* counter, const float* beta_dev, void* stream) {
   B2RL_REQUIRE(log_prob && prob_next_target && action && reward && mask && kl_out && counter, "null pointer");
-  B2RL_REQUIRE(B > 0 && A > 0 && N >= 2 && N <= 4096 && A <= 4096, "bad shape");
+  B2RL_REQUIRE(B > 0 && A > 0 && N >= 2 && N <= DIST_MAX_N && A <= DIST_MAX_A, "bad shape");
   const double start = (double)v_min, step = ((double)v_max - (double)v_min) / (double)(N - 1);
   const float delta_atom = (float)(((double)v_max - (double)v_min) / (double)(N - 1));   // CategoricalDQN_agent.py:46
-  size_t smem = (size_t)(3 * N + A) * sizeof(float);
+  const size_t smem = (size_t)(3 * N + A) * sizeof(float);
+  if (int rc = raise_dyn_smem(c51_loss_kernel, smem, "b2rl_c51_loss")) return rc;
   launch_pdl(c51_loss_kernel, dim3(B), dim3(64), smem, (cudaStream_t)stream, log_prob, prob_next_target, prob_next_online, action, reward,
                                                          mask, gamma_n, v_min, v_max, start, step, delta_atom, B, A, N,
                                                          is_prob, beta, eps, alpha, kl_out, priority_out, loss_out,
@@ -327,8 +345,9 @@ extern "C" int b2rl_qr_loss(const float* quantile, const float* quantile_next, c
                             int32_t* counter, const float* grad_weight, void* stream) {
   B2RL_REQUIRE(quantile && quantile_next && action && reward && mask, "null pointer");
   B2RL_REQUIRE((partial && counter) || dquant_out, "nothing to compute");
-  B2RL_REQUIRE(B > 0 && A > 0 && N > 0 && N <= 4096 && A <= 4096, "bad shape");
-  size_t smem = (size_t)(3 * N + A) * sizeof(float);
+  B2RL_REQUIRE(B > 0 && A > 0 && N > 0 && N <= DIST_MAX_N && A <= DIST_MAX_A, "bad shape");
+  const size_t smem = (size_t)(3 * N + A) * sizeof(float);
+  if (int rc = raise_dyn_smem(qr_loss_kernel, smem, "b2rl_qr_loss")) return rc;
   launch_pdl(qr_loss_kernel, dim3(B), dim3(256), smem, (cudaStream_t)stream, quantile, quantile_next, action, reward, mask, gamma_n, kappa,
                                                          B, A, N, vec_out, loss_out, dquant_out, partial, counter,
                                                          grad_weight);

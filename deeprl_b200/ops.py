@@ -22,14 +22,21 @@ def _c(x, dtype=None):
 
 
 class _Scratch:
-    """Per-device reusable scratch (zero-initialised counters the kernels re-arm themselves)."""
+    """Per-device reusable scratch (zero-initialised counters the kernels re-arm themselves).
+
+    Every tensor handed out stays alive for the life of the process, also after a larger request replaced it: a CUDA graph
+    captured while it was current keeps using its address, and freeing it would let the caching allocator give that memory
+    to another tensor that every replay then overwrites."""
     _store = {}
+    _retired = []
 
     @classmethod
     def get(cls, device, name, numel, dtype):
         key = (str(device), name, dtype)
         t = cls._store.get(key)
         if t is None or t.numel() < numel:
+            if t is not None:
+                cls._retired.append(t)
             t = torch.zeros(numel, dtype=dtype, device=device)
             cls._store[key] = t
         return t
