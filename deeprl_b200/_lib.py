@@ -26,6 +26,8 @@ c_p, c_i32, c_i64, c_u64, c_f32, c_f64 = (ctypes.c_void_p, ctypes.c_int32, ctype
 SIGNATURES = {
     "b2rl_replay_feed": [c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_i32, c_i32, c_p],
     "b2rl_replay_select_uniform": [c_p, c_p, c_i32, c_u64, c_i32, c_i32, c_i32, c_p, c_p, c_p],
+    "b2rl_replay_select_uniform_scalars": [c_p, c_p, c_i32, c_u64, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p, c_f64, c_p,
+                                           c_p, c_p, c_p],
     "b2rl_replay_gather": [c_p, c_p, c_p, c_p, c_i64, c_i64, c_p, c_i32, c_i32, c_i32, c_f64, c_p, c_i32, c_i32, c_i32,
                            c_p, c_p, c_p, c_p, c_p, c_p],
     "b2rl_sumtree_add": [c_p, c_p, c_i64, c_p, c_p, c_i32, c_p, c_p],

@@ -303,8 +303,16 @@ class UniformReplay:
             self._lut_cache[scale] = torch.from_numpy(t).to(self.device)
         return self._lut_cache[scale]
 
-    def select(self, B, idx_out, candidates=None):
+    def select(self, B, idx_out, candidates=None, scalars=None):
+        """Draw B valid indices into ``idx_out``; with ``scalars`` (a buffer set) the same launch also writes their action /
+        n-step reward / mask, as ``gather_scalars`` does."""
         n_cand = min(8192, max(2 * B, B + 256)) if candidates is None else min(8192, candidates.numel())
+        if scalars is not None:
+            _lib.call("b2rl_replay_select_uniform_scalars", _lib.ptr(self.ring_state), _lib.ptr(candidates), int(n_cand), self.seed,
+                      self.history_length, self.n_step, int(B), _lib.ptr(idx_out), _lib.ptr(self._status), _lib.ptr(self.action),
+                      _lib.ptr(self.reward), _lib.ptr(self.mask), self.discount, _lib.ptr(scalars["action"]),
+                      _lib.ptr(scalars["reward"]), _lib.ptr(scalars["mask"]), _lib.stream())
+            return
         _lib.call("b2rl_replay_select_uniform", _lib.ptr(self.ring_state), _lib.ptr(candidates), int(n_cand), self.seed,
                   self.history_length, self.n_step, int(B), _lib.ptr(idx_out), _lib.ptr(self._status), _lib.stream())
 
@@ -382,13 +390,16 @@ class UniformReplay:
         if candidates is not None and not isinstance(candidates, torch.Tensor):
             candidates = torch.as_tensor(np.asarray(candidates, dtype=np.int64), device=self.device)
         # phase "select": draw the indices only; phase "gather": build the batch from the indices drawn before (the learner
-        # draws early, on tiny kernels, and gathers late, beside its update tail); None: both
+        # draws early, on tiny kernels, and gathers late, beside its update tail); None: both.  layout "ring" (K1): no batch
+        # is materialised, conv1 reads the ring through the sampled indices, and the draw writes action / reward / mask itself
+        ring = layout == "ring"
         if phase != "gather":
-            self.select(B, bufs["idx"], candidates)
+            self.select(B, bufs["idx"], candidates, scalars=bufs if ring else None)
         if phase == "select":
             return None
-        if layout == "ring":             # K1: no batch is materialised, conv1 reads the ring through the sampled indices
-            self.gather_scalars(bufs["idx"], B, bufs)
+        if ring:
+            if phase == "gather":
+                self.gather_scalars(bufs["idx"], B, bufs)
             return Transition(self.ring_frames(bufs["idx"], 0), bufs["action"], bufs["reward"], self.ring_frames(bufs["idx"], 1),
                               bufs["mask"])
         self.gather(bufs["idx"], B, bufs, out_dtype, None if scale is None else self.lut(scale), layout)

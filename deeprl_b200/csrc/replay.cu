@@ -67,6 +67,22 @@ __device__ __forceinline__ bool valid_index(int64_t i, int64_t pos, int64_t size
   return false;
 }
 
+__device__ __forceinline__ void gather_scalars(const int32_t* action, const double* reward, const int32_t* mask,
+                                               int64_t i, int n, double discount, int64_t* a_out, float* r_out,
+                                               float* m_out, int b) {
+  // replay.py:128-140: cum_r = reward[k] + mask[k]*discount*cum_r for k reversed (float64); cum_mask = AND
+  double cum_r = 0.0;
+  int cum_m = 1;
+  for (int k = n - 1; k >= 0; --k) {
+    double mk = (double)mask[i + k];
+    cum_r = __dadd_rn(reward[i + k], __dmul_rn(__dmul_rn(mk, discount), cum_r));
+    cum_m = (cum_m && mask[i + k]) ? 1 : 0;
+  }
+  if (a_out) a_out[b] = (int64_t)action[i];
+  if (r_out) r_out[b] = (float)cum_r;          // one rounding float64 -> float32, as np.asarray(x, float32)
+  if (m_out) m_out[b] = (float)cum_m;
+}
+
 constexpr int SEL_THREADS = 1024;
 constexpr int SEL_PER_THREAD = 8;
 
@@ -74,7 +90,10 @@ __global__ void __launch_bounds__(SEL_THREADS) select_uniform_kernel(int64_t* __
                                                                      const int64_t* __restrict__ cand, int n_cand,
                                                                      uint64_t seed, int hl, int n, int B,
                                                                      int64_t* __restrict__ idx_out,
-                                                                     int32_t* __restrict__ status) {
+                                                                     int32_t* __restrict__ status, const int32_t* action,
+                                                                     const double* reward, const int32_t* mask,
+                                                                     double discount, int64_t* a_out, float* r_out,
+                                                                     float* m_out) {
   pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return
   __shared__ int warp_tot[32];
   __shared__ int last_used;
@@ -138,6 +157,12 @@ __global__ void __launch_bounds__(SEL_THREADS) select_uniform_kernel(int64_t* __
     const int total = s_total;
     for (int j = total + t; j < B; j += SEL_THREADS) idx_out[j] = total > 0 ? idx_out[j % total] : (int64_t)(hl - 1);
   }
+  // action / n-step reward / mask of the chosen indices (K1: the frame stacks stay in the ring), in the same launch: the
+  // separate gather_scalars_kernel would be one more dependent launch between the draw and the forward pass
+  if (a_out || r_out || m_out) {
+    __syncthreads();                                  // idx_out complete, including the cycled tail
+    for (int j = t; j < B; j += SEL_THREADS) gather_scalars(action, reward, mask, idx_out[j], n, discount, a_out, r_out, m_out, j);
+  }
   if (t == 0) {
     status[1] = last_used ? last_used : n_cand;       // candidates consumed (all of them if the stream ran dry)
     if (!cand) ring_state[4] = (int64_t)(ctr + (uint64_t)n_cand);
@@ -186,22 +211,6 @@ template <typename T> struct Cvt;
 template <> struct Cvt<float> { __device__ static float f(float x) { return x; } };
 template <> struct Cvt<__half> { __device__ static __half f(float x) { return __float2half_rn(x); } };
 template <> struct Cvt<__nv_bfloat16> { __device__ static __nv_bfloat16 f(float x) { return __float2bfloat16_rn(x); } };
-
-__device__ __forceinline__ void gather_scalars(const int32_t* action, const double* reward, const int32_t* mask,
-                                               int64_t i, int n, double discount, int64_t* a_out, float* r_out,
-                                               float* m_out, int b) {
-  // replay.py:128-140: cum_r = reward[k] + mask[k]*discount*cum_r for k reversed (float64); cum_mask = AND
-  double cum_r = 0.0;
-  int cum_m = 1;
-  for (int k = n - 1; k >= 0; --k) {
-    double mk = (double)mask[i + k];
-    cum_r = __dadd_rn(reward[i + k], __dmul_rn(__dmul_rn(mk, discount), cum_r));
-    cum_m = (cum_m && mask[i + k]) ? 1 : 0;
-  }
-  if (a_out) a_out[b] = (int64_t)action[i];
-  if (r_out) r_out[b] = (float)cum_r;          // one rounding float64 -> float32, as np.asarray(x, float32)
-  if (m_out) m_out[b] = (float)cum_m;
-}
 
 // scalars only (action, n-step reward, mask): the frame stacks stay in the ring and are read by conv1 itself (K1, csrc/gemm.cu)
 __global__ void __launch_bounds__(128) gather_scalars_kernel(const int32_t* __restrict__ action, const double* __restrict__ reward,
@@ -553,8 +562,23 @@ extern "C" int b2rl_replay_select_uniform(int64_t* ring_state, const int64_t* ca
   B2RL_REQUIRE(B > 0 && n_cand >= B && n_cand <= SEL_THREADS * SEL_PER_THREAD, "need B <= n_cand <= 8192");
   B2RL_REQUIRE(history >= 1 && n_step >= 1, "history and n_step must be >= 1");
   launch_pdl(select_uniform_kernel, dim3(1), dim3(SEL_THREADS), 0, (cudaStream_t)stream, ring_state, candidates, n_cand, seed, history,
-                                                                      n_step, B, idx_out, status_out);
+                                                                      n_step, B, idx_out, status_out, (const int32_t*)nullptr,
+             (const double*)nullptr, (const int32_t*)nullptr, 0.0, (int64_t*)nullptr, (float*)nullptr, (float*)nullptr);
   return check_launch("b2rl_replay_select_uniform");
+}
+
+extern "C" int b2rl_replay_select_uniform_scalars(int64_t* ring_state, const int64_t* candidates, int32_t n_cand,
+                                                  uint64_t seed, int32_t history, int32_t n_step, int32_t B,
+                                                  int64_t* idx_out, int32_t* status_out, const int32_t* action,
+                                                  const double* reward, const int32_t* mask, double discount,
+                                                  int64_t* action_out, float* reward_out, float* mask_out, void* stream) {
+  B2RL_REQUIRE(ring_state && idx_out && status_out && action && reward && mask, "null pointer");
+  B2RL_REQUIRE(action_out || reward_out || mask_out, "no scalar output: use b2rl_replay_select_uniform");
+  B2RL_REQUIRE(B > 0 && n_cand >= B && n_cand <= SEL_THREADS * SEL_PER_THREAD, "need B <= n_cand <= 8192");
+  B2RL_REQUIRE(history >= 1 && n_step >= 1, "history and n_step must be >= 1");
+  launch_pdl(select_uniform_kernel, dim3(1), dim3(SEL_THREADS), 0, (cudaStream_t)stream, ring_state, candidates, n_cand, seed, history,
+             n_step, B, idx_out, status_out, action, reward, mask, discount, action_out, reward_out, mask_out);
+  return check_launch("b2rl_replay_select_uniform_scalars");
 }
 
 extern "C" int b2rl_replay_gather(const uint8_t* frames, const int32_t* action, const double* reward,

@@ -94,9 +94,16 @@ class GraphedDQNLearner:
         self._overlap = False             # multi-GPU: NCCL captured inside the update graph, fc4's all-reduce beside the backward
         self._early_work = None
         body = getattr(network, "body", None)
-        self.ring = (not self.prefetch and not self.dual and compute_dtype == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
+        # K1: conv1 reads the sampled frame stacks from the uint8 ring, no batch is materialised.  With async replay the feeds
+        # and the index draw of the next batch then run after this update's last ring read (_main).  Prioritized replay keeps
+        # the materialising gather there: its draw of the next batch must precede this update's priority update, which comes
+        # before the backward pass, while the feeds may only overwrite ring rows after the backward pass.  The fused-head
+        # path keeps it as well.
+        fused_head = kind == "dqn" and os.environ.get("B2RL_FUSED_HEAD", "0") != "0"
+        self.ring = (not self.dual and compute_dtype == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
                      and hasattr(body, "repack") and not getattr(body, "noisy_linear", False) and replay.history_length == 4
-                     and tuple(getattr(replay, "item_shape", ())) == (84, 84) and os.environ.get("B2RL_K1", "1") != "0")
+                     and tuple(getattr(replay, "item_shape", ())) == (84, 84) and os.environ.get("B2RL_K1", "1") != "0"
+                     and not (self.prefetch and (self.per or fused_head)))
         self.opt.zero_grad()              # the fused tail writes / re-zeroes the gradient arena itself: start from zeros
 
     # ------------------------------------------------------------------ fused tail / fused head (csrc/tail.cu, csrc/head.cu)
@@ -161,8 +168,8 @@ class GraphedDQNLearner:
             rp.quirk = quirk
         if self.dtype == torch.bfloat16:
             # exact integer frames, space-to-depth layout; ImageNormalizer's scale is folded into conv1's weights.
-            # K1 (self.ring): no batch at all -- conv1 reads the sampled stacks from the uint8 ring (synchronous replay only:
-            # a prefetched index could be overwritten by the next update's feeds before its frames are read)
+            # K1 (self.ring): no batch at all -- conv1 reads the sampled stacks from the uint8 ring; the frames of a batch are
+            # those of the ring until the next feed, which _main orders after the batch's last read
             kw = dict(phase=phase) if phase else {}
             return rp.sample_normalized(out_dtype=self.dtype, scale=None, layout="ring" if self.ring else "s2d", tag=tag, **kw)
         kw = dict(phase=phase) if phase else {}
@@ -188,11 +195,16 @@ class GraphedDQNLearner:
             with torch.cuda.stream(side):
                 self._repack(self.net, fs)
                 self._packed_ev.record(side)
-        # async replay: the batch of the NEXT update is fed + sampled on a parallel branch.  Uniform replay: that branch starts
-        # after the backward pass, beside the (small-footprint, L2-bound) update tail -- started beside the forward pass its 512
+        # async replay: the batch of the NEXT update is fed + sampled on a parallel branch.  Uniform replay with the
+        # materialising gather: that branch starts after the backward pass, beside the (small-footprint, L2-bound) update tail -- started beside the forward pass its 512
         # gather CTAs would hold the shared memory the convolution kernels need and delay them.  Prioritized replay keeps the early start: the reference's replay worker draws the next
         # batch BEFORE this update's priorities arrive (replay.py:219-261), and the graph keeps that order.
-        late = (self.prefetch and not self.per and getattr(self, "_one_graph", True)
+        # K1 with async replay: this update's batch is read from the ring by both conv1 forwards and, last, by conv1's weight
+        # gradient.  The whole prefetch branch -- this update's feeds, the index draw and the action / reward / mask gather of
+        # the next batch into the other buffer set -- forks after that last read, so every batch sees the ring exactly as the
+        # materialising form gathers it (after the previous update's feeds, before this update's)
+        ring_pre = self.prefetch and self.ring
+        late = (self.prefetch and not self.per and not self.ring and getattr(self, "_one_graph", True)
                 and os.environ.get("B2RL_PREFETCH_LATE", "1") == "1")
         if self.prefetch:
             eager = parity is None
@@ -203,7 +215,7 @@ class GraphedDQNLearner:
             t = self._batch[parity]
             if late:
                 self._prefetch_branch(parity, "select")  # feed + index draw now (two one-CTA kernels), the gather later
-            else:
+            elif not ring_pre:                           # (K1: the whole branch after the last ring read, below)
                 self._prefetch_branch(parity)
             if eager:
                 self._parity = 1 - parity
@@ -266,7 +278,11 @@ class GraphedDQNLearner:
         if tail is None:
             self.opt.zero_grad()
         fired = []
-        if late and os.environ.get("B2RL_PREFETCH_AT", "end") == "dgrad":
+        if ring_pre:
+            # forked right after the launch of conv1's weight gradient from the ring, beside the rest of the backward pass and
+            # the update tail (kernels A / B)
+            nature_tc.AFTER_RING_READ = lambda stream: fired or (self._prefetch_branch(parity, after=stream), fired.append(1))
+        elif late and os.environ.get("B2RL_PREFETCH_AT", "end") == "dgrad":
             # option (B2RL_PREFETCH_AT=dgrad): fork the gather right after the last dgrad GEMM, beside the conv2 / conv1
             # weight-gradient GEMMs.  The default forks after the backward pass: beside the weight gradients the gather slows the
             # conv1 weight gradient and kernel A
@@ -276,18 +292,24 @@ class GraphedDQNLearner:
                 head.backward(grad)
         finally:
             nature_tc.AFTER_DGRAD = None
+            nature_tc.AFTER_RING_READ = None
         nature_tc.mark("bwd_done")
         self.loss.copy_(r["loss"])
-        if late:
-            if not fired:
-                self._prefetch_branch(parity, "gather")
-            self._late_join = True                       # joined after the optimizer kernels (_opt)
+        if late or ring_pre:
+            if not fired:                                # (no ring read in the backward pass: fork after it)
+                self._prefetch_branch(parity, None if ring_pre else "gather")
+            if getattr(self, "_one_graph", True):
+                self._late_join = True                   # joined after the optimizer kernels (_opt)
+            else:
+                cur.wait_stream(pre)                     # split-graph form: joined inside the first graph
         elif self.prefetch:
             cur.wait_stream(pre)
 
-    def _prefetch_branch(self, parity, phase=None):
+    def _prefetch_branch(self, parity, phase=None, after=None):
         cur, pre = torch.cuda.current_stream(), self._pre
         pre.wait_stream(cur)                                             # after the host->device copy of this update's feeds
+        if after is not None:
+            pre.wait_stream(after)                                       # and after the ring read launched there
         with torch.cuda.stream(pre):
             b = self._sample(1 - parity, phase)
             if phase != "select":

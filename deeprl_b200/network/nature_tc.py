@@ -49,6 +49,9 @@ def mark(name, stream=None):
 
 AFTER_DGRAD = None         # callable run once, on the current stream, right after the last dgrad GEMM of the backward pass was
                            # launched (the learner forks its late prefetch branch there: beside the weight-gradient tail)
+AFTER_RING_READ = None     # callable(stream) run on the current stream right after conv1's weight gradient was launched from the
+                           # uint8 ring (K1) on ``stream`` (None: the current stream); that launch is the batch's last ring read,
+                           # so the learner forks the next update's ring feeds there
 SINK = None                # network/tail.py NatureTail while ``grad_sink`` is active: backward hands it the GEMM-layout gradients
 RELU_FEATURES = {}         # data_ptr -> weak reference to the feature tensor y4 = relu(fc4(.)) nature_body produced there
 PREMASKED = {}             # data_ptr of a feature gradient already masked by head_bwd_relu -> (that gradient, its column sums = db4)
@@ -112,6 +115,19 @@ class RingFrames:
         g = self.grid
         x = x.view(self.batch, self.history, g, 4, g, 4).permute(0, 2, 4, 1, 3, 5).reshape(self.batch, g, g, 16 * self.history)
         return x.to(_bf16).permute(0, 3, 1, 2)
+
+    # inspection (tests, debugging): a RingFrames reads as the batch it stands for, as the ring holds it now
+    def data_ptr(self):
+        """Address of the index buffer: batches drawn into different buffer sets differ here."""
+        return self.idx.data_ptr()
+
+    def clone(self):
+        return self.materialize()
+
+    @classmethod
+    def __torch_function__(cls, func, types, args=(), kwargs=None):
+        m = lambda x: x.materialize() if isinstance(x, RingFrames) else x
+        return func(*[m(a) for a in args], **{k: m(v) for k, v in (kwargs or {}).items()})
 
     def args(self):
         return (_lib.ptr(self.frames), int(self.frames.shape[0]), _lib.ptr(self.idx), self.first, self.row_bytes, self.frame_w,
@@ -198,6 +214,8 @@ def _backward_fused(ctx, gy4):
         AFTER_DGRAD()
     if ctx.ring is not None:
         gw1p, p1 = wgrad_partials_ring(ctx.ring, g1, 32, stream=_fork())
+        if AFTER_RING_READ is not None:
+            AFTER_RING_READ(_WGRAD["stream"])
     else:
         gw1p, p1 = wgrad_partials(x0m, g1, 32, 4, 2, 21, stream=_fork())
     mark("w_conv1", _WGRAD["stream"])
@@ -405,6 +423,8 @@ def _backward_unfused(ctx, gy4):
     g1, db1 = act_bwd_bias_grad(gy1, x1, True, row_map=2, G=21, V=20, out_rows=B * 441)
     if ctx.ring is not None:
         gw1p, p1 = wgrad_partials_ring(ctx.ring, g1, 32, stream=_fork())
+        if AFTER_RING_READ is not None:
+            AFTER_RING_READ(_WGRAD["stream"])
     else:
         gw1p, p1 = wgrad_partials(x0m, g1, 32, 4, 2, 21, stream=_fork())
     _join()

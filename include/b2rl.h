@@ -64,6 +64,14 @@ int b2rl_replay_select_uniform(int64_t* ring_state, const int64_t* candidates, i
                                int32_t history, int32_t n_step, int32_t B, int64_t* idx_out, int32_t* status_out,
                                void* stream);
 
+/* b2rl_replay_select_uniform + the action / n-step reward / mask of the chosen indices in the same launch (exactly the
+ * scalar outputs of b2rl_replay_gather, same rounding): the sample of a consumer that reads the frame stacks from the
+ * ring itself (K1).  At least one *_out must be non-NULL; a NULL one is skipped. */
+int b2rl_replay_select_uniform_scalars(int64_t* ring_state, const int64_t* candidates, int32_t n_cand, uint64_t seed,
+                                       int32_t history, int32_t n_step, int32_t B, int64_t* idx_out, int32_t* status_out,
+                                       const int32_t* action, const double* reward, const int32_t* mask, double discount,
+                                       int64_t* action_out, float* reward_out, float* mask_out, void* stream);
+
 /* construct_transition for B indices (replay.py:112-140): frame-stack gather + n-step return.
  * out_dtype B2RL_U8: raw stacks [B][history][row_bytes] (lut must be NULL, layout 0).
  * converted dtypes (F16/BF16/F32): value = lut[v] (float32 [256] table, e.g. float32(float64(v)/255) = the reference's
