@@ -220,14 +220,21 @@ PPO_FN AdamCoef adam_coef(float lr, float b1, float b2, float eps, int t) {
   return c;
 }
 
+// The three updates are written as explicit fmaf, the same at every Adam site (adam_elem, wgrad_adam_tile): left to
+// contraction, nvcc fused `p - step_size * q` into one FFMA in wgrad_adam_tile but rounded step_size * q first in the
+// data-parallel reduce, so the W = 1 data-parallel kernel drifted from the single-process one by that rounding every step.
+PPO_FN float adam_m(float m, float g, const AdamCoef& c) { return fmaf(1.0f - c.b1, g - m, m); }          // exp_avg.lerp_
+PPO_FN float adam_v(float v, float g, const AdamCoef& c) { return fmaf((1.0f - c.b2) * g, g, c.b2 * v); } // .addcmul_
+PPO_FN float adam_p(float p, float m, float v, const AdamCoef& c) {
+  const float denom = sqrtf(v) / c.bc2s + c.eps;
+  return fmaf(-c.step_size, m / denom, p);
+}
+
 PPO_FN float adam_elem(float p, float g, float* m, float* v, int idx, const AdamCoef& c) {
-  float mi = m[idx];
-  mi = mi + (1.0f - c.b1) * (g - mi);                              // exp_avg.lerp_(grad, 1 - beta1)
-  const float vi = c.b2 * v[idx] + (1.0f - c.b2) * g * g;          // exp_avg_sq.mul_(beta2).addcmul_(g, g, 1 - beta2)
+  const float mi = adam_m(m[idx], g, c), vi = adam_v(v[idx], g, c);
   m[idx] = mi;
   v[idx] = vi;
-  const float denom = sqrtf(vi) / c.bc2s + c.eps;
-  return p - c.step_size * (mi / denom);
+  return adam_p(p, mi, vi, c);
 }
 
 // Number of 4 x 4 tiles of a [J][K] weight
@@ -306,10 +313,9 @@ PPO_FN void wgrad_adam_tile(int t, const float* d, int ldd, const float* in, int
     float wn[4], mn[4], vn[4];
     for (int c = 0; c < 4; ++c) {
       const float g = acc[r][c];
-      mn[c] = mo[r][c] + (1.0f - ac.b1) * (g - mo[r][c]);             // exp_avg.lerp_(grad, 1 - beta1)
-      vn[c] = ac.b2 * vo[r][c] + (1.0f - ac.b2) * g * g;              // exp_avg_sq.mul_(beta2).addcmul_(g, g, 1 - beta2)
-      const float denom = sqrtf(vn[c]) / ac.bc2s + ac.eps;
-      wn[c] = (4 * tk + c < K ? wp[c] : 0.0f) - ac.step_size * (mn[c] / denom);
+      mn[c] = adam_m(mo[r][c], g, ac);
+      vn[c] = adam_v(vo[r][c], g, ac);
+      wn[c] = adam_p(4 * tk + c < K ? wp[c] : 0.0f, mn[c], vn[c], ac);
     }
     const int e = off + (4 * tj + r) * K + 4 * tk;
     if (vec) {

@@ -356,11 +356,11 @@ def test_cuda_dp_with_one_rank_matches_the_single_process_kernel(case):
               c["a_lr"], HYPER["a_b1"], HYPER["a_b2"], HYPER["a_eps"], HYPER["c_lr"], HYPER["c_b1"], HYPER["c_b2"], HYPER["c_eps"],
               HYPER["clip"], HYPER["ent_w"], 1.5 * c["target_kl"], p(t["stats"]), _lib.stream())
     torch.cuda.synchronize()
-    diffs = {k: float(np.abs(getattr(s, k) - t[k].cpu().numpy()).max()) for k in ("a_flat", "c_flat", "a_m", "a_v", "c_m", "c_v", "stats")}
-    print("W=1 data-parallel vs single-process kernel, max |difference|:", diffs)
+    # every Adam site evaluates the update as the same explicit fmaf (ppo_phases.h adam_m / adam_v / adam_p), and 1/W = 1:
+    # the two kernels agree bit for bit
     assert int(s.a_step[0]) == int(t["a_step"]) and int(s.c_step[0]) == int(t["c_step"])
-    for k in ("a_flat", "c_flat"):
-        assert diffs[k] <= 2e-5, (k, diffs)
+    for k in ("a_flat", "c_flat", "a_m", "a_v", "c_m", "c_v", "stats"):
+        assert np.array_equal(getattr(s, k), t[k].cpu().numpy()), k
 
 
 @pytest.mark.gpu
