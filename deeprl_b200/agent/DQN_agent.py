@@ -304,6 +304,5 @@ class DQNAgent(BaseAgent):
             lr.d_beta.fill_(float(config.replay_beta()))
         with config.lock:                                  # the actor reads the shared parameters (DQN_agent.py:30,133)
             lr.update()
-            if lr.tail() is None:                          # (the fused tail writes the packed operands itself)
-                lr._repack(self.network, lr.scale if lr.dtype == torch.bfloat16 else 1.0)   # the actor's next forward sees theta_k
+            lr.repack_online()                             # the actor's next forward sees theta_k
         self.last_loss = lr.loss

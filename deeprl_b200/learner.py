@@ -8,6 +8,7 @@ Multi-GPU (SURVEY 8e): one learner per rank, rank-local replay shard, parameters
 gradients are summed with ONE NCCL all-reduce of the flat gradient arena between the two graphs and scaled by
 1 / world_size inside the clip kernel.
 """
+import dataclasses
 import os
 import sys
 
@@ -39,6 +40,63 @@ class StepTrace:
         return [(n, t0.elapsed_time(e) * 1e3) for n, e in self.marks]
 
 
+@dataclasses.dataclass(frozen=True)
+class UpdatePlan:
+    """The layout of one ``GraphedDQNLearner`` update, as decided by ``update_plan``."""
+    ring: bool            # K1: conv1 reads the sampled frame stacks from the uint8 ring, no batch is materialised
+    tail: bool            # the two-launch fused update tail (network/tail.py) replaces unpack + FlatOptimizer.step
+    repack_online: bool   # no fused tail: the online operands are re-packed on the side branch at the start of each update
+    dist_head: bool       # C51 / QR: the heads read bf16 weight copies on the wgmma GEMM
+    head: str             # "separate" (head_fwd | loss | head_bwd), "fused-two" or "fused-one" (csrc/head.cu on the features)
+    forward: str          # "two-branch" (target on the side stream), "dual" (one launch per layer for both) or "one-stream"
+    single_stream: bool   # the side-branch work (target forward, re-pack, weight gradients) runs on the main stream
+    prefetch: object      # where the next batch is sampled: None, "start", "gather-after-bwd" / "-dgrad", "after-ring-read"
+    join: object          # where the prefetch branch joins: None, "main" (end of _main) or "opt" (after the optimizer kernels)
+    one_graph: bool       # multi-GPU: the all-reduce is captured inside the update graph
+
+
+def update_plan(kind="dqn", per=False, prefetch=False, dual=False, k1_body=True, dual_body=True, tail=True,
+                narrow_head=True, world=1, one_graph=True, env=None):
+    """Decide the update schedule from plain values: the learner's options, what the networks support (``k1_body``: a
+    wgmma NatureConvBody on a 4 x 84 x 84 uint8 ring; ``dual_body``: both bodies on the wgmma kernels; ``tail``: the fused
+    update tail applies; ``narrow_head``: VanillaNet / DuelingNet heads the fused head kernel takes) and the ``B2RL_*``
+    switches in ``env``.  ``one_graph=False``: the split-graph form after a failed NCCL capture."""
+    env = env or {}
+    on = lambda name, default: env.get(name, default) != "0"
+    fused_env = kind == "dqn" and on("B2RL_FUSED_HEAD", "0")
+    # K1 with async replay: the feeds and the index draw of the next batch run after this update's last ring read.
+    # Prioritized replay keeps the materialising gather: its draw of the next batch must precede this update's priority
+    # update, which comes before the backward pass, while the feeds may only overwrite ring rows after the backward pass.
+    # The fused-head switch keeps it as well (whether or not the fused head then applies).
+    ring = k1_body and not dual and on("B2RL_K1", "1") and not (prefetch and (per or fused_env))
+    tail = tail and on("B2RL_TAIL", "1")
+    # the fused head (off by default: the separate kernels run the target head on the side branch, which it gives up)
+    head = "separate"
+    if fused_env and tail and narrow_head:
+        head = "fused-one" if env.get("B2RL_FUSED_HEAD") == "one" else "fused-two"
+    single = head == "separate" and env.get("B2RL_SINGLE_STREAM", "0") == "1"       # experiment: no parallel branches
+    forward = "dual" if head == "separate" and dual and dual_body else ("one-stream" if single else "two-branch")
+    one_graph = one_graph and (world == 1 or env.get("B2RL_NCCL_IN_GRAPH", "1") == "1")
+    # async replay, uniform with the materialising gather: feed + index draw at the start, the gather after the backward
+    # pass beside the (small-footprint, L2-bound) update tail -- started beside the forward pass its 512 gather CTAs would
+    # hold the shared memory the convolution kernels need.  Prioritized replay keeps the whole branch at the start: the
+    # reference's replay worker draws the next batch BEFORE this update's priorities arrive (replay.py:219-261).
+    pf = join = None
+    if prefetch:
+        if ring:
+            pf, join = "after-ring-read", "opt" if one_graph else "main"
+        elif not per and one_graph and env.get("B2RL_PREFETCH_LATE", "1") == "1":
+            # B2RL_PREFETCH_AT=dgrad forks the gather after the last dgrad GEMM, beside the conv2 / conv1 weight gradients,
+            # where it slows the conv1 weight gradient and kernel A
+            at_dgrad = head == "separate" and env.get("B2RL_PREFETCH_AT", "end") == "dgrad"
+            pf, join = "gather-after-dgrad" if at_dgrad else "gather-after-bwd", "opt" if head == "separate" else "main"
+        else:
+            pf, join = "start", "main"
+    return UpdatePlan(ring=ring, tail=tail, repack_online=not tail, head=head, forward=forward, single_stream=single,
+                      dist_head=kind in ("c51", "qr") and tail and on("B2RL_DIST_HEAD", "1"), prefetch=pf, join=join,
+                      one_graph=one_graph)
+
+
 class GraphedDQNLearner:
     def __init__(self, network, target_network, optimizer, replay, kind="dqn", discount=0.99, n_step=1, double_q=False,
                  gradient_clip=5.0, feeds_per_update=4, compute_dtype=torch.bfloat16, state_scale=1.0 / 255,
@@ -52,10 +110,8 @@ class GraphedDQNLearner:
         self.world = world_size
         self.per = isinstance(replay, PrioritizedReplay)
         self.sync_every = target_sync_every
-        dev = replay.device
-        self.dev = dev
-        B = replay.batch_size
-        self.B = B
+        self.dev = dev = replay.device
+        self.B = replay.batch_size
         n = max(self.feeds, 1)
         rb = replay.row_bytes
         # ONE packed pinned staging buffer for the env transitions of an update (+ PER beta) and ONE device mirror:
@@ -93,18 +149,32 @@ class GraphedDQNLearner:
         self._tail = None                 # network/tail.py NatureTail (built on first use), False = not applicable
         self._overlap = False             # multi-GPU: NCCL captured inside the update graph, fc4's all-reduce beside the backward
         self._early_work = None
-        body = getattr(network, "body", None)
-        # K1: conv1 reads the sampled frame stacks from the uint8 ring, no batch is materialised.  With async replay the feeds
-        # and the index draw of the next batch then run after this update's last ring read (_main).  Prioritized replay keeps
-        # the materialising gather there: its draw of the next batch must precede this update's priority update, which comes
-        # before the backward pass, while the feeds may only overwrite ring rows after the backward pass.  The fused-head
-        # path keeps it as well.
-        fused_head = kind == "dqn" and os.environ.get("B2RL_FUSED_HEAD", "0") != "0"
-        self.ring = (not self.dual and compute_dtype == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
-                     and hasattr(body, "repack") and not getattr(body, "noisy_linear", False) and replay.history_length == 4
-                     and tuple(getattr(replay, "item_shape", ())) == (84, 84) and os.environ.get("B2RL_K1", "1") != "0"
-                     and not (self.prefetch and (self.per or fused_head)))
+        self._env = {k: v for k, v in os.environ.items() if k.startswith("B2RL_")}     # update_plan's switches, as constructed
+        self._plan = None
         self.opt.zero_grad()              # the fused tail writes / re-zeroes the gradient arena itself: start from zeros
+
+    @property
+    def plan(self):
+        """The ``UpdatePlan`` of this learner, decided on first use (the module flags the fused tail depends on are read
+        then, as the tail itself is built lazily)."""
+        if self._plan is None:
+            self._plan = self._resolve_plan()
+        return self._plan
+
+    def _resolve_plan(self, one_graph=True):
+        body, rp = getattr(self.net, "body", None), self.replay
+        wgmma = self.dtype == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05" and hasattr(body, "repack")
+        plain = wgmma and not getattr(body, "noisy_linear", False)
+        return update_plan(
+            self.kind, self.per, self.prefetch, self.dual, world=self.world, one_graph=one_graph, env=self._env,
+            k1_body=plain and rp.history_length == 4 and tuple(getattr(rp, "item_shape", ())) == (84, 84),
+            dual_body=wgmma and hasattr(getattr(self.tgt, "body", None), "repack"),
+            tail=plain and nature_tc.FUSED_BWD and bool(_lib.CONV_SLAB) and self.opt.kind in ("rmsprop", "adam"),
+            narrow_head=self._heads() is not None)
+
+    @property
+    def ring(self):
+        return self.plan.ring
 
     # ------------------------------------------------------------------ fused tail / fused head (csrc/tail.cu, csrc/head.cu)
     def tail(self):
@@ -112,13 +182,9 @@ class GraphedDQNLearner:
         wgmma NatureConvBody and the backward epilogues are fused; None otherwise (generic unpack + FlatOptimizer.step)."""
         if self._tail is None:
             from .network.tail import NatureTail
-            body = getattr(self.net, "body", None)
-            ok = (self.dtype == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05" and nature_tc.FUSED_BWD and _lib.CONV_SLAB
-                  and hasattr(body, "repack") and not getattr(body, "noisy_linear", False)
-                  and os.environ.get("B2RL_TAIL", "1") != "0" and self.opt.kind in ("rmsprop", "adam"))
-            if ok:
-                self._repack(self.net, self.scale)
-                self._tail = NatureTail(self.opt, body, self.scale)
+            if self.plan.tail:
+                self._repack(self.net)
+                self._tail = NatureTail(self.opt, self.net.body, self.scale)
                 self._tail.max_norm, self._tail.grad_scale = self.clip, 1.0 / self.world
                 self._refresh_head_operands(True)
                 if self.world > 1:
@@ -131,11 +197,8 @@ class GraphedDQNLearner:
         return self._tail or None
 
     def _heads(self):
-        """(online head modules, target head modules) when the DQN head can run in the fused head + loss + backward kernel."""
-        # (off by default: the separate head_fwd | dqn_loss | head_bwd kernels run the target head on the side branch, which the
-        # fused forms give up)
-        if self.kind != "dqn" or self.tail() is None or os.environ.get("B2RL_FUSED_HEAD", "0") == "0":
-            return None
+        """(online head modules, target head modules) when the heads fit the fused head + loss + backward kernel: narrow,
+        16-byte aligned VanillaNet / DuelingNet heads."""
         out = []
         for n in (self.net, self.tgt):
             fa = getattr(n, "fc_head", None) or getattr(n, "fc_advantage", None)
@@ -166,46 +229,37 @@ class GraphedDQNLearner:
             else:
                 rp.feed_device(self.d_frames, self.d_action, self.d_reward, self.d_mask, self.feeds)
             rp.quirk = quirk
+        kw = dict(phase=phase) if phase else {}
         if self.dtype == torch.bfloat16:
             # exact integer frames, space-to-depth layout; ImageNormalizer's scale is folded into conv1's weights.
             # K1 (self.ring): no batch at all -- conv1 reads the sampled stacks from the uint8 ring; the frames of a batch are
             # those of the ring until the next feed, which _main orders after the batch's last read
-            kw = dict(phase=phase) if phase else {}
             return rp.sample_normalized(out_dtype=self.dtype, scale=None, layout="ring" if self.ring else "s2d", tag=tag, **kw)
-        kw = dict(phase=phase) if phase else {}
         return rp.sample_normalized(out_dtype=self.dtype, scale=self.scale, layout="nchw", tag=tag, **kw)
 
     def _main(self, parity=None):
-        rp = self.replay
+        plan = self.plan
         cur = torch.cuda.current_stream()
         nature_tc.mark("start")
         if self._side is None:
             self._side = torch.cuda.Stream(device=self.dev)
             self._pre = torch.cuda.Stream(device=self.dev)
             self._packed_ev, self._sampled_ev = torch.cuda.Event(), torch.cuda.Event()
-        side, pre = self._side, self._pre
-        if os.environ.get("B2RL_SINGLE_STREAM", "0") == "1":       # experiment: no parallel graph branches except the prefetch
-            side = cur
+        side, pre = cur if plan.single_stream else self._side, self._pre
         fs = self.scale if self.dtype == torch.bfloat16 else 1.0
         tail = self.tail()
-        if tail is None:
+        if plan.repack_online:
             # online weights changed in the previous optimizer step: re-pack them on the side branch, next to feed + sample
             # (with the fused tail the optimizer kernel itself writes the packed bf16 operands)
             side.wait_stream(cur)
             with torch.cuda.stream(side):
-                self._repack(self.net, fs)
+                self._repack(self.net)
                 self._packed_ev.record(side)
-        # async replay: the batch of the NEXT update is fed + sampled on a parallel branch.  Uniform replay with the
-        # materialising gather: that branch starts after the backward pass, beside the (small-footprint, L2-bound) update tail -- started beside the forward pass its 512
-        # gather CTAs would hold the shared memory the convolution kernels need and delay them.  Prioritized replay keeps the early start: the reference's replay worker draws the next
-        # batch BEFORE this update's priorities arrive (replay.py:219-261), and the graph keeps that order.
-        # K1 with async replay: this update's batch is read from the ring by both conv1 forwards and, last, by conv1's weight
-        # gradient.  The whole prefetch branch -- this update's feeds, the index draw and the action / reward / mask gather of
-        # the next batch into the other buffer set -- forks after that last read, so every batch sees the ring exactly as the
-        # materialising form gathers it (after the previous update's feeds, before this update's)
-        ring_pre = self.prefetch and self.ring
-        late = (self.prefetch and not self.per and not self.ring and getattr(self, "_one_graph", True)
-                and os.environ.get("B2RL_PREFETCH_LATE", "1") == "1")
+        # async replay: the batch of the NEXT update is fed + sampled on a parallel branch.  K1: this update's batch is read
+        # from the ring by both conv1 forwards and, last, by conv1's weight gradient.  The whole prefetch branch -- this
+        # update's feeds, the index draw and the action / reward / mask gather of the next batch into the other buffer set --
+        # forks after that last read, so every batch sees the ring exactly as the materialising form gathers it (after the
+        # previous update's feeds, before this update's)
         if self.prefetch:
             eager = parity is None
             if eager:
@@ -213,96 +267,88 @@ class GraphedDQNLearner:
             if self._batch[parity] is None:                              # very first update: nothing prefetched yet
                 self._batch[parity] = self._sample(parity)
             t = self._batch[parity]
-            if late:
-                self._prefetch_branch(parity, "select")  # feed + index draw now (two one-CTA kernels), the gather later
-            elif not ring_pre:                           # (K1: the whole branch after the last ring read, below)
+            if plan.prefetch == "start":
                 self._prefetch_branch(parity)
+            elif plan.prefetch != "after-ring-read":
+                self._prefetch_branch(parity, "select")  # feed + index draw now (two one-CTA kernels), the gather later
             if eager:
                 self._parity = 1 - parity
         else:
             t = self._sample(0)
         per = dict(is_prob=t.sampling_prob, eps=self.eps, alpha=self.alpha, beta_dev=self.d_beta) if self.per else {}
-        heads = self._heads()
-        if heads is not None:
-            self._main_fused_head(t, per, heads, tail, fs)
-            if late:
-                self._prefetch_branch(parity, "gather")
-            if self.prefetch:
-                cur.wait_stream(pre)
-            return
-        body_a, body_b = getattr(self.net, "body", None), getattr(self.tgt, "body", None)
-        if (self.dual and self.dtype == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
-                and hasattr(body_a, "repack") and hasattr(body_b, "repack")):
+        # the fused head takes the features of the bodies: the forward fork below runs the bodies only
+        fused = plan.head != "separate"
+        net, tgt = (self.net.body, self.tgt.body) if fused else (self.net, self.tgt)
+        if plan.forward == "dual":
             # online(s) and target(s') share every launch of the convolutional body (nature_tc.forward_dual): the grid of
             # each kernel is split between the two networks, so the per-launch fixed cost is paid once
             if tail is None:
                 cur.wait_event(self._packed_ev)
-            with nature_tc.dual_forward(body_a, body_b, t.next_state), frame_scale(fs):
-                out = self.net(t.state)
+            with nature_tc.dual_forward(net.body, tgt.body, t.next_state), frame_scale(fs):
+                out = net(t.state)
                 with torch.no_grad():
-                    nxt_t = self.tgt(t.next_state)
-                    nxt_o = self.net(t.next_state) if self.double_q else None
+                    nxt_t = tgt(t.next_state)
+                    nxt_o = net(t.next_state) if self.double_q else None
         else:
             # the target forward on s' and the online forward on s are independent: fork them onto two streams (two
             # parallel branches of the captured graph) so that the prologue / tail of one chain overlaps the other
             side.wait_stream(cur)
             with torch.cuda.stream(side), frame_scale(fs), torch.no_grad():
-                nxt_t = self.tgt(t.next_state)
+                nxt_t = tgt(t.next_state)
             if tail is None:
                 cur.wait_event(self._packed_ev)
             with frame_scale(fs):
                 with torch.no_grad():
-                    nxt_o = self.net(t.next_state) if self.double_q else None
-                out = self.net(t.state)
+                    nxt_o = net(t.next_state) if self.double_q else None
+                out = net(t.state)
             cur.wait_stream(side)
         nature_tc.mark("fwd_joined")
-        if self.kind == "dqn":
-            head = out["q"]
-            r = ops.dqn_loss_fused(head.detach(), nxt_t["q"], nxt_o["q"] if nxt_o else None, t.action, t.reward, t.mask,
+        if fused:
+            # ONE launch for the online / target [/ double-Q] head forwards + target / loss / PER block + head backward
+            heads = self._heads()
+            r = ops.dqn_head_fused(out.detach(), nxt_t, nxt_o, heads[0], heads[1], t.action, t.reward, t.mask, self.gamma_n,
+                                   tail.db4, two=plan.head == "fused-two", **per)
+            root, grad = out, r["gphi"]
+        elif self.kind == "dqn":
+            root = out["q"]
+            r = ops.dqn_loss_fused(root.detach(), nxt_t["q"], nxt_o["q"] if nxt_o else None, t.action, t.reward, t.mask,
                                    self.gamma_n, **per)
             grad = r["dq"]
         elif self.kind == "c51":
-            head = out["log_prob"]
-            r = ops.c51_loss_fused(head.detach(), nxt_t["prob"], nxt_o["prob"] if nxt_o else None, t.action, t.reward,
+            root = out["log_prob"]
+            r = ops.c51_loss_fused(root.detach(), nxt_t["prob"], nxt_o["prob"] if nxt_o else None, t.action, t.reward,
                                    t.mask, self.gamma_n, self.cat[0], self.cat[1], **per)
             grad = r["dlogp"]
         else:
-            head = out["quantile"]
-            r = ops.qr_loss_fused(head.detach(), nxt_t["quantile"], t.action, t.reward, t.mask, self.gamma_n)
+            root = out["quantile"]
+            r = ops.qr_loss_fused(root.detach(), nxt_t["quantile"], t.action, t.reward, t.mask, self.gamma_n)
             grad = r["dquant"]
         if self.per:
             if self.prefetch:                            # the sum tree is read by the prefetch branch: update after it
                 cur.wait_event(self._sampled_ev)
-            rp.update_priorities((t.idx, r["priority"]))
-        nature_tc.mark("loss")
+            self.replay.update_priorities((t.idx, r["priority"]))
+        nature_tc.mark("head" if fused else "loss")
+        if fused:
+            nature_tc.premask(grad, tail.db4)            # already masked by relu(fc4); its column sums are in the tail's db4
         if tail is None:
             self.opt.zero_grad()
-        fired = []
-        if ring_pre:
-            # forked right after the launch of conv1's weight gradient from the ring, beside the rest of the backward pass and
-            # the update tail (kernels A / B)
-            nature_tc.AFTER_RING_READ = lambda stream: fired or (self._prefetch_branch(parity, after=stream), fired.append(1))
-        elif late and os.environ.get("B2RL_PREFETCH_AT", "end") == "dgrad":
-            # option (B2RL_PREFETCH_AT=dgrad): fork the gather right after the last dgrad GEMM, beside the conv2 / conv1
-            # weight-gradient GEMMs.  The default forks after the backward pass: beside the weight gradients the gather slows the
-            # conv1 weight gradient and kernel A
-            nature_tc.AFTER_DGRAD = lambda: (self._prefetch_branch(parity, "gather"), fired.append(1))
+        # the late prefetch fork: after conv1's weight gradient from the ring (beside the rest of the backward pass and the
+        # update tail), after the last dgrad GEMM, or -- the fallback when neither fired -- after the backward pass
+        fired, phase = [], None if plan.prefetch == "after-ring-read" else "gather"
+        fork = lambda after=None: fired or (self._prefetch_branch(parity, phase, after), fired.append(1))
+        nature_tc.AFTER_RING_READ = fork if plan.prefetch == "after-ring-read" else None
+        nature_tc.AFTER_DGRAD = fork if plan.prefetch == "gather-after-dgrad" else None
         try:
             with nature_tc.wgrad_stream(None if side is cur else side), nature_tc.grad_sink(tail):   # weight-gradient GEMMs on the side branch
-                head.backward(grad)
+                root.backward(grad)
         finally:
-            nature_tc.AFTER_DGRAD = None
-            nature_tc.AFTER_RING_READ = None
-        nature_tc.mark("bwd_done")
+            nature_tc.AFTER_DGRAD = nature_tc.AFTER_RING_READ = None
+        if not fused:
+            nature_tc.mark("bwd_done")
         self.loss.copy_(r["loss"])
-        if late or ring_pre:
-            if not fired:                                # (no ring read in the backward pass: fork after it)
-                self._prefetch_branch(parity, None if ring_pre else "gather")
-            if getattr(self, "_one_graph", True):
-                self._late_join = True                   # joined after the optimizer kernels (_opt)
-            else:
-                cur.wait_stream(pre)                     # split-graph form: joined inside the first graph
-        elif self.prefetch:
+        if plan.prefetch not in (None, "start"):
+            fork()
+        if plan.join == "main":
             cur.wait_stream(pre)
 
     def _prefetch_branch(self, parity, phase=None, after=None):
@@ -317,77 +363,48 @@ class GraphedDQNLearner:
                 self._sampled_ev.record(pre)
                 nature_tc.mark("sampled")
 
-    def _main_fused_head(self, t, per, heads, tail, fs):
-        """DQN with a VanillaNet / DuelingNet head: bodies on the wgmma kernels, then ONE launch for the online / target
-        [/ double-Q] head forwards + target / loss / PER block + head backward (csrc/head.cu dqn_head_fused_kernel)."""
-        cur, side = torch.cuda.current_stream(), self._side
-        side.wait_stream(cur)
-        with torch.cuda.stream(side), frame_scale(fs), torch.no_grad():
-            phi_t = self.tgt.body(t.next_state)
-        with frame_scale(fs):
-            with torch.no_grad():
-                phi_o = self.net.body(t.next_state) if self.double_q else None
-            phi = self.net.body(t.state)
-        cur.wait_stream(side)
-        nature_tc.mark("fwd_joined")
-        r = ops.dqn_head_fused(phi.detach(), phi_t, phi_o, heads[0], heads[1], t.action, t.reward, t.mask, self.gamma_n,
-                               tail.db4, two=os.environ.get("B2RL_FUSED_HEAD", "0") != "one", **per)
-        if self.per:
-            if self.prefetch:                            # the sum tree is read by the prefetch branch: update after it
-                cur.wait_event(self._sampled_ev)
-            self.replay.update_priorities((t.idx, r["priority"]))
-        gphi = r["gphi"]
-        nature_tc.mark("head")
-        nature_tc.premask(gphi, tail.db4)                # already masked by relu(fc4); its column sums are in the tail's db4
-        with nature_tc.wgrad_stream(side), nature_tc.grad_sink(tail):
-            phi.backward(gphi)
-        self.loss.copy_(r["loss"])
-
-    def _repack(self, net, fs):
+    def _repack(self, net):
         """wgmma backend: the learner owns the packed bf16 operands of both networks -- the online body is re-packed
         once per update (one launch), the target body only when it is synchronised."""
         body = getattr(net, "body", None)
         if body is not None and hasattr(body, "repack") and self.dtype == torch.bfloat16:
             body.auto_repack = False
-            body.repack(fs)
+            body.repack(self.scale)
+
+    def repack_online(self):
+        """Bring the online network's packed bf16 operands up to date after ``update()``, for a forward outside the learner
+        (the actor).  The fused tail's optimizer kernel writes them itself; without it this is one re-pack launch."""
+        if self.tail() is None:
+            self._repack(self.net)
 
     def sync_target(self):
         self.tgt.load_state_dict(self.net.state_dict())        # DQN_agent.py:136-138
-        self._repack(self.tgt, self.scale if self.dtype == torch.bfloat16 else 1.0)
+        self._repack(self.tgt)
         self._refresh_head_operands(False)
 
     def _opt(self):
-        self._opt_kernels()
-        if getattr(self, "_late_join", False):           # the late prefetch branch ran beside the update tail
-            torch.cuda.current_stream().wait_stream(self._pre)
-            self._late_join = False
-
-    def _opt_kernels(self):
         tail = self.tail()
         if tail is not None:
             tail.step(max_norm=self.clip, grad_scale=1.0 / self.world, reduced_elsewhere=self.world > 1)
-            nature_tc.mark("opt")
         else:
             self.opt.step(max_norm=self.clip, grad_scale=1.0 / self.world)
-            nature_tc.mark("opt")
+        nature_tc.mark("opt")
+        if self.plan.join == "opt":                      # the late prefetch branch ran beside the update tail
+            torch.cuda.current_stream().wait_stream(self._pre)
 
     def refresh_packed(self):
         """Re-derive the packed bf16 operands of both networks from the fp32 parameters (after the parameters were changed
         from outside: load_state_dict, a broadcast, a copied arena)."""
-        fs = self.scale if self.dtype == torch.bfloat16 else 1.0
-        self._repack(self.net, fs)
-        self._repack(self.tgt, fs)
+        self._repack(self.net)
+        self._repack(self.tgt)
         self._refresh_head_operands(True)
-
-    def _dist_fc(self, net):
-        return getattr(net, "fc_categorical", None) or getattr(net, "fc_quantiles", None)
 
     def _refresh_head_operands(self, online):
         """Distributional heads (C51 / QR-DQN) on the wgmma GEMM: the online head reads its bf16 weight from the optimizer's
         arena-wide bf16 shadow (written by the fused optimizer kernel), the target head from a copy refreshed at target sync."""
-        if self.kind not in ("c51", "qr") or self.tail() is None or os.environ.get("B2RL_DIST_HEAD", "1") == "0":
+        if not self.plan.dist_head or self.tail() is None:
             return
-        fa, ft = self._dist_fc(self.net), self._dist_fc(self.tgt)
+        fa, ft = (getattr(n, "fc_categorical", None) or getattr(n, "fc_quantiles", None) for n in (self.net, self.tgt))
         if not isinstance(fa, torch.nn.Linear) or not isinstance(ft, torch.nn.Linear) or fa.weight.data_ptr() % 16:
             return
         o = self.opt
@@ -410,9 +427,7 @@ class GraphedDQNLearner:
         # the bytes) is all-reduced asynchronously right after its weight-gradient GEMM, beside the convolution backward, the
         # small remainder after the last GEMM.  B2RL_NCCL_IN_GRAPH=0: [sample..backward] graph | eager all-reduce of the whole
         # arena | [clip + optimizer] graph (the older form; it exposes the whole all-reduce).
-        one_graph = self.world == 1 or os.environ.get("B2RL_NCCL_IN_GRAPH", "1") == "1"
-        self._one_graph = one_graph      # (the late prefetch branch is joined after the optimizer kernels: one graph only)
-        self._overlap = self.world > 1 and one_graph and self.tail() is not None
+        self._overlap = self.world > 1 and self.plan.one_graph and self.tail() is not None
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
@@ -426,18 +441,17 @@ class GraphedDQNLearner:
         torch.cuda.synchronize()
         self.g_main, self.g_opt = [], None
         try:
-            self._capture_main(with_h2d, one_graph)
+            self._capture_main(with_h2d)
         except Exception as e:                            # noqa: BLE001 -- any capture error: use the split form
-            if self.world == 1 or not one_graph:
+            if self.world == 1 or not self.plan.one_graph:
                 raise
             print("b2rl: NCCL capture failed (%s); using the split-graph form" % str(e).splitlines()[0], file=sys.stderr)
             torch.cuda.synchronize()
-            one_graph = False
-            self._one_graph = False
+            self._plan = self._resolve_plan(one_graph=False)
             self._overlap = False
             self.g_main = []
-            self._capture_main(with_h2d, False)
-        if not one_graph:                                # [sample..backward] | NCCL all-reduce | [clip+opt]
+            self._capture_main(with_h2d)
+        if not self.plan.one_graph:                      # [sample..backward] | NCCL all-reduce | [clip+opt]
             self.g_opt = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.g_opt):
                 self._opt()
@@ -447,14 +461,14 @@ class GraphedDQNLearner:
         self.launches_per_update = None
         return self
 
-    def _capture_main(self, with_h2d, one_graph):
+    def _capture_main(self, with_h2d):
         for parity in ((0, 1) if self.prefetch else (None,)):
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, pool=self.g_main[0].pool() if self.g_main else None):
                 if with_h2d:
                     self._h2d()
                 self._main(parity)
-                if one_graph:
+                if self.plan.one_graph:
                     self._allreduce()
                     self._opt()
             self.g_main.append(g)
@@ -474,7 +488,7 @@ class GraphedDQNLearner:
         if tail is not None and self._overlap:
             for lo, hi in tail.late_slices:
                 parallel.allreduce_gradients(self.opt.grad[lo:hi])
-            if getattr(self, "_early_work", None) is not None:
+            if self._early_work is not None:
                 self._early_work.wait()
                 self._early_work = None
         else:
@@ -515,16 +529,9 @@ class GraphedDQNLearner:
         return self.h_pack.numel()
 
 
-class GraphedPPOLearner:
-    """The PPO minibatch update (PPO_agent.py:73-99, non-shared representation) as ONE captured graph replayed once per
-    minibatch: row gather by a device-resident index matrix, network forward, ``b2rl_ppo_loss`` (clipped surrogate, value
-    loss, approx-KL and their gradients in one launch), backward, KL-GATED actor Adam step (``b2rl_clip_adam_gated``: the
-    reference's ``if approx_kl <= 1.5 * target_kl`` decided on the device) and the critic Adam step.  An iteration of
-    examples.py:496-522 is 5 120 such updates of an 11 k-parameter MLP: eager, each is dominated by Python and launch
-    latency; as a graph replay the host cost is one ``cudaGraphLaunch``.
-
-    The rollout rows live in persistent device buffers (``load``); the minibatch index rows of ALL epochs are uploaded
-    once per iteration (``set_batches``) and consumed through a device cursor."""
+class _PPOLearner:
+    """What both PPO learners share: the rollout rows in persistent device buffers (``load``), the minibatch index rows of
+    ALL epochs of an iteration uploaded once (``set_batches``) and the statistics of the last update."""
 
     KEYS = ("state", "action", "log_pi_a", "ret", "advantage")
 
@@ -532,15 +539,12 @@ class GraphedPPOLearner:
                  entropy_weight, target_kl, max_batches):
         self.net, self.actor_opt, self.critic_opt = network, actor_opt, critic_opt
         self.mb, self.clip, self.ent_w, self.target_kl = int(mini_batch_size), ppo_ratio_clip, entropy_weight, target_kl
-        dev = actor_opt.flat.device
+        dev = self.dev = actor_opt.flat.device
         f = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)
         self.buf = dict(state=f(rows, state_dim), action=f(rows, action_dim), log_pi_a=f(rows, 1), ret=f(rows, 1),
                         advantage=f(rows, 1))
         self.perm = torch.zeros((max_batches, self.mb), dtype=torch.int64, device=dev)
-        self.cursor = torch.zeros(1, dtype=torch.int64, device=dev)
         self.stats = torch.zeros(4, dtype=torch.float32, device=dev)      # policy loss, value loss, approx KL of the last update
-        self.graph = None
-        self.dev = dev
 
     def load(self, entries):
         for k in self.KEYS:
@@ -550,8 +554,27 @@ class GraphedPPOLearner:
         rows = np.stack([np.asarray(r, dtype=np.int64) for r in index_rows])
         assert rows.shape[1] == self.mb and rows.shape[0] <= self.perm.shape[0]
         self.perm[:rows.shape[0]].copy_(torch.from_numpy(rows), non_blocking=False)
-        self.cursor.zero_()
         return rows.shape[0]
+
+
+class GraphedPPOLearner(_PPOLearner):
+    """The PPO minibatch update (PPO_agent.py:73-99, non-shared representation) as ONE captured graph replayed once per
+    minibatch: row gather by a device-resident index matrix, network forward, ``b2rl_ppo_loss`` (clipped surrogate, value
+    loss, approx-KL and their gradients in one launch), backward, KL-GATED actor Adam step (``b2rl_clip_adam_gated``: the
+    reference's ``if approx_kl <= 1.5 * target_kl`` decided on the device) and the critic Adam step.  An iteration of
+    examples.py:496-522 is 5 120 such updates of an 11 k-parameter MLP: eager, each is dominated by Python and launch
+    latency; as a graph replay the host cost is one ``cudaGraphLaunch``.  The minibatch index rows (``set_batches``) are
+    consumed through a device cursor."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.cursor = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self.graph = None
+
+    def set_batches(self, index_rows):
+        n = super().set_batches(index_rows)
+        self.cursor.zero_()
+        return n
 
     def _step(self):
         idx = self.perm.index_select(0, self.cursor).view(-1)
@@ -605,14 +628,13 @@ class GraphedPPOLearner:
             self.graph.replay()
 
 
-class PersistentPPOLearner:
+class PersistentPPOLearner(_PPOLearner):
     """The whole minibatch loop of a PPO iteration (PPO_agent.py:68-99, non-shared representation) as ONE launch of one
     persistent thread block (``b2rl_ppo_minibatch_updates``, csrc/ppo_persistent.cu): weights in shared memory, Adam moments in
     L2, the rows of the next minibatch fetched during the current update, the KL gate decided on the device.  Same interface as
     ``GraphedPPOLearner`` (which replays ~45 small kernels per update and remains the path for every network this kernel does
     not cover)."""
 
-    KEYS = GraphedPPOLearner.KEYS
     A_NAMES = ("actor_body.layers.0.weight", "actor_body.layers.0.bias", "actor_body.layers.1.weight",
                "actor_body.layers.1.bias", "fc_action.weight", "fc_action.bias", "std")
     C_NAMES = ("critic_body.layers.0.weight", "critic_body.layers.0.bias", "critic_body.layers.1.weight",
@@ -640,18 +662,11 @@ class PersistentPPOLearner:
 
     def __init__(self, network, actor_opt, critic_opt, rows, state_dim, action_dim, mini_batch_size, ppo_ratio_clip,
                  entropy_weight, target_kl, max_batches, world=1, rank=0, exchange_timeout_s=5.0):
-        self.net, self.actor_opt, self.critic_opt = network, actor_opt, critic_opt
-        self.mb, self.clip, self.ent_w, self.target_kl = int(mini_batch_size), ppo_ratio_clip, entropy_weight, target_kl
-        self.world, self.rank, self.rows = int(world), int(rank), int(rows)
         if actor_opt.kind != "adam" or critic_opt.kind != "adam":
             raise NotImplementedError("the persistent PPO kernel implements Adam (examples.py:508-509)")
-        dev = actor_opt.flat.device
-        self.dev = dev
-        f = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)
-        self.buf = dict(state=f(rows, state_dim), action=f(rows, action_dim), log_pi_a=f(rows, 1), ret=f(rows, 1),
-                        advantage=f(rows, 1))
-        self.perm = torch.zeros((max_batches, self.mb), dtype=torch.int64, device=dev)
-        self.stats = torch.zeros(4, dtype=torch.float32, device=dev)
+        super().__init__(network, actor_opt, critic_opt, rows, state_dim, action_dim, mini_batch_size, ppo_ratio_clip,
+                         entropy_weight, target_kl, max_batches)
+        self.world, self.rank, self.rows = int(world), int(rank), int(rows)
         named = dict(network.named_parameters())
         self.a_off = self._offsets(actor_opt, [named[n] for n in self.A_NAMES])
         self.c_off = self._offsets(critic_opt, [named[n] for n in self.C_NAMES])
@@ -664,8 +679,8 @@ class PersistentPPOLearner:
             # data parallel (one process per GPU): every update exchanges the ranks' gradients inside the kernel, through
             # exchange regions mapped into every peer (parallel.ExchangeRegions); seq = updates exchanged so far
             a_n, c_n = actor_opt.flat.numel(), critic_opt.flat.numel()
-            self.exchange = parallel.ExchangeRegions(int(_lib.lib().b2rl_ppo_dp_region_bytes(a_n, c_n)), dev)
-            self.status = torch.zeros(1, dtype=torch.int64, device=dev)
+            self.exchange = parallel.ExchangeRegions(int(_lib.lib().b2rl_ppo_dp_region_bytes(a_n, c_n)), self.dev)
+            self.status = torch.zeros(1, dtype=torch.int64, device=self.dev)
             self.seq = 0
             self.timeout_ns = int(exchange_timeout_s * 1e9)
 
@@ -689,16 +704,6 @@ class PersistentPPOLearner:
             offs.append(off)
         return torch.tensor(offs, dtype=torch.int32)
 
-    def load(self, entries):
-        for k in self.KEYS:
-            self.buf[k].copy_(getattr(entries, k).reshape(self.buf[k].shape))
-
-    def set_batches(self, index_rows):
-        rows = np.stack([np.asarray(r, dtype=np.int64) for r in index_rows])
-        assert rows.shape[1] == self.mb and rows.shape[0] <= self.perm.shape[0]
-        self.perm[:rows.shape[0]].copy_(torch.from_numpy(rows), non_blocking=False)
-        return rows.shape[0]
-
     def capture(self, warmup=0):
         return self
 
@@ -707,24 +712,17 @@ class PersistentPPOLearner:
         if self.world > 1:
             self.check_exchange()                      # (the previous iteration's launch)
             n_batches = parallel.agree(n_batches, self.dev, "PPO minibatches per iteration")
-            _lib.call("b2rl_ppo_minibatch_updates_dp", _lib.ptr(b["state"]), _lib.ptr(b["action"]), _lib.ptr(b["log_pi_a"]),
-                      _lib.ptr(b["ret"]), _lib.ptr(b["advantage"]), self.D, self.A, self.H1, self.H2, self.mb,
-                      _lib.ptr(self.perm), int(n_batches), _lib.ptr(a.flat), _lib.ptr(a.s1), _lib.ptr(a.s2),
-                      _lib.ptr(a.step_dev), _lib.ptr(self.a_off), _lib.ptr(c.flat), _lib.ptr(c.s1), _lib.ptr(c.s2),
-                      _lib.ptr(c.step_dev), _lib.ptr(self.c_off), float(a.lr), float(a.betas[0]), float(a.betas[1]), float(a.eps),
-                      float(c.lr), float(c.betas[0]), float(c.betas[1]), float(c.eps), float(self.clip), float(self.ent_w),
-                      float(1.5 * self.target_kl), _lib.ptr(self.stats), self.rows, a.flat.numel(), c.flat.numel(), self.world,
-                      self.rank, self.exchange.table, self.seq, self.timeout_ns, _lib.ptr(self.status), 1, _lib.stream())
+        args = (*[_lib.ptr(b[k]) for k in self.KEYS], self.D, self.A, self.H1, self.H2, self.mb, _lib.ptr(self.perm),
+                int(n_batches), *[_lib.ptr(t) for t in (a.flat, a.s1, a.s2, a.step_dev, self.a_off)],
+                *[_lib.ptr(t) for t in (c.flat, c.s1, c.s2, c.step_dev, self.c_off)],
+                *[float(x) for x in (a.lr, a.betas[0], a.betas[1], a.eps, c.lr, c.betas[0], c.betas[1], c.eps)],
+                float(self.clip), float(self.ent_w), float(1.5 * self.target_kl), _lib.ptr(self.stats))
+        if self.world > 1:
+            _lib.call("b2rl_ppo_minibatch_updates_dp", *args, self.rows, a.flat.numel(), c.flat.numel(), self.world, self.rank,
+                      self.exchange.table, self.seq, self.timeout_ns, _lib.ptr(self.status), 1, _lib.stream())
             self.seq_last = self.seq
             self.seq += int(n_batches)
-            self.n = int(n_batches)
-            return
-        _lib.call("b2rl_ppo_minibatch_updates", _lib.ptr(b["state"]), _lib.ptr(b["action"]), _lib.ptr(b["log_pi_a"]),
-                  _lib.ptr(b["ret"]), _lib.ptr(b["advantage"]), self.D, self.A, self.H1, self.H2, self.mb, _lib.ptr(self.perm),
-                  int(n_batches), _lib.ptr(a.flat), _lib.ptr(a.s1), _lib.ptr(a.s2), _lib.ptr(a.step_dev), _lib.ptr(self.a_off),
-                  _lib.ptr(c.flat), _lib.ptr(c.s1), _lib.ptr(c.s2), _lib.ptr(c.step_dev), _lib.ptr(self.c_off),
-                  float(a.lr), float(a.betas[0]), float(a.betas[1]), float(a.eps), float(c.lr), float(c.betas[0]),
-                  float(c.betas[1]), float(c.eps), float(self.clip), float(self.ent_w), float(1.5 * self.target_kl),
-                  _lib.ptr(self.stats), _lib.stream())
+        else:
+            _lib.call("b2rl_ppo_minibatch_updates", *args, _lib.stream())
         self.n = int(n_batches)         # (the one launch is counted by _lib.call itself; launches_per_update stays 0)
 

@@ -19,7 +19,7 @@ rl.select_device(0)
 rl.Config.COMPUTE_DTYPE = torch.bfloat16
 bench.CAP = a.capacity
 learner = bench.build_learner(rl, a.workload, torch.device("cuda", 0), 0, 1, prefetch=(a.replay == "async"))
-learner._repack(learner.tgt, learner.scale)          # as capture() does: the target operands are packed at sync time only
+learner.refresh_packed()                             # as capture() does: the target operands are otherwise packed at sync only
 for _ in range(2):                                     # warm-up (cuDNN plan selection)
     learner._main(), learner._opt()
 torch.cuda.synchronize()
