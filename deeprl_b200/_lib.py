@@ -82,6 +82,9 @@ SIGNATURES = {
     "b2rl_nstep_dqn_actor_step": [c_i32, c_p, c_f64, c_p, c_p] + [c_i32] * 5 + [c_f32, c_p, c_p, c_p, c_u64, c_p, c_p],
     "b2rl_nstep_dqn_update": ([c_i32] + [c_p] * 4 + [c_i32] * 6 + [c_p, c_p, c_i32] + [c_p] * 4 + [c_f32] * 3 + [c_i32]
                               + [c_f32] * 2 + [c_p, c_p]),
+    "b2rl_dqn_replay_smem_bytes": [c_i32] * 7,
+    "b2rl_dqn_replay_update": ([c_i32, c_i32, c_p, c_p, c_i32, c_f64, c_p, c_p, c_p] + [c_i32] * 5 + [c_p] * 6 + [c_f32] * 3
+                               + [c_i32, c_f32, c_i32, c_f32, c_p] + [c_f32] * 3 + [c_p] * 4),
     "b2rl_ipc_alloc": [c_i64, c_p],
     "b2rl_ipc_get_handle": [c_p, c_p],
     "b2rl_ipc_open_handle": [c_p, c_p],
@@ -159,6 +162,7 @@ def lib():
             fn.restype = ctypes.c_int
         L.b2rl_a2c_smem_bytes.restype = ctypes.c_int64       # (a size, not a status)
         L.b2rl_nstep_dqn_smem_bytes.restype = ctypes.c_int64
+        L.b2rl_dqn_replay_smem_bytes.restype = ctypes.c_int64
         _lib = L
     return _lib
 

@@ -9,6 +9,12 @@ sum-tree priority update on the device (``csrc/sumtree.cu``).  Nothing of the up
 ``compute_loss`` / ``reduce_loss`` keep the reference's contract (per-sample tensor, then reduction,
 DQN_agent.py:78-99) and differentiate through the same kernel; a subclass that overrides either is served by
 the generic autograd path in ``_generic_update``.
+
+``config.device_dqn = True`` (off by default) runs a VanillaNet / DuelingNet on a two-layer FCBody (``dqn_feature``) on the
+device: one ``b2rl_nstep_dqn_actor_step`` launch per env step (epsilon-greedy on the device's Philox stream, not numpy's) and
+one ``b2rl_dqn_replay_update`` launch per gradient update on the batch ``replay.sample()`` returns (csrc/a2c.cu,
+component/actor.py ``DeviceDQN``).  Configurations the kernels do not cover raise ``NotImplementedError`` naming the unmet
+condition.
 """
 import threading
 
@@ -53,6 +59,12 @@ class DQNActor(BaseActor):
         if self._state is None:
             self._state = self._task.reset()
         config = self.config
+        dev = getattr(self, "_device_dqn", None)
+        if dev is not None:                                # config.device_dqn: rescale + forward + epsilon-greedy, one launch
+            epsilon = 1 if self._total_steps < config.exploration_steps else config.random_action_prob()
+            with config.lock:
+                action = dev.act(self._state, epsilon)
+            return self._env_step(action)
         if config.noisy_linear:
             self._network.reset_noise()
         ga = self._graphed() if getattr(config, "cuda_graph", False) else None
@@ -70,6 +82,9 @@ class DQNActor(BaseActor):
         else:
             epsilon = config.random_action_prob()
         action = epsilon_greedy(epsilon, q_values)
+        return self._env_step(action)
+
+    def _env_step(self, action):
         next_state, reward, done, info = self._task.step(action)
         entry = [self._state, action, reward, next_state, done, info]
         self._total_steps += 1
@@ -110,6 +125,11 @@ class DQNAgent(BaseAgent):
         self.actor.set_network(self.network)
         self.total_steps = 0
         self.last_loss = None
+        self.device_dqn = None
+        if getattr(config, "device_dqn", False):
+            from ..component.actor import DeviceDQN
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
+            self.device_dqn = self.actor._device_dqn = DeviceDQN(self, seed)
 
     def close(self):
         close_obj(self.replay)
@@ -252,7 +272,9 @@ class DQNAgent(BaseAgent):
             for d in feeds:
                 self.replay.feed(d)
 
-        if self.total_steps > config.exploration_steps and self._graph_ok():
+        if self.total_steps > config.exploration_steps and self.device_dqn is not None:
+            self._device_update()                          # config.device_dqn: the whole update is one launch
+        elif self.total_steps > config.exploration_steps and self._graph_ok():
             self._graph_update()                           # config.cuda_graph: the whole update is one graph replay
         elif self.total_steps > config.exploration_steps:
             transitions = self._sample()
@@ -266,10 +288,25 @@ class DQNAgent(BaseAgent):
                     self.last_loss = self._fused_update(transitions)
 
         if self.total_steps / config.sgd_update_frequency % config.target_network_update_freq == 0:
-            if getattr(self, "_learner", None) is not None:
+            if self.device_dqn is not None:
+                self.device_dqn.sync_target()              # one copy of the online arena into the target arena
+            elif getattr(self, "_learner", None) is not None:
                 self._learner.sync_target()                # load_state_dict + re-pack of the target's bf16 operands
             else:
                 self.target_network.load_state_dict(self.network.state_dict())
+
+    # ------------------------------------------------------------------ config.device_dqn (opt-in)
+    def _device_update(self):
+        """DQN_agent.py:115-134 for the batch ``replay.sample()`` returns (sync or async wrapper, uniform or prioritized) as
+        ONE ``b2rl_dqn_replay_update`` launch; the new priorities go to the tree from the device (:120-123)."""
+        config = self.config
+        transitions = self.replay.sample()
+        per = isinstance(transitions, PrioritizedTransition)
+        beta = config.replay_beta() if per else 0.0
+        with config.lock:                                  # the actor reads the shared parameters (DQN_agent.py:30,133)
+            self.last_loss, priority = self.device_dqn.update(transitions, beta)
+        if per:
+            self.replay.update_priorities((transitions.idx, priority))
 
     # ------------------------------------------------------------------ config.cuda_graph (opt-in)
     _graph_kind = "dqn"

@@ -509,3 +509,140 @@ class DeviceNStepDQN(_DeviceRollout):
                   _lib.ptr(o.s1), _lib.ptr(o.s2), _lib.ptr(o.step_dev), self._off, float(o.lr), float(o.alpha), float(o.eps),
                   int(o.centered), float(c.discount), float(c.gradient_clip), _lib.ptr(loss), _lib.stream())
         return loss
+
+
+# ------------------------------------------------------------------------------------------------ replay DQN on the device
+def dqn_kernel_order(net):
+    """A VanillaNet's / DuelingNet's parameters in the kernels' tensor order: w1 b1 w2 b2, then fc_head.w fc_head.b, or
+    fc_advantage.w fc_advantage.b fc_value.w fc_value.b."""
+    from ..network.network_heads import DuelingNet
+    body = [t for m in net.body.layers for t in (m.weight, m.bias)]
+    if isinstance(net, DuelingNet):
+        return body + [net.fc_advantage.weight, net.fc_advantage.bias, net.fc_value.weight, net.fc_value.bias]
+    return body + [net.fc_head.weight, net.fc_head.bias]
+
+
+def dqn_unsupported(agent):
+    """``None`` when ``config.device_dqn``'s kernels (csrc/a2c.cu: b2rl_nstep_dqn_actor_step, b2rl_dqn_replay_update) cover
+    this ``DQNAgent``, else the unmet condition."""
+    import torch.nn.functional as F
+
+    from ..network.network_bodies import NatureConvBody
+    from ..network.network_heads import DuelingNet, VanillaNet
+    from ..utils.normalizer import RescaleNormalizer
+    config, network = agent.config, agent.network
+    if type(network) not in (VanillaNet, DuelingNet):
+        return ("the network is a %s; the device kernels implement VanillaNet and DuelingNet (C51, QR and Rainbow heads are "
+                "not covered)" % type(network).__name__)
+    if agent._uses_reference_hooks():
+        return "%s overrides compute_loss / reduce_loss; the device update implements DQNAgent's" % type(agent).__name__
+    body = network.body
+    if isinstance(body, NatureConvBody):
+        return "the body is a NatureConvBody; the device kernels implement a two-layer FCBody"
+    if not isinstance(body, FCBody):
+        return "the network needs an FCBody body (got %s)" % type(body).__name__
+    if body.noisy_linear or config.noisy_linear:
+        return "the network has NoisyLinear layers; the device kernels implement nn.Linear"
+    if len(body.layers) != 2:
+        return "the device kernels implement a two-layer FCBody (got %d layers)" % len(body.layers)
+    if body.gate not in (torch.tanh, F.relu):
+        return "the FCBody gate must be torch.tanh or F.relu"
+    if not body.layers[0].weight.is_cuda:
+        return "the network is not on a CUDA device (select_device(0))"
+    head = network.fc_advantage if isinstance(network, DuelingNet) else network.fc_head
+    D, H1, H2, A = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features, head.out_features
+    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32:
+        return "sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32" % (D, H1, H2, A)
+    if not isinstance(agent.optimizer, torch.optim.RMSprop) or agent._flat is None:
+        return "the optimizer is %s; the device update implements RMSprop" % type(agent.optimizer).__name__
+    if type(config.state_normalizer) is not RescaleNormalizer:
+        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
+    if config.async_actor:
+        return "async_actor is set; the device actor runs in the agent's thread (async_actor=False)"
+    if config.history_length != 1:
+        return "history_length is %d; the device kernels read single 1-D states, not frame stacks" % config.history_length
+    smem = _lib.lib().b2rl_dqn_replay_smem_bytes(int(isinstance(network, DuelingNet)), D, H1, H2, A, int(config.batch_size),
+                                                 int(bool(config.double_q)))
+    if not 0 < smem <= 227 * 1024:
+        return ("a batch of %d needs %d bytes of shared memory, more than one SM has (b2rl_dqn_replay_smem_bytes)"
+                % (config.batch_size, smem))
+    return None
+
+
+class DeviceDQN(_DeviceRollout):
+    """``DQNAgent.step()`` on the device (``config.device_dqn``): one ``b2rl_nstep_dqn_actor_step`` launch per env step
+    (rescale, forward, epsilon-greedy on the device's Philox stream) and one ``b2rl_dqn_replay_update`` launch per gradient
+    update on the batch ``replay.sample()`` returned.  The update trains ``DQNAgent._flat``'s arena; the target network's
+    parameters become views into a second arena of the same layout (``target``), so the target sync is one device copy and both
+    modules' ``state_dict()`` are always current.
+
+    ``forced``: test hook -- a callable returning the actions of the next env step, which the actor step then writes through
+    unchanged instead of drawing."""
+
+    def __init__(self, agent, seed):
+        from ..network.network_heads import DuelingNet
+        why = dqn_unsupported(agent)
+        if why is not None:
+            raise NotImplementedError("config.device_dqn: " + why)
+        config, network = agent.config, agent.network
+        self.net, self.target_net, self.cfg = network, agent.target_network, config
+        body = network.body
+        self.head = int(isinstance(network, DuelingNet))
+        self.gate = 0 if body.gate is torch.tanh else 1
+        self.tensors = dqn_kernel_order(network)
+        self.opt = agent._flat
+        self.dev = self.opt.flat.device
+        self.target = torch.zeros_like(self.opt.flat)
+        with torch.no_grad():
+            for p, o in zip(agent.target_network.parameters(), self.opt.offsets):
+                k = p.numel()
+                self.target[o:o + k].copy_(p.detach().reshape(-1))
+                p.data = self.target[o:o + k].view_as(p)
+        self.N, self.T = int(config.num_workers), 1
+        self.D, self.H1, self.H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
+        self.A = self.tensors[4].shape[0]
+        self.acols = 1
+        self._buffers(seed)
+        self._dims = (self.D, self.H1, self.H2, self.A)
+        self._offsets()
+
+    def _offsets(self):
+        """``_arena_offsets``, and the check that the target parameters still live in the target arena."""
+        self._arena_offsets()
+        base = self.target.data_ptr()
+        for t, o in zip(dqn_kernel_order(self.target_net), self.off.tolist()):
+            if t.data_ptr() != base + 4 * o:
+                raise _lib.B2RLError("DeviceDQN: a target parameter no longer lives in the target arena")
+
+    def act(self, raw_obs, epsilon):
+        """One env step's actions: rescale + forward + epsilon-greedy in one launch, downloaded for ``task.step``."""
+        obs, given = self._stage(raw_obs)
+        _lib.call("b2rl_nstep_dqn_actor_step", self.gate + 2 * self.head, obs, self._scale, self._flat, self._off, *self._dims,
+                  self.N, float(epsilon), None, self._row_ptrs(0)[1], given, self.seed, _lib.ptr(self.counter), _lib.stream())
+        return self._fetch(0)[:, 0].astype(np.int64)
+
+    def update(self, tr, beta=0.0):
+        """One gradient update on a sampled batch (``Transition`` / ``PrioritizedTransition`` of device tensors).  Returns the
+        objective (0-dim device tensor) and, for a prioritized batch, the new priorities (float32 device tensor [B])."""
+        c, o = self.cfg, self.opt
+        s, s2 = tr.state, tr.next_state
+        if s.dtype not in (_f32, _f64) or s.dim() != 2 or s.shape[1] != self.D:
+            raise NotImplementedError("config.device_dqn: the replay returned %s states of shape %s; the device update reads "
+                                      "1-D float32 / float64 rows of %d" % (s.dtype, tuple(s.shape), self.D))
+        self._offsets()
+        B = s.shape[0]
+        per = getattr(tr, "sampling_prob", None) is not None
+        loss = torch.empty((), dtype=_f32, device=self.dev)
+        prio = torch.empty(B, dtype=_f32, device=self.dev) if per else None
+        ptr = lambda t: _lib.ptr(None if t is None else t.contiguous())
+        _lib.call("b2rl_dqn_replay_update", self.head, self.gate, ptr(s), ptr(s2), int(s.dtype == _f64), self._scale,
+                  ptr(tr.action), ptr(tr.reward), ptr(tr.mask), B, *self._dims, self._flat, _lib.ptr(self.target),
+                  _lib.ptr(o.s1), _lib.ptr(o.s2), _lib.ptr(o.step_dev), self._off, float(o.lr), float(o.alpha), float(o.eps),
+                  int(o.centered), float(c.discount ** c.n_step), int(bool(c.double_q)), float(c.gradient_clip or 0.0),
+                  ptr(tr.sampling_prob if per else None), float(beta), float(getattr(c, "replay_eps", 0.01)),
+                  float(getattr(c, "replay_alpha", 0.5)), ptr(prio), None, _lib.ptr(loss), _lib.stream())
+        return loss, prio
+
+    def sync_target(self):
+        """DQN_agent.py:136-138: the target arena becomes the online arena (one device copy)."""
+        self.target.copy_(self.opt.flat)

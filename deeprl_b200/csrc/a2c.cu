@@ -12,6 +12,9 @@
 //   b2rl_nstep_dqn_*      NStepDQNAgent.step() (NStepDQN_agent.py:26-67) for a VanillaNet on a two-layer FCBody the same way: an
 //                         actor step with epsilon-greedy on Philox uniforms, and one update launch (nstep_sequence.inc) that also
 //                         does the rollout's target sync.
+//   b2rl_dqn_replay_*     DQNAgent's gradient update (DQN_agent.py:81-134) for a VanillaNet or DuelingNet on a two-layer FCBody:
+//                         one launch on the sampled batch (dqn_sequence.inc); its actor step is b2rl_nstep_dqn_actor_step's
+//                         dqn_actor_kernel (DuelingNet head, no state row).
 //
 // sm_90a only.
 #include "common.cuh"
@@ -163,6 +166,109 @@ __global__ void __launch_bounds__(A2C_ACT_NT, 1) nstep_dqn_actor_kernel(const __
   if (tid == 0 && !a.given) *a.counter = ctr0 + 2 * (int64_t)a.N;
 }
 
+// ------------------------------------------------------------------------------------------------ replay Q (DQN_agent.py)
+// the actor step of the replay DQN agent: the forward of nstep_dqn_actor_kernel for a VanillaNet (HEAD = Q) or a DuelingNet
+// (HEAD = DUEL, which also needs fc_value and the q = v + (adv - mean(adv)) phase) and the same epsilon-greedy on the same
+// Philox stream; the state row is optional (the replay agent keeps no rollout arena).  A kernel of its own, so that the n-step
+// instantiations above keep their code.
+template <int HEAD, int GATE>
+__global__ void __launch_bounds__(A2C_ACT_NT, 1) dqn_actor_kernel(const __grid_constant__ A2cActorArgs a, float epsilon) {
+  using namespace b2rl_a2c;
+  pdl_sync();
+  extern __shared__ __align__(16) float a2c_smem[];
+  A2cShared S;
+  a2c_carve<HEAD, true>(S, a2c_smem, a.net.D, a.net.H1, a.net.H2, a.net.A, a.N, 0);
+  const int tid = threadIdx.x, NT = A2C_ACT_NT, D = a.net.D, A = a.net.A;
+  const int64_t ctr0 = *a.counter;
+  constexpr bool actor_only = HEAD == Q;
+  ph_load_weights<HEAD, true>(S, a.net, actor_only, tid, NT);
+  for (int e = tid; e < a.N * D; e += NT) {
+    const int n = e / D, k = e - n * D;
+    const float x = (float)(a.scale * a.obs[e]);
+    S.x[n * S.ldx + k] = x;
+    if (a.state_out) a.state_out[e] = x;
+  }
+  __syncthreads();
+  ph_fwd1<HEAD, true, GATE>(S, a.net, actor_only, tid, NT);
+  __syncthreads();
+  ph_fwd2<HEAD, true, GATE>(S, a.net, actor_only, tid, NT);
+  __syncthreads();
+  ph_heads<HEAD, true>(S, a.net, actor_only, tid, NT);
+  __syncthreads();
+  if (HEAD == DUEL) {
+    ph_duel_q(S, a.N, A, tid, NT);
+    __syncthreads();
+  }
+  for (int n = tid; n < a.N; n += NT) {
+    if (a.given) {
+      a.action_out[n] = a.given[n];
+      continue;
+    }
+    const uint64_t c = (uint64_t)(ctr0 + 2 * (int64_t)n);
+    int pick;
+    if (Philox::u24(a.seed, c, NSTEP_PHILOX_STREAM) < epsilon) {
+      pick = min((int)(Philox::u24(a.seed, c + 1, NSTEP_PHILOX_STREAM) * (float)A), A - 1);
+    } else {
+      const float* z = S.z + n * S.lda;
+      pick = 0;
+      for (int j = 1; j < A; ++j)
+        if (z[j] > z[pick]) pick = j;
+    }
+    a.action_out[n] = (float)pick;
+  }
+  if (tid == 0 && !a.given) *a.counter = ctr0 + 2 * (int64_t)a.N;
+}
+
+// DQNAgent's update for one sampled batch as ONE launch of one block (dqn_sequence.inc)
+template <int HEAD, int GATE>
+__global__ void __launch_bounds__(A2C_NT, 1) dqn_replay_update_kernel(const __grid_constant__ b2rl_a2c::DqnArgs d) {
+  using namespace b2rl_a2c;
+  pdl_sync();
+  extern __shared__ __align__(16) float a2c_smem[];
+  DqnShared DS;
+  dqn_carve<HEAD>(DS, a2c_smem, d.a.net.D, d.a.net.H1, d.a.net.H2, d.a.net.A, d.a.N, d.double_q);
+  A2cShared& S = DS.s;
+  const int NT = A2C_NT;
+#define A2C_PHASE(...) { const int tid = threadIdx.x; __VA_ARGS__; } __syncthreads();
+#include "dqn_sequence.inc"
+#undef A2C_PHASE
+}
+
+template <int HEAD, int GATE> struct DqnActorLaunch {
+  static void run(const A2cActorArgs& a, float epsilon, size_t smem, cudaStream_t st) {
+    static size_t attr = 0;
+    if (smem > attr) {
+      cudaFuncSetAttribute(dqn_actor_kernel<HEAD, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      attr = smem;
+    }
+    launch_pdl(dqn_actor_kernel<HEAD, GATE>, dim3(1), dim3(A2C_ACT_NT), smem, st, a, epsilon);
+  }
+};
+
+template <int HEAD, int GATE> struct DqnUpdateLaunch {
+  static void run(const b2rl_a2c::DqnArgs& d, size_t smem, cudaStream_t st) {
+    static size_t attr = 0;
+    if (smem > attr) {
+      cudaFuncSetAttribute(dqn_replay_update_kernel<HEAD, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      attr = smem;
+    }
+    launch_pdl(dqn_replay_update_kernel<HEAD, GATE>, dim3(1), dim3(A2C_NT), smem, st, d);
+  }
+};
+
+// the instantiated replay Q configurations: VanillaNet / DuelingNet (head 0 / 1) x tanh / ReLU
+template <template <int, int> class F, typename... Args>
+static void dqn_dispatch(int head, int gate, Args&&... args) {
+  using namespace b2rl_a2c;
+  if (head == 0) {
+    if (gate == TANH) F<Q, TANH>::run(args...);
+    else F<Q, RELU>::run(args...);
+  } else {
+    if (gate == TANH) F<DUEL, TANH>::run(args...);
+    else F<DUEL, RELU>::run(args...);
+  }
+}
+
 template <int GATE>
 static void nstep_update_launch(const b2rl_a2c::NStepArgs& q, size_t smem, cudaStream_t st) {
   static size_t attr = 0;
@@ -311,22 +417,78 @@ extern "C" int64_t b2rl_nstep_dqn_smem_bytes(int32_t D, int32_t H1, int32_t H2, 
   return (int64_t)nstep_bytes(D, H1, H2, A, (T + 1) * N, T * N);
 }
 
-extern "C" int b2rl_nstep_dqn_actor_step(int32_t gate, const double* obs, double obs_scale, const float* flat, const int32_t* off,
-                                         int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, float epsilon,
-                                         float* state_out, float* action_out, const float* given_action, uint64_t seed,
-                                         int64_t* counter, void* stream) {
+// net_kind = gate + 2 * head: gate 0 tanh / 1 ReLU, head 0 VanillaNet / 1 DuelingNet.  state_out may be NULL.
+extern "C" int b2rl_nstep_dqn_actor_step(int32_t net_kind, const double* obs, double obs_scale, const float* flat,
+                                         const int32_t* off, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N,
+                                         float epsilon, float* state_out, float* action_out, const float* given_action,
+                                         uint64_t seed, int64_t* counter, void* stream) {
+  B2RL_REQUIRE(net_kind >= 0 && net_kind <= 3, "net_kind must be gate (0 tanh, 1 relu) + 2 x head (0 VanillaNet, 1 DuelingNet)");
+  const int32_t gate = net_kind & 1, head = net_kind >> 1;
   NSTEP_CHECK_NET();
-  B2RL_REQUIRE(obs && state_out && action_out && counter, "null pointer");
+  B2RL_REQUIRE(obs && action_out && counter, "null pointer");
   B2RL_REQUIRE(N > 0 && N <= 1024, "N must be in [1, 1024]");
   A2cActorArgs a;
-  a.net = a2c_net(const_cast<float*>(flat), off, b2rl_a2c::Q, 1, D, H1, H2, A);
+  a.net = a2c_net(const_cast<float*>(flat), off, head ? b2rl_a2c::DUEL : b2rl_a2c::Q, 1, D, H1, H2, A);
   a.obs = obs; a.scale = obs_scale; a.N = N; a.state_out = state_out; a.action_out = action_out; a.given = given_action;
   a.seed = seed; a.counter = counter;
-  const size_t smem = nstep_bytes(D, H1, H2, A, N, 0);
+  b2rl_a2c::A2cShared probe;
+  const size_t smem = head ? b2rl_a2c::a2c_carve<b2rl_a2c::DUEL, true>(probe, reinterpret_cast<float*>(uintptr_t(4096)), D, H1,
+                                                                        H2, A, N, 0) * sizeof(float)
+                           : nstep_bytes(D, H1, H2, A, N, 0);
   B2RL_REQUIRE(smem <= 227 * 1024, "network / worker count too large for the shared memory of one SM");
-  if (gate == b2rl_a2c::TANH) nstep_actor_launch<b2rl_a2c::TANH>(a, epsilon, smem, (cudaStream_t)stream);
-  else nstep_actor_launch<b2rl_a2c::RELU>(a, epsilon, smem, (cudaStream_t)stream);
+  if (head == 0 && state_out) {                  // the n-step agent's form: the state row goes to its rollout arena
+    if (gate == b2rl_a2c::TANH) nstep_actor_launch<b2rl_a2c::TANH>(a, epsilon, smem, (cudaStream_t)stream);
+    else nstep_actor_launch<b2rl_a2c::RELU>(a, epsilon, smem, (cudaStream_t)stream);
+  } else {
+    dqn_dispatch<DqnActorLaunch>(head, gate, a, epsilon, smem, (cudaStream_t)stream);
+  }
   return check_launch("b2rl_nstep_dqn_actor_step");
+}
+
+// ------------------------------------------------------------------------------------------------ replay Q entry points
+static size_t dqn_bytes(int head, int D, int H1, int H2, int A, int B, int double_q) {
+  b2rl_a2c::DqnShared probe;
+  float* dummy = reinterpret_cast<float*>(uintptr_t(4096));
+  return (head ? b2rl_a2c::dqn_carve<b2rl_a2c::DUEL>(probe, dummy, D, H1, H2, A, B, double_q)
+               : b2rl_a2c::dqn_carve<b2rl_a2c::Q>(probe, dummy, D, H1, H2, A, B, double_q)) * sizeof(float);
+}
+
+// dynamic shared memory of the replay Q update for these sizes (the caller checks it against the 227 KB of one SM)
+extern "C" int64_t b2rl_dqn_replay_smem_bytes(int32_t head, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t B,
+                                              int32_t double_q) {
+  if (D <= 0 || H1 <= 0 || H2 <= 0 || A <= 0 || B <= 0 || (head != 0 && head != 1)) return 0;
+  return (int64_t)dqn_bytes(head, D, H1, H2, A, B, double_q != 0);
+}
+
+extern "C" int b2rl_dqn_replay_update(int32_t head, int32_t gate, const void* state, const void* next_state, int32_t state_f64,
+                                      double state_scale, const int64_t* action, const float* reward, const float* mask,
+                                      int32_t B, int32_t D, int32_t H1, int32_t H2, int32_t A, float* flat, const float* target,
+                                      float* square_avg, float* grad_avg, int64_t* step, const int32_t* off, float lr,
+                                      float alpha, float eps, int32_t centered, float discount_n, int32_t double_q,
+                                      float max_norm, const float* sampling_prob, float beta, float replay_eps,
+                                      float replay_alpha, float* priority_out, float* delta_out, float* loss, void* stream) {
+  NSTEP_CHECK_NET();
+  B2RL_REQUIRE(head == 0 || head == 1, "head must be 0 (VanillaNet) or 1 (DuelingNet)");
+  B2RL_REQUIRE(state && next_state && action && reward && mask && target && square_avg && step && loss &&
+                   (grad_avg || !centered) && (priority_out || !sampling_prob),
+               "null pointer");
+  B2RL_REQUIRE(B > 0, "bad batch size");
+  b2rl_a2c::DqnArgs d = {};
+  b2rl_a2c::A2cArgs& a = d.a;
+  a.net = a2c_net(flat, off, head ? b2rl_a2c::DUEL : b2rl_a2c::Q, 1, D, H1, H2, A);
+  a.N = B; a.T = 1;
+  a.sq = square_avg; a.ga = grad_avg; a.step = step;
+  a.lr = lr; a.alpha = alpha; a.eps = eps; a.centered = centered;
+  a.discount = discount_n; a.max_norm = max_norm; a.loss = loss;
+  d.state = state; d.next_state = next_state; d.f64 = state_f64 != 0; d.scale = state_scale;
+  d.action = action; d.reward = reward; d.mask = mask; d.target = target; d.double_q = double_q != 0;
+  d.prob = sampling_prob; d.beta = beta; d.per_eps = replay_eps; d.per_alpha = replay_alpha;
+  d.priority = priority_out; d.delta = delta_out;
+  const size_t smem = (size_t)b2rl_dqn_replay_smem_bytes(head, D, H1, H2, A, B, double_q);
+  B2RL_REQUIRE(smem > 0 && smem <= 227 * 1024,
+               "batch / network too large for the shared memory of one SM (b2rl_dqn_replay_smem_bytes)");
+  dqn_dispatch<DqnUpdateLaunch>(head, gate, d, smem, (cudaStream_t)stream);
+  return check_launch("b2rl_dqn_replay_update");
 }
 
 extern "C" int b2rl_nstep_dqn_update(int32_t gate, const float* states, const float* actions, const float* reward,

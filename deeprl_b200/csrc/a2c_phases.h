@@ -19,6 +19,10 @@
 //             clip_grad_norm_ (:63); RMSprop on the FlatOptimizer arena (:64)
 //   n-step Q  (NStepDQN_agent.py:26-67, nstep_sequence.inc) forward of the T N rollout rows, the target network on row block T
 //             and its max over actions (:56-57), the return scan (:58-60), 0.5 mean((q[a] - ret)^2) (:63), backward, clip, RMSprop
+//   replay Q  (DQN_agent.py:81-134, dqn_sequence.inc) HEAD = Q or DUEL (DuelingNet: q = v + (adv - mean(adv)), fc_advantage in
+//             the fc_action slot, fc_value in the fc_critic slot): forward of the B sampled states (and of the B next states
+//             with double_q), the target network on the next states, the TD target, delta, the PER priorities and importance
+//             weights, 0.5 mean((w delta)^2), backward, clip, RMSprop
 #pragma once
 #include <math.h>
 #include <stddef.h>
@@ -42,7 +46,7 @@
 
 namespace b2rl_a2c {
 
-enum { CAT = 0, GAUSS = 1, Q = 2 };      // head kind
+enum { CAT = 0, GAUSS = 1, Q = 2, DUEL = 3 };   // head kind
 enum { TANH = 0, RELU = 1, LINEAR = 2 }; // gate of a layer
 constexpr int A2C_MAX_TENSORS = 13;      // two trunks x (w1 b1 w2 b2) + fc_action w b + fc_critic w b + std
 constexpr int A2C_CHUNK = 64;            // gradient elements per partial sum of the global norm
@@ -426,6 +430,10 @@ A2C_FN void ph_head_wgrad(A2cShared& S, const A2cArgs& a, int tid, int NT) {
     return;
   }
   dense_wgrad(S.dv, 1, a2c_h(S, K::critic_trunk, 1), S.ldh, S.G + fc.woff, fc.ld, S.G + bc.woff, M, 1, net.H2, tid, NT);
+  if (HEAD == DUEL) {                                   // fc_value's gradient above; the objective of the Q head
+    if (tid == NT - 1) S.scal[0] = 0.5f * (sum4(S.red, M) * (1.0f / (float)M));
+    return;
+  }
   if (HEAD == GAUSS) {                                  // d / d std_param: summed over rows, then through softplus
     const TensorDesc sd = a2c_tensor(K::sd, K::ntr, net.D, net.H1, net.H2, A);
     const float invM = 1.0f / (float)M, gent = -a.ent_w * invM;
@@ -609,6 +617,196 @@ A2C_FN void ph_nstep_loss_grad(A2cShared& S, const A2cArgs& a, int tid, int NT) 
     const float err = A2C_SUB(S.z[(size_t)n * S.lda + an], S.ret[n]);
     S.dz[(size_t)n * S.lda + j] = j == an ? A2C_MUL(err, invM) : 0.0f;
     if (j == 0) S.red[n] = A2C_MUL(err, err);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ phases (replay Q)
+#ifdef __CUDACC__
+#define A2C_DIV(x, y) __fdiv_rn(x, y)
+#else
+#define A2C_DIV(x, y) ((x) / (y))
+#endif
+
+// the replay Q update's arguments besides A2cArgs, of which it reads net, the RMSprop fields, max_norm, loss, N (= B) and
+// discount (= discount ** n_step)
+struct DqnArgs {
+  A2cArgs a;
+  const void* state; const void* next_state;     // [B][D] sampled rows: float64 (f64) or float32
+  int f64; double scale;                         // RescaleNormalizer: float32(scale * double(x)), rounded once
+  const int64_t* action; const float* reward; const float* mask;   // [B]
+  const float* target;                           // the target network's arena: the layout of a.net.flat, the same offsets
+  int double_q;
+  const float* prob; float beta, per_eps, per_alpha;   // PER when prob is set: sampling probabilities [B], beta, eps, alpha
+  float* priority;                               // [B] (|delta| + eps)^alpha, PER only
+  float* delta;                                  // [B] y - q[a], optional
+};
+
+struct DqnShared {
+  A2cShared s;
+  float *delta, *wt;                             // [B] delta, importance weights before the max-normalisation
+};
+
+// the shared block of the replay Q update: x holds the B states, then the B next states.  The online forward covers S.R rows
+// (the states, and with double_q the next states too, for the argmax), the target network's forward the B rows after them in
+// h / z / v.  The backward covers the first S.M = B rows.  base may be a dummy when only the size is wanted.
+template <int HEAD>
+A2C_HD size_t dqn_carve(DqnShared& DS, float* base, int D, int H1, int H2, int A, int B, int double_q) {
+  using K = A2cKind<HEAD, true>;
+  A2cShared& S = DS.s;
+  const TensorDesc last = a2c_tensor(K::ntensors - 1, K::ntr, D, H1, H2, A);
+  const size_t wsize = (size_t)last.woff + (size_t)last.rows * last.ld;
+  int nchunks = 0;
+  for (int i = 0; i < K::ntensors; ++i) {
+    const TensorDesc d = a2c_tensor(i, K::ntr, D, H1, H2, A);
+    nchunks += (d.rows * d.cols + A2C_CHUNK - 1) / A2C_CHUNK;
+  }
+  const int R = (double_q ? 2 : 1) * B, Rt = R + B;
+  const bool duel = HEAD == DUEL;
+  S.ldx = a2c_odd(D);
+  S.ldh = a2c_odd(H1 > H2 ? H1 : H2);
+  S.lda = a2c_odd(A);
+  S.hstride = Rt * S.ldh;
+  S.R = R;
+  S.M = B;
+  S.nchunks = nchunks;
+  S.adv = S.ret = S.logp = S.ent = S.lse = S.sdv = S.lsd = nullptr;
+  size_t off = 0;
+#define A2C_TAKE(n) (base + (off += ((size_t)(n) + 3) / 4 * 4) - ((size_t)(n) + 3) / 4 * 4)
+  S.W = A2C_TAKE(wsize);
+  S.G = A2C_TAKE(wsize);
+  S.x = A2C_TAKE((size_t)2 * B * S.ldx);
+  S.h = A2C_TAKE((size_t)2 * S.hstride);
+  S.z = A2C_TAKE((size_t)Rt * S.lda);
+  S.dz = A2C_TAKE((size_t)B * S.lda);
+  S.v = duel ? A2C_TAKE(Rt) : nullptr;
+  S.dv = duel ? A2C_TAKE(B) : nullptr;
+  S.red = A2C_TAKE(B);
+  S.part = A2C_TAKE(nchunks);
+  S.scal = A2C_TAKE(4);
+  DS.delta = A2C_TAKE(B);
+  DS.wt = A2C_TAKE(B);
+#undef A2C_TAKE
+  return off;
+}
+
+// at::pow(Tensor, Scalar)'s special cases (losses.cu pow_like_torch)
+A2C_FN float a2c_pow_torch(float x, float e) {
+  if (e == 0.5f) return sqrtf(x);
+  if (e == 1.0f) return x;
+  if (e == 2.0f) return x * x;
+  if (e == -0.5f) return 1.0f / sqrtf(x);
+  if (e == -1.0f) return 1.0f / x;
+  return powf(x, e);
+}
+
+// DuelingNet (network_heads.py DuelingNet.forward): q = v + (adv - mean(adv)) in place over the advantages of rows 0..rows-1
+A2C_FN void ph_duel_q(A2cShared& S, int rows, int A, int tid, int NT) {
+  for (int n = tid; n < rows; n += NT) {
+    float* z = S.z + (size_t)n * S.lda;
+    float s = 0.0f;
+    for (int j = 0; j < A; ++j) s += z[j];
+    const float mean = A2C_DIV(s, (float)A), v = S.v[n];
+    for (int j = 0; j < A; ++j) z[j] = A2C_ADD(v, A2C_SUB(z[j], mean));
+  }
+}
+
+// P0: parameters, and the rescaled states / next states
+template <int HEAD>
+A2C_FN void ph_dqn_load(DqnShared& DS, const DqnArgs& d, int tid, int NT) {
+  A2cShared& S = DS.s;
+  ph_load_weights<HEAD, true>(S, d.a.net, false, tid, NT);
+  const int D = d.a.net.D, n1 = S.M * D;
+  for (int e = tid; e < 2 * n1; e += NT) {
+    const int n = e / D, k = e - n * D, e1 = e < n1 ? e : e - n1;
+    const void* src = e < n1 ? d.state : d.next_state;
+    const double x = d.f64 ? static_cast<const double*>(src)[e1] : (double)static_cast<const float*>(src)[e1];
+    S.x[n * S.ldx + k] = (float)(d.scale * x);
+  }
+}
+
+// layer l (0, 1: the trunk, 2: the head) of the target network on the B next states, into the rows S.R.. of h / z (/ v).  Its
+// weights are read from the target arena in global memory (rows of `cols` floats).  Runs in the phase of the online layer l.
+template <int HEAD, int GATE>
+A2C_FN void ph_dqn_target_fwd(DqnShared& DS, const DqnArgs& d, int l, int tid, int NT) {
+  using K = A2cKind<HEAD, true>;
+  A2cShared& S = DS.s;
+  const A2cNet& net = d.a.net;
+  const float* w = d.target;
+  const int B = S.M;
+  const size_t rh = (size_t)S.R * S.ldh;
+  if (l == 0) {
+    dense_fwd<GATE>(S.x + (size_t)B * S.ldx, S.ldx, w + net.off[0], net.D, w + net.off[1], a2c_h(S, 0, 0) + rh, S.ldh, B, net.D,
+                    net.H1, tid, NT);
+  } else if (l == 1) {
+    dense_fwd<GATE>(a2c_h(S, 0, 0) + rh, S.ldh, w + net.off[2], net.H1, w + net.off[3], a2c_h(S, 0, 1) + rh, S.ldh, B, net.H1,
+                    net.H2, tid, NT);
+  } else {
+    dense_fwd<LINEAR>(a2c_h(S, 0, 1) + rh, S.ldh, w + net.off[K::fa], net.H2, w + net.off[K::ba], S.z + (size_t)S.R * S.lda,
+                      S.lda, B, net.H2, net.A, tid, NT);
+    if (HEAD == DUEL)
+      dense_fwd<LINEAR>(a2c_h(S, 0, 1) + rh, S.ldh, w + net.off[K::fc], net.H2, w + net.off[K::bc], S.v + S.R, 1, B, net.H2, 1,
+                        tid, NT);
+  }
+}
+
+// per sample (one thread each; the arithmetic of losses.cu dqn_loss_kernel): the bootstrap q (DQN_agent.py:88-92: the target's
+// max, or with double_q the target's q at the online argmax, first maximal index), y = r + discount^n q_next mask (:95),
+// delta = y - q[a] (:99); PER: the priority (|delta| + eps)^alpha (:121) and the unnormalised weight (P B + 1e-6)^-beta (:125)
+template <int HEAD>
+A2C_FN void ph_dqn_delta(DqnShared& DS, const DqnArgs& d, int tid, int NT) {
+  A2cShared& S = DS.s;
+  const int B = S.M, A = d.a.net.A;
+  for (int n = tid; n < B; n += NT) {
+    const float* zt = S.z + (size_t)(S.R + n) * S.lda;
+    float qn;
+    if (d.double_q) {
+      const float* zo = S.z + (size_t)(B + n) * S.lda;
+      int best = 0;
+      float bv = zo[0];
+      for (int j = 1; j < A; ++j)
+        if (zo[j] > bv) { bv = zo[j]; best = j; }
+      qn = zt[best];
+    } else {
+      qn = zt[0];
+      for (int j = 1; j < A; ++j) qn = fmaxf(qn, zt[j]);
+    }
+    const float y = A2C_ADD(d.reward[n], A2C_MUL(A2C_MUL(d.a.discount, qn), d.mask[n]));
+    const float dl = A2C_SUB(y, S.z[(size_t)n * S.lda + (int)d.action[n]]);
+    DS.delta[n] = dl;
+    if (d.delta) d.delta[n] = dl;
+    if (d.prob) {
+      d.priority[n] = a2c_pow_torch(A2C_ADD(fabsf(dl), d.per_eps), d.per_alpha);
+      DS.wt[n] = a2c_pow_torch(A2C_ADD(A2C_MUL(d.prob[n], (float)B), 1e-6f), -d.beta);
+    }
+  }
+}
+
+// w = weight / max(weights) (:126, every thread takes the max in the same order), wl = delta w (:127), (wl)^2 for the objective
+// 0.5 mean(wl^2) (:79), and its gradient d / dq[n][j] = (j == a_n) (-wl w / B); DUEL: through q = v + (adv - mean(adv)) into
+// d / d adv (the fc_action slot) and d / d v (the fc_critic slot)
+template <int HEAD>
+A2C_FN void ph_dqn_loss_grad(DqnShared& DS, const DqnArgs& d, int tid, int NT) {
+  A2cShared& S = DS.s;
+  const int B = S.M, A = d.a.net.A;
+  const float invB = 1.0f / (float)B;
+  float wmax = 1.0f;
+  if (d.prob) {
+    wmax = 0.0f;
+    for (int i = 0; i < B; ++i) wmax = fmaxf(wmax, DS.wt[i]);
+  }
+  for (int e = tid; e < B * A; e += NT) {
+    const int n = e / A, j = e - n * A, an = (int)d.action[n];
+    const float w = d.prob ? A2C_DIV(DS.wt[n], wmax) : 1.0f;
+    const float wl = A2C_MUL(DS.delta[n], w);
+    const float g = A2C_MUL(A2C_MUL(-wl, w), invB);
+    float* dz = S.dz + (size_t)n * S.lda;
+    if (HEAD == DUEL) {
+      dz[j] = A2C_SUB(j == an ? g : 0.0f, A2C_DIV(g, (float)A));
+      if (j == 0) S.dv[n] = g;
+    } else {
+      dz[j] = j == an ? g : 0.0f;
+    }
+    if (j == 0) S.red[n] = A2C_MUL(wl, wl);
   }
 }
 

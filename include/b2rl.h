@@ -474,15 +474,34 @@ int b2rl_a2c_update(int32_t head, int32_t shared, int32_t gate, const float* sta
  * update: forward of states [T][N][D], bootstrap max_a q_target(states[T]), ret = r + discount * mask * ret backwards over T,
  *   0.5 mean((q[a] - ret)^2) into *loss (device), its gradient, clip_grad_norm_(max_norm) and RMSprop on flat / square_avg /
  *   grad_avg; *step += 1.  target: the target network's arena (same offsets).  sync_target != 0: target = flat (before the
- *   RMSprop step) first, and the bootstrap uses those weights. */
+ *   RMSprop step) first, and the bootstrap uses those weights.
+ * actor_step also serves DQNAgent (b2rl_dqn_replay_*): net_kind = gate + 2 * head, head 0 = VanillaNet, 1 = DuelingNet (off:
+ *   w1 b1 w2 b2 fc_advantage.w fc_advantage.b fc_value.w fc_value.b; q = v + (adv - mean(adv))).  state_out may be NULL. */
 int64_t b2rl_nstep_dqn_smem_bytes(int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, int32_t T);
-int b2rl_nstep_dqn_actor_step(int32_t gate, const double* obs, double obs_scale, const float* flat, const int32_t* off, int32_t D,
-                              int32_t H1, int32_t H2, int32_t A, int32_t N, float epsilon, float* state_out, float* action_out,
-                              const float* given_action, uint64_t seed, int64_t* counter, void* stream);
+int b2rl_nstep_dqn_actor_step(int32_t net_kind, const double* obs, double obs_scale, const float* flat, const int32_t* off,
+                              int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t N, float epsilon, float* state_out,
+                              float* action_out, const float* given_action, uint64_t seed, int64_t* counter, void* stream);
 int b2rl_nstep_dqn_update(int32_t gate, const float* states, const float* actions, const float* reward, const float* mask,
                           int32_t T, int32_t N, int32_t D, int32_t H1, int32_t H2, int32_t A, float* flat, float* target,
                           int32_t sync_target, float* square_avg, float* grad_avg, int64_t* step, const int32_t* off, float lr,
                           float alpha, float eps, int32_t centered, float discount, float max_norm, float* loss, void* stream);
+
+/* DQNAgent's gradient update (DQN_agent.py:81-134) for one sampled batch on the device, as ONE launch of one block: head 0 =
+ * VanillaNet, 1 = DuelingNet on a two-layer FCBody (gate 0 = tanh, 1 = ReLU); flat / off / target as for b2rl_nstep_dqn_*.
+ * state / next_state [B][D]: float64 (state_f64) or float32 rows, rescaled as float32(state_scale * double(x)).  action int64,
+ * reward / mask float32 [B].  y = reward + discount_n * q_next * mask with q_next = max_a q_target(s') or, double_q, q_target(s')
+ * at the online argmax; delta = y - q[a] (delta_out, optional).  sampling_prob != NULL (PER): priority_out = (|delta| +
+ * replay_eps)^replay_alpha, w = (P B + 1e-6)^-beta / max; the objective 0.5 mean((w delta)^2) into *loss, its gradient,
+ * clip_grad_norm_(max_norm) and RMSprop on flat / square_avg / grad_avg; *step += 1.  The target arena is only read.
+ * smem_bytes: dynamic shared memory for a batch of B; it must fit the 227 KB of one SM. */
+int64_t b2rl_dqn_replay_smem_bytes(int32_t head, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t B, int32_t double_q);
+int b2rl_dqn_replay_update(int32_t head, int32_t gate, const void* state, const void* next_state, int32_t state_f64,
+                           double state_scale, const int64_t* action, const float* reward, const float* mask, int32_t B, int32_t D,
+                           int32_t H1, int32_t H2, int32_t A, float* flat, const float* target, float* square_avg, float* grad_avg,
+                           int64_t* step, const int32_t* off, float lr, float alpha, float eps, int32_t centered,
+                           float discount_n, int32_t double_q, float max_norm, const float* sampling_prob, float beta,
+                           float replay_eps, float replay_alpha, float* priority_out, float* delta_out, float* loss,
+                           void* stream);
 
 int b2rl_ipc_alloc(int64_t bytes, void** out);
 int b2rl_ipc_get_handle(void* ptr, void* handle_out);

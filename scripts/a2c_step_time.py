@@ -1,6 +1,7 @@
 """Agent steps per second of the rollout launchers' configurations, eager (the torch path of ``step()``) against the launcher's
-device flag (one actor-step launch per env step, one update launch per rollout: csrc/a2c.cu) -- ``config.device_a2c`` for
-A2CAgent (a2c_feature, a2c_continuous), ``config.device_nstep_dqn`` for NStepDQNAgent (n_step_dqn_feature) -- in one process on
+device flag (one actor-step launch per env step, one update launch per rollout or gradient update: csrc/a2c.cu) --
+``config.device_a2c`` for A2CAgent (a2c_feature, a2c_continuous), ``config.device_nstep_dqn`` for NStepDQNAgent
+(n_step_dqn_feature), ``config.device_dqn`` for DQNAgent (dqn_feature, timed past its exploration steps) -- in one process on
 one card, the two alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
 left to the learner is visible.  Prints the card's name and power limit with the numbers.
 
@@ -21,7 +22,8 @@ sys.path.insert(0, ROOT)
 
 # (launcher, game, its device flag, the agent's name in the output keys)
 CONFIGS = [("a2c_feature", "CartPole-v0", "device_a2c", "a2c"), ("a2c_continuous", "SyntheticCheetah-v0", "device_a2c", "a2c"),
-           ("n_step_dqn_feature", "CartPole-v0", "device_nstep_dqn", "nstep_dqn")]
+           ("n_step_dqn_feature", "CartPole-v0", "device_nstep_dqn", "nstep_dqn"),
+           ("dqn_feature", "CartPole-v0", "device_dqn", "dqn")]
 
 
 def card():
@@ -54,15 +56,31 @@ def timed(agent, steps):
     return steps / (time.perf_counter() - t0)
 
 
+def env_steps(agent):
+    """Env steps per agent step: the rollout, or DQNAgent's sgd_update_frequency transitions."""
+    from deeprl_b200 import DQNAgent
+    return agent.config.sgd_update_frequency if isinstance(agent, DQNAgent) else agent.config.rollout_length
+
+
+def past_exploration(agent):
+    """DQNAgent: step until the gradient updates run, so that the timed steps include them."""
+    from deeprl_b200 import DQNAgent
+    if isinstance(agent, DQNAgent):
+        while agent.total_steps <= agent.config.exploration_steps:
+            agent.step()
+
+
 def env_only(agent, steps):
-    """task.step alone, T * steps times, with the actions of one draw (what the host envs cost per agent step)."""
-    from deeprl_b200 import CategoricalActorCriticNet, VanillaNet
+    """task.step alone, env_steps * steps times, with the actions of one draw (what the host envs cost per agent step)."""
+    from deeprl_b200 import CategoricalActorCriticNet, DuelingNet, VanillaNet
     c = agent.config
-    a = (np.zeros(c.num_workers, dtype=np.int64) if isinstance(agent.network, (CategoricalActorCriticNet, VanillaNet))
+    a = (np.zeros(c.num_workers, dtype=np.int64)
+         if isinstance(agent.network, (CategoricalActorCriticNet, VanillaNet, DuelingNet))
          else np.zeros((c.num_workers, c.action_dim), dtype=np.float32))
+    task = agent.task if hasattr(agent, "task") else agent.actor._task
     t0 = time.perf_counter()
-    for _ in range(steps * c.rollout_length):
-        agent.task.step(a)
+    for _ in range(steps * env_steps(agent)):
+        task.step(a)
     return steps / (time.perf_counter() - t0)
 
 
@@ -83,6 +101,7 @@ def main():
     for name, game, flag, unit in CONFIGS:
         agents = {"eager": make_agent(name, game, flag, False), flag: make_agent(name, game, flag, True)}
         for ag in agents.values():
+            past_exploration(ag)
             timed(ag, args.warmup)
         rates = {k: [] for k in agents}
         for _ in range(args.rounds):                        # alternated: both see the same host / card conditions
@@ -92,13 +111,13 @@ def main():
         c = agents["eager"].config
         med = {k: float(np.median(v)) for k, v in rates.items()}
         learner_ms = {k: 1e3 / med[k] - 1e3 / env for k in med}
-        row = {"game": game, "num_workers": c.num_workers, "rollout_length": c.rollout_length, unit + "_steps_per_s": rates,
+        row = {"game": game, "num_workers": c.num_workers, "env_steps_per_agent_step": env_steps(agents["eager"]), unit + "_steps_per_s": rates,
                "median_%s_steps_per_s" % unit: med, "speedup": med[flag] / med["eager"], "env_only_%s_steps_per_s" % unit: env,
                "ms_per_step_besides_envs": learner_ms}
         result["configs"][name] = row
-        print("%-18s %-20s N=%d T=%d  eager %8.1f steps/s  %s %8.1f steps/s  (x%.2f)  envs alone %8.1f steps/s;  "
+        print("%-18s %-20s N=%d env steps %d  eager %8.1f steps/s  %s %8.1f steps/s  (x%.2f)  envs alone %8.1f steps/s;  "
               "ms per step besides the envs: eager %.3f, %s %.3f"
-              % (name, game, c.num_workers, c.rollout_length, med["eager"], flag, med[flag], row["speedup"], env,
+              % (name, game, c.num_workers, env_steps(agents["eager"]), med["eager"], flag, med[flag], row["speedup"], env,
                  learner_ms["eager"], flag, learner_ms[flag]))
         for ag in agents.values():
             ag.close()
