@@ -163,11 +163,6 @@ struct GemmParams {
   int64_t mask_ld;
   float* dbias;
   int dbias_mod, sub_c;
-  // out_mode 3: split-K with an in-kernel fix-up -- every split stores its fp32 partial tile to ws[split][row][col], the split
-  // that arrives last at counters[tile] adds the partials in split order (deterministic), applies bias / ReLU and stores bf16
-  float* ws;
-  int ws_rows, ws_ld;
-  int* counters;
 };
 
 __device__ __forceinline__ int tap_shift(const GemmParams& p, int tap) {
@@ -176,8 +171,7 @@ __device__ __forceinline__ int tap_shift(const GemmParams& p, int tap) {
 
 // accumulator staging tile of the epilogue: 128 rows x (BN + 8) fp32.  The 8-float pad puts consecutive rows 32 bytes apart
 // in the bank pattern: the float2 writes of stage_acc (4 rows x 32 bytes per half-warp) and the float4 reads of
-// epilogue_half (see there) are free of bank conflicts.  The split-K fix-up (epilogue_fixup, out_mode 3, off by default)
-// still reads one row per lane; its float4 reads see 2-way conflicts at this stride.
+// epilogue_half (see there) are free of bank conflicts.
 __host__ __device__ constexpr int acc_ld(int bn) { return bn + 8; }
 __host__ __device__ constexpr size_t acc_stage_bytes(int bn) { return (size_t)GEMM_BM * acc_ld(bn) * 4; }
 
@@ -206,7 +200,7 @@ __device__ __forceinline__ int epi_row(int t, int k) { return t / (BN / 8) + k *
 // 64-row mask boxes in shared memory fits beside the dgrad slab kernels only by giving up slab stages (conv2, BN 128: two
 // 16 KB boxes leave three of its five; conv3, BN 64: four 8 KB boxes leave four of six).  Built and measured that way, against the
 // old epilogue in the same session, it took conv2's dgrad from 59.5 to 52.7 us per update where these register loads take
-// it to 44.7 (from 60.1), and conv3's to 31.7 as these do to 31.1: the mask stays in global memory (DESIGN section 9).  fc4's dgrad, gemm_wgmma_kernel, has one tile per CTA.
+// it to 44.7 (from 60.1), and conv3's to 31.7 as these do to 31.1: the mask stays in global memory (DESIGN section 9).  fc4's dgrad, dense_gemm_kernel, has one tile per CTA.
 // 16-byte shared-memory load through an explicit shared-space address (a generic pointer would go through the L1 path
 // and hold a 64-bit address)
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
@@ -417,81 +411,6 @@ __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int
   if (EXT && p.dbias) dbias_flush<BN>(p, n0, t, dsum, s_dbias);
 }
 
-// Epilogue of a split-K GEMM with in-kernel fix-up (out_mode 3; fc4 forward at batch 512: 32 output tiles cannot fill the
-// SMs).  Replaces zero-fill + atomic split-K + bias/ReLU pass (three launches) by one launch.  Every CTA owns exactly ONE tile
-// (the host sizes the grid so).  All 256 MMA threads store their rows of the staged partial tile to the fp32 scratch; the
-// CTA that arrived last at the tile's counter adds the `splits` partials -- each thread requests all its partials of a
-// 32-column chunk before adding them (in split order: deterministic), so the fix-up costs about one L2 round trip.
-template <int BN>
-__device__ __forceinline__ void epilogue_fixup(const GemmParams& p, int tile, int m0, int n0, int rl, int c0, int ct,
-                                               const float* srow, int* s_flag) {
-  const int row = m0 + rl;
-  const int splits = (int)gridDim.z;
-  float* wrow = p.ws + ((int64_t)blockIdx.z * p.ws_rows + row) * p.ws_ld + n0;
-  for (int c = c0; c < BN; c += 64) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) __stcg(reinterpret_cast<float4*>(wrow + c + j), *reinterpret_cast<const float4*>(srow + c + j));
-  }
-  __threadfence();
-  named_sync(1, 256);
-  if (ct == 0) *s_flag = atomicAdd(p.counters + tile, 1) == splits - 1;
-  named_sync(1, 256);
-  if (!*s_flag) return;
-  __threadfence();
-  if (ct == 0) p.counters[tile] = 0;                                       // re-armed for the next launch
-  const bool valid = row < p.M;
-  for (int c = c0; c < BN; c += 64) {
-    float acc[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = 0.0f;
-    for (int sp0 = 0; sp0 < splits; sp0 += 2) {                            // 2 splits x 8 float4 requested before any is added
-      float4 v[2][8];                                                      // (more in flight spills beside the accumulators)
-#pragma unroll
-      for (int s4 = 0; s4 < 2; ++s4) {
-        if (sp0 + s4 < splits) {
-          const float4* src = reinterpret_cast<const float4*>(p.ws + ((int64_t)(sp0 + s4) * p.ws_rows + row) * p.ws_ld + n0 + c);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[s4][j] = __ldcg(src + j);
-        }
-      }
-#pragma unroll
-      for (int s4 = 0; s4 < 2; ++s4) {
-        if (sp0 + s4 < splits) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            acc[4 * j] += v[s4][j].x; acc[4 * j + 1] += v[s4][j].y; acc[4 * j + 2] += v[s4][j].z; acc[4 * j + 3] += v[s4][j].w;
-          }
-        }
-      }
-    }
-    if (valid && n0 + c < p.N) {
-      if (p.bias) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (n0 + c + j < p.N) acc[j] += __ldg(p.bias + n0 + c + j);
-      }
-      if (p.relu) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = fmaxf(acc[j], 0.0f);
-      }
-      __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(p.D) + (int64_t)row * p.ldd + n0 + c;
-      if (n0 + c + 32 <= p.N && (reinterpret_cast<uintptr_t>(d) & 15) == 0) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          int4 o;
-          __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) h[t] = __floats2bfloat162_rn(acc[j + 2 * t], acc[j + 2 * t + 1]);
-          *reinterpret_cast<int4*>(d + j) = o;
-        }
-      } else {
-        for (int j = 0; j < 32; ++j)
-          if (n0 + c + j < p.N) d[j] = __float2bfloat16_rn(acc[j]);
-      }
-    }
-  }
-}
-
 template <int BN, int STAGES, bool EXT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                      const __grid_constant__ CUtensorMap tmB,
@@ -524,7 +443,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
   const int n_kt = max(kt_end - kt_begin, 0);
 
   __shared__ float s_dbias[128];                    // per-CTA bias-gradient accumulator (backward extras)
-  __shared__ int s_fix[2];                          // out_mode 3: "this CTA arrived last at the tile's counter"
   if (threadIdx.x < 128) s_dbias[threadIdx.x] = 0.0f;
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS); }
@@ -579,7 +497,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: rows 64 g .. 64 g + 63
     // (K-major A: rows 64.. start 64 x 128 bytes into the stage; MN-major A: the second [64 k][64 m] box)
     const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
-    const int rl = g * 64 + (wl & 1) * 32 + lane, c0 = (wl >> 1) * 32;   // split-K fix-up: tile row and first 32-column chunk
     const int t = wl * 32 + lane;                                          // epilogue_half's thread index in the warpgroup
     float* sAcc_g = sAcc + g * 64 * ACC_LD;
     const uint64_t a0 = make_desc(s2u(sA) + g * 8192, 8192), b0 = make_desc(s2u(sB), 8192);
@@ -610,13 +527,195 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
       epi_mask_load<BN, EXT>(p, m0 + 64 * g, n0, t, mk);     // in flight during the staging (fc4 dgrad: one tile per CTA)
       stage_acc<BN>(d, sAcc_g, ACC_LD, wl, lane);
       named_sync(2 + g, 128);
-      if (!EXT && p.out_mode == 3) epilogue_fixup<BN>(p, tile, m0, n0, rl, c0, cw * 32 + lane, sAcc + rl * ACC_LD, s_fix);
-      else epilogue_half<BN, EXT>(p, m0 + 64 * g, n0, t, sAcc_g, mk, s_dbias);
+      epilogue_half<BN, EXT>(p, m0 + 64 * g, n0, t, sAcc_g, mk, s_dbias);
       named_sync(2 + g, 128);                        // staging tile read: the next tile may overwrite it
     }
   }
   __syncthreads();
   if (EXT && p0.dbias && (int)threadIdx.x < dbias_slots(p0)) atomicAdd(p0.dbias + threadIdx.x, s_dbias[threadIdx.x]);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Plain GEMM (no tap addressing): fc4 forward / dgrad / weight gradient and the distributional heads.  Same roles, ring and
+// epilogue as gemm_wgmma_kernel, with two differences:
+//  * the operand majors TA / TB are template parameters, so a tile's k-tiles form one chain of wgmmas of one shape.  Each
+//    k-tile is one commit group: after issuing k-tile i a warpgroup waits for k-tile i - 1 only (wgmma.wait_group 1) and
+//    releases its stage, and it drains once per tile, so its MMAs overlap the next k-tile's barrier wait and issue.
+//  * cluster split-K: launched with clusters of S > 1 CTAs (one output tile per cluster), CTA rank r computes the tile over
+//    k-tiles [r kps, (r + 1) kps) and stages its partial accumulators in its own shared memory.  After a cluster barrier
+//    each CTA adds, for its 128 / S rows of the tile, the S partials in rank order through distributed shared memory (the
+//    sum is the same in every launch), and a second barrier ends all remote reads.  The CTA then runs the epilogue on its
+//    rows only: one launch, no global workspace, no atomics.  Without a cluster (S = 1) the CTAs are persistent over the
+//    tiles, and blockIdx.z selects the k range of an atomic split-K (out_mode 2).
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_size() {
+  uint32_t n;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+  return n;
+}
+// every thread of every CTA of the cluster arrives (release: its shared-memory writes become visible to the cluster) and
+// waits for all others (acquire)
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// 16 bytes at shared-memory address `addr` of cluster CTA `rank`
+__device__ __forceinline__ float4 ld_dsmem128(uint32_t addr, uint32_t rank) {
+  uint32_t ra;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(addr), "r"(rank));
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(ra) : "memory");
+  return v;
+}
+
+constexpr int DENSE_MAX_CLUSTER = 8;
+
+template <int BN, int STAGES, int TA, int TB, bool EXT>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) dense_gemm_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                     const __grid_constant__ CUtensorMap tmB,
+                                                                     const GemmParams p) {
+  constexpr uint32_t A_BYTES = GEMM_BM * GEMM_BK * 2, B_BYTES = BN * GEMM_BK * 2;
+  constexpr int ACC_LD = acc_ld(BN);
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + STAGES * A_BYTES;
+  float* sAcc = reinterpret_cast<float*>(sB + STAGES * B_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sAcc + GEMM_BM * ACC_LD);
+  uint64_t* empty = full + STAGES;
+
+  const int S = (int)cluster_size(), rank = (int)cluster_rank();   // 1 / 0 without a cluster launch
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+  const int n_tiles = (p.N + BN - 1) / BN, tiles = ((p.M + GEMM_BM - 1) / GEMM_BM) * n_tiles;
+  const int n_cta = (int)gridDim.x / S, cta = (int)blockIdx.x / S;
+  const int kt_total = (p.K + GEMM_BK - 1) / GEMM_BK;
+  const int kt_begin = (S > 1 ? rank : (int)blockIdx.z) * p.k_tiles_per_split;
+  const int n_kt = max(min(kt_total, kt_begin + p.k_tiles_per_split) - kt_begin, 0);
+
+  __shared__ float s_dbias[128];
+  if (threadIdx.x < 128) s_dbias[threadIdx.x] = 0.0f;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+  }
+  __syncthreads();
+  pdl_sync();
+
+  if (warp == 0 && n_kt > 0 && elect_one()) {
+    // ---------------------------------------------------------------------- TMA producer
+    uint32_t it = 0;
+    for (int tile = cta; tile < tiles; tile += n_cta) {
+      const int mt = tile / n_tiles;
+      const int m0 = mt * GEMM_BM, n0 = (tile - mt * n_tiles) * BN;
+      for (int i = 0; i < n_kt; ++i, ++it) {
+        const int s = it % STAGES;
+        mb_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+        mb_expect_tx(&full[s], A_BYTES + B_BYTES);
+        const int k0 = (kt_begin + i) * GEMM_BK;
+        uint8_t* a = sA + s * A_BYTES;
+        uint8_t* b = sB + s * B_BYTES;
+        if constexpr (!TA) {
+          tma_load_2d(a, &tmA, &full[s], k0, m0);                        // box [128 rows][64 k]
+        } else {
+          tma_load_2d(a, &tmA, &full[s], m0, k0);                        // 2 boxes [64 k][64 m]
+          tma_load_2d(a + 8192, &tmA, &full[s], m0 + 64, k0);
+        }
+        if constexpr (!TB) {
+          tma_load_2d(b, &tmB, &full[s], k0, n0);                        // box [BN rows][64 k]
+        } else {
+#pragma unroll
+          for (int q = 0; q < BN / 64; ++q) tma_load_2d(b + q * 8192, &tmB, &full[s], n0 + q * 64, k0);
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: rows 64 g .. 64 g + 63
+    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
+    const int t = wl * 32 + lane;
+    const uint64_t a0 = make_desc(s2u(sA) + g * 8192, 8192), b0 = make_desc(s2u(sB), 8192);
+    uint32_t it = 0;
+    for (int tile = cta; tile < tiles; tile += n_cta) {
+      const int mt = tile / n_tiles;
+      const int m0 = mt * GEMM_BM, n0 = (tile - mt * n_tiles) * BN;
+      float d[BN / 2];
+      acc_zero<BN>(d);
+      for (int i = 0; i < n_kt; ++i, ++it) {
+        const int s = it % STAGES;
+        mb_wait(&full[s], (it / STAGES) & 1);
+        wg_fence();
+        mma_ktile<BN, TA, TB>(d, a0 + (uint64_t)s * (A_BYTES >> 4), b0 + (uint64_t)s * (B_BYTES >> 4));
+        wg_commit();
+        wg_wait1();                                          // k-tile i - 1 has retired: release its stage
+        if (i > 0 && lane == 0) mb_arrive(&empty[(it - 1) % STAGES]);
+      }
+      wg_wait0();
+      acc_fence<BN>(d);
+      if (n_kt > 0 && lane == 0) mb_arrive(&empty[(it - 1) % STAGES]);
+      float* sAcc_g = sAcc + g * 64 * ACC_LD;
+      if (S > 1) {                                           // partial tile: reduced across the cluster below
+        stage_acc<BN>(d, sAcc_g, ACC_LD, wl, lane);
+        continue;
+      }
+      int4 mk[BN / 16];
+      epi_mask_load<BN, EXT>(p, m0 + 64 * g, n0, t, mk);
+      stage_acc<BN>(d, sAcc_g, ACC_LD, wl, lane);
+      named_sync(2 + g, 128);
+      epilogue_half<BN, EXT>(p, m0 + 64 * g, n0, t, sAcc_g, mk, s_dbias);
+      named_sync(2 + g, 128);                                // staging tile read: the next tile may overwrite it
+    }
+  }
+  if (S > 1) {
+    // one tile per cluster (the launcher sizes the grid so): every thread of the CTA takes part in both cluster barriers
+    const int R = GEMM_BM / S;                               // rows of the tile this CTA reduces and stores
+    const int mt = cta / n_tiles;
+    const int m0 = mt * GEMM_BM, n0 = (cta - mt * n_tiles) * BN;
+    const int g = (warp - 4) >> 2, t = (warp & 3) * 32 + lane, tid = (int)threadIdx.x - 128;
+    // warpgroup g stores rows R/2 g .. R/2 g + R/2 - 1 of the CTA's rows: the half-tile epilogue with the rows past them cut off
+    GemmParams pe = p;
+    const int row0 = m0 + rank * R + g * (R / 2);
+    pe.M = min(p.M, row0 + R / 2);
+    int4 mk[BN / 16];
+    if (warp >= 4) epi_mask_load<BN, EXT>(pe, row0, n0, t, mk);
+    cluster_sync();                                          // every CTA's partial tile is staged
+    // An MMA thread owns BN / (8 S) float4s of the CTA's R x BN rows (e = tid + 256 j; at BN 32, S 8 half the threads own one)
+    // and loads each from all S ranks: slot f = S j + q, all issued before the first add so that their remote latencies
+    // overlap.  Then each slot adds its predecessor's sum (rank order: the same sum in every launch); slot S j + S - 1 ends
+    // with float4 j.
+    constexpr int NL = BN / 8 > DENSE_MAX_CLUSTER ? BN / 8 : DENSE_MAX_CLUSTER;
+    const int ls = __ffs(S) - 1;
+    float4 x[NL];
+    const uint32_t base = s2u(sAcc);
+    if (warp >= 4) {
+#pragma unroll
+      for (int f = 0; f < NL; ++f) {
+        const int e = tid + 256 * (f >> ls), r = e / (BN / 4), c = 4 * (e % (BN / 4));
+        x[f] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (r < R) x[f] = ld_dsmem128(base + (uint32_t)(((rank * R + r) * ACC_LD + c) * 4), (uint32_t)(f & (S - 1)));
+      }
+#pragma unroll
+      for (int f = 1; f < NL; ++f) {
+        if (f & (S - 1)) { x[f].x += x[f - 1].x; x[f].y += x[f - 1].y; x[f].z += x[f - 1].z; x[f].w += x[f - 1].w; }
+      }
+    }
+    cluster_sync();                                          // no CTA reads another's staging tile any more
+    if (warp >= 4) {
+#pragma unroll
+      for (int f = 0; f < NL; ++f) {
+        const int e = tid + 256 * (f >> ls), r = e / (BN / 4), c = 4 * (e % (BN / 4));
+        if ((f & (S - 1)) == S - 1 && r < R) *reinterpret_cast<float4*>(sAcc + r * ACC_LD + c) = x[f];   // compacted: rows 0 .. R-1
+      }
+      named_sync(1, 256);
+      epilogue_half<BN, EXT>(pe, row0, n0, t, sAcc + g * (R / 2) * ACC_LD, mk, s_dbias);
+    }
+  }
+  __syncthreads();
+  if (EXT && p.dbias && (int)threadIdx.x < dbias_slots(p)) atomicAdd(p.dbias + threadIdx.x, s_dbias[threadIdx.x]);
 }
 
 
@@ -1218,7 +1317,7 @@ static int sm_count() {
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 
 // dynamic shared memory kernel `k` may request: the per-CTA limit of the device minus the kernel's own static shared memory
-// (s_dbias, s_fix and the alignment of the extern region); 0 if the runtime cannot tell
+// (s_dbias and the alignment of the extern region); 0 if the runtime cannot tell
 template <typename K>
 static size_t dyn_smem_limit(K k) {
   static int optin = 0;
@@ -1255,10 +1354,6 @@ static int launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   int ctas = sm_count() / splits / (p.dual ? 2 : 1);                 // per operand set
   if (ctas < 1) ctas = 1;
   if (ctas > tiles) ctas = tiles;
-  if (p.out_mode == 3 && ctas != tiles) {
-    set_error("b2rl_gemm_splitk_bf16: tiles x splits (%d x %d) must fit one CTA per SM (%d) and splits <= 8", tiles, splits, sm_count());
-    return B2RL_ERR_ARG;
-  }
   dim3 grid(p.dual ? 2 * ctas : ctas, 1, splits);
   launch_pdl(k, dim3(grid), dim3(GEMM_THREADS), smem, st, ta, tb, ta2, tb2, p);
   return check_launch("b2rl_gemm_bf16");
@@ -1297,6 +1392,139 @@ static int gemm_dispatch(const uint16_t* A, int a_mn, int64_t lda, int64_t a_row
   if (block_n == 32) return launch_gemm<32, 6>(ta, tb, ta2, tb2, p, splits, st);
   if (block_n == 64) return launch_gemm<64, 6>(ta, tb, ta2, tb2, p, splits, st);
   return launch_gemm<128, 4>(ta, tb, ta2, tb2, p, splits, st);
+}
+
+// ---- plain GEMMs: dense_gemm_kernel
+
+// clusters of `S` CTAs of kernel `k` the device can hold at once (0: none -- e.g. no GPC has S free SMs for it)
+template <typename K>
+static int cluster_capacity(K k, size_t smem, int S) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(S);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = S;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, k, &cfg) != cudaSuccess) {
+    cudaGetLastError();
+    n = 0;
+  }
+  return n;
+}
+
+// Cluster size of a launch the caller leaves to the launcher, from the shape: per wave of tiles a CTA streams
+// ceil(K tiles / S) k-tiles, and a cluster launch costs about CLUSTER_COST k-tiles more (the two cluster barriers, the
+// DSMEM reduction and the epilogue on fewer rows; measured on fc4's forward, DESIGN section 7).  The size with the fewest
+// k-tile steps, waves x (k-tiles per CTA [+ CLUSTER_COST]), wins; ties go to the smaller cluster.  fc4 forward at batch 512,
+// BN 64 (32 tiles, 49 k-tiles): S = 2, since 32 clusters of 4 do not fit in one wave on an H100 SXM; the fc4 dgrad / weight
+// gradient and the head GEMMs (8 k-tiles or fewer): S = 1.
+// The wave count uses the clusters the device can hold (cap), not SMs / S: a GPC whose SMs do not divide by S leaves some idle.
+constexpr int CLUSTER_COST = 16;
+static int auto_cluster(int tiles, int kt_total, const int (&cap)[DENSE_MAX_CLUSTER + 1]) {
+  int best = 1, best_cost = ((tiles + sm_count() - 1) / sm_count()) * kt_total;
+  for (int S = 2; S <= 4; S *= 2) {
+    if (cap[S] <= 0) continue;
+    const int cost = ((tiles + cap[S] - 1) / cap[S]) * ((kt_total + S - 1) / S + CLUSTER_COST);
+    if (cost < best_cost) best = S, best_cost = cost;
+  }
+  return best;
+}
+
+// cluster: 0 = chosen from the shape (auto_cluster), else the requested size (a power of two <= 8; halved while the device
+// cannot hold a cluster of that size).  splits > 1 (atomic split-K over blockIdx.z) launches without clusters.
+template <int BN, int STAGES, int TA, int TB, bool EXT>
+static int launch_dense_t(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, int splits, int cluster, cudaStream_t st) {
+  constexpr size_t smem = 1024 + (size_t)STAGES * (GEMM_BM * GEMM_BK * 2 + BN * GEMM_BK * 2) + acc_stage_bytes(BN) + 2 * STAGES * 8;
+  static_assert(smem <= SMEM_LIMIT, "GEMM stages do not fit in shared memory");
+  auto k = dense_gemm_kernel<BN, STAGES, TA, TB, EXT>;
+  static const size_t limit = dyn_smem_limit(k);
+  if (smem > limit) {
+    set_error("b2rl_gemm_bf16: %zu bytes of shared memory per CTA exceed the %zu the device allows", smem, limit);
+    return B2RL_ERR_ARG;
+  }
+  static int cap[DENSE_MAX_CLUSTER + 1] = {};
+  static bool init = false;
+  if (!init) {
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    for (int S = 2; S <= DENSE_MAX_CLUSTER; S *= 2) cap[S] = cluster_capacity(k, smem, S);
+    init = true;
+  }
+  const int tiles = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + BN - 1) / BN);
+  const int kt_total = (p.K + GEMM_BK - 1) / GEMM_BK;
+  int S = 1;
+  if (splits == 1) {
+    S = cluster > 0 ? cluster : auto_cluster(tiles, kt_total, cap);
+    while (S > 1 && cap[S] <= 0) S >>= 1;
+  }
+  int ctas = S > 1 ? tiles * S : (tiles < sm_count() / splits ? tiles : sm_count() / splits);
+  if (ctas < 1) ctas = 1;
+  if (S > 1) p.k_tiles_per_split = (kt_total + S - 1) / S;   // rank r: k-tiles [r kps, (r + 1) kps); trailing ranks may get none
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(ctas, 1, splits);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  int na = 0;
+  if (pdl_enabled()) {
+    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[na++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (S > 1) {
+    attr[na].id = cudaLaunchAttributeClusterDimension;
+    attr[na].val.clusterDim.x = S;
+    attr[na].val.clusterDim.y = 1;
+    attr[na++].val.clusterDim.z = 1;
+  }
+  cfg.attrs = attr;
+  cfg.numAttrs = na;
+  cudaLaunchKernelEx(&cfg, k, ta, tb, p);
+  return check_launch("b2rl_gemm_bf16");
+}
+
+// instantiations: K-major or MN-major A and B (MN-major B from BN 64); the backward extras with a K-major A (dgrad)
+template <int BN, int STAGES, bool EXT>
+static int launch_dense_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int splits, int cluster,
+                           cudaStream_t st) {
+  if constexpr (BN >= 64) {
+    if (p.b_mn) {
+      if (!p.a_mn) return launch_dense_t<BN, STAGES, 0, 1, EXT>(ta, tb, p, splits, cluster, st);
+      if constexpr (!EXT) return launch_dense_t<BN, STAGES, 1, 1, false>(ta, tb, p, splits, cluster, st);
+    }
+  }
+  if (!p.b_mn) {
+    if (!p.a_mn) return launch_dense_t<BN, STAGES, 0, 0, EXT>(ta, tb, p, splits, cluster, st);
+    if constexpr (!EXT) return launch_dense_t<BN, STAGES, 1, 0, false>(ta, tb, p, splits, cluster, st);
+  }
+  set_error("b2rl_gemm_bf16: no kernel for a_mn %d, b_mn %d, block_n %d%s", p.a_mn, p.b_mn, BN, EXT ? " with backward extras" : "");
+  return B2RL_ERR_ARG;
+}
+
+static int dense_dispatch(const uint16_t* A, int a_mn, int64_t lda, int64_t a_rows, int64_t a_cols, const uint16_t* B,
+                          int b_mn, int64_t ldb, int64_t b_rows, int64_t b_cols, GemmParams p, int splits, int block_n,
+                          int cluster, cudaStream_t st) {
+  CUtensorMap ta, tb;
+  int rc = make_map(&ta, A, a_cols, a_rows, lda, a_mn ? 64 : GEMM_BM);
+  if (rc) return rc;
+  rc = make_map(&tb, B, b_cols, b_rows, ldb, b_mn ? 64 : block_n);
+  if (rc) return rc;
+  const int kt_total = (p.K + GEMM_BK - 1) / GEMM_BK;
+  if (splits > kt_total) splits = kt_total;
+  p.k_tiles_per_split = (kt_total + splits - 1) / splits;
+  splits = (kt_total + p.k_tiles_per_split - 1) / p.k_tiles_per_split;
+  const bool ext = has_ext(p);
+  if (block_n == 32) return ext ? launch_dense_bn<32, 6, true>(ta, tb, p, splits, cluster, st)
+                                : launch_dense_bn<32, 6, false>(ta, tb, p, splits, cluster, st);
+  if (block_n == 64) return ext ? launch_dense_bn<64, 6, true>(ta, tb, p, splits, cluster, st)
+                                : launch_dense_bn<64, 6, false>(ta, tb, p, splits, cluster, st);
+  return ext ? launch_dense_bn<128, 4, true>(ta, tb, p, splits, cluster, st)
+             : launch_dense_bn<128, 4, false>(ta, tb, p, splits, cluster, st);
 }
 
 template <int BN, bool EXT, bool U8, int TX, int TY, int CB>
@@ -1482,8 +1710,8 @@ extern "C" int b2rl_gemm_bf16(const uint16_t* A, int32_t a_mn, int64_t lda, cons
   p.a_mn = a_mn; p.b_mn = b_mn; p.relu = relu; p.out_mode = out_mode; p.bias = bias; p.D = D;
   p.taps_x = 1; p.shift_sign = 1;
   // K-major: stored [rows][K]; MN-major: stored [K][rows]
-  return gemm_dispatch(A, a_mn, lda, a_mn ? K : M, a_mn ? M : K, B, b_mn, ldb, b_mn ? K : N, b_mn ? N : K, p, splits,
-                       block_n, (cudaStream_t)stream);
+  return dense_dispatch(A, a_mn, lda, a_mn ? K : M, a_mn ? M : K, B, b_mn, ldb, b_mn ? K : N, b_mn ? N : K, p, splits,
+                        block_n, 0, (cudaStream_t)stream);
 }
 
 // Convolution over a G x G grid as a shifted-row GEMM (see the header of this file).
@@ -1668,7 +1896,7 @@ extern "C" int b2rl_gemm_bwd_bf16(const uint16_t* A, int64_t lda, const uint16_t
   p.out_map = out_map; p.G = G; p.V = V;
   rc = apply_ext(p, ext, N);
   if (rc) return rc;
-  return gemm_dispatch(A, 0, lda, M, K, B, b_mn, ldb, b_mn ? K : N, b_mn ? N : K, p, 1, block_n, (cudaStream_t)stream);
+  return dense_dispatch(A, 0, lda, M, K, B, b_mn, ldb, b_mn ? K : N, b_mn ? N : K, p, 1, block_n, 0, (cudaStream_t)stream);
 }
 
 // Weight gradient as split-K PARTIALS: partial i (one per CTA, n_partials_host of them, at most one per SM) is stored at
@@ -1687,27 +1915,21 @@ extern "C" int b2rl_conv_wgrad_partials(const uint16_t* X, int64_t rows, int32_t
   return rc;
 }
 
-// D = act(A B^T + bias) in bf16 with split-K over `splits` CTAs per output tile and an in-kernel fix-up (out_mode 3): ONE
-// launch instead of zero-fill + atomic split-K + bias/activation pass.  A [M][K], B [N][K] K-major bf16.  ws: fp32
-// [splits][ceil(M/128)*128][ceil(N/block_n)*block_n] scratch; counters: int32 [tiles], zero-initialised once (the kernel
-// re-arms them).  Launches on different streams must not share ws / counters.  fc4 of NatureConvBody (network_bodies.py:33).
+// D = act(A B^T + bias) in bf16, K split over the `splits` CTAs of a cluster per output tile and the partials summed in
+// distributed shared memory in rank order (dense_gemm_kernel): one launch, no scratch, the same bits in every launch.
+// A [M][K], B [N][K] K-major bf16; splits 1, 2, 4 or 8 (1: one CTA per tile over all of K), or 0: the cluster size the
+// launcher picks from the shape (auto_cluster).  fc4 of NatureConvBody (network_bodies.py:33).
 extern "C" int b2rl_gemm_splitk_bf16(const uint16_t* A, int64_t lda, const uint16_t* B, int64_t ldb, void* D, int64_t ldd,
                                      int32_t M, int32_t N, int32_t K, const float* bias, int32_t relu, int32_t splits,
-                                     int32_t block_n, float* ws, int32_t* counters, void* stream) {
-  B2RL_REQUIRE(A && B && D && ws && counters, "null pointer");
-  B2RL_REQUIRE(M > 0 && N > 0 && K > 0 && splits >= 1 && splits <= 8, "bad shape (1 <= splits <= 8)");
-  B2RL_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "operand row strides must be multiples of 8 elements (16 bytes)");
-  B2RL_REQUIRE((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(ws)) % 16 == 0,
-               "operands and scratch must be 16-byte aligned");
-  B2RL_REQUIRE(block_n == 32 || block_n == 64 || block_n == 128, "block_n must be 32, 64 or 128");
+                                     int32_t block_n, void* stream) {
+  B2RL_REQUIRE(splits == 0 || splits == 1 || splits == 2 || splits == 4 || splits == 8, "splits must be 0, 1, 2, 4 or 8");
+  int rc = check_common(A, B, D, lda, ldb, M, N, K, 0, 1, block_n, 0, relu);
+  if (rc) return rc;
   GemmParams p = {};
   p.M = M; p.N = N; p.K = K; p.ldd = (int)ldd;
-  p.relu = relu; p.out_mode = 3; p.bias = bias; p.D = D;
+  p.relu = relu; p.out_mode = 0; p.bias = bias; p.D = D;
   p.taps_x = 1; p.shift_sign = 1;
-  p.ws = ws; p.counters = counters;
-  p.ws_rows = (M + GEMM_BM - 1) / GEMM_BM * GEMM_BM;
-  p.ws_ld = (N + block_n - 1) / block_n * block_n;
-  return gemm_dispatch(A, 0, lda, M, K, B, 0, ldb, N, K, p, splits, block_n, (cudaStream_t)stream);
+  return dense_dispatch(A, 0, lda, M, K, B, 0, ldb, N, K, p, 1, block_n, splits, (cudaStream_t)stream);
 }
 
 

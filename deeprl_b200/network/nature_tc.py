@@ -28,13 +28,10 @@ from .fused import act_bwd_bias_grad
 
 _bf16 = torch.bfloat16
 _f32 = torch.float32
-# fc4 forward at small batch: split-K factor (zero fill + split-K GEMM with fp32 atomics + bias/ReLU pass, 3 launches) or 1 =
-# one GEMM launch with the fused bias/ReLU epilogue
-FC4_SPLITS = int(os.environ.get("B2RL_FC4_SPLITS", "4"))
-# split-K with the in-kernel fix-up (one launch) instead of zero fill + atomic split-K + bias/ReLU pass (three)
-# (off by default: the last-arriver's L2 round trips are exposed, while the three small launches overlap with the other
-# network's chain)
-FC4_FIXUP = os.environ.get("B2RL_FC4_FIXUP", "0") == "1"
+# fc4 forward, one launch with the bias / ReLU / bf16 epilogue: K split over the FC4_SPLITS CTAs (2, 4 or 8) of a
+# thread-block cluster per output tile, the partials summed in distributed shared memory in a fixed order; 0 = the cluster
+# size the launcher picks from the shape and the SMs of the device; 1 = one CTA per output tile over all of K
+FC4_SPLITS = int(os.environ.get("B2RL_FC4_SPLITS", "0"))
 # backward: ReLU mask + bias gradient + re-layout fused into the dgrad GEMM epilogues (b2rl_*_bwd_bf16) instead of three
 # b2rl_act_bwd_bias_grad_bf16 passes (B2RL_FUSED_BWD=0 restores them).
 FUSED_BWD = os.environ.get("B2RL_FUSED_BWD", "1") == "1"
@@ -352,17 +349,9 @@ def forward_only(x0, packed, b1, b2, b3, b4):
     y3 = torch.empty((B * 49, 64), dtype=_bf16, device=dev)
     conv_gemm(0, y2, w3f, 64, 9, 3, 10, 1, y3, bias=b3, relu=True, out_map=2, G=10, V=7, block_n=64)
     mark("f_conv3")
-    n4 = w4p.shape[0]
-    if B <= 1024 and FC4_SPLITS > 1 and FC4_FIXUP:
-        # few output tiles, long K (3136): split K over CTAs; the last split of a tile adds the partials, bias + ReLU + bf16
-        y4 = gemm_splitk_bf16(y3.view(B, 3136), w4p, bias=b4, relu=True, splits=FC4_SPLITS, block_n=64)
-    elif B <= 1024 and FC4_SPLITS > 1:
-        # few output tiles, long K (3136): split K over CTAs, finish (bias + ReLU + bf16) in a streaming pass
-        acc = gemm_bf16(y3.view(B, 3136), w4p, out_dtype=_f32, splits=FC4_SPLITS, block_n=64)
-        y4 = torch.empty((B, n4), dtype=_bf16, device=dev)
-        _lib.call("b2rl_bias_act_f32_to_bf16", _lib.ptr(acc), _lib.ptr(b4), _lib.ptr(y4), B, n4, 1, _lib.stream())
-    else:
-        y4 = gemm_bf16(y3.view(B, 3136), w4p, bias=b4, relu=True, block_n=32 if B <= 1024 else 64)
+    # BN 64: at batch 512 the launcher's clusters of 2 make 64 CTAs, so the online and the target network's fc4 (two graph
+    # branches) fit the SMs side by side; BN 32 is faster alone (128 CTAs) but not beside the other branch (DESIGN section 7)
+    y4 = gemm_splitk_bf16(y3.view(B, 3136), w4p, bias=b4, relu=True, splits=FC4_SPLITS, block_n=64)
     mark("f_fc4")
     return y4, (x0m, x1, y2, y3)
 

@@ -358,20 +358,16 @@ def gemm_bf16(a, b, a_major="k", b_major="k", bias=None, relu=False, out_dtype=t
 
 
 def gemm_splitk_bf16(a, b, bias=None, relu=False, splits=4, block_n=64, out=None):
-    """``act(a @ b.T + bias)`` in bf16 with split-K and an in-kernel fix-up (csrc/gemm.cu out_mode 3): ONE launch where
-    ``gemm_bf16(splits > 1)`` needs a zero fill, the atomic split-K GEMM and a bias / activation pass.  ``a`` [M, K] and ``b``
-    [N, K] bf16 row-major.  The fp32 scratch and the tile counters are kept per (shape, stream): the online and the target
-    network run this concurrently on two streams."""
+    """``act(a @ b.T + bias)`` in bf16, ONE launch: K split over the ``splits`` CTAs (1, 2, 4 or 8; 0: the launcher picks the
+    size from the shape) of a thread-block cluster per output tile, whose partials are summed in distributed shared memory
+    in a fixed order, so every launch gives the same bits (csrc/gemm.cu dense_gemm_kernel).  ``a`` [M, K] and ``b`` [N, K]
+    bf16 row-major."""
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.dim() == 2 and b.dim() == 2
     assert a.stride(1) == 1 and b.stride(1) == 1 and a.shape[1] == b.shape[1]
     M, K = a.shape
     N = b.shape[0]
-    rows, cols = (M + 127) // 128 * 128, (N + block_n - 1) // block_n * block_n
-    key = "splitk_%d_%d_%d_%d_%d" % (rows, cols, splits, block_n, torch.cuda.current_stream().cuda_stream)
-    ws = _Scratch.get(a.device, key + "_ws", splits * rows * cols, _f32)
-    counters = _Scratch.get(a.device, key + "_cnt", (rows // 128) * (cols // block_n), torch.int32)
     if out is None:
         out = torch.empty((M, N), dtype=torch.bfloat16, device=a.device)
     _lib.call("b2rl_gemm_splitk_bf16", _lib.ptr(a), a.stride(0), _lib.ptr(b), b.stride(0), _lib.ptr(out), out.stride(0), int(M),
-              int(N), int(K), _lib.ptr(bias), int(relu), int(splits), int(block_n), _lib.ptr(ws), _lib.ptr(counters), _lib.stream())
+              int(N), int(K), _lib.ptr(bias), int(relu), int(splits), int(block_n), _lib.stream())
     return out

@@ -324,13 +324,11 @@ int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capacity, const 
                                  int32_t frame_w, int32_t batch, int32_t history, const uint16_t* G_rows, int32_t n_out, float* partials,
                                  int32_t* n_partials_host, void* stream);
 
-/* D = act(A B^T + bias) (bf16 out) with split-K and an in-kernel fix-up: one launch instead of zero-fill + atomic split-K +
- * bias/activation pass (fc4 of NatureConvBody at small batch, network_bodies.py:33).  A [M][K], B [N][K] bf16 K-major.
- * ws: fp32 [splits][ceil(M/128)*128][ceil(N/block_n)*block_n]; counters: int32 [tiles], zeroed once (self re-arming).
- * Concurrent launches (different streams) need their own ws / counters. */
+/* D = act(A B^T + bias) (bf16 out) in one launch: K split over the `splits` CTAs (1, 2, 4 or 8; 0: chosen from the shape) of
+ * a thread-block cluster per output tile, the partials summed in distributed shared memory in a fixed order (deterministic),
+ * bias / ReLU in the same epilogue (fc4 of NatureConvBody, network_bodies.py:33).  A [M][K], B [N][K] bf16 K-major. */
 int b2rl_gemm_splitk_bf16(const uint16_t* A, int64_t lda, const uint16_t* B, int64_t ldb, void* D, int64_t ldd, int32_t M,
-                          int32_t N, int32_t K, const float* bias, int32_t relu, int32_t splits, int32_t block_n, float* ws,
-                          int32_t* counters, void* stream);
+                          int32_t N, int32_t K, const float* bias, int32_t relu, int32_t splits, int32_t block_n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Tail of one gradient update for a NatureConvBody network on the wgmma path (csrc/tail.cu):
