@@ -1,6 +1,11 @@
 """C51 agent (also Rainbow through ``RainbowNet`` + PER + double-Q + n-step) behind the reference's interface
 (``deep_rl/agent/CategoricalDQN_agent.py``: ``CategoricalDQNActor``:14, ``CategoricalDQNAgent``:27).
-The categorical projection + KL + gradient run as one kernel (``csrc/losses.cu: c51_loss_kernel``)."""
+The categorical projection + KL + gradient run as one kernel (``csrc/losses.cu: c51_loss_kernel``).
+
+``config.device_c51 = True`` (off by default; ``categorical_dqn_feature(game=..., device_c51=True)``) runs a CategoricalNet on a
+two-layer FCBody on the device: one ``b2rl_dist_dqn_actor_step`` launch per env step (epsilon-greedy on the device's Philox
+stream, not numpy's) and one ``b2rl_dist_dqn_replay_update`` launch per gradient update (csrc/dist_dqn.cu, component/actor.py
+``DeviceDistDQN``), also with ``async_actor``.  Configurations the kernels do not cover raise ``NotImplementedError``."""
 import threading
 
 import numpy as np
@@ -32,6 +37,7 @@ class CategoricalDQNAgent(DQNAgent):
         self.delta_atom = (config.categorical_v_max - config.categorical_v_min) / float(config.categorical_n_atoms - 1)
 
     _graph_kind = "c51"
+    _device_flag = "device_c51"
 
     def _fused_owner(self):
         return CategoricalDQNAgent

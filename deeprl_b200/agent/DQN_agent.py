@@ -14,7 +14,9 @@ the generic autograd path in ``_generic_update``.
 device: one ``b2rl_nstep_dqn_actor_step`` launch per env step (epsilon-greedy on the device's Philox stream, not numpy's) and
 one ``b2rl_dqn_replay_update`` launch per gradient update on the batch ``replay.sample()`` returns (csrc/a2c.cu,
 component/actor.py ``DeviceDQN``).  Configurations the kernels do not cover raise ``NotImplementedError`` naming the unmet
-condition.
+condition.  ``CategoricalDQNAgent`` / ``QuantileRegressionDQNAgent`` have their own flags, ``config.device_c51`` /
+``config.device_qr``, served by the same ``step()`` with ``DeviceDistDQN`` (csrc/dist_dqn.cu); they also run with
+``async_actor``, the actor thread launching its actor steps under ``config.lock``.
 """
 import threading
 
@@ -126,7 +128,15 @@ class DQNAgent(BaseAgent):
         self.total_steps = 0
         self.last_loss = None
         self.device_dqn = None
-        if getattr(config, "device_dqn", False):
+        flag = self._device_flag
+        if flag is not None and getattr(config, flag, False):
+            if getattr(config, "device_dqn", False):
+                raise NotImplementedError("config.device_dqn and config.%s are both set; %s runs on the device with "
+                                          "config.%s alone" % (flag, type(self).__name__, flag))
+            from ..component.actor import DeviceDistDQN
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
+            self.device_dqn = self.actor._device_dqn = DeviceDistDQN(self, seed)
+        elif getattr(config, "device_dqn", False):
             from ..component.actor import DeviceDQN
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
             self.device_dqn = self.actor._device_dqn = DeviceDQN(self, seed)
@@ -296,6 +306,8 @@ class DQNAgent(BaseAgent):
                 self.target_network.load_state_dict(self.network.state_dict())
 
     # ------------------------------------------------------------------ config.device_dqn (opt-in)
+    _device_flag = None                                    # the distributional agents' own flag (device_c51 / device_qr)
+
     def _device_update(self):
         """DQN_agent.py:115-134 for the batch ``replay.sample()`` returns (sync or async wrapper, uniform or prioritized) as
         ONE ``b2rl_dqn_replay_update`` launch; the new priorities go to the tree from the device (:120-123)."""

@@ -2,7 +2,13 @@
 ``QuantileRegressionDQNActor``:14, ``QuantileRegressionDQNAgent``:23).  The pairwise quantile-Huber loss
 (N x B x N terms, six 82 MB temporaries in the reference at N=200, B=512) is one kernel that never
 materialises the pair tensor (``csrc/losses.cu: qr_loss_kernel``).  As in the reference the loss tensor is
-indexed by TARGET quantile, shape (N,), so QR-DQN + prioritized replay is not defined (SURVEY 7.3-7)."""
+indexed by TARGET quantile, shape (N,), so QR-DQN + prioritized replay is not defined (SURVEY 7.3-7).
+
+``config.device_qr = True`` (off by default; ``quantile_regression_dqn_feature(game=..., device_qr=True)``) runs a QuantileNet
+on a two-layer FCBody on the device: one ``b2rl_dist_dqn_actor_step`` launch per env step (epsilon-greedy on the device's
+Philox stream, not numpy's) and one ``b2rl_dist_dqn_replay_update`` launch per gradient update (csrc/dist_dqn.cu,
+component/actor.py ``DeviceDistDQN``), also with ``async_actor``.  Configurations the kernels do not cover raise
+``NotImplementedError``."""
 import threading
 
 import numpy as np
@@ -31,6 +37,7 @@ class QuantileRegressionDQNAgent(DQNAgent):
         self.cumulative_density = tensor((2 * np.arange(config.num_quantiles) + 1) / (2.0 * config.num_quantiles)).view(1, -1)
 
     _graph_kind = "qr"
+    _device_flag = "device_qr"
 
     def _fused_owner(self):
         return QuantileRegressionDQNAgent

@@ -513,29 +513,23 @@ class DeviceNStepDQN(_DeviceRollout):
 
 # ------------------------------------------------------------------------------------------------ replay DQN on the device
 def dqn_kernel_order(net):
-    """A VanillaNet's / DuelingNet's parameters in the kernels' tensor order: w1 b1 w2 b2, then fc_head.w fc_head.b, or
-    fc_advantage.w fc_advantage.b fc_value.w fc_value.b."""
+    """A VanillaNet's / DuelingNet's / CategoricalNet's / QuantileNet's parameters in the kernels' tensor order: w1 b1 w2 b2,
+    then fc_head.w fc_head.b, or fc_advantage.w fc_advantage.b fc_value.w fc_value.b, or fc_categorical.w fc_categorical.b, or
+    fc_quantiles.w fc_quantiles.b."""
     from ..network.network_heads import DuelingNet
     body = [t for m in net.body.layers for t in (m.weight, m.bias)]
     if isinstance(net, DuelingNet):
         return body + [net.fc_advantage.weight, net.fc_advantage.bias, net.fc_value.weight, net.fc_value.bias]
-    return body + [net.fc_head.weight, net.fc_head.bias]
+    head = next(getattr(net, k) for k in ("fc_head", "fc_categorical", "fc_quantiles") if hasattr(net, k))
+    return body + [head.weight, head.bias]
 
 
-def dqn_unsupported(agent):
-    """``None`` when ``config.device_dqn``'s kernels (csrc/a2c.cu: b2rl_nstep_dqn_actor_step, b2rl_dqn_replay_update) cover
-    this ``DQNAgent``, else the unmet condition."""
+def _fc_body_unsupported(network, config):
+    """The body checks of ``dqn_unsupported`` and ``dist_dqn_unsupported``: a two-layer, non-noisy FCBody with tanh or ReLU on
+    a CUDA device."""
     import torch.nn.functional as F
 
     from ..network.network_bodies import NatureConvBody
-    from ..network.network_heads import DuelingNet, VanillaNet
-    from ..utils.normalizer import RescaleNormalizer
-    config, network = agent.config, agent.network
-    if type(network) not in (VanillaNet, DuelingNet):
-        return ("the network is a %s; the device kernels implement VanillaNet and DuelingNet (C51, QR and Rainbow heads are "
-                "not covered)" % type(network).__name__)
-    if agent._uses_reference_hooks():
-        return "%s overrides compute_loss / reduce_loss; the device update implements DQNAgent's" % type(agent).__name__
     body = network.body
     if isinstance(body, NatureConvBody):
         return "the body is a NatureConvBody; the device kernels implement a two-layer FCBody"
@@ -549,6 +543,24 @@ def dqn_unsupported(agent):
         return "the FCBody gate must be torch.tanh or F.relu"
     if not body.layers[0].weight.is_cuda:
         return "the network is not on a CUDA device (select_device(0))"
+    return None
+
+
+def dqn_unsupported(agent):
+    """``None`` when ``config.device_dqn``'s kernels (csrc/a2c.cu: b2rl_nstep_dqn_actor_step, b2rl_dqn_replay_update) cover
+    this ``DQNAgent``, else the unmet condition."""
+    from ..network.network_heads import DuelingNet, VanillaNet
+    from ..utils.normalizer import RescaleNormalizer
+    config, network = agent.config, agent.network
+    if type(network) not in (VanillaNet, DuelingNet):
+        return ("the network is a %s; the device kernels implement VanillaNet and DuelingNet (C51, QR and Rainbow heads are "
+                "not covered)" % type(network).__name__)
+    if agent._uses_reference_hooks():
+        return "%s overrides compute_loss / reduce_loss; the device update implements DQNAgent's" % type(agent).__name__
+    why = _fc_body_unsupported(network, config)
+    if why is not None:
+        return why
+    body = network.body
     head = network.fc_advantage if isinstance(network, DuelingNet) else network.fc_head
     D, H1, H2, A = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features, head.out_features
     if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32:
@@ -579,11 +591,17 @@ class DeviceDQN(_DeviceRollout):
     ``forced``: test hook -- a callable returning the actions of the next env step, which the actor step then writes through
     unchanged instead of drawing."""
 
+    flag = "config.device_dqn"
+
+    @staticmethod
+    def unsupported(agent):
+        return dqn_unsupported(agent)
+
     def __init__(self, agent, seed):
         from ..network.network_heads import DuelingNet
-        why = dqn_unsupported(agent)
+        why = self.unsupported(agent)
         if why is not None:
-            raise NotImplementedError("config.device_dqn: " + why)
+            raise NotImplementedError(self.flag + ": " + why)
         config, network = agent.config, agent.network
         self.net, self.target_net, self.cfg = network, agent.target_network, config
         body = network.body
@@ -621,14 +639,17 @@ class DeviceDQN(_DeviceRollout):
                   self.N, float(epsilon), None, self._row_ptrs(0)[1], given, self.seed, _lib.ptr(self.counter), _lib.stream())
         return self._fetch(0)[:, 0].astype(np.int64)
 
+    def _check_states(self, s):
+        if s.dtype not in (_f32, _f64) or s.dim() != 2 or s.shape[1] != self.D:
+            raise NotImplementedError("%s: the replay returned %s states of shape %s; the device update reads 1-D float32 / "
+                                      "float64 rows of %d" % (self.flag, s.dtype, tuple(s.shape), self.D))
+
     def update(self, tr, beta=0.0):
         """One gradient update on a sampled batch (``Transition`` / ``PrioritizedTransition`` of device tensors).  Returns the
         objective (0-dim device tensor) and, for a prioritized batch, the new priorities (float32 device tensor [B])."""
         c, o = self.cfg, self.opt
         s, s2 = tr.state, tr.next_state
-        if s.dtype not in (_f32, _f64) or s.dim() != 2 or s.shape[1] != self.D:
-            raise NotImplementedError("config.device_dqn: the replay returned %s states of shape %s; the device update reads "
-                                      "1-D float32 / float64 rows of %d" % (s.dtype, tuple(s.shape), self.D))
+        self._check_states(s)
         self._offsets()
         B = s.shape[0]
         per = getattr(tr, "sampling_prob", None) is not None
@@ -646,3 +667,115 @@ class DeviceDQN(_DeviceRollout):
     def sync_target(self):
         """DQN_agent.py:136-138: the target arena becomes the online arena (one device copy)."""
         self.target.copy_(self.opt.flat)
+
+
+# ------------------------------------------------------------------------------------------------ C51 / QR-DQN on the device
+def dist_dqn_unsupported(agent):
+    """``None`` when ``config.device_c51`` / ``config.device_qr``'s kernels (csrc/dist_dqn.cu: b2rl_dist_dqn_actor_step,
+    b2rl_dist_dqn_replay_update) cover this ``CategoricalDQNAgent`` / ``QuantileRegressionDQNAgent``, else the unmet
+    condition."""
+    from ..agent.CategoricalDQN_agent import CategoricalDQNAgent
+    from ..component.replay import PrioritizedReplay
+    from ..network.network_heads import CategoricalNet, QuantileNet, RainbowNet
+    from ..utils.normalizer import RescaleNormalizer
+    config, network = agent.config, agent.network
+    c51 = isinstance(agent, CategoricalDQNAgent)
+    want = CategoricalNet if c51 else QuantileNet
+    if isinstance(network, RainbowNet):
+        return "the network is a RainbowNet; the device kernels implement CategoricalNet (RainbowNet / NoisyLinear is not covered)"
+    if type(network) is not want:
+        return "the network is a %s; the device kernels implement %s" % (type(network).__name__, want.__name__)
+    if agent._uses_reference_hooks():
+        return "%s overrides compute_loss / reduce_loss; the device update implements %s's" % (
+            type(agent).__name__, agent._fused_owner().__name__)
+    why = _fc_body_unsupported(network, config)
+    if why is not None:
+        return why
+    body = network.body
+    D, H1, H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
+    A, K = network.action_dim, network.num_atoms if c51 else network.num_quantiles
+    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32 or not 2 <= K <= 256:
+        return ("sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32, "
+                "2 <= %s %d <= 256" % (D, H1, H2, A, "atoms" if c51 else "quantiles", K))
+    if not isinstance(agent.optimizer, torch.optim.RMSprop) or agent._flat is None:
+        return "the optimizer is %s; the device update implements RMSprop" % type(agent.optimizer).__name__
+    if type(config.state_normalizer) is not RescaleNormalizer:
+        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
+    if config.history_length not in (None, 1):
+        return "history_length is %d; the device kernels read single 1-D states, not frame stacks" % config.history_length
+    replay_cls = getattr(agent.replay, "replay_cls", type(agent.replay))
+    if not c51 and issubclass(replay_cls, PrioritizedReplay):
+        return ("QR-DQN with prioritized replay is undefined in the reference: its loss is per target quantile, not per sample "
+                "(QuantileRegressionDQN_agent.py:74)")
+    smem = _lib.lib().b2rl_dist_dqn_smem_bytes(int(not c51), D, H1, H2, A, K, int(config.batch_size),
+                                               int(bool(config.double_q)))
+    if not 0 < smem <= 227 * 1024:
+        return ("a batch of %d needs %d bytes of shared memory, more than one SM has (b2rl_dist_dqn_smem_bytes)"
+                % (config.batch_size, smem))
+    return None
+
+
+class DeviceDistDQN(DeviceDQN):
+    """``CategoricalDQNAgent.step()`` / ``QuantileRegressionDQNAgent.step()`` on the device (``config.device_c51`` /
+    ``config.device_qr``): one ``b2rl_dist_dqn_actor_step`` launch per env step (rescale, forward, the action values,
+    epsilon-greedy on the device's Philox stream) and one ``b2rl_dist_dqn_replay_update`` launch per gradient update.  The
+    arenas, the target network's parameters as views into the target arena, the staging buffers and the target sync are
+    ``DeviceDQN``'s.
+
+    With ``async_actor`` the actor thread calls ``act`` (inside ``config.lock``, as ``DQNActor._transition`` does) and the agent
+    calls ``update`` under the same lock; both launch on torch's current stream.  The staging buffers and the Philox counter are
+    only touched by ``act``."""
+
+    @property
+    def flag(self):
+        return "config.device_c51" if self.kind == 0 else "config.device_qr"
+
+    @staticmethod
+    def unsupported(agent):
+        return dist_dqn_unsupported(agent)
+
+    def __init__(self, agent, seed):
+        from ..agent.CategoricalDQN_agent import CategoricalDQNAgent
+        self.kind = 0 if isinstance(agent, CategoricalDQNAgent) else 1      # C51, QR
+        super().__init__(agent, seed)
+        n, c = agent.network, agent.config
+        self.A = n.action_dim
+        self.K = n.num_atoms if self.kind == 0 else n.num_quantiles
+        self.v_min = float(getattr(c, "categorical_v_min", 0.0)) if self.kind == 0 else 0.0
+        self.v_max = float(getattr(c, "categorical_v_max", 1.0)) if self.kind == 0 else 1.0
+        self._dims = (self.D, self.H1, self.H2, self.A, self.K)
+
+    def act(self, raw_obs, epsilon):
+        """One env step's actions: rescale + forward + action values + epsilon-greedy in one launch, downloaded for
+        ``task.step``."""
+        obs, given = self._stage(raw_obs)
+        _lib.call("b2rl_dist_dqn_actor_step", self.kind, self.gate, obs, self._scale, self._flat, self._off, *self._dims, self.N,
+                  self.v_min, self.v_max, float(epsilon), self._row_ptrs(0)[1], given, self.seed, _lib.ptr(self.counter),
+                  _lib.stream())
+        return self._fetch(0)[:, 0].astype(np.int64)
+
+    def update(self, tr, beta=0.0, loss_vec=None):
+        """One gradient update on a sampled batch (``Transition`` / ``PrioritizedTransition`` of device tensors; C51 only for
+        the latter).  Returns the objective (0-dim device tensor) and, for a prioritized batch, the new priorities (float32
+        device tensor [B]).  ``loss_vec``: optional float32 device tensor for the per-sample KL [B] (C51) / the loss vector [K]
+        (QR)."""
+        c, o = self.cfg, self.opt
+        s, s2 = tr.state, tr.next_state
+        self._check_states(s)
+        self._offsets()
+        B = s.shape[0]
+        per = getattr(tr, "sampling_prob", None) is not None
+        if per and self.kind == 1:
+            raise NotImplementedError("config.device_qr: QR-DQN with prioritized replay is undefined in the reference: its loss "
+                                      "is per target quantile, not per sample (QuantileRegressionDQN_agent.py:74)")
+        loss = torch.empty((), dtype=_f32, device=self.dev)
+        prio = torch.empty(B, dtype=_f32, device=self.dev) if per else None
+        ptr = lambda t: _lib.ptr(None if t is None else t.contiguous())
+        _lib.call("b2rl_dist_dqn_replay_update", self.kind, self.gate, ptr(s), ptr(s2), int(s.dtype == _f64), self._scale,
+                  ptr(tr.action), ptr(tr.reward), ptr(tr.mask), B, *self._dims, self._flat, _lib.ptr(self.target),
+                  _lib.ptr(o.s1), _lib.ptr(o.s2), _lib.ptr(o.step_dev), self._off, float(o.lr), float(o.alpha), float(o.eps),
+                  int(o.centered), float(c.discount ** c.n_step), int(bool(c.double_q)), self.v_min, self.v_max,
+                  float(c.gradient_clip or 0.0), ptr(tr.sampling_prob if per else None), float(beta),
+                  float(getattr(c, "replay_eps", 0.01)), float(getattr(c, "replay_alpha", 0.5)), ptr(prio), ptr(loss_vec),
+                  _lib.ptr(loss), _lib.stream())
+        return loss, prio

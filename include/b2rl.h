@@ -501,6 +501,35 @@ int b2rl_dqn_replay_update(int32_t head, int32_t gate, const void* state, const 
                            float replay_eps, float replay_alpha, float* priority_out, float* delta_out, float* loss,
                            void* stream);
 
+/* C51 / QR-DQN on the device (csrc/dist_dqn.cu): CategoricalDQNAgent / QuantileRegressionDQNAgent for a CategoricalNet /
+ * QuantileNet on a two-layer FCBody.  kind 0 = C51, 1 = QR-DQN; gate 0 tanh / 1 ReLU.  The parameters: flat at off[6] in the
+ * order w1 b1 w2 b2 fc.weight [A K][H2] fc.bias [A K] (fc_categorical / fc_quantiles).  Limits: D <= 256, H1, H2 <= 128,
+ * 2 <= A <= 32, 2 <= K <= 256.  C51's support is np.linspace(v_min, v_max, K) in float64, rounded to float32.
+ *
+ * actor_step: rescale + forward + the action values (C51: sum_k softmax z_k; QR: the mean of the quantiles) + epsilon-greedy
+ * on Philox stream 17 as b2rl_nstep_dqn_actor_step (two uniforms per row; the counter advances by 2 N; given_action != NULL:
+ * written through, nothing drawn).
+ *
+ * replay_update: one launch on a sampled batch (the layout of b2rl_dqn_replay_update's arguments).  C51: the projection of the
+ * target's p(a*) (a* the first maximum of sum_k p z_k of the target, or with double_q of the online network), KL = sum m log(m +
+ * 1e-5) - m log p[a] (loss_vec_out [B], optional), PER when sampling_prob != NULL (priority_out = (|KL| + replay_eps)^alpha),
+ * the objective mean(w KL).  QR (double_q ignored, no PER): T_j = r + discount_n mask theta'_j(a*), the quantile-Huber loss
+ * vector indexed by target quantile (loss_vec_out [K], optional) and its mean.  Then the backward, clip_grad_norm_(max_norm)
+ * and RMSprop as b2rl_dqn_replay_update.  smem_bytes: 0 for invalid input; the result must fit the 227 KB of one SM. */
+int64_t b2rl_dist_dqn_smem_bytes(int32_t kind, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t K, int32_t B,
+                                 int32_t double_q);
+int b2rl_dist_dqn_actor_step(int32_t kind, int32_t gate, const double* obs, double obs_scale, const float* flat,
+                             const int32_t* off, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t K, int32_t N, double v_min,
+                             double v_max, float epsilon, float* action_out, const float* given_action, uint64_t seed,
+                             int64_t* counter, void* stream);
+int b2rl_dist_dqn_replay_update(int32_t kind, int32_t gate, const void* state, const void* next_state, int32_t state_f64,
+                                double state_scale, const int64_t* action, const float* reward, const float* mask, int32_t B,
+                                int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t K, float* flat, const float* target,
+                                float* square_avg, float* grad_avg, int64_t* step, const int32_t* off, float lr, float alpha,
+                                float eps, int32_t centered, float discount_n, int32_t double_q, double v_min, double v_max,
+                                float max_norm, const float* sampling_prob, float beta, float replay_eps, float replay_alpha,
+                                float* priority_out, float* loss_vec_out, float* loss, void* stream);
+
 int b2rl_ipc_alloc(int64_t bytes, void** out);
 int b2rl_ipc_get_handle(void* ptr, void* handle_out);
 int b2rl_ipc_open_handle(const void* handle, void** out);

@@ -1,8 +1,10 @@
 """Agent steps per second of the rollout launchers' configurations, eager (the torch path of ``step()``) against the launcher's
 device flag (one actor-step launch per env step, one update launch per rollout or gradient update: csrc/a2c.cu) --
 ``config.device_a2c`` for A2CAgent (a2c_feature, a2c_continuous), ``config.device_nstep_dqn`` for NStepDQNAgent
-(n_step_dqn_feature), ``config.device_dqn`` for DQNAgent (dqn_feature, timed past its exploration steps) -- in one process on
-one card, the two alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
+(n_step_dqn_feature), ``config.device_dqn`` for DQNAgent (dqn_feature, timed past its exploration steps), ``config.device_c51``
+/ ``config.device_qr`` for CategoricalDQNAgent / QuantileRegressionDQNAgent (categorical_dqn_feature,
+quantile_regression_dqn_feature: csrc/dist_dqn.cu, with the launchers' async actor) -- in one process on one card, the two
+alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
 left to the learner is visible.  Prints the card's name and power limit with the numbers.
 
     python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--out DIR]
@@ -23,7 +25,9 @@ sys.path.insert(0, ROOT)
 # (launcher, game, its device flag, the agent's name in the output keys)
 CONFIGS = [("a2c_feature", "CartPole-v0", "device_a2c", "a2c"), ("a2c_continuous", "SyntheticCheetah-v0", "device_a2c", "a2c"),
            ("n_step_dqn_feature", "CartPole-v0", "device_nstep_dqn", "nstep_dqn"),
-           ("dqn_feature", "CartPole-v0", "device_dqn", "dqn")]
+           ("dqn_feature", "CartPole-v0", "device_dqn", "dqn"),
+           ("categorical_dqn_feature", "CartPole-v0", "device_c51", "c51"),
+           ("quantile_regression_dqn_feature", "CartPole-v0", "device_qr", "qr")]
 
 
 def card():
@@ -71,17 +75,24 @@ def past_exploration(agent):
 
 
 def env_only(agent, steps):
-    """task.step alone, env_steps * steps times, with the actions of one draw (what the host envs cost per agent step)."""
-    from deeprl_b200 import CategoricalActorCriticNet, DuelingNet, VanillaNet
+    """task.step alone, env_steps * steps times, with the actions of one draw (what the host envs cost per agent step).  With
+    an async actor its thread owns its task, so a new one is made."""
+    from deeprl_b200 import CategoricalActorCriticNet, CategoricalNet, DuelingNet, QuantileNet, VanillaNet
     c = agent.config
     a = (np.zeros(c.num_workers, dtype=np.int64)
-         if isinstance(agent.network, (CategoricalActorCriticNet, VanillaNet, DuelingNet))
+         if isinstance(agent.network, (CategoricalActorCriticNet, VanillaNet, DuelingNet, CategoricalNet, QuantileNet))
          else np.zeros((c.num_workers, c.action_dim), dtype=np.float32))
-    task = agent.task if hasattr(agent, "task") else agent.actor._task
+    own = hasattr(agent, "actor") and c.async_actor
+    task = agent.task if hasattr(agent, "task") else c.task_fn() if own else agent.actor._task
+    if own:
+        task.reset()
     t0 = time.perf_counter()
     for _ in range(steps * env_steps(agent)):
         task.step(a)
-    return steps / (time.perf_counter() - t0)
+    rate = steps / (time.perf_counter() - t0)
+    if own:
+        task.close()
+    return rate
 
 
 def main():
