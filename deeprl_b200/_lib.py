@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(CSRC, "libb2rl.so")
-SOURCES = ["core.cu", "replay.cu", "sumtree.cu", "losses.cu", "onpolicy.cu", "optim.cu", "dense.cu", "gemm.cu", "pack.cu", "head.cu", "tail.cu", "disthead.cu", "actor.cu", "ppo_persistent.cu", "a2c.cu", "dist_dqn.cu"]
+SOURCES = ["core.cu", "replay.cu", "sumtree.cu", "losses.cu", "onpolicy.cu", "optim.cu", "dense.cu", "gemm.cu", "pack.cu", "head.cu", "tail.cu", "disthead.cu", "actor.cu", "ppo_persistent.cu", "a2c.cu", "dist_dqn.cu", "rainbow.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
@@ -90,6 +90,12 @@ SIGNATURES = {
                                                                                        c_p],
     "b2rl_dist_dqn_replay_update": ([c_i32, c_i32, c_p, c_p, c_i32, c_f64, c_p, c_p, c_p] + [c_i32] * 6 + [c_p] * 6
                                     + [c_f32] * 3 + [c_i32, c_f32, c_i32, c_f64, c_f64, c_f32, c_p] + [c_f32] * 3 + [c_p] * 4),
+    "b2rl_rainbow_smem_bytes": [c_i32] * 8,
+    "b2rl_rainbow_actor_step": [c_i32, c_i32, c_p, c_f64, c_p, c_p] + [c_i32] * 6 + [c_f64, c_f64, c_f32, c_p, c_p, c_u64, c_p,
+                                                                                      c_f32, c_p, c_p, c_p, c_p],
+    "b2rl_rainbow_replay_update": ([c_i32, c_i32, c_p, c_p, c_i32, c_f64, c_p, c_p, c_p] + [c_i32] * 6 + [c_p] * 6
+                                   + [c_f32] * 3 + [c_i32, c_f32, c_i32, c_f64, c_f64, c_f32, c_p] + [c_f32] * 3 + [c_p] * 3
+                                   + [c_u64, c_f32] + [c_p] * 5),
     "b2rl_ipc_alloc": [c_i64, c_p],
     "b2rl_ipc_get_handle": [c_p, c_p],
     "b2rl_ipc_open_handle": [c_p, c_p],
@@ -169,6 +175,7 @@ def lib():
         L.b2rl_nstep_dqn_smem_bytes.restype = ctypes.c_int64
         L.b2rl_dqn_replay_smem_bytes.restype = ctypes.c_int64
         L.b2rl_dist_dqn_smem_bytes.restype = ctypes.c_int64
+        L.b2rl_rainbow_smem_bytes.restype = ctypes.c_int64
         _lib = L
     return _lib
 

@@ -5,7 +5,12 @@ The categorical projection + KL + gradient run as one kernel (``csrc/losses.cu: 
 ``config.device_c51 = True`` (off by default; ``categorical_dqn_feature(game=..., device_c51=True)``) runs a CategoricalNet on a
 two-layer FCBody on the device: one ``b2rl_dist_dqn_actor_step`` launch per env step (epsilon-greedy on the device's Philox
 stream, not numpy's) and one ``b2rl_dist_dqn_replay_update`` launch per gradient update (csrc/dist_dqn.cu, component/actor.py
-``DeviceDistDQN``), also with ``async_actor``.  Configurations the kernels do not cover raise ``NotImplementedError``."""
+``DeviceDistDQN``), also with ``async_actor``.  Configurations the kernels do not cover raise ``NotImplementedError``.
+
+``config.device_rainbow = True`` (off by default; ``rainbow_feature(game=..., device_rainbow=True)``) is the same for a
+RainbowNet on a two-layer FCBody, all layers NoisyLinear or all nn.Linear: one ``b2rl_rainbow_actor_step`` launch per env step
+and one ``b2rl_rainbow_replay_update`` launch per gradient update (csrc/rainbow.cu, component/actor.py ``DeviceRainbow``), the
+factorised noise drawn in the kernels from a Philox stream of its own."""
 import threading
 
 import numpy as np

@@ -16,7 +16,9 @@ one ``b2rl_dqn_replay_update`` launch per gradient update on the batch ``replay.
 component/actor.py ``DeviceDQN``).  Configurations the kernels do not cover raise ``NotImplementedError`` naming the unmet
 condition.  ``CategoricalDQNAgent`` / ``QuantileRegressionDQNAgent`` have their own flags, ``config.device_c51`` /
 ``config.device_qr``, served by the same ``step()`` with ``DeviceDistDQN`` (csrc/dist_dqn.cu); they also run with
-``async_actor``, the actor thread launching its actor steps under ``config.lock``.
+``async_actor``, the actor thread launching its actor steps under ``config.lock``.  ``config.device_rainbow`` does the same for
+a ``CategoricalDQNAgent`` on a RainbowNet (``DeviceRainbow``, csrc/rainbow.cu): the NoisyLinear noise is drawn in the kernels,
+so the ``reset_noise()`` calls of the eager path do not run.
 """
 import threading
 
@@ -63,7 +65,10 @@ class DQNActor(BaseActor):
         config = self.config
         dev = getattr(self, "_device_dqn", None)
         if dev is not None:                                # config.device_dqn: rescale + forward + epsilon-greedy, one launch
-            epsilon = 1 if self._total_steps < config.exploration_steps else config.random_action_prob()
+            if config.noisy_linear:                        # config.device_rainbow: the noise explores (DQN_agent.py:34-35)
+                epsilon = 0
+            else:
+                epsilon = 1 if self._total_steps < config.exploration_steps else config.random_action_prob()
             with config.lock:
                 action = dev.act(self._state, epsilon)
             return self._env_step(action)
@@ -129,7 +134,15 @@ class DQNAgent(BaseAgent):
         self.last_loss = None
         self.device_dqn = None
         flag = self._device_flag
-        if flag is not None and getattr(config, flag, False):
+        if getattr(config, "device_rainbow", False):
+            for other in ("device_dqn", flag):
+                if other is not None and getattr(config, other, False):
+                    raise NotImplementedError("config.device_rainbow and config.%s are both set; a RainbowNet runs on the "
+                                              "device with config.device_rainbow alone" % other)
+            from ..component.actor import DeviceRainbow
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
+            self.device_dqn = self.actor._device_dqn = DeviceRainbow(self, seed)
+        elif flag is not None and getattr(config, flag, False):
             if getattr(config, "device_dqn", False):
                 raise NotImplementedError("config.device_dqn and config.%s are both set; %s runs on the device with "
                                           "config.%s alone" % (flag, type(self).__name__, flag))

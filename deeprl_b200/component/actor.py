@@ -607,7 +607,7 @@ class DeviceDQN(_DeviceRollout):
         body = network.body
         self.head = int(isinstance(network, DuelingNet))
         self.gate = 0 if body.gate is torch.tanh else 1
-        self.tensors = dqn_kernel_order(network)
+        self.tensors = self._tensors(network)
         self.opt = agent._flat
         self.dev = self.opt.flat.device
         self.target = torch.zeros_like(self.opt.flat)
@@ -624,11 +624,15 @@ class DeviceDQN(_DeviceRollout):
         self._dims = (self.D, self.H1, self.H2, self.A)
         self._offsets()
 
+    @staticmethod
+    def _tensors(net):
+        return dqn_kernel_order(net)
+
     def _offsets(self):
         """``_arena_offsets``, and the check that the target parameters still live in the target arena."""
         self._arena_offsets()
         base = self.target.data_ptr()
-        for t, o in zip(dqn_kernel_order(self.target_net), self.off.tolist()):
+        for t, o in zip(self._tensors(self.target_net), self.off.tolist()):
             if t.data_ptr() != base + 4 * o:
                 raise _lib.B2RLError("DeviceDQN: a target parameter no longer lives in the target arena")
 
@@ -778,4 +782,178 @@ class DeviceDistDQN(DeviceDQN):
                   float(c.gradient_clip or 0.0), ptr(tr.sampling_prob if per else None), float(beta),
                   float(getattr(c, "replay_eps", 0.01)), float(getattr(c, "replay_alpha", 0.5)), ptr(prio), ptr(loss_vec),
                   _lib.ptr(loss), _lib.stream())
+        return loss, prio
+
+
+# ------------------------------------------------------------------------------------------------ Rainbow on the device
+RAINBOW_NOISE_BUFFERS = ("noise_in", "noise_out_weight", "noise_out_bias")
+
+
+def rainbow_layers(net):
+    """A RainbowNet's four layers in the kernels' order: body.layers.0, body.layers.1, fc_advantage, fc_value."""
+    return list(net.body.layers) + [net.fc_advantage, net.fc_value]
+
+
+def rainbow_kernel_order(net):
+    """A RainbowNet's parameters in the kernels' tensor order: per layer of ``rainbow_layers`` weight_mu weight_sigma bias_mu
+    bias_sigma (NoisyLinear) or weight bias (nn.Linear)."""
+    names = ("weight_mu", "weight_sigma", "bias_mu", "bias_sigma") if net.noisy_linear else ("weight", "bias")
+    return [getattr(m, k) for m in rainbow_layers(net) for k in names]
+
+
+def rainbow_unsupported(agent):
+    """``None`` when ``config.device_rainbow``'s kernels (csrc/rainbow.cu: b2rl_rainbow_actor_step, b2rl_rainbow_replay_update)
+    cover this agent, else the unmet condition."""
+    import torch.nn.functional as F
+
+    from ..agent.CategoricalDQN_agent import CategoricalDQNAgent
+    from ..network.network_bodies import NatureConvBody
+    from ..network.network_heads import RainbowNet
+    from ..network.network_utils import NoisyLinear
+    from ..utils.normalizer import RescaleNormalizer
+    config, network = agent.config, agent.network
+    if not isinstance(agent, CategoricalDQNAgent):
+        return "the agent is a %s; Rainbow is a CategoricalDQNAgent on a RainbowNet" % type(agent).__name__
+    if type(network) is not RainbowNet:
+        return "the network is a %s; the device kernels implement RainbowNet" % type(network).__name__
+    if agent._uses_reference_hooks():
+        return "%s overrides compute_loss / reduce_loss; the device update implements CategoricalDQNAgent's" % type(agent).__name__
+    body = network.body
+    if isinstance(body, NatureConvBody):
+        return "the body is a NatureConvBody; the device kernels implement a two-layer FCBody"
+    if not isinstance(body, FCBody):
+        return "the network needs an FCBody body (got %s)" % type(body).__name__
+    if len(body.layers) != 2:
+        return "the device kernels implement a two-layer FCBody (got %d layers)" % len(body.layers)
+    noisy = [isinstance(m, NoisyLinear) for m in rainbow_layers(network)]
+    if len(set(noisy + [bool(network.noisy_linear), bool(body.noisy_linear), bool(config.noisy_linear)])) != 1:
+        return ("the body, the head and config.noisy_linear disagree: the device kernels implement all four layers NoisyLinear "
+                "or all four nn.Linear, not a mix")
+    if body.gate not in (torch.tanh, F.relu):
+        return "the FCBody gate must be torch.tanh or F.relu"
+    if not next(network.parameters()).is_cuda:
+        return "the network is not on a CUDA device (select_device(0))"
+    D, H1, H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
+    A, K = network.action_dim, network.num_atoms
+    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32 or not 2 <= K <= 256:
+        return ("sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32, "
+                "2 <= atoms %d <= 256" % (D, H1, H2, A, K))
+    if not isinstance(agent.optimizer, torch.optim.RMSprop) or agent._flat is None:
+        return "the optimizer is %s; the device update implements RMSprop" % type(agent.optimizer).__name__
+    if type(config.state_normalizer) is not RescaleNormalizer:
+        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
+    if config.history_length not in (None, 1):
+        return "history_length is %d; the device kernels read single 1-D states, not frame stacks" % config.history_length
+    smem = _lib.lib().b2rl_rainbow_smem_bytes(int(noisy[0]), D, H1, H2, A, K, int(config.batch_size), int(bool(config.double_q)))
+    if not 0 < smem <= 227 * 1024:
+        return ("a batch of %d needs %d bytes of shared memory, more than one SM has (b2rl_rainbow_smem_bytes)"
+                % (config.batch_size, smem))
+    return None
+
+
+class DeviceRainbow(DeviceDistDQN):
+    """``CategoricalDQNAgent.step()`` for a RainbowNet on the device (``config.device_rainbow``): one ``b2rl_rainbow_actor_step``
+    launch per env step and one ``b2rl_rainbow_replay_update`` launch per gradient update (csrc/rainbow.cu).  The arenas, the
+    target network's parameters as views into the target arena, the staging buffers, the target sync and the locking with
+    ``async_actor`` are ``DeviceDistDQN``'s / ``DeviceDQN``'s.
+
+    NoisyLinear: the kernels draw the factorised noise themselves (Philox stream 29 under the agent's key, position
+    ``noise_counter``: an actor step advances it by ``noise_len``, an update by twice that, the target network's vector first),
+    so the eager ``reset_noise()`` calls do not run.  The online module's noise buffers become views into ``noise`` (the vectors
+    of all layers, then every bias_epsilon, then every weight_epsilon), which every update writes: ``eval_step``, ``save`` and
+    any eager code see the noise of the latest update.  The actor steps' noise and the target module's buffers are not written
+    back.
+
+    Test hooks: ``forced`` (the actions of the next env step) and ``forced_noise``, a callable ``(count)`` returning the noise
+    vector(s) of the next launch: ``count`` is 1 for an actor step (``noise_len`` floats) and 2 for an update (the target's, then
+    the online network's); then nothing is drawn and the counter does not move."""
+
+    flag = "config.device_rainbow"
+
+    @staticmethod
+    def unsupported(agent):
+        return rainbow_unsupported(agent)
+
+    def __init__(self, agent, seed):
+        from ..utils import Config
+        self.kind = 0
+        DeviceDQN.__init__(self, agent, seed)
+        n, c = agent.network, agent.config
+        self.noisy = int(bool(n.noisy_linear))
+        self.A, self.K = n.action_dim, n.num_atoms
+        self.v_min, self.v_max = float(c.categorical_v_min), float(c.categorical_v_max)
+        self._dims = (self.D, self.H1, self.H2, self.A, self.K)
+        self.noise_std = float(Config.NOISY_LAYER_STD)
+        self.noise_counter = torch.zeros(1, dtype=torch.int64, device=self.dev)
+        self.forced_noise = None
+        shapes = [(m.in_features, m.out_features) for m in rainbow_layers(n)]
+        self.noise_len = sum(i + 2 * o for i, o in shapes)
+        self.noise = torch.zeros(self.noise_len + sum(o + o * i for i, o in shapes), dtype=_f32, device=self.dev)
+        self._given_noise = torch.zeros(2 * self.noise_len, dtype=_f32, device=self.dev)
+        if self.noisy:
+            self._adopt_noise_buffers()
+
+    @staticmethod
+    def _tensors(net):
+        return rainbow_kernel_order(net)
+
+    def _adopt_noise_buffers(self):
+        """The online module's noise buffers as views into ``noise`` (their present values kept)."""
+        layers = rainbow_layers(self.net)
+        o, views = 0, []
+        for m in layers:
+            for k in RAINBOW_NOISE_BUFFERS:
+                views.append((m, k, o))
+                o += getattr(m, k).numel()
+        for k in ("bias_epsilon", "weight_epsilon"):
+            for m in layers:
+                views.append((m, k, o))
+                o += getattr(m, k).numel()
+        assert o == self.noise.numel()
+        with torch.no_grad():
+            for m, k, o in views:
+                old = getattr(m, k)
+                view = self.noise[o:o + old.numel()].view_as(old)
+                view.copy_(old)
+                setattr(m, k, view)
+
+    def _noise_arg(self, count):
+        if self.forced_noise is None or not self.noisy:
+            return None
+        v = torch.as_tensor(np.asarray(self.forced_noise(count), dtype=np.float32).reshape(count * self.noise_len))
+        self._given_noise[:v.numel()].copy_(v)
+        return _lib.ptr(self._given_noise)
+
+    def act(self, raw_obs, epsilon, noise_out=None):
+        """One env step's actions: fresh noise + rescale + forward + dueling combination + action values + the choice in one
+        launch, downloaded for ``task.step``.  ``noise_out``: optional float32 device tensor [noise_len] for the noise used."""
+        obs, given = self._stage(raw_obs)
+        _lib.call("b2rl_rainbow_actor_step", self.noisy, self.gate, obs, self._scale, self._flat, self._off, *self._dims, self.N,
+                  self.v_min, self.v_max, float(epsilon), self._row_ptrs(0)[1], given, self.seed, _lib.ptr(self.counter),
+                  self.noise_std, self._noise_arg(1), _lib.ptr(noise_out), _lib.ptr(self.noise_counter), _lib.stream())
+        return self._fetch(0)[:, 0].astype(np.int64)
+
+    def update(self, tr, beta=0.0, loss_vec=None, target_noise_out=None):
+        """One gradient update on a sampled batch (``Transition`` / ``PrioritizedTransition`` of device tensors).  Returns the
+        objective (0-dim device tensor) and, for a prioritized batch, the new priorities (float32 device tensor [B]).
+        ``loss_vec``: optional float32 device tensor [B] for the per-sample KL; ``target_noise_out``: optional [noise_len] for
+        the target network's noise."""
+        c, o = self.cfg, self.opt
+        s, s2 = tr.state, tr.next_state
+        self._check_states(s)
+        self._offsets()
+        B = s.shape[0]
+        per = getattr(tr, "sampling_prob", None) is not None
+        loss = torch.empty((), dtype=_f32, device=self.dev)
+        prio = torch.empty(B, dtype=_f32, device=self.dev) if per else None
+        ptr = lambda t: _lib.ptr(None if t is None else t.contiguous())
+        _lib.call("b2rl_rainbow_replay_update", self.noisy, self.gate, ptr(s), ptr(s2), int(s.dtype == _f64), self._scale,
+                  ptr(tr.action), ptr(tr.reward), ptr(tr.mask), B, *self._dims, self._flat, _lib.ptr(self.target),
+                  _lib.ptr(o.s1), _lib.ptr(o.s2), _lib.ptr(o.step_dev), self._off, float(o.lr), float(o.alpha), float(o.eps),
+                  int(o.centered), float(c.discount ** c.n_step), int(bool(c.double_q)), self.v_min, self.v_max,
+                  float(c.gradient_clip or 0.0), ptr(tr.sampling_prob if per else None), float(beta),
+                  float(getattr(c, "replay_eps", 0.01)), float(getattr(c, "replay_alpha", 0.5)), ptr(prio), ptr(loss_vec),
+                  _lib.ptr(loss), self.seed, self.noise_std, self._noise_arg(2),
+                  _lib.ptr(self.noise) if self.noisy else None, ptr(target_noise_out), _lib.ptr(self.noise_counter),
+                  _lib.stream())
         return loss, prio

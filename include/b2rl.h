@@ -530,6 +530,47 @@ int b2rl_dist_dqn_replay_update(int32_t kind, int32_t gate, const void* state, c
                                 float max_norm, const float* sampling_prob, float beta, float replay_eps, float replay_alpha,
                                 float* priority_out, float* loss_vec_out, float* loss, void* stream);
 
+/* Rainbow on the device (csrc/rainbow.cu): CategoricalDQNAgent for a RainbowNet on a two-layer FCBody.  noisy 1: all four
+ * layers (body.layers.0, body.layers.1, fc_advantage [A K][H2], fc_value [K][H2], the kernels' layer order) are NoisyLinear and
+ * flat holds weight_mu weight_sigma bias_mu bias_sigma of layer l at off[4 l .. 4 l + 3]; noisy 0: all four are nn.Linear,
+ * weight bias at off[2 l], off[2 l + 1].  gate 0 tanh / 1 ReLU.  Limits and the support as b2rl_dist_dqn_*.
+ *
+ * A network's noise vector is, layer after layer, noise_in [in], noise_out_weight [out], noise_out_bias [out]: noise_len =
+ * sum (in + 2 out) floats.  Element i of a drawn vector is noise_std times the standard normal of Philox stream 29 under
+ * `seed` at position *noise_counter + i.  f(x) = sign(x) sqrt|x|; the effective parameters mu + sigma (f(out_w) (x) f(in)),
+ * mu_b + sigma_b f(out_b) are formed as the weights are read.  With noisy 0 nothing is drawn and the noise arguments are ignored.
+ *
+ * actor_step: one noise vector for the online network (given_noise != NULL: that vector [noise_len], nothing drawn, the
+ * counter stays; else *noise_counter advances by noise_len), rescale + forward + q[a][k] = v[k] + adv[a][k] - mean_a adv[.][k]
+ * + sum_k softmax(q[a])_k z_k + the action.  noisy 1: the argmax, epsilon is not read and *counter stays (DQN_agent.py:34-35);
+ * noisy 0: b2rl_dist_dqn_actor_step's epsilon-greedy on stream 17 (*counter advances by 2 N).  given_action != NULL: written
+ * through.  noise_out (optional) [noise_len]: the vector used.
+ *
+ * replay_update: one launch on a sampled batch (the arguments of b2rl_dist_dqn_replay_update with kind C51, then the noise).
+ * Noise for the target network, then for the online network (given_noise != NULL: [2][noise_len] in that order, nothing drawn;
+ * else *noise_counter advances by 2 noise_len).  The forwards, C51's projection, KL (loss_vec_out [B], optional), PER and logit
+ * gradient, the backward through the dueling combination and the effective weights; d mu = dW, d sigma = dW eps_w, d mu_b = db,
+ * d sigma_b = db eps_b; clip_grad_norm_(max_norm) over all tensors and RMSprop.  noise_out (optional): the online module's
+ * noise arena -- the online vector [noise_len], then every layer's bias_epsilon [out], then every layer's weight_epsilon
+ * [out][in].  target_noise_out (optional) [noise_len].  smem_bytes: 0 for invalid input; double_q does not change it (the
+ * online forward of the next states uses the rows the target's forward takes afterwards); it must fit the 227 KB of one SM. */
+int64_t b2rl_rainbow_smem_bytes(int32_t noisy, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t K, int32_t B,
+                                int32_t double_q);
+int b2rl_rainbow_actor_step(int32_t noisy, int32_t gate, const double* obs, double obs_scale, const float* flat,
+                            const int32_t* off, int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t K, int32_t N, double v_min,
+                            double v_max, float epsilon, float* action_out, const float* given_action, uint64_t seed,
+                            int64_t* counter, float noise_std, const float* given_noise, float* noise_out,
+                            int64_t* noise_counter, void* stream);
+int b2rl_rainbow_replay_update(int32_t noisy, int32_t gate, const void* state, const void* next_state, int32_t state_f64,
+                               double state_scale, const int64_t* action, const float* reward, const float* mask, int32_t B,
+                               int32_t D, int32_t H1, int32_t H2, int32_t A, int32_t K, float* flat, const float* target,
+                               float* square_avg, float* grad_avg, int64_t* step, const int32_t* off, float lr, float alpha,
+                               float eps, int32_t centered, float discount_n, int32_t double_q, double v_min, double v_max,
+                               float max_norm, const float* sampling_prob, float beta, float replay_eps, float replay_alpha,
+                               float* priority_out, float* loss_vec_out, float* loss, uint64_t seed, float noise_std,
+                               const float* given_noise, float* noise_out, float* target_noise_out, int64_t* noise_counter,
+                               void* stream);
+
 int b2rl_ipc_alloc(int64_t bytes, void** out);
 int b2rl_ipc_get_handle(void* ptr, void* handle_out);
 int b2rl_ipc_open_handle(const void* handle, void** out);

@@ -3,11 +3,16 @@ device flag (one actor-step launch per env step, one update launch per rollout o
 ``config.device_a2c`` for A2CAgent (a2c_feature, a2c_continuous), ``config.device_nstep_dqn`` for NStepDQNAgent
 (n_step_dqn_feature), ``config.device_dqn`` for DQNAgent (dqn_feature, timed past its exploration steps), ``config.device_c51``
 / ``config.device_qr`` for CategoricalDQNAgent / QuantileRegressionDQNAgent (categorical_dqn_feature,
-quantile_regression_dqn_feature: csrc/dist_dqn.cu, with the launchers' async actor) -- in one process on one card, the two
+quantile_regression_dqn_feature: csrc/dist_dqn.cu, with the launchers' async actor), ``config.device_rainbow`` for
+CategoricalDQNAgent on a noisy RainbowNet (rainbow_feature: csrc/rainbow.cu) -- in one process on one card, the two
 alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
 left to the learner is visible.  Prints the card's name and power limit with the numbers.
 
-    python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--out DIR]
+    python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--only LAUNCHER[,LAUNCHER]] [--out DIR]
+
+A side whose ``step()`` raises while it is warmed up is reported with its error and not timed (rainbow_feature's eager path:
+its actor thread resets the NoisyLinear noise buffers in place while the learner's autograd graph holds them, and torch's
+version check stops the backward).
 """
 import argparse
 import json
@@ -27,7 +32,8 @@ CONFIGS = [("a2c_feature", "CartPole-v0", "device_a2c", "a2c"), ("a2c_continuous
            ("n_step_dqn_feature", "CartPole-v0", "device_nstep_dqn", "nstep_dqn"),
            ("dqn_feature", "CartPole-v0", "device_dqn", "dqn"),
            ("categorical_dqn_feature", "CartPole-v0", "device_c51", "c51"),
-           ("quantile_regression_dqn_feature", "CartPole-v0", "device_qr", "qr")]
+           ("quantile_regression_dqn_feature", "CartPole-v0", "device_qr", "qr"),
+           ("rainbow_feature", "CartPole-v0", "device_rainbow", "rainbow")]
 
 
 def card():
@@ -77,10 +83,10 @@ def past_exploration(agent):
 def env_only(agent, steps):
     """task.step alone, env_steps * steps times, with the actions of one draw (what the host envs cost per agent step).  With
     an async actor its thread owns its task, so a new one is made."""
-    from deeprl_b200 import CategoricalActorCriticNet, CategoricalNet, DuelingNet, QuantileNet, VanillaNet
+    from deeprl_b200 import CategoricalActorCriticNet, CategoricalNet, DuelingNet, QuantileNet, RainbowNet, VanillaNet
     c = agent.config
     a = (np.zeros(c.num_workers, dtype=np.int64)
-         if isinstance(agent.network, (CategoricalActorCriticNet, VanillaNet, DuelingNet, CategoricalNet, QuantileNet))
+         if isinstance(agent.network, (CategoricalActorCriticNet, VanillaNet, DuelingNet, CategoricalNet, QuantileNet, RainbowNet))
          else np.zeros((c.num_workers, c.action_dim), dtype=np.float32))
     own = hasattr(agent, "actor") and c.async_actor
     task = agent.task if hasattr(agent, "task") else c.task_fn() if own else agent.actor._task
@@ -100,6 +106,7 @@ def main():
     ap.add_argument("--steps", type=int, default=300)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--only", default=None, help="comma-separated launcher names (default: all of CONFIGS)")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -109,27 +116,38 @@ def main():
     rl.random_seed(0)
     result = dict(card=card(), steps_per_round=args.steps, rounds=args.rounds, configs={})
     print(result["card"])
+    only = None if args.only is None else set(args.only.split(","))
+    if only is not None and not only <= {c[0] for c in CONFIGS}:
+        raise SystemExit("--only: unknown launcher in %s" % sorted(only))
     for name, game, flag, unit in CONFIGS:
+        if only is not None and name not in only:
+            continue
         agents = {"eager": make_agent(name, game, flag, False), flag: make_agent(name, game, flag, True)}
-        for ag in agents.values():
-            past_exploration(ag)
-            timed(ag, args.warmup)
-        rates = {k: [] for k in agents}
+        failed = {}
+        for k, ag in agents.items():
+            try:
+                past_exploration(ag)
+                timed(ag, args.warmup)
+            except RuntimeError as e:
+                failed[k] = "%s: %s" % (type(e).__name__, str(e).split(". Hint")[0])
+        timed_agents = {k: ag for k, ag in agents.items() if k not in failed}
+        rates = {k: [] for k in timed_agents}
         for _ in range(args.rounds):                        # alternated: both see the same host / card conditions
-            for k, ag in agents.items():
+            for k, ag in timed_agents.items():
                 rates[k].append(timed(ag, args.steps))
-        env = env_only(agents["eager"], args.steps)
-        c = agents["eager"].config
+        env = env_only(agents[flag], args.steps)
+        c = agents[flag].config
         med = {k: float(np.median(v)) for k, v in rates.items()}
         learner_ms = {k: 1e3 / med[k] - 1e3 / env for k in med}
-        row = {"game": game, "num_workers": c.num_workers, "env_steps_per_agent_step": env_steps(agents["eager"]), unit + "_steps_per_s": rates,
-               "median_%s_steps_per_s" % unit: med, "speedup": med[flag] / med["eager"], "env_only_%s_steps_per_s" % unit: env,
-               "ms_per_step_besides_envs": learner_ms}
+        row = {"game": game, "num_workers": c.num_workers, "env_steps_per_agent_step": env_steps(agents[flag]), unit + "_steps_per_s": rates,
+               "median_%s_steps_per_s" % unit: med, "speedup": med[flag] / med["eager"] if len(med) == 2 else None,
+               "env_only_%s_steps_per_s" % unit: env, "ms_per_step_besides_envs": learner_ms, "failed": failed}
         result["configs"][name] = row
-        print("%-18s %-20s N=%d env steps %d  eager %8.1f steps/s  %s %8.1f steps/s  (x%.2f)  envs alone %8.1f steps/s;  "
-              "ms per step besides the envs: eager %.3f, %s %.3f"
-              % (name, game, c.num_workers, env_steps(agents["eager"]), med["eager"], flag, med[flag], row["speedup"], env,
-                 learner_ms["eager"], flag, learner_ms[flag]))
+        print("%-18s %-20s N=%d env steps %d  %s;  envs alone %8.1f steps/s;  ms per step besides the envs: %s%s"
+              % (name, game, c.num_workers, env_steps(agents[flag]),
+                 "  ".join("%s %8.1f steps/s" % kv for kv in med.items()) + ("  (x%.2f)" % row["speedup"] if row["speedup"] else ""),
+                 env, ", ".join("%s %.3f" % kv for kv in learner_ms.items()),
+                 "".join(";  %s not timed (%s)" % kv for kv in failed.items())))
         for ag in agents.values():
             ag.close()
     print(json.dumps(result))
