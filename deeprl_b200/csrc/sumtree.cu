@@ -192,10 +192,15 @@ __global__ void __launch_bounds__(ST_MAX_B) sumtree_sample_kernel(const double* 
     if (!uniforms || !fills) ring_state[4] = (int64_t)(ctr + 2ull * B);
   }
   __syncthreads();
-  if (i < B && n_valid > 0) {
-    tidx_out[i] = s_t[i];
-    didx_out[i] = s_t[i] - cap + 1;
-    prob_out[i] = s_p[i];
+  // With no valid draw the reference has nothing to back-fill from (random.choice raises).  The consumers (gather, conv1's
+  // ring reads) use the outputs without a host check inside a captured graph, so they must still hold valid indices: as in
+  // select_uniform_kernel, every row gets the smallest data index that cannot read below the ring (hl - 1), its leaf and that
+  // leaf's probability.  status[0] = 0 tells the host check.
+  if (i < B) {
+    const int64_t t = n_valid > 0 ? s_t[i] : (int64_t)(hl - 1) + cap - 1;
+    tidx_out[i] = t;
+    didx_out[i] = t - cap + 1;
+    prob_out[i] = n_valid > 0 ? s_p[i] : __ddiv_rn(tree[t], total);
   }
 }
 
@@ -273,6 +278,7 @@ extern "C" int b2rl_sumtree_sample(const double* tree, uint8_t* pending, int64_t
                "null pointer");
   B2RL_REQUIRE(capacity >= 2, "capacity must be >= 2");
   B2RL_REQUIRE(B > 0 && B <= ST_MAX_B, "B must be in [1, 1024]");
+  B2RL_REQUIRE(history >= 1 && history <= capacity, "history must be in [1, capacity]");
   sumtree_sample_kernel<<<1, ST_MAX_B, 0, (cudaStream_t)stream>>>(tree, pending, capacity, ring_state, uniforms, fills,
                                                                   seed, history, n_step, B, tree_idx_out, data_idx_out,
                                                                   sampling_prob_out, status_out);

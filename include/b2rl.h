@@ -101,8 +101,12 @@ int b2rl_sumtree_add(double* tree, uint8_t* pending, int64_t capacity, int64_t* 
  * (seg*(i+1) - seg*i) * u_i (CPython random.uniform), sum_tree.py:23-33 descent rule, validity filter in batch
  * order, back-fill.  uniforms: float64 [B] in [0,1) or NULL (Philox, 53-bit).  fills: int64 [B] positions for
  * the back-fill draws (used modulo the current list length) or NULL (Philox).
+ * Philox draws: u_i = u53 at ring_state[4] + i (stream 2), back-fill k = below(len) at ring_state[4] + B + k (stream 3);
+ * ring_state[4] advances by 2B unless both uniforms and fills are given.  history must be in [1, capacity].
  * Outputs: tree_idx int64 [B], data_idx int64 [B], sampling_prob float64 [B] (= p / total), status int32[2] =
- * {valid before back-fill, 0}. */
+ * {valid before back-fill, 0}.  With no valid draw (status[0] == 0, where the reference's random.choice raises) every
+ * row gets data index history - 1, its leaf and that leaf's p / total, so that consumers reading frames through the
+ * outputs without a host check stay inside the ring. */
 int b2rl_sumtree_sample(const double* tree, uint8_t* pending, int64_t capacity, int64_t* ring_state,
                         const double* uniforms, const int64_t* fills, uint64_t seed, int32_t history, int32_t n_step,
                         int32_t B, int64_t* tree_idx_out, int64_t* data_idx_out, double* sampling_prob_out,
