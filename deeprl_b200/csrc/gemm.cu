@@ -216,6 +216,10 @@ __device__ __forceinline__ int4 ldg_v4_here(const void* ptr) {
   asm volatile("ld.global.nc.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(ptr));
   return v;
 }
+// 16-byte global store of a 16-byte aligned address
+__device__ __forceinline__ void stg128(void* ptr, const int4 v) {
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(ptr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
 template <int BN, bool EXT>
 __device__ __forceinline__ void epi_mask_load(const GemmParams& p, int row0, int n0, int t, int4 (&m)[BN / 16]) {
   if constexpr (EXT) {
@@ -303,18 +307,23 @@ __device__ __forceinline__ int64_t epi_col_off(const GemmParams& p, int n) {
 
 // Epilogue of one 64-row half of a 128 x BN tile (first row row0, first column n0) for warpgroup thread t: `s` is the
 // half's fp32 staging tile, `m` its mask (epi_mask_load).  The bias-gradient column sums of the half stay in registers
-// (dsum: the thread's 8 columns over its BN/16 rows) until one dbias_flush at the end.
-template <int BN, bool EXT>
+// (dsum: the thread's 8 columns over its BN/16 rows) until one dbias_flush at the end.  PAIR (paired conv1 forward, n0 = 0):
+// tile columns 0 .. BN/2 - 1 are columns of (D, bias), columns BN/2 .. BN - 1 those of (D2, bias2); p.N = BN / 2.
+template <int BN, bool EXT, bool PAIR = false>
 __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int n0, int t, const float* s,
                                               const int4 (&m)[BN / 16], float* s_dbias) {
   constexpr int ACC_LD = acc_ld(BN);
   float dsum[8] = {};
-  const int c = epi_col<BN>(t), n = n0 + c;
+  const int c = epi_col<BN>(t);
+  const bool second = PAIR && c >= BN / 2;                    // the thread's 8 columns all lie in one half
+  const int n = n0 + c - (second ? BN / 2 : 0);
+  const float* bias = second ? p.bias2 : p.bias;
+  void* D = second ? p.D2 : p.D;
   const bool cols = n < p.N, full = n + 8 <= p.N;
-  const bool add_bias = p.bias && blockIdx.z == 0 && cols;
+  const bool add_bias = bias && blockIdx.z == 0 && cols;
   float b[8];
   if (add_bias) {
-    const float* bp = p.bias + n;
+    const float* bp = bias + n;
     if (full && (reinterpret_cast<uintptr_t>(bp) & 15) == 0) {
       const float4 b0 = __ldg(reinterpret_cast<const float4*>(bp)), b1 = __ldg(reinterpret_cast<const float4*>(bp + 4));
       b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
@@ -373,8 +382,17 @@ __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int
           if (full || n + j < p.N) dsum[j] += v[j];
       }
     }
-    if (p.out_mode == 0) {
-      __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(p.D) + off;
+    if constexpr (PAIR) {
+      // bf16, whole 16-byte column groups (b2rl_conv1_u8_fwd_pair): the one store form, which keeps the code of this
+      // epilogue small beside the converters' and the producer's (explicit store: through the selected pointer the compiler
+      // splits it)
+      int4 o;
+      __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
+      stg128(reinterpret_cast<__nv_bfloat16*>(D) + off, o);
+    } else if (p.out_mode == 0) {
+      __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(D) + off;
       if (full && off % 8 == 0) {
         int4 o;
         __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
@@ -387,7 +405,7 @@ __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int
           if (n + j < p.N) d[j] = __float2bfloat16_rn(v[j]);
       }
     } else if (p.out_mode == 1) {
-      float* d = reinterpret_cast<float*>(p.D) + off;
+      float* d = reinterpret_cast<float*>(D) + off;
       if (full && off % 4 == 0) {
         *reinterpret_cast<float4*>(d) = make_float4(v[0], v[1], v[2], v[3]);
         *reinterpret_cast<float4*>(d + 4) = make_float4(v[4], v[5], v[6], v[7]);
@@ -397,7 +415,7 @@ __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int
           if (n + j < p.N) d[j] = v[j];
       }
     } else {
-      float* d = reinterpret_cast<float*>(p.D) + off;
+      float* d = reinterpret_cast<float*>(D) + off;
       if (full && (reinterpret_cast<uintptr_t>(d) & 15) == 0) {
         atomicAdd(reinterpret_cast<float4*>(d), make_float4(v[0], v[1], v[2], v[3]));
         atomicAdd(reinterpret_cast<float4*>(d + 4), make_float4(v[4], v[5], v[6], v[7]));
@@ -746,6 +764,7 @@ struct U8Src {
   int G;                     // grid width = frame_w / 4 (21); slab rows are (b, gy, gx) over G x G positions per image
   int rows;                  // batch * G * G
   int stages;                // uint8 staging tiles in flight (set by the launcher, <= U8_MAX_STAGES)
+  int nf;                    // frames per image box: history (4), or 5 for the paired forward's window of s and s'
 };
 
 __device__ __forceinline__ int4 cvt8_u8_bf16(uint32_t w0, uint32_t w1) {
@@ -771,14 +790,17 @@ __device__ __forceinline__ int4 cvt8_u8_bf16(uint32_t w0, uint32_t w1) {
 // ONE image are the box [4 frames][slots grid rows][frame_w words] at (word 0, grid row q0 - b*G, ring row idx[b] + first) --
 // one tensor load per image the slab touches (at most two), instead of one bulk copy per (image, frame) whose fixed cost
 // is serialised per SM.  Grid rows past the end of the image are
-// zero-filled by the TMA and never read.
-//   staging layout of one tile: [image segment 0 | 1][frame f][slot = grid-row index q - qseg][4 * frame_w bytes]
+// zero-filled by the TMA and never read.  The paired forward (b2rl_conv1_u8_fwd_pair) loads nf = 5 frames per image: the
+// window idx-3 .. idx+1 that holds both s (frames 0-3) and s' (frames 1-4).
+//   staging layout of one tile: [image segment 0 | 1][frame f < nf][slot = grid-row index q - qseg][4 * frame_w bytes]
 constexpr int U8_MAX_STAGES = 8;
 __host__ __device__ inline int u8_slots(int slab_rows, int G) { return (slab_rows + G - 2) / G + 1; }
-__host__ __device__ inline int u8_box_bytes(int slab_rows, int G, int frame_w) {
-  return (4 * u8_slots(slab_rows, G) * 4 * frame_w + 127) & ~127;
+__host__ __device__ inline int u8_box_bytes(int slab_rows, int G, int frame_w, int nf) {
+  return (nf * u8_slots(slab_rows, G) * 4 * frame_w + 127) & ~127;
 }
-__host__ __device__ inline int u8_stage_bytes(int slab_rows, int G, int frame_w) { return 2 * u8_box_bytes(slab_rows, G, frame_w); }
+__host__ __device__ inline int u8_stage_bytes(int slab_rows, int G, int frame_w, int nf) {
+  return 2 * u8_box_bytes(slab_rows, G, frame_w, nf);
+}
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
@@ -807,7 +829,7 @@ __device__ __forceinline__ U8Plan u8_plan(const U8Src& u, int R0, int slab_rows)
 // ONE thread: arm `bar` with the tile's byte count and issue its one or two tensor loads; i0 / i1 = idx[b0] / idx[b0 + 1]
 __device__ __forceinline__ void u8_issue(const U8Src& u, const CUtensorMap* map, const U8Plan& pl, long long i0, long long i1,
                                          uint8_t* stage, uint64_t* bar, int slots) {
-  const uint32_t box = (uint32_t)(4 * slots * 4 * u.frame_w);          // bytes the TMA reports per box (zero fill included)
+  const uint32_t box = (uint32_t)(u.nf * slots * 4 * u.frame_w);       // bytes the TMA reports per box (zero fill included)
   const int nb = (pl.n0 > 0) + (pl.n1 > 0);
   if (nb == 0) { mb_arrive(bar); return; }
   mb_expect_tx(bar, box * nb);
@@ -827,9 +849,17 @@ __device__ __forceinline__ void sts128(uint32_t addr, const int4 v) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
+// shared-memory address of chunk j (16 bytes = 8 channels) of slab row rl: chunks 0-7 (frames 0-3) lie in the 128B-swizzled
+// 64-channel block `slab`; chunks 8-9 (frame 4, paired forward only) in block `slab_b` of 32-byte rows with the 32-byte swizzle
+// (address bit 4 ^= bit 7; slab_b is 256-byte aligned, so bit 7 is bit 2 of the row)
+__device__ __forceinline__ uint32_t slab_chunk(uint32_t slab, uint32_t slab_b, int rl, int j) {
+  return j < 8 ? slab + (uint32_t)(rl * 128 + ((j ^ (rl & 7)) << 4)) : slab_b + (uint32_t)(rl * 32 + (((j - 8) ^ ((rl >> 2) & 1)) << 4));
+}
+
 template <int J0, int NJ>
-__device__ __forceinline__ void u8_store_chunks(uint32_t stage, uint32_t slab, int rl, int so, int fstride, int frame_w) {
-  // chunks J0 .. J0+NJ-1 (16 bytes = 8 channels each) of slab row rl; so = staging offset of pixel (4gy, 4gx) of frame 0, or -1: zeros
+__device__ __forceinline__ void u8_store_chunks(uint32_t stage, uint32_t slab, uint32_t slab_b, int rl, int so, int fstride,
+                                                int frame_w) {
+  // chunks J0 .. J0+NJ-1 of slab row rl; so = staging offset of pixel (4gy, 4gx) of frame 0, or -1: zeros
   uint32_t w0[NJ], w1[NJ];
 #pragma unroll
   for (int jj = 0; jj < NJ; ++jj) {                       // all loads first, then the conversions
@@ -842,26 +872,24 @@ __device__ __forceinline__ void u8_store_chunks(uint32_t stage, uint32_t slab, i
     }
   }
 #pragma unroll
-  for (int jj = 0; jj < NJ; ++jj) {
-    const int j = J0 + jj;
-    sts128(slab + (uint32_t)(rl * 128 + ((j ^ (rl & 7)) << 4)), cvt8_u8_bf16(w0[jj], w1[jj]));
-  }
+  for (int jj = 0; jj < NJ; ++jj) sts128(slab_chunk(slab, slab_b, rl, J0 + jj), cvt8_u8_bf16(w0[jj], w1[jj]));
 }
 
 // NT = 128 or 256 threads (tid 0..NT-1, named barrier `bar_id`) convert one staged tile into the swizzled bf16 slab of
-// `slab_rows` rows x 64 channels whose first row is grid-matrix row R0; rows >= u.rows are zero (what the TMA's out-of-bounds
-// fill gave).  Thread t owns slab row t & 127 (consecutive threads -> consecutive pixels of the staging rows and the 8 distinct
-// swizzle positions of a 128-byte window: conflict-free both ways) and, with 256 threads, one half of its 8 chunks; rows beyond
-// 128 are shared out chunk-wise.  On return every thread's stores are fenced towards the async proxy (wgmma reads shared
-// memory through it) and all NT threads have arrived.
-template <int NT>
-__device__ __forceinline__ void u8_convert(const U8Src& u, const uint8_t* stage_p, uint8_t* slab_p, int R0, int slab_rows,
-                                           int slots, int tid, int bar_id) {
-  const uint32_t stage = s2u(stage_p), slab = s2u(slab_p);
+// `slab_rows` rows x 8 NCH channels whose first row is grid-matrix row R0 (NCH = 8: one 64-channel block; 10: the paired
+// forward's block A of frames 0-3 and block B of frame 4, see slab_chunk); rows >= u.rows are zero (what the TMA's
+// out-of-bounds fill gave).  Thread t owns slab row t & 127 (consecutive threads -> consecutive pixels of the staging rows and
+// the 8 distinct swizzle positions of a 128-byte window: conflict-free both ways) and, with 256 threads, one half of its NCH
+// chunks; rows beyond 128 are shared out chunk-wise.  On return every thread's stores are fenced towards the async proxy
+// (wgmma reads shared memory through it) and all NT threads have arrived.
+template <int NT, int NCH>
+__device__ __forceinline__ void u8_convert(const U8Src& u, const uint8_t* stage_p, uint8_t* slab_p, uint8_t* slab_b_p, int R0,
+                                           int slab_rows, int slots, int tid, int bar_id) {
+  const uint32_t stage = s2u(stage_p), slab = s2u(slab_p), slab_b = NCH > 8 ? s2u(slab_b_p) : 0u;
   const int rowb = 4 * u.frame_w, fstride = slots * rowb;
   const int q0 = R0 / u.G;
   const int qb1 = (q0 / u.G + 1) * u.G;                   // first grid row of the second image the slab may touch
-  const int seg1 = (4 * fstride + 127) & ~127;            // its box sits behind the first image's
+  const int seg1 = (u.nf * fstride + 127) & ~127;         // its box sits behind the first image's
   const int rl0 = tid & 127;
   if (rl0 < slab_rows) {
     const int r = R0 + rl0;
@@ -871,15 +899,15 @@ __device__ __forceinline__ void u8_convert(const U8Src& u, const uint8_t* stage_
       so = (q >= qb1 ? seg1 + (q - qb1) * rowb : (q - q0) * rowb) + 4 * (r - q * u.G);
     }
     if (NT == 128) {
-      u8_store_chunks<0, 8>(stage, slab, rl0, so, fstride, u.frame_w);
+      u8_store_chunks<0, NCH>(stage, slab, slab_b, rl0, so, fstride, u.frame_w);
     } else if (tid < 128) {
-      u8_store_chunks<0, 4>(stage, slab, rl0, so, fstride, u.frame_w);
+      u8_store_chunks<0, NCH / 2>(stage, slab, slab_b, rl0, so, fstride, u.frame_w);
     } else {
-      u8_store_chunks<4, 4>(stage, slab, rl0, so, fstride, u.frame_w);
+      u8_store_chunks<NCH / 2, NCH / 2>(stage, slab, slab_b, rl0, so, fstride, u.frame_w);
     }
   }
-  for (int e = tid; e < (slab_rows - 128) * 8; e += NT) {
-    const int rl = 128 + (e >> 3), j = e & 7, r = R0 + rl;
+  for (int e = tid; e < (slab_rows - 128) * NCH; e += NT) {
+    const int rl = 128 + e / NCH, j = e % NCH, r = R0 + rl;
     uint32_t w0 = 0, w1 = 0;
     if (r < u.rows) {
       const int q = r / u.G;
@@ -888,7 +916,7 @@ __device__ __forceinline__ void u8_convert(const U8Src& u, const uint8_t* stage_
       w0 = lds32(src);
       w1 = lds32(src + u.frame_w);
     }
-    sts128(slab + (uint32_t)(rl * 128 + ((j ^ (rl & 7)) << 4)), cvt8_u8_bf16(w0, w1));
+    sts128(slab_chunk(slab, slab_b, rl, j), cvt8_u8_bf16(w0, w1));
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "n"(NT) : "memory");
@@ -902,21 +930,48 @@ struct SlabParams {
   int stages;
   int base_offset_mode;    // 1: descriptor base_offset = (window start >> 7) & 7; 2: base_offset = 0 (address-based swizzle)
   U8Src u8;                // U8 kernels: the activation slabs are built from the uint8 frame ring (K1), tmA is unused
+  unsigned long long* clk; // U8 kernels, profiling hook (normally null): cycles per role summed over the CTAs, K1_CLK_*
 };
 
+// slots of the K1 phase probe (b2rl_conv1_set_phase_clocks): clock64() cycles summed over all CTAs -- the CTA's whole run
+// (thread 0), the producer's waits for a free uint8 stage, the converters' (thread 0 of warp 12) waits for a free slab and for
+// the pixels and their conversion, the MMA warpgroups' (thread 0 of each) waits for the MMA turn and the slab, their chain
+// from the first issue to its retirement, their whole epilogue and its accumulator staging part (stage_acc + barrier); the
+// last slot counts the tiles the MMA warpgroups took.
+enum { K1_CLK_CTA, K1_CLK_PRODUCER_WAIT, K1_CLK_CONVERT_WAIT_SLAB, K1_CLK_CONVERT_WAIT_PIXELS, K1_CLK_CONVERT, K1_CLK_MMA_WAIT,
+       K1_CLK_MMA, K1_CLK_EPILOGUE, K1_CLK_EPILOGUE_STAGE, K1_CLK_TILES, K1_CLK_SLOTS };
+__device__ __forceinline__ long long clk_now(const unsigned long long* clk) { return clk ? clock64() : 0; }
+
 constexpr int SLAB_U8_THREADS = GEMM_THREADS + 128;   // K1: a fourth warpgroup (warps 12-15) converts the uint8 pixels
+
+// Paired conv1 forward (PAIR: U8, BN 64, 2 x 2 taps, one column block): x1 = conv1_online(s) and z1 = conv1_target(s') in ONE
+// launch from the five-frame ring window idx-3 .. idx+1 shared by s (frames 0-3) and s' (frames 1-4, n_step 1).
+//   slab:    block A = window frames 0-3, the 128B-swizzled 64-channel slab of s as above; block B = window frame 4, 16
+//            channels, rows of 32 bytes with the 32-byte swizzle (slab_chunk), pair_block_b_bytes behind block A
+//   weights: N = 64 stacked, per tap a 128B-swizzled [64 n][64 k] tile (k16 step j reads window frame j) and a 32B-swizzled
+//            [64 n][16 k] tile for frame 4.  Rows 0-31 = online: frames 0-3 as stored, zero at frame 4 (set in the prologue);
+//            rows 32-63 = target: zero at frame 0 (the TMA's out-of-bounds fill of a box that starts at channel -16), its
+//            frames 0-3 at window frames 1-4.
+// Per tap and accumulator half the chain is the four k16 steps over block A, then one over block B: every output column sees
+// the products of today's separate launch in the same k16 groups and tap order, plus exact zeros -- the same bits.
+__host__ __device__ inline uint32_t pair_block_b_bytes(int slab_rows) { return ((uint32_t)slab_rows * 32 + 1023) & ~1023u; }
+// wgmma descriptor of a K-major operand with 32-byte rows and the 32-byte swizzle (layout type 3): 8-row groups 256 B apart
+__device__ __forceinline__ uint64_t make_desc_sw32(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)3 << 62);
+}
 // The tap grid (TX x TY taps) and the column blocks (CB = channels / 64) are template parameters: a tile's 2 x TX x TY x CB
 // k-tiles are then one unrolled chain of wgmmas in ONE commit group (a chain carried through runtime loops makes ptxas
 // serialize every wgmma).  The two MMA warpgroups ping-pong: warpgroup g takes every other tile of the CTA (the CTA's
 // i-th tile goes to warpgroup i % 2), whole 128-row tiles as two m64 accumulator halves, and "MMA turn" named barriers
 // let a warpgroup issue its tile's MMAs only after the other one has issued the previous tile's -- so one warpgroup's
 // epilogue runs while the other's MMAs keep the tensor cores busy.
-template <int BN, bool EXT, bool U8, int TX, int TY, int CB>
-__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_slab_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                          const __grid_constant__ CUtensorMap tmB,
-                                                                          const __grid_constant__ CUtensorMap tmA2,
-                                                                          const __grid_constant__ CUtensorMap tmB2,
-                                                                          const SlabParams sp) {
+// The body of conv_slab_wgmma_kernel and of its paired conv1 instantiation conv1_pair_wgmma_kernel (below); the tensor maps
+// are the kernels' __grid_constant__ parameters.  PAIR: tmA = ring, tmB = online weights (box [32 n][1 tap][64 k]),
+// tmA2 / tmB2 = target weights (boxes [32][1][64] / [32][1][16]).
+template <int BN, bool EXT, bool U8, int TX, int TY, int CB, bool PAIR>
+__device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2,
+                                               const CUtensorMap& tmB2, const SlabParams& sp) {
+  static_assert(!PAIR || (U8 && !EXT && BN == 64 && TX == 2 && TY == 2 && CB == 1), "the paired forward is conv1's K1 shape");
   const int n_cta = sp.g.dual ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   const bool second = sp.g.dual && (int)blockIdx.x >= n_cta;
   const int cta = second ? (int)blockIdx.x - n_cta : (int)blockIdx.x;
@@ -925,22 +980,24 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
   GemmParams p = sp.g;
   if (second) { p.D = sp.g.D2; p.bias = sp.g.bias2; }
   constexpr uint32_t W_TILE = BN * 128;                               // one 64-wide k-tile of the weights
+  constexpr uint32_t WB_TILE = BN * 32;                               // PAIR: one tap's frame-4 weights
   constexpr int ACC_LD = acc_ld(BN);
   constexpr int MAX_STAGES = 6;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int k_tiles = TX * TY * CB;
   const uint32_t slab_block = (uint32_t)sp.slab_rows * 128;          // one 64-channel column block of a slab
-  const uint32_t slab_bytes = slab_block * CB;
+  const uint32_t slab_bytes = slab_block * CB + (PAIR ? pair_block_b_bytes(sp.slab_rows) : 0u);
   uint8_t* sW = smem;
-  uint8_t* sS = smem + (size_t)k_tiles * W_TILE;
+  uint8_t* sWB = smem + (size_t)k_tiles * W_TILE;                     // PAIR: frame-4 weight tiles
+  uint8_t* sS = sWB + (PAIR ? (size_t)k_tiles * WB_TILE : 0);
   float* sAcc = reinterpret_cast<float*>(sS + (size_t)sp.stages * slab_bytes);
   uint64_t* full = reinterpret_cast<uint64_t*>(sAcc + GEMM_BM * ACC_LD);
   uint64_t* empty = full + MAX_STAGES;
   uint64_t* w_full = empty + MAX_STAGES;
   // U8 (K1): uint8 staging tiles + their full / empty barriers live behind the barriers (launch_slab_t sizes the allocation)
   const int u8_slots_ = U8 ? u8_slots(sp.slab_rows, sp.u8.G) : 0;
-  const int u8_bytes = U8 ? u8_stage_bytes(sp.slab_rows, sp.u8.G, sp.u8.frame_w) : 0;
+  const int u8_bytes = U8 ? u8_stage_bytes(sp.slab_rows, sp.u8.G, sp.u8.frame_w, sp.u8.nf) : 0;
   uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(w_full + 2) + 127) & ~uintptr_t(127));
   const int U8_STAGES = U8 ? sp.u8.stages : 1;
   uint64_t* u8_full = reinterpret_cast<uint64_t*>(sU + (size_t)U8_STAGES * u8_bytes);
@@ -960,16 +1017,38 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(mA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(mB) : "memory");
+    if (PAIR) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA2) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB2) : "memory");
+    }
+  }
+  if constexpr (PAIR) {
+    // the online rows (0-31) of every tap's frame-4 weights are zero; the wgmmas read them through the async proxy
+    for (int i = threadIdx.x; i < k_tiles * (int)WB_TILE / 32; i += blockDim.x)
+      sts128(s2u(sWB) + (uint32_t)((i / 64) * WB_TILE + (i % 64) * 16), make_int4(0, 0, 0, 0));
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
   pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
+  unsigned long long* const clk = U8 ? sp.clk : nullptr;
+  const long long t_start = clk_now(clk);
+  long long c_wait = 0, c_wait2 = 0, c_work = 0, c_epi = 0, c_stage = 0;   // per-role sums of the probe (thread 0 of its role)
   // register file split of the 384-thread kernel (setmaxnreg): the producer warpgroup needs few, the MMA warpgroups hold two
   // m64 x BN accumulator halves across the epilogue of the first (BN 128: 128 registers); 128 x 56 + 256 x 224 <= 64K
   if (warp < 4) {
     if constexpr (!U8) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
     if (warp == 0 && elect_one()) {
-    mb_expect_tx(w_full, (uint32_t)k_tiles * W_TILE);
-    for (int kt = 0; kt < k_tiles; ++kt) tma_load_2d(sW + (size_t)kt * W_TILE, mB, w_full, kt * GEMM_BK, 0);
+    if constexpr (PAIR) {
+      mb_expect_tx(w_full, (uint32_t)k_tiles * (W_TILE + WB_TILE / 2));
+      for (int kt = 0; kt < k_tiles; ++kt) {
+        tma_load_3d(sW + (size_t)kt * W_TILE, mB, w_full, 0, kt, 0);                           // online, frames 0-3
+        tma_load_3d(sW + (size_t)kt * W_TILE + W_TILE / 2, &tmA2, w_full, -16, kt, 0);         // target: zero, frames 0-2
+        tma_load_3d(sWB + (size_t)kt * WB_TILE + WB_TILE / 2, &tmB2, w_full, 48, kt, 0);       // target: frame 3
+      }
+    } else {
+      mb_expect_tx(w_full, (uint32_t)k_tiles * W_TILE);
+      for (int kt = 0; kt < k_tiles; ++kt) tma_load_2d(sW + (size_t)kt * W_TILE, mB, w_full, kt * GEMM_BK, 0);
+    }
     if constexpr (U8) {
       // -------------------------------------------------------------------- K1 producer: the uint8 pixels of every tile (one
       // tensor load per image the slab touches), up to sp.u8.stages tiles ahead; idx[] is requested one tile early
@@ -986,9 +1065,12 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
           if (pl.n0 > 0) { i0 = __ldg(sp.u8.idx + pl.b0); i1 = __ldg(sp.u8.idx + min(pl.b0 + 1, nimg - 1)); }
         }
         const int us = it % U8_STAGES;
+        const long long t0 = clk_now(clk);
         mb_wait(&u8_empty[us], ((it / U8_STAGES) & 1) ^ 1);
+        c_wait += clk_now(clk) - t0;
         u8_issue(sp.u8, mA, cur, c0, c1, sU + (size_t)us * u8_bytes, &u8_full[us], u8_slots_);
       }
+      if (clk) atomicAdd(clk + K1_CLK_PRODUCER_WAIT, (unsigned long long)c_wait);
     } else {
       // -------------------------------------------------------------------- TMA producer: one slab per tile
       uint32_t it = 0;
@@ -1014,11 +1096,21 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
     uint32_t it = 0;
     for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
       const int s = it % sp.stages, us = it % U8_STAGES;
+      const long long t0 = clk_now(clk);
       mb_wait(&empty[s], ((it / sp.stages) & 1) ^ 1);
+      const long long t1 = clk_now(clk);
       mb_wait(&u8_full[us], (it / U8_STAGES) & 1);
-      u8_convert<128>(sp.u8, sU + (size_t)us * u8_bytes, sS + (size_t)s * slab_bytes, tile * GEMM_BM + sp.min_shift,
-                      sp.slab_rows, u8_slots_, tid, 4);
+      const long long t2 = clk_now(clk);
+      u8_convert<128, PAIR ? 10 : 8>(sp.u8, sU + (size_t)us * u8_bytes, sS + (size_t)s * slab_bytes,
+                                     sS + (size_t)s * slab_bytes + slab_block, tile * GEMM_BM + sp.min_shift, sp.slab_rows,
+                                     u8_slots_, tid, 4);
       if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
+      c_wait += t1 - t0, c_wait2 += t2 - t1, c_work += clk_now(clk) - t2;
+    }
+    if (clk && tid == 0) {
+      atomicAdd(clk + K1_CLK_CONVERT_WAIT_SLAB, (unsigned long long)c_wait);
+      atomicAdd(clk + K1_CLK_CONVERT_WAIT_PIXELS, (unsigned long long)c_wait2);
+      atomicAdd(clk + K1_CLK_CONVERT, (unsigned long long)c_work);
     }
   } else {
     // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: tiles i = g, g + 2, ...
@@ -1028,13 +1120,16 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
     const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
     const int t = wl * 32 + lane;                                   // epilogue_half's thread index in the warpgroup
     float* sAcc_g = sAcc + g * 64 * ACC_LD;
-    const uint32_t w0 = s2u(sW);
+    const uint32_t w0 = s2u(sW), wb0 = s2u(sWB);
     mb_wait(w_full, 0);
     uint32_t it = g;
+    int n_tiles_g = 0;
     for (int tile = cta + g * n_cta; tile < tiles; tile += 2 * n_cta, it += 2) {
       const int s = it % sp.stages;
+      const long long t0 = clk_now(clk);
       if (it > 0) named_sync(5 + g, 256);                           // the other warpgroup has issued tile it - 1
       mb_wait(&full[s], (it / sp.stages) & 1);
+      const long long t1 = clk_now(clk);
       float d[2][BN / 2];
       acc_zero<BN>(d[0]);
       acc_zero<BN>(d[1]);
@@ -1056,6 +1151,9 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
               const int row = 64 * h - sp.min_shift + p.shift_sign * (dy * p.grid_w + dx);
               const uint32_t a_addr = slab + cb * slab_block + (uint32_t)row * 128;
               mma_ktile<BN, 0, 0>(d[h], make_desc(a_addr, 16, sp.base_offset_mode == 1 ? (a_addr >> 7) & 7 : 0), b);
+              if constexpr (PAIR)                                     // window frame 4: block B
+                wgmma_n64<0, 0>(d[h], make_desc_sw32(slab + slab_block + (uint32_t)row * 32),
+                                make_desc_sw32(wb0 + (dy * TX + dx) * WB_TILE));
             }
           }
         }
@@ -1070,20 +1168,49 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
       acc_fence<BN>(d[0]);
       acc_fence<BN>(d[1]);
       if (lane == 0) mb_arrive(&empty[s]);
+      const long long t2 = clk_now(clk);
       if constexpr (BN > 64) epi_mask_load<BN, EXT>(p, tile * GEMM_BM, 0, t, mk[0]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (BN > 64 && h == 1) epi_mask_load<BN, EXT>(p, tile * GEMM_BM + 64, 0, t, mk[1]);
+        const long long t3 = clk_now(clk);
         stage_acc<BN>(d[h], sAcc_g, ACC_LD, wl, lane);
         named_sync(2 + g, 128);
+        c_stage += clk_now(clk) - t3;
         if (BN <= 64 && h == 0) epi_mask_load<BN, EXT>(p, tile * GEMM_BM + 64, 0, t, mk[1]);   // in flight during the first half
-        epilogue_half<BN, EXT>(p, tile * GEMM_BM + 64 * h, 0, t, sAcc_g, mk[h], s_dbias);
+        epilogue_half<BN, EXT, PAIR>(p, tile * GEMM_BM + 64 * h, 0, t, sAcc_g, mk[h], s_dbias);
         named_sync(2 + g, 128);
       }
+      c_wait += t1 - t0, c_work += t2 - t1, c_epi += clk_now(clk) - t2, ++n_tiles_g;
+    }
+    if (clk && t == 0) {
+      atomicAdd(clk + K1_CLK_MMA_WAIT, (unsigned long long)c_wait);
+      atomicAdd(clk + K1_CLK_MMA, (unsigned long long)c_work);
+      atomicAdd(clk + K1_CLK_EPILOGUE, (unsigned long long)c_epi);
+      atomicAdd(clk + K1_CLK_EPILOGUE_STAGE, (unsigned long long)c_stage);
+      atomicAdd(clk + K1_CLK_TILES, (unsigned long long)n_tiles_g);
     }
   }
   __syncthreads();
+  if (clk && threadIdx.x == 0) atomicAdd(clk + K1_CLK_CTA, (unsigned long long)(clock64() - t_start));
   if (EXT && sp.g.dbias && (int)threadIdx.x < dbias_slots(sp.g)) atomicAdd(sp.g.dbias + threadIdx.x, s_dbias[threadIdx.x]);
+}
+
+template <int BN, bool EXT, bool U8, int TX, int TY, int CB>
+__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_slab_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                          const __grid_constant__ CUtensorMap tmB,
+                                                                          const __grid_constant__ CUtensorMap tmA2,
+                                                                          const __grid_constant__ CUtensorMap tmB2,
+                                                                          const SlabParams sp) {
+  conv_slab_body<BN, EXT, U8, TX, TY, CB, false>(tmA, tmB, tmA2, tmB2, sp);
+}
+// conv1's K1 instantiation with the PAIR flag: b2rl_conv1_u8_fwd_pair
+__global__ void __launch_bounds__(SLAB_U8_THREADS, 1) conv1_pair_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                             const __grid_constant__ CUtensorMap tmB,
+                                                                             const __grid_constant__ CUtensorMap tmA2,
+                                                                             const __grid_constant__ CUtensorMap tmB2,
+                                                                             const SlabParams sp) {
+  conv_slab_body<64, false, true, 2, 2, 1, true>(tmA, tmB, tmA2, tmB2, sp);
 }
 
 
@@ -1136,7 +1263,7 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
   uint64_t* empty = full + MAX_STAGES;
   // U8 (K1): uint8 staging tiles + their full / empty barriers behind the operand ring (launch_wgrad sizes the allocation)
   const int u8_slots_ = U8 ? u8_slots(w.slab_rows, w.u8.G) : 0;
-  const int u8_bytes = U8 ? u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w) : 0;
+  const int u8_bytes = U8 ? u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w, w.u8.nf) : 0;
   uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(empty + MAX_STAGES) + 127) & ~uintptr_t(127));
   const int U8_STAGES = U8 ? w.u8.stages : 1;
   uint64_t* u8_full = reinterpret_cast<uint64_t*>(sU + (size_t)U8_STAGES * u8_bytes);
@@ -1202,8 +1329,8 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
       const int s = i % w.stages, us = i % U8_STAGES;
       mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
       mb_wait(&u8_full[us], (i / U8_STAGES) & 1);
-      u8_convert<128>(w.u8, sU + (size_t)us * u8_bytes, smem + (size_t)s * stage_bytes + A_BYTES, (kt_begin + i) * GEMM_BK,
-                      w.slab_rows, u8_slots_, tid, 4);
+      u8_convert<128, 8>(w.u8, sU + (size_t)us * u8_bytes, smem + (size_t)s * stage_bytes + A_BYTES, nullptr,
+                         (kt_begin + i) * GEMM_BK, w.slab_rows, u8_slots_, tid, 4);
       if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
     }
   } else if (warp >= 4 && warp < 12 && n_kt > 0 && (warp - 4) / 4 >= w.a_boxes) {
@@ -1527,15 +1654,21 @@ static int dense_dispatch(const uint16_t* A, int a_mn, int64_t lda, int64_t a_ro
              : launch_dense_bn<128, 4, false>(ta, tb, p, splits, cluster, st);
 }
 
-template <int BN, bool EXT, bool U8, int TX, int TY, int CB>
+template <int BN, bool EXT, bool U8, int TX, int TY, int CB, bool PAIR>
+static auto slab_kernel() {
+  if constexpr (PAIR) return &conv1_pair_wgmma_kernel;
+  else return &conv_slab_wgmma_kernel<BN, EXT, U8, TX, TY, CB>;
+}
+
+template <int BN, bool EXT, bool U8, int TX, int TY, int CB, bool PAIR = false>
 static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ta2, const CUtensorMap& tb2,
                          SlabParams sp, cudaStream_t st) {
-  const size_t w_bytes = (size_t)TX * TY * CB * BN * 128;
-  const size_t slab_bytes = (size_t)sp.slab_rows * 128 * CB;
+  const size_t w_bytes = (size_t)TX * TY * CB * BN * 128 + (PAIR ? (size_t)TX * TY * BN * 32 : 0);
+  const size_t slab_bytes = (size_t)sp.slab_rows * 128 * CB + (PAIR ? pair_block_b_bytes(sp.slab_rows) : 0);
   const int tiles = (sp.g.M + GEMM_BM - 1) / GEMM_BM;
   // weights + slab ring + accumulator staging + barriers (+ uint8 staging) within the shared memory of one SM
   const size_t fixed = 1024 + acc_stage_bytes(BN) + (2 * 6 + 2) * 8 + 128;
-  auto k = conv_slab_wgmma_kernel<BN, EXT, U8, TX, TY, CB>;
+  auto k = slab_kernel<BN, EXT, U8, TX, TY, CB, PAIR>();
   static const size_t limit = dyn_smem_limit(k);
   if (limit <= fixed) return 1;
   size_t u8_extra = 0;
@@ -1543,7 +1676,7 @@ static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   if (U8) {
     // K1: three bf16 slabs are enough (shared -> shared conversion); everything else goes to uint8 staging tiles, each of which
     // is held for the copy latency plus the conversion
-    const size_t ub = u8_stage_bytes(sp.slab_rows, sp.u8.G, sp.u8.frame_w);
+    const size_t ub = u8_stage_bytes(sp.slab_rows, sp.u8.G, sp.u8.frame_w, sp.u8.nf);
     if (w_bytes + 3 * slab_bytes + 2 * ub + 2 * U8_MAX_STAGES * 8 > budget) return 1;
     int us = (int)((budget - w_bytes - 3 * slab_bytes - 2 * U8_MAX_STAGES * 8) / ub);
     if (us > U8_MAX_STAGES) us = U8_MAX_STAGES;
@@ -1623,7 +1756,7 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   size_t u8_extra = 0;
   int stages = (int)(budget / stage);
   if (U8) {                                                          // K1: four operand stages, the rest for uint8 staging tiles
-    const size_t ub = u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w);
+    const size_t ub = u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w, w.u8.nf);
     if (4 * stage + 2 * ub + 512 > budget) return 1;
     stages = 4;
     int us = (int)((budget - 4 * stage - 512) / ub);
@@ -1684,6 +1817,13 @@ static float* g_partial_buf = nullptr;
 static int64_t g_partial_stride = 0;
 static int g_partial_count = 0;
 static int g_use_slab = 2;   // 2: shifted windows with base_offset 0 -- the 128B swizzle is a pure function of the smem address
+static unsigned long long* g_k1_clocks = nullptr;
+// Profiling hook of the K1 conv1 forwards (b2rl_conv1_u8_fwd, b2rl_conv1_u8_fwd_pair): while set, every launch adds its
+// K1_CLK_SLOTS phase-cycle sums to clocks[] (scripts/conv1_pair_time.py --phases).  Null (the default): no probe.
+extern "C" int b2rl_conv1_set_phase_clocks(int64_t* clocks) {
+  g_k1_clocks = reinterpret_cast<unsigned long long*>(clocks);
+  return B2RL_OK;
+}
 extern "C" void b2rl_set_conv_slab(int32_t on) { g_use_slab = on; }
 
 static int check_common(const void* A, const void* B, const void* D, int64_t lda, int64_t ldb, int M, int N, int K,
@@ -1940,13 +2080,14 @@ extern "C" int b2rl_gemm_splitk_bf16(const uint16_t* A, int64_t lda, const uint1
 // of the oldest stacked frame relative to idx[b] (-(history-1) for the state, n_step-(history-1) for the next state).
 // The frame values enter as exact integers 0..255; ImageNormalizer's 1/255 is folded into W (b2rl_nature_pack_weights).
 // ---------------------------------------------------------------------------------------------------------------
-// 3-D tensor map over the uint8 ring as 32-bit words: [capacity][G grid rows][frame_w words], box [4 frames][slots][frame_w]
-static int make_ring_map(CUtensorMap* m, const uint8_t* frames, int64_t capacity, int64_t row_bytes, int frame_w, int slots) {
+// 3-D tensor map over the uint8 ring as 32-bit words: [capacity][G grid rows][frame_w words], box [nf frames][slots][frame_w]
+static int make_ring_map(CUtensorMap* m, const uint8_t* frames, int64_t capacity, int64_t row_bytes, int frame_w, int slots,
+                         int nf) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return B2RL_ERR_CUDA; }
   cuuint64_t gdim[3] = {(cuuint64_t)frame_w, (cuuint64_t)(frame_w / 4), (cuuint64_t)capacity};
   cuuint64_t gstr[2] = {(cuuint64_t)4 * frame_w, (cuuint64_t)row_bytes};
-  cuuint32_t box[3] = {(cuuint32_t)frame_w, (cuuint32_t)slots, 4u};
+  cuuint32_t box[3] = {(cuuint32_t)frame_w, (cuuint32_t)slots, (cuuint32_t)nf};
   cuuint32_t estr[3] = {1u, 1u, 1u};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, const_cast<uint8_t*>(frames), gdim, gstr, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1966,6 +2107,7 @@ static int u8_src(U8Src& u, const uint8_t* frames, const int64_t* idx, int32_t f
   B2RL_REQUIRE(batch > 0 && (int64_t)batch * (frame_w / 4) * (frame_w / 4) < (1LL << 31), "bad batch");
   u.frames = frames; u.idx = idx; u.row_bytes = row_bytes; u.first = first; u.frame_w = frame_w; u.G = frame_w / 4;
   u.rows = batch * u.G * u.G;
+  u.nf = history;
   return B2RL_OK;
 }
 
@@ -1996,10 +2138,71 @@ extern "C" int b2rl_conv1_u8_fwd(const uint8_t* frames, int64_t capacity, const 
   CUtensorMap tb, tr;
   rc = make_map(&tb, W, K, n_out, K, 32);
   if (rc) return rc;
-  rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(sp.slab_rows, G));
+  rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(sp.slab_rows, G), sp.u8.nf);
   if (rc) return rc;
+  sp.clk = g_k1_clocks;
   int r2 = launch_slab<32>(tr, tb, tr, tb, sp, (cudaStream_t)stream);
   if (r2 > 0) { set_error("b2rl_conv1_u8_fwd: the slab does not fit in shared memory"); return B2RL_ERR_ARG; }
+  return r2;
+}
+
+// 3-D bf16 tensor map over conv1's packed weights [32 n][4 taps][64 k] (K-major, tap-major columns), box [32 n][1 tap][box_k k]
+static int make_w1_map(CUtensorMap* m, const uint16_t* W, int box_k, CUtensorMapSwizzle swizzle) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return B2RL_ERR_CUDA; }
+  cuuint64_t gdim[3] = {64u, 4u, 32u};
+  cuuint64_t gstr[2] = {64u * 2, 4u * 64 * 2};
+  cuuint32_t box[3] = {(cuuint32_t)box_k, 1u, 32u};
+  cuuint32_t estr[3] = {1u, 1u, 1u};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<uint16_t*>(W), gdim, gstr, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (conv1 weights) failed (%d)", (int)r); return B2RL_ERR_CUDA; }
+  return B2RL_OK;
+}
+
+// D = act(conv1_W(s) + bias) and D2 = act(conv1_W2(s') + bias2) in ONE launch (PAIR in conv_slab_wgmma_kernel), s the stacks
+// idx[b] + first .. + 3 and s' the stacks one ring row later (n_step 1): both are read from the five ring rows
+// idx[b] + first .. + 4.  W, W2: [32][4 taps * 64] as b2rl_conv1_u8_fwd takes them; D, D2: as its D (n_out 32, row stride ldd).
+// The bits equal those of two b2rl_conv1_u8_fwd launches (first and first + 1).
+extern "C" int b2rl_conv1_u8_fwd_pair(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first,
+                                      int64_t row_bytes, int32_t frame_w, int32_t batch, int32_t history, const uint16_t* W,
+                                      const uint16_t* W2, void* D, void* D2, int64_t ldd, const float* bias, const float* bias2,
+                                      int32_t relu, int32_t out_map, int32_t V, void* stream) {
+  SlabParams sp = {};
+  int rc = u8_src(sp.u8, frames, idx, first, row_bytes, frame_w, batch, history);
+  if (rc) return rc;
+  B2RL_REQUIRE(W && W2 && D && D2, "null pointer");
+  B2RL_REQUIRE(D != D2, "the two outputs must be distinct buffers");
+  B2RL_REQUIRE((bias == nullptr) == (bias2 == nullptr), "both or neither bias");
+  B2RL_REQUIRE(out_map >= 0 && out_map <= 2, "out_map 0..2");
+  B2RL_REQUIRE(ldd >= (out_map == 1 ? 128 : 32) && ldd % 8 == 0, "ldd must hold the 32 output channels (x 4 for out_map 1), multiple of 8");
+  B2RL_REQUIRE(frame_w == 84, "the paired forward serves 84 x 84 frames");
+  B2RL_REQUIRE((reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(W2) | reinterpret_cast<uintptr_t>(D) |
+                reinterpret_cast<uintptr_t>(D2)) % 16 == 0, "operands and outputs must be 16-byte aligned");
+  B2RL_REQUIRE(capacity >= history + 1, "bad capacity");
+  sp.u8.nf = history + 1;                                  // the window of s and s'
+  const int G = sp.u8.G;
+  GemmParams p = {};
+  p.M = sp.u8.rows; p.N = 32; p.K = 4 * 64; p.ldd = (int)ldd;
+  p.relu = relu; p.out_mode = 0; p.bias = bias; p.D = D; p.bias2 = bias2; p.D2 = D2;
+  p.taps_x = 2; p.grid_w = G; p.shift_sign = 1; p.a_tap_tiles = 1;
+  p.out_map = out_map; p.G = G; p.V = V;
+  sp.g = p; sp.taps = 4; sp.col_blocks = 1;
+  sp.slab_rows = (GEMM_BM + G + 1 + 7) / 8 * 8;
+  sp.min_shift = 0;
+  sp.base_offset_mode = 2;
+  CUtensorMap tr, tw, tw2a, tw2b;
+  rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(sp.slab_rows, G), sp.u8.nf);
+  if (rc) return rc;
+  rc = make_w1_map(&tw, W, 64, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  rc = make_w1_map(&tw2a, W2, 64, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  rc = make_w1_map(&tw2b, W2, 16, CU_TENSOR_MAP_SWIZZLE_32B);
+  if (rc) return rc;
+  sp.clk = g_k1_clocks;
+  int r2 = launch_slab_t<64, false, true, 2, 2, 1, true>(tr, tw, tw2a, tw2b, sp, (cudaStream_t)stream);
+  if (r2 > 0) { set_error("b2rl_conv1_u8_fwd_pair: the slab does not fit in shared memory"); return B2RL_ERR_ARG; }
   return r2;
 }
 
@@ -2028,7 +2231,7 @@ extern "C" int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capac
   CUtensorMap tg, tr;
   rc = make_map(&tg, G_rows, n_out, w.rows, n_out, 64);
   if (rc) return rc;
-  rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(w.slab_rows, G));
+  rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(w.slab_rows, G), w.u8.nf);
   if (rc) return rc;
   int n = 0;
   int r2 = launch_wgrad<true>(tg, tr, w, (cudaStream_t)stream, &n);

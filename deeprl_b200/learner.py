@@ -8,6 +8,7 @@ Multi-GPU (SURVEY 8e): one learner per rank, rank-local replay shard, parameters
 gradients are summed with ONE NCCL all-reduce of the flat gradient arena between the two graphs and scaled by
 1 / world_size inside the clip kernel.
 """
+import contextlib
 import dataclasses
 import os
 import sys
@@ -49,6 +50,7 @@ class UpdatePlan:
     dist_head: bool       # C51 / QR: the heads read bf16 weight copies on the wgmma GEMM
     head: str             # "separate" (head_fwd | loss | head_bwd), "fused-two" or "fused-one" (csrc/head.cu on the features)
     forward: str          # "two-branch" (target on the side stream), "dual" (one launch per layer for both) or "one-stream"
+    conv1: str            # "pair": online conv1(s) and target conv1(s') in one launch from the ring (K1, n_step 1); "separate"
     single_stream: bool   # the side-branch work (target forward, re-pack, weight gradients) runs on the main stream
     prefetch: object      # where the next batch is sampled: None, "start", "gather-after-bwd" / "-dgrad", "after-ring-read"
     join: object          # where the prefetch branch joins: None, "main" (end of _main) or "opt" (after the optimizer kernels)
@@ -56,11 +58,12 @@ class UpdatePlan:
 
 
 def update_plan(kind="dqn", per=False, prefetch=False, dual=False, k1_body=True, dual_body=True, tail=True,
-                narrow_head=True, world=1, one_graph=True, env=None):
+                narrow_head=True, world=1, one_graph=True, env=None, n_step=1):
     """Decide the update schedule from plain values: the learner's options, what the networks support (``k1_body``: a
     wgmma NatureConvBody on a 4 x 84 x 84 uint8 ring; ``dual_body``: both bodies on the wgmma kernels; ``tail``: the fused
-    update tail applies; ``narrow_head``: VanillaNet / DuelingNet heads the fused head kernel takes) and the ``B2RL_*``
-    switches in ``env``.  ``one_graph=False``: the split-graph form after a failed NCCL capture."""
+    update tail applies; ``narrow_head``: VanillaNet / DuelingNet heads the fused head kernel takes), the replay's
+    ``n_step`` and the ``B2RL_*`` switches in ``env``.  ``one_graph=False``: the split-graph form after a failed NCCL
+    capture."""
     env = env or {}
     on = lambda name, default: env.get(name, default) != "0"
     fused_env = kind == "dqn" and on("B2RL_FUSED_HEAD", "0")
@@ -77,6 +80,9 @@ def update_plan(kind="dqn", per=False, prefetch=False, dual=False, k1_body=True,
     single = head == "separate" and env.get("B2RL_SINGLE_STREAM", "0") == "1"       # experiment: no parallel branches
     forward = "dual" if head == "separate" and dual and dual_body else ("one-stream" if single else "two-branch")
     one_graph = one_graph and (world == 1 or env.get("B2RL_NCCL_IN_GRAPH", "1") == "1")
+    # with n_step 1 the next state's stacks are the state's shifted by one ring row: one conv1 launch reads each sample's
+    # five-frame window once for the online forward on s and the target forward on s' (nature_tc.paired_conv1)
+    conv1 = "pair" if ring and forward != "dual" and dual_body and n_step == 1 else "separate"
     # async replay, uniform with the materialising gather: feed + index draw at the start, the gather after the backward
     # pass beside the (small-footprint, L2-bound) update tail -- started beside the forward pass its 512 gather CTAs would
     # hold the shared memory the convolution kernels need.  Prioritized replay keeps the whole branch at the start: the
@@ -92,7 +98,7 @@ def update_plan(kind="dqn", per=False, prefetch=False, dual=False, k1_body=True,
             pf, join = "gather-after-dgrad" if at_dgrad else "gather-after-bwd", "opt" if head == "separate" else "main"
         else:
             pf, join = "start", "main"
-    return UpdatePlan(ring=ring, tail=tail, repack_online=not tail, head=head, forward=forward, single_stream=single,
+    return UpdatePlan(ring=ring, tail=tail, repack_online=not tail, head=head, forward=forward, conv1=conv1, single_stream=single,
                       dist_head=kind in ("c51", "qr") and tail and on("B2RL_DIST_HEAD", "1"), prefetch=pf, join=join,
                       one_graph=one_graph)
 
@@ -170,7 +176,7 @@ class GraphedDQNLearner:
             k1_body=plain and rp.history_length == 4 and tuple(getattr(rp, "item_shape", ())) == (84, 84),
             dual_body=wgmma and hasattr(getattr(self.tgt, "body", None), "repack"),
             tail=plain and nature_tc.FUSED_BWD and bool(_lib.CONV_SLAB) and self.opt.kind in ("rmsprop", "adam"),
-            narrow_head=self._heads() is not None)
+            narrow_head=self._heads() is not None, n_step=rp.n_step)
 
     @property
     def ring(self):
@@ -291,17 +297,25 @@ class GraphedDQNLearner:
                     nxt_o = net(t.next_state) if self.double_q else None
         else:
             # the target forward on s' and the online forward on s are independent: fork them onto two streams (two
-            # parallel branches of the captured graph) so that the prologue / tail of one chain overlaps the other
-            side.wait_stream(cur)
-            with torch.cuda.stream(side), frame_scale(fs), torch.no_grad():
-                nxt_t = tgt(t.next_state)
-            if tail is None:
-                cur.wait_event(self._packed_ev)
-            with frame_scale(fs):
-                with torch.no_grad():
-                    nxt_o = net(t.next_state) if self.double_q else None
-                out = net(t.state)
-            cur.wait_stream(side)
+            # parallel branches of the captured graph) so that the prologue / tail of one chain overlaps the other.  With
+            # the paired conv1 both conv1s run first, as one launch on this stream; the branches continue from its outputs
+            pair = contextlib.nullcontext()
+            if plan.conv1 == "pair":
+                if tail is None:
+                    cur.wait_event(self._packed_ev)
+                pair = nature_tc.paired_conv1(self.net.body, self.tgt.body, t.state, t.next_state, fs)
+                nature_tc.mark("conv1_pair")
+            with pair:
+                side.wait_stream(cur)
+                with torch.cuda.stream(side), frame_scale(fs), torch.no_grad():
+                    nxt_t = tgt(t.next_state)
+                if tail is None:
+                    cur.wait_event(self._packed_ev)
+                with frame_scale(fs):
+                    with torch.no_grad():
+                        nxt_o = net(t.next_state) if self.double_q else None
+                    out = net(t.state)
+                cur.wait_stream(side)
         nature_tc.mark("fwd_joined")
         if fused:
             # ONE launch for the online / target [/ double-Q] head forwards + target / loss / PER block + head backward

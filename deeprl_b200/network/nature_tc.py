@@ -334,13 +334,17 @@ def forward_only(x0, packed, b1, b2, b3, b4):
     w1f, w2f, _, w3f, _, w4p = packed
     B = x0.shape[0]
     dev = x0.device
-    x1 = torch.empty((B * 100, 128), dtype=_bf16, device=dev)
-    if isinstance(x0, RingFrames):                                             # K1: conv1 reads the uint8 ring itself
+    x1 = paired_conv1.take(x0, w1f) if paired_conv1.current is not None else None
+    if x1 is not None:                                                         # computed by the paired conv1 launch
         x0m = x0
+    elif isinstance(x0, RingFrames):                                           # K1: conv1 reads the uint8 ring itself
+        x0m = x0
+        x1 = torch.empty((B * 100, 128), dtype=_bf16, device=dev)
         _lib.call("b2rl_conv1_u8_fwd", *x0.args(), _lib.ptr(w1f), 32, _lib.ptr(x1), x1.stride(0), _lib.ptr(b1), 1, 1, 20,
                   _lib.stream())
     else:
         x0m = x0.permute(0, 2, 3, 1).reshape(B * 441, x0.shape[1])            # free view of the NHWC memory
+        x1 = torch.empty((B * 100, 128), dtype=_bf16, device=dev)
         conv_gemm(0, x0m, w1f, 32, 4, 2, 21, 1, x1, bias=b1, relu=True, out_map=1, G=21, V=20, block_n=32)
     mark("f_conv1")
     y2 = torch.empty((B * 100, 64), dtype=_bf16, device=dev)
@@ -488,6 +492,66 @@ class dual_forward:
         return False
 
 
+def conv1_pair(state, next_state, w1f, b1, v1f, c1):
+    """relu(conv1_w1f(state) + b1) and relu(conv1_v1f(next_state) + c1) in ONE launch (b2rl_conv1_u8_fwd_pair): the two
+    ``RingFrames`` must be the same batch of one ring, ``next_state`` one ring row after ``state`` (n_step 1), so that the
+    kernel reads each sample's five-frame window once.  Returns (x1, z1), conv2's space-to-depth(2) input rows."""
+    s, n = state, next_state
+    if not (isinstance(s, RingFrames) and isinstance(n, RingFrames)):
+        raise ValueError("conv1_pair takes the RingFrames of a state and its next state")
+    if n.first != s.first + 1:
+        raise ValueError("conv1_pair: the next state must start one ring row after the state (n_step 1), got first %d and %d"
+                         % (s.first, n.first))
+    if (n.frames.data_ptr(), n.idx.data_ptr(), n.batch, n.row_bytes, n.frame_w, n.history) != \
+            (s.frames.data_ptr(), s.idx.data_ptr(), s.batch, s.row_bytes, s.frame_w, s.history):
+        raise ValueError("conv1_pair: the state and the next state must be the same batch of the same ring")
+    e = lambda: torch.empty((s.batch * 100, 128), dtype=_bf16, device=s.device)
+    x1, z1 = e(), e()
+    _lib.call("b2rl_conv1_u8_fwd_pair", *s.args(), _lib.ptr(w1f), _lib.ptr(v1f), _lib.ptr(x1), _lib.ptr(z1), x1.stride(0),
+              _lib.ptr(b1), _lib.ptr(c1), 1, 1, 20, _lib.stream())
+    return x1, z1
+
+
+class paired_conv1:
+    """``with paired_conv1(online_body, target_body, state, next_state, scale):`` -- launches conv1 of the online body on
+    ``state`` and of the target body on ``next_state`` as ONE kernel (``conv1_pair``) on the current stream; inside the
+    context ``forward_only`` takes those outputs instead of launching conv1 for exactly these two (RingFrames, weights)
+    pairs, so the two forwards may continue on different streams.  Every other conv1 (double-Q's online(next_state))
+    launches its own kernel.  Used by the graph learner."""
+    current = None
+
+    def __init__(self, online, target, state, next_state, scale):
+        pk, pt = packed_operands(online, scale, state.device), packed_operands(target, scale, state.device)
+        x1, z1 = conv1_pair(state, next_state, pk.w1f, online.conv1.bias.detach(), pt.w1f, target.conv1.bias.detach())
+        self.out = [(state, pk.w1f, x1), (next_state, pt.w1f, z1)]
+
+    @staticmethod
+    def take(x0, w1f):
+        for x, w, y in paired_conv1.current.out:
+            if x is x0 and w is w1f:
+                return y
+        return None
+
+    def __enter__(self):
+        paired_conv1.current = self
+        return self
+
+    def __exit__(self, *exc):
+        paired_conv1.current = None
+        return False
+
+
+def packed_operands(body, scale, device):
+    """The packed bf16 operands of ``body`` (built on first use), re-packed here unless the owner manages them
+    (``body.auto_repack = False`` + ``body.repack(scale)`` after every parameter change)."""
+    pk = getattr(body, "_packed", None)
+    if pk is None:
+        pk = body._packed = PackedWeights(body.conv1.in_channels, body.fc4.out_features, device)
+    if getattr(body, "auto_repack", True) or pk.scale != float(scale):
+        repack(body, scale)
+    return pk
+
+
 def nature_body(body, x0, scale):
     """``relu(fc4(flatten(relu(conv3(relu(conv2(relu(conv1(x * scale)))))))))`` for space-to-depth bf16 frames ``x0``.
     ``body`` is the NatureConvBody; its packed bf16 operands are refreshed here unless the owner manages them
@@ -497,11 +561,7 @@ def nature_body(body, x0, scale):
             x0 = x0.materialize()
     if not isinstance(x0, RingFrames) and not x0.is_contiguous(memory_format=torch.channels_last):
         x0 = x0.contiguous(memory_format=torch.channels_last)
-    pk = getattr(body, "_packed", None)
-    if pk is None:
-        pk = body._packed = PackedWeights(body.conv1.in_channels, body.fc4.out_features, x0.device)
-    if getattr(body, "auto_repack", True) or pk.scale != float(scale):
-        repack(body, scale)
+    pk = packed_operands(body, scale, x0.device)
     c1, c2, c3, f4 = body.conv1, body.conv2, body.conv3, body.fc4
     d = dual_forward.current
     companion = None

@@ -327,6 +327,19 @@ int b2rl_conv1_u8_fwd(const uint8_t* frames, int64_t capacity, const int64_t* id
 int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first, int64_t row_bytes,
                                  int32_t frame_w, int32_t batch, int32_t history, const uint16_t* G_rows, int32_t n_out, float* partials,
                                  int32_t* n_partials_host, void* stream);
+/* The online forward on the state and the target forward on the next state (n_step 1) in ONE launch: D = act(conv1_W(s) +
+ * bias) and D2 = act(conv1_W2(s') + bias2), s the stacks idx[b] + first .. + history - 1 and s' the stacks one ring row
+ * later, read together from the history + 1 ring rows they span.  W, W2 [32][4 taps * 64]; D, D2 as D of b2rl_conv1_u8_fwd
+ * with n_out 32 (row stride ldd).  Bit-identical to b2rl_conv1_u8_fwd(first, W, D, bias) and (first + 1, W2, D2, bias2).
+ * history 4 and 84 x 84 frames only. */
+int b2rl_conv1_u8_fwd_pair(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first, int64_t row_bytes,
+                           int32_t frame_w, int32_t batch, int32_t history, const uint16_t* W, const uint16_t* W2, void* D,
+                           void* D2, int64_t ldd, const float* bias, const float* bias2, int32_t relu, int32_t out_map, int32_t V,
+                           void* stream);
+/* Profiling hook of the two conv1 forwards above: while `clocks` (device, 10 int64, zeroed by the caller) is set, every launch
+ * adds per-role clock64() cycle sums to it -- CTA run, producer waits, converter waits (slab, pixels) and conversion, MMA waits,
+ * MMA chain, epilogue and its staging part, tiles (csrc/gemm.cu K1_CLK_*).  NULL (the default) turns it off. */
+int b2rl_conv1_set_phase_clocks(int64_t* clocks);
 
 /* D = act(A B^T + bias) (bf16 out) in one launch: K split over the `splits` CTAs (1, 2, 4 or 8; 0: chosen from the shape) of
  * a thread-block cluster per output tile, the partials summed in distributed shared memory in a fixed order (deterministic),
