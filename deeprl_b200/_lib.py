@@ -58,6 +58,7 @@ SIGNATURES = {
                        c_p],
     "b2rl_conv1_u8_fwd": [c_p, c_i64, c_p, c_i32, c_i64, c_i32, c_i32, c_i32, c_p, c_i32, c_p, c_i64, c_p, c_i32, c_i32, c_i32, c_p],
     "b2rl_conv1_u8_wgrad_partials": [c_p, c_i64, c_p, c_i32, c_i64, c_i32, c_i32, c_i32, c_p, c_i32, c_p, c_p, c_p],
+    "b2rl_conv1_wgrad_partials": [c_p, c_i64, c_i32, c_p, c_i32, c_p, c_p, c_p],
     "b2rl_conv1_u8_fwd_pair": [c_p, c_i64, c_p, c_i32, c_i64, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_i64, c_p, c_p, c_i32,
                                c_i32, c_i32, c_p],
     "b2rl_conv1_set_phase_clocks": [c_p],

@@ -1241,7 +1241,6 @@ struct WgradParams {
   // run_low[j] = first output column of the lower half of run j, or -1 (a duplicate of an upper tap: dropped).
   int stack_delta, stack_rows;
   int run_low[9];
-  U8Src u8;                                    // U8 kernels: the activation slabs come from the uint8 frame ring (K1)
 };
 
 // The windows of a CTA are a compile-time shape WIN: WGRAD_N128 (one n128 window, C = 128), WGRAD_2X64 (two n64 windows) or
@@ -1249,10 +1248,10 @@ struct WgradParams {
 // accumulator chain, ptxas keeps the wgmmas asynchronous: every k-tile is one commit group, and the group of k-tile i - 1 is
 // retired (its stage released) only after k-tile i has been issued.
 constexpr int WGRAD_N128 = 0, WGRAD_2X64 = 1, WGRAD_1X64 = 2;
-template <bool U8, int WIN>
-__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmG,
-                                                                                             const __grid_constant__ CUtensorMap tmX,
-                                                                                             const WgradParams w) {
+template <int WIN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) conv_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmG,
+                                                                          const __grid_constant__ CUtensorMap tmX,
+                                                                          const WgradParams w) {
   constexpr int MAX_STAGES = 6;
   constexpr uint32_t A_BYTES = 2 * 8192;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -1261,23 +1260,13 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
   const uint32_t stage_bytes = A_BYTES + slab_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)w.stages * stage_bytes);
   uint64_t* empty = full + MAX_STAGES;
-  // U8 (K1): uint8 staging tiles + their full / empty barriers behind the operand ring (launch_wgrad sizes the allocation)
-  const int u8_slots_ = U8 ? u8_slots(w.slab_rows, w.u8.G) : 0;
-  const int u8_bytes = U8 ? u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w, w.u8.nf) : 0;
-  uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(empty + MAX_STAGES) + 127) & ~uintptr_t(127));
-  const int U8_STAGES = U8 ? w.u8.stages : 1;
-  uint64_t* u8_full = reinterpret_cast<uint64_t*>(sU + (size_t)U8_STAGES * u8_bytes);
-  uint64_t* u8_empty = u8_full + U8_MAX_STAGES;
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
   const int kt_total = (w.rows + GEMM_BK - 1) / GEMM_BK;
   const int kt_begin = blockIdx.x * w.k_tiles_per_cta;
   const int n_kt = max(min(kt_total, kt_begin + w.k_tiles_per_cta) - kt_begin, 0);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], U8 ? 2 : 1); mb_init(&empty[s], MMA_WARPS); }   // U8: TMA + converters
-    if (U8) {
-      for (int s = 0; s < U8_STAGES; ++s) { mb_init(&u8_full[s], 1); mb_init(&u8_empty[s], 1); }
-    }
+    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
@@ -1286,60 +1275,24 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
   pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
 
   if (warp == 0 && elect_one()) {
-    if constexpr (U8) {
-      // K1 producer: the uint8 pixels of every k-tile (one tensor load per image its slab touches, up to w.u8.stages k-tiles
-      // ahead, idx[] one k-tile early) and the gradient rows
-      const int nimg = w.u8.rows / (w.u8.G * w.u8.G);
-      U8Plan pl = u8_plan(w.u8, kt_begin * GEMM_BK, w.slab_rows);
-      long long i0 = 0, i1 = 0;
-      if (n_kt > 0 && pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
-      for (int i = 0; i < n_kt; ++i) {
-        const U8Plan cur = pl;
-        const long long c0 = i0, c1 = i1;
-        if (i + 1 < n_kt) {
-          pl = u8_plan(w.u8, (kt_begin + i + 1) * GEMM_BK, w.slab_rows);
-          if (pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
-        }
-        const int us = i % U8_STAGES, s = i % w.stages;
-        mb_wait(&u8_empty[us], ((i / U8_STAGES) & 1) ^ 1);
-        u8_issue(w.u8, &tmX, cur, c0, c1, sU + (size_t)us * u8_bytes, &u8_full[us], u8_slots_);
-        mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
-        mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192);
-        uint8_t* st = smem + (size_t)s * stage_bytes;
-        for (int g = 0; g < w.a_boxes; ++g)
-          tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, (kt_begin + i) * GEMM_BK + (g ? w.stack_delta : 0));
-      }
-    } else {
-      for (int i = 0; i < n_kt; ++i) {
-        const int s = i % w.stages;
-        mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
-        mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192 + slab_bytes);
-        uint8_t* st = smem + (size_t)s * stage_bytes;
-        const int k0 = (kt_begin + i) * GEMM_BK;
-        for (int g = 0; g < w.a_boxes; ++g)                                                                 // [64 k][64 n]
-          tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, k0 + (g ? w.stack_delta : 0));
-        for (int cb = 0; cb < w.col_blocks; ++cb)
-          tma_load_2d(st + A_BYTES + (size_t)cb * slab_block, &tmX, &full[s], cb * GEMM_BK, k0);           // [slab_rows][64 c]
-      }
-    }
-  } else if (U8 && warp >= 12) {
-    // K1 converters (warps 12-15): the activation slab of every k-tile from the staged uint8 pixels
-    const int tid = (int)threadIdx.x - GEMM_THREADS;
     for (int i = 0; i < n_kt; ++i) {
-      const int s = i % w.stages, us = i % U8_STAGES;
+      const int s = i % w.stages;
       mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
-      mb_wait(&u8_full[us], (i / U8_STAGES) & 1);
-      u8_convert<128, 8>(w.u8, sU + (size_t)us * u8_bytes, smem + (size_t)s * stage_bytes + A_BYTES, nullptr,
-                         (kt_begin + i) * GEMM_BK, w.slab_rows, u8_slots_, tid, 4);
-      if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
+      mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192 + slab_bytes);
+      uint8_t* st = smem + (size_t)s * stage_bytes;
+      const int k0 = (kt_begin + i) * GEMM_BK;
+      for (int g = 0; g < w.a_boxes; ++g)                                                                 // [64 k][64 n]
+        tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, k0 + (g ? w.stack_delta : 0));
+      for (int cb = 0; cb < w.col_blocks; ++cb)
+        tma_load_2d(st + A_BYTES + (size_t)cb * slab_block, &tmX, &full[s], cb * GEMM_BK, k0);           // [slab_rows][64 c]
     }
-  } else if (warp >= 4 && warp < 12 && n_kt > 0 && (warp - 4) / 4 >= w.a_boxes) {
+  } else if (warp >= 4 && n_kt > 0 && (warp - 4) / 4 >= w.a_boxes) {
     // one A box (n_out <= 64, not stacked): warpgroup 2 only releases the stages
     for (int i = 0; i < n_kt; ++i) {
       mb_wait(&full[i % w.stages], (i / w.stages) & 1);
       if (lane == 0) mb_arrive(&empty[i % w.stages]);
     }
-  } else if (warp >= 4 && warp < 12 && n_kt > 0) {
+  } else if (warp >= 4 && n_kt > 0) {
     // ---------------------------------------------------------------------- MMA, warpgroup g: accumulator rows (output
     // channels) 64 g .. 64 g + 63 from A box g -- or, M-stacked, the same channels one tap row further down
     constexpr int NJ = WIN == WGRAD_2X64 ? 2 : 1, WC = WIN == WGRAD_N128 ? 128 : 64;   // windows, columns per window
@@ -1396,6 +1349,185 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_w
     }
   }
   __syncthreads();
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// conv1's weight gradient with the taps in the MMA rows.  conv1 has n_out = 32 channels and 2 x 2 taps at row shifts
+// s_t = 0, 1, G, G + 1 of the G x G grid.  The sum is written with the activations unshifted and the gradient rows carrying
+// the shift:
+//   dW[n][t*64 + c] = sum_r G[r][n] x[r + s_t][c] = sum_r' G[r' - s_t][n] x[r'][c]
+// (r' - s_t < 0: the TMA's out-of-bounds zero fill; r' >= rows: x is zero there -- the same products as the slab form).
+// Each MMA warpgroup g holds ONE m64n64 accumulator over two taps: rows 0-31 are tap 2g + 1, rows 32-63 tap 2g, so every
+// accumulator row is a result.  The A operand (MN-major, K = rows r') is one TMA box of the gradient rows [k0 - G - 1,
+// k0 + BK) stored with the 64-byte swizzle (one 64-byte row per grid row = 32 channels = one swizzle atom column): the
+// descriptor of warpgroup g starts at the row of its larger shift and reaches the smaller one through the MN-direction
+// atom stride (LBO) of one row, 64 bytes.  The 64-byte swizzle, like the 128-byte one of the slab kernels, is a function of
+// the shared-memory address (bits 4-5 ^= bits 7-8), so a descriptor may start at any 64-byte row with base_offset 0.  The
+// B operand is the 64-channel activation block of rows [k0, k0 + BK) with no halo, 128B-swizzled MN-major.
+// A CTA takes a contiguous range of 128-row k-blocks (at most one CTA per SM, equal ranges) and stores its [32][256] fp32
+// partial block at D + blockIdx.x * 8192.  Two producers of the activation block give bit-identical partials: U8 builds it
+// from the uint8 frame ring (K1: u8_issue / u8_convert with a 128-row slab), the bf16 form loads it by TMA from x0m.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int C1W_BK = 128;                           // rows of one k-block
+constexpr uint32_t C1W_X_BYTES = C1W_BK * 128;        // activation block: 128 rows x 64 channels bf16
+struct Conv1WgradParams {
+  int rows, grid_w;             // batch * G * G rows of the G x G grid; G
+  int blocks, blocks_per_cta;   // 128-row k-blocks in all / per CTA
+  int stages;                   // operand stages (G box + activation block)
+  float* D;                     // partials: CTA i at D + i * 32 * 256
+  U8Src u8;                     // U8: the activation blocks come from the uint8 frame ring (K1)
+  unsigned long long* clk;      // profiling hook (normally null), K1_CLK_* slots: see conv1_wgrad_body
+};
+// bytes of one gradient box: rows [k0 - G - 1, k0 + BK) of 64 bytes, padded to the 1024-byte alignment of the stage ring
+__host__ __device__ inline uint32_t c1w_g_bytes(int grid_w) { return ((uint32_t)(C1W_BK + grid_w + 1) * 64 + 1023) & ~1023u; }
+// wgmma descriptor of an MN-major operand with the 64-byte swizzle (layout type 2): 32-element MN atoms `lbo` bytes apart,
+// 8-K-row groups 512 bytes apart
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t smem_addr, uint32_t lbo_bytes) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)(512 >> 4) << 32) |
+         ((uint64_t)2 << 62);
+}
+
+// Phase probe (b2rl_conv1_set_phase_clocks) slots used here: K1_CLK_CTA (thread 0's run), K1_CLK_PRODUCER_WAIT (the
+// producer's waits for a free uint8 stage and a free operand stage), K1_CLK_CONVERT_WAIT_SLAB / _PIXELS / K1_CLK_CONVERT
+// (U8 converters), K1_CLK_MMA_WAIT (MMA warpgroups' waits for a full stage), K1_CLK_MMA (their issue, retire-one wait and
+// release), K1_CLK_TILES (k-blocks, counted by the MMA warpgroups).
+template <bool U8>
+__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv1_taps_conv_wgrad_wgmma_kernel(
+    const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX, const Conv1WgradParams w) {
+  constexpr int MAX_STAGES = 6;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int halo = w.grid_w + 1;
+  const uint32_t g_bytes = c1w_g_bytes(w.grid_w), stage_bytes = g_bytes + C1W_X_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)w.stages * stage_bytes);
+  uint64_t* empty = full + MAX_STAGES;
+  // U8: uint8 staging tiles + their full / empty barriers behind the operand ring (launch_conv1_wgrad sizes the allocation)
+  const int u8_slots_ = U8 ? u8_slots(C1W_BK, w.u8.G) : 0;
+  const int u8_bytes = U8 ? u8_stage_bytes(C1W_BK, w.u8.G, w.u8.frame_w, w.u8.nf) : 0;
+  uint8_t* sU = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(empty + MAX_STAGES) + 127) & ~uintptr_t(127));
+  const int U8_STAGES = U8 ? w.u8.stages : 1;
+  uint64_t* u8_full = reinterpret_cast<uint64_t*>(sU + (size_t)U8_STAGES * u8_bytes);
+  uint64_t* u8_empty = u8_full + U8_MAX_STAGES;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
+  const int blk0 = (int)blockIdx.x * w.blocks_per_cta;
+  const int n_blk = max(min(w.blocks, blk0 + w.blocks_per_cta) - blk0, 0);
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], U8 ? 2 : 1); mb_init(&empty[s], MMA_WARPS); }   // U8: TMA + converters
+    if (U8) {
+      for (int s = 0; s < U8_STAGES; ++s) { mb_init(&u8_full[s], 1); mb_init(&u8_empty[s], 1); }
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
+  }
+  __syncthreads();
+  pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
+  unsigned long long* const clk = w.clk;
+  const long long t_start = clk_now(clk);
+  long long c_wait = 0, c_wait2 = 0, c_work = 0;                 // per-role sums of the probe (one thread per role)
+
+  if (warp == 0 && elect_one()) {
+    // ------------------------------------------------------------------------ producer: per k-block the gradient box and
+    // (bf16) the activation block, or (U8) the uint8 pixels of the block, up to w.u8.stages blocks ahead, idx[] one block early
+    U8Plan pl = {};
+    long long i0 = 0, i1 = 0;
+    int nimg = 1;
+    if constexpr (U8) {
+      nimg = w.u8.rows / (w.u8.G * w.u8.G);
+      pl = u8_plan(w.u8, blk0 * C1W_BK, C1W_BK);
+      if (n_blk > 0 && pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
+    }
+    for (int i = 0; i < n_blk; ++i) {
+      const int s = i % w.stages, k0 = (blk0 + i) * C1W_BK;
+      uint8_t* st = smem + (size_t)s * stage_bytes;
+      const long long t0 = clk_now(clk);
+      if constexpr (U8) {
+        const U8Plan cur = pl;
+        const long long c0 = i0, c1 = i1;
+        if (i + 1 < n_blk) {
+          pl = u8_plan(w.u8, k0 + C1W_BK, C1W_BK);
+          if (pl.n0 > 0) { i0 = __ldg(w.u8.idx + pl.b0); i1 = __ldg(w.u8.idx + min(pl.b0 + 1, nimg - 1)); }
+        }
+        const int us = i % U8_STAGES;
+        mb_wait(&u8_empty[us], ((i / U8_STAGES) & 1) ^ 1);
+        u8_issue(w.u8, &tmX, cur, c0, c1, sU + (size_t)us * u8_bytes, &u8_full[us], u8_slots_);
+        mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
+        mb_expect_tx(&full[s], (uint32_t)(C1W_BK + halo) * 64);
+      } else {
+        mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
+        mb_expect_tx(&full[s], (uint32_t)(C1W_BK + halo) * 64 + C1W_X_BYTES);
+        tma_load_2d(st + g_bytes, &tmX, &full[s], 0, k0);                                // [128 rows][64 c]
+      }
+      c_wait += clk_now(clk) - t0;
+      tma_load_2d(st, &tmG, &full[s], 0, k0 - halo);                                     // [BK + halo rows][32 n]
+    }
+    if (clk) atomicAdd(clk + K1_CLK_PRODUCER_WAIT, (unsigned long long)c_wait);
+  } else if (U8 && warp >= 12) {
+    // ------------------------------------------------------------------------ K1 converters (warps 12-15): the activation
+    // block of every k-block from the staged uint8 pixels, one block row per thread
+    const int tid = (int)threadIdx.x - GEMM_THREADS;
+    for (int i = 0; i < n_blk; ++i) {
+      const int s = i % w.stages, us = i % U8_STAGES;
+      const long long t0 = clk_now(clk);
+      mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
+      const long long t1 = clk_now(clk);
+      mb_wait(&u8_full[us], (i / U8_STAGES) & 1);
+      const long long t2 = clk_now(clk);
+      u8_convert<128, 8>(w.u8, sU + (size_t)us * u8_bytes, smem + (size_t)s * stage_bytes + g_bytes, nullptr,
+                         (blk0 + i) * C1W_BK, C1W_BK, u8_slots_, tid, 4);
+      if (tid == 0) { mb_arrive(&full[s]); mb_arrive(&u8_empty[us]); }
+      c_wait += t1 - t0, c_wait2 += t2 - t1, c_work += clk_now(clk) - t2;
+    }
+    if (clk && tid == 0) {
+      atomicAdd(clk + K1_CLK_CONVERT_WAIT_SLAB, (unsigned long long)c_wait);
+      atomicAdd(clk + K1_CLK_CONVERT_WAIT_PIXELS, (unsigned long long)c_wait2);
+      atomicAdd(clk + K1_CLK_CONVERT, (unsigned long long)c_work);
+    }
+  } else if (warp >= 4 && warp < 12 && n_blk > 0) {
+    // ------------------------------------------------------------------------ MMA, warpgroup g: taps 2g + 1 (rows 0-31) and
+    // 2g (rows 32-63); shift of the larger tap: 1 (g = 0) or G + 1 (g = 1), its rows start halo - shift rows into the box
+    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
+    const uint32_t a0 = s2u(smem) + (uint32_t)(g ? 0 : halo - 1) * 64, b0 = s2u(smem) + g_bytes;
+    float d[32];
+    acc_zero<64>(d);
+#pragma unroll 2
+    for (int i = 0; i < n_blk; ++i) {
+      const int s = i % w.stages;
+      const long long t0 = clk_now(clk);
+      mb_wait(&full[s], (i / w.stages) & 1);
+      const long long t1 = clk_now(clk);
+      const uint32_t st = (uint32_t)s * stage_bytes;
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < C1W_BK / 16; ++k)                         // k16 step: 16 rows = 1024 bytes of A, 2048 of B
+        wgmma_n64<1, 1>(d, make_desc_sw64(a0 + st + k * 1024, 64), make_desc(b0 + st + k * 2048, 8192));
+      wg_commit();
+      wg_wait1();                                                    // k-block i - 1 has retired: release its stage
+      if (i > 0 && lane == 0) mb_arrive(&empty[(i - 1) % w.stages]);
+      c_wait += t1 - t0, c_work += clk_now(clk) - t1;
+    }
+    wg_wait0();
+    acc_fence<64>(d);
+    if (lane == 0) mb_arrive(&empty[(n_blk - 1) % w.stages]);
+    // accumulator element d[4 jj + 2 h + e]: row m = 16 wl + lane / 4 + 8 h (channel m & 31, tap 2g + 1 - m / 32), column
+    // c = 8 jj + 2 (lane % 4) + e
+    float* base = w.D + (int64_t)blockIdx.x * (32 * 256) + 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = 16 * wl + (lane >> 2) + 8 * h;
+      float* dst = base + (m & 31) * 256 + (2 * g + 1 - (m >> 5)) * 64;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(d[4 * jj + 2 * h], d[4 * jj + 2 * h + 1]);
+    }
+    if (clk && (threadIdx.x & 127) == 0) {
+      atomicAdd(clk + K1_CLK_MMA_WAIT, (unsigned long long)c_wait);
+      atomicAdd(clk + K1_CLK_MMA, (unsigned long long)c_work);
+      if (g == 0) atomicAdd(clk + K1_CLK_TILES, (unsigned long long)n_blk);
+    }
+  }
+  __syncthreads();
+  if (clk && threadIdx.x == 0) atomicAdd(clk + K1_CLK_CTA, (unsigned long long)(clock64() - t_start));
 }
 
 // ------------------------------------------------------------------------------------------------- host side
@@ -1735,39 +1867,28 @@ static int launch_slab(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
 }
 
 // one launch of the weight-gradient instantiation for window shape WIN over `groups` tap groups from window w.win0 on
-template <bool U8, int WIN>
+template <int WIN>
 static void launch_wgrad_k(const CUtensorMap& tg, const CUtensorMap& tx, const WgradParams& w, int ctas, int groups,
                            size_t smem, cudaStream_t st) {
-  auto k = conv_wgrad_wgmma_kernel<U8, WIN>;
+  auto k = conv_wgrad_wgmma_kernel<WIN>;
   static size_t attr = 0;
   if (attr < smem) {
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     attr = smem;
   }
-  launch_pdl(k, dim3(ctas, groups), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, tg, tx, w);
+  launch_pdl(k, dim3(ctas, groups), dim3(GEMM_THREADS), smem, st, tg, tx, w);
 }
 
-template <bool U8 = false>
 static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParams w, cudaStream_t st, int* n_ctas = nullptr) {
   const size_t slab_bytes = (size_t)w.slab_rows * 128 * w.col_blocks, stage = 16384 + slab_bytes;
-  static const size_t limit = dyn_smem_limit(conv_wgrad_wgmma_kernel<U8, WGRAD_2X64>);
-  const size_t fixed = 1024 + 2 * 6 * 8 + 16 + (U8 ? 2 * U8_MAX_STAGES * 8 + 144 : 0);
+  static const size_t limit = dyn_smem_limit(conv_wgrad_wgmma_kernel<WGRAD_2X64>);
+  const size_t fixed = 1024 + 2 * 6 * 8 + 16;
   const size_t budget = limit > fixed + 200 * 1024 ? 200 * 1024 : (limit > fixed ? limit - fixed : 0);
-  size_t u8_extra = 0;
   int stages = (int)(budget / stage);
-  if (U8) {                                                          // K1: four operand stages, the rest for uint8 staging tiles
-    const size_t ub = u8_stage_bytes(w.slab_rows, w.u8.G, w.u8.frame_w, w.u8.nf);
-    if (4 * stage + 2 * ub + 512 > budget) return 1;
-    stages = 4;
-    int us = (int)((budget - 4 * stage - 512) / ub);
-    if (us > U8_MAX_STAGES) us = U8_MAX_STAGES;
-    w.u8.stages = us;
-    u8_extra = (size_t)us * ub + 2 * U8_MAX_STAGES * 8 + 144;
-  }
   if (stages > 6) stages = 6;
   if (stages < 2) return 1;
   w.stages = stages;
-  const size_t smem = 1024 + stages * stage + 2 * 6 * 8 + 16 + u8_extra;
+  const size_t smem = 1024 + stages * stage + 2 * 6 * 8 + 16;
   // one window per tap; a CTA accumulates the taps of one 128-column group (blockIdx.y)
   if (w.ntaps > 9 || (w.C != 64 && w.C != 128)) return 1;
   for (int n = 0; n < w.ntaps; ++n) {
@@ -1793,19 +1914,54 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   ctas = (kt_total + w.k_tiles_per_cta - 1) / w.k_tiles_per_cta;
   if (n_ctas) *n_ctas = ctas;
   w.win0 = 0;
-  if constexpr (U8) {                                                // conv1 from the ring: two windows of 64 channels
-    if (w.C != 64 || w.ntaps != 2) return 1;
-    launch_wgrad_k<true, WGRAD_2X64>(tg, tx, w, ctas, 1, smem, st);
-  } else if (w.C == 128) {
-    launch_wgrad_k<false, WGRAD_N128>(tg, tx, w, ctas, groups, smem, st);
+  if (w.C == 128) {
+    launch_wgrad_k<WGRAD_N128>(tg, tx, w, ctas, groups, smem, st);
   } else {                                                           // pairs of windows, then the odd one out on its own
-    if (w.ntaps >= 2) launch_wgrad_k<false, WGRAD_2X64>(tg, tx, w, ctas, w.ntaps / 2, smem, st);
+    if (w.ntaps >= 2) launch_wgrad_k<WGRAD_2X64>(tg, tx, w, ctas, w.ntaps / 2, smem, st);
     if (w.ntaps % 2) {
       w.win0 = w.ntaps - 1;
-      launch_wgrad_k<false, WGRAD_1X64>(tg, tx, w, ctas, 1, smem, st);
+      launch_wgrad_k<WGRAD_1X64>(tg, tx, w, ctas, 1, smem, st);
     }
   }
   return check_launch("b2rl_conv_gemm_bf16(wgrad slab)");
+}
+
+// conv1_taps_conv_wgrad_wgmma_kernel: the 128-row k-blocks in equal contiguous ranges over at most one CTA per SM; returns
+// the CTA count (= partial blocks written) through n_ctas, or 1 when the operand ring does not fit in shared memory
+template <bool U8>
+static int launch_conv1_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, Conv1WgradParams w, cudaStream_t st, int* n_ctas) {
+  auto k = conv1_taps_conv_wgrad_wgmma_kernel<U8>;
+  static const size_t limit = dyn_smem_limit(k);
+  const size_t stage = c1w_g_bytes(w.grid_w) + C1W_X_BYTES;
+  // alignment of the ring + its barriers (+ U8: alignment of the uint8 staging tiles and their barriers)
+  const size_t fixed = 1024 + 2 * 6 * 8 + (U8 ? 128 + 2 * U8_MAX_STAGES * 8 : 0);
+  if (limit <= fixed) return 1;
+  const size_t budget = limit - fixed;
+  int stages = (int)(budget / stage);
+  size_t u8_extra = 0;
+  if (U8) {                                                          // K1: four operand stages, the rest for uint8 staging tiles
+    const size_t ub = u8_stage_bytes(C1W_BK, w.u8.G, w.u8.frame_w, w.u8.nf);
+    if (4 * stage + 2 * ub > budget) return 1;
+    stages = 4;
+    w.u8.stages = (int)((budget - 4 * stage) / ub);
+    if (w.u8.stages > U8_MAX_STAGES) w.u8.stages = U8_MAX_STAGES;
+    u8_extra = (size_t)w.u8.stages * ub;
+  }
+  if (stages > 6) stages = 6;
+  if (stages < 2) return 1;
+  w.stages = stages;
+  const size_t smem = fixed + stages * stage + u8_extra;
+  static size_t attr = 0;
+  if (attr < smem) {
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    attr = smem;
+  }
+  w.blocks = (w.rows + C1W_BK - 1) / C1W_BK;
+  const int ctas = w.blocks < sm_count() ? w.blocks : sm_count();
+  w.blocks_per_cta = (w.blocks + ctas - 1) / ctas;
+  *n_ctas = (w.blocks + w.blocks_per_cta - 1) / w.blocks_per_cta;
+  launch_pdl(k, dim3(*n_ctas), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, tg, tx, w);
+  return check_launch("conv1 weight gradient");
 }
 
 }  // namespace b2rl
@@ -1818,8 +1974,9 @@ static int64_t g_partial_stride = 0;
 static int g_partial_count = 0;
 static int g_use_slab = 2;   // 2: shifted windows with base_offset 0 -- the 128B swizzle is a pure function of the smem address
 static unsigned long long* g_k1_clocks = nullptr;
-// Profiling hook of the K1 conv1 forwards (b2rl_conv1_u8_fwd, b2rl_conv1_u8_fwd_pair): while set, every launch adds its
-// K1_CLK_SLOTS phase-cycle sums to clocks[] (scripts/conv1_pair_time.py --phases).  Null (the default): no probe.
+// Profiling hook of the K1 conv1 forwards (b2rl_conv1_u8_fwd, b2rl_conv1_u8_fwd_pair) and of conv1's weight gradient
+// (b2rl_conv1_u8_wgrad_partials, b2rl_conv1_wgrad_partials): while set, every launch adds its K1_CLK_SLOTS phase-cycle sums
+// to clocks[] (scripts/conv1_pair_time.py --phases, scripts/conv1_wgrad_time.py --phases).  Null (the default): no probe.
 extern "C" int b2rl_conv1_set_phase_clocks(int64_t* clocks) {
   g_k1_clocks = reinterpret_cast<unsigned long long*>(clocks);
   return B2RL_OK;
@@ -2206,36 +2363,74 @@ extern "C" int b2rl_conv1_u8_fwd_pair(const uint8_t* frames, int64_t capacity, c
   return r2;
 }
 
+// 2-D bf16 tensor map over conv1's output gradient [rows][32] (64-byte rows), box [BK + G + 1 rows][32], 64-byte swizzle
+static int make_g1_map(CUtensorMap* m, const uint16_t* G_rows, int64_t rows, int grid_w) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return B2RL_ERR_CUDA; }
+  cuuint64_t gdim[2] = {32u, (cuuint64_t)rows};
+  cuuint64_t gstr[1] = {64u};
+  cuuint32_t box[2] = {32u, (cuuint32_t)(C1W_BK + grid_w + 1)};
+  cuuint32_t estr[2] = {1u, 1u};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<uint16_t*>(G_rows), gdim, gstr, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (conv1 output gradient) failed (%d)", (int)r); return B2RL_ERR_CUDA; }
+  return B2RL_OK;
+}
+
+static int conv1_wgrad_args(const uint16_t* G_rows, int32_t n_out, int grid_w, const float* partials, const int32_t* n_partials_host) {
+  B2RL_REQUIRE(G_rows && partials && n_partials_host, "null pointer");
+  B2RL_REQUIRE(n_out == 32, "conv1's weight gradient has n_out 32");
+  B2RL_REQUIRE(grid_w > 0 && C1W_BK + grid_w + 1 <= 256, "grid too wide for one gradient box");
+  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(G_rows) % 16 == 0, "operands must be 16-byte aligned");
+  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(partials) % 8 == 0, "partials must be 8-byte aligned");
+  return B2RL_OK;
+}
+
 // split-K partials of conv1's weight gradient dW[n][tap*64 + c] = sum_r G[r][n] * x[r + shift(tap)][c] with x read from the
-// ring as above (G_rows: bf16 [batch*G*G][n_out], the masked output gradient on conv1's grid).  Same output contract as
-// b2rl_conv_wgrad_partials.
+// ring as above (G_rows: bf16 [batch*G*G][32], the masked output gradient on conv1's grid; n_out must be 32).  Same output
+// contract as b2rl_conv_wgrad_partials (partial i at partials + i * 32 * 256, at most one per SM), same bits as
+// b2rl_conv1_wgrad_partials on the materialised stacks.
 extern "C" int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first,
                                             int64_t row_bytes, int32_t frame_w, int32_t batch, int32_t history, const uint16_t* G_rows,
                                             int32_t n_out, float* partials, int32_t* n_partials_host, void* stream) {
-  WgradParams w = {};
+  Conv1WgradParams w = {};
   int rc = u8_src(w.u8, frames, idx, first, row_bytes, frame_w, batch, history);
   if (rc) return rc;
-  B2RL_REQUIRE(G_rows && partials && n_partials_host, "null pointer");
-  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(partials) % 8 == 0, "partials must be 8-byte aligned");
-  B2RL_REQUIRE(n_out > 0 && n_out <= 64 && n_out % 8 == 0, "n_out <= 64, multiple of 8");
-  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(G_rows) % 16 == 0, "operands must be 16-byte aligned");
-  const int G = w.u8.G, C = 64, taps = 4;
-  w.rows = w.u8.rows; w.n_out = n_out; w.C = C; w.col_blocks = 1; w.taps_x = 2; w.grid_w = G;
-  // M-stacking (WgradParams): windows of tap row 0 only; accumulator lanes 64-127 (gradient rows read G rows earlier) give row 1
-  w.stack_delta = -G; w.stack_rows = 2; w.a_boxes = 2;
-  w.slab_rows = (GEMM_BK + 1 + 7) / 8 * 8;
-  w.D = partials; w.ldd = taps * C; w.partial_stride = (int64_t)n_out * taps * C;
-  w.tap0 = 0; w.ntaps = 2;
-  B2RL_REQUIRE(w.slab_rows <= 256, "frame too wide for one slab");
-  B2RL_REQUIRE(capacity > 0, "bad capacity");
-  CUtensorMap tg, tr;
-  rc = make_map(&tg, G_rows, n_out, w.rows, n_out, 64);
+  rc = conv1_wgrad_args(G_rows, n_out, w.u8.G, partials, n_partials_host);
   if (rc) return rc;
-  rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(w.slab_rows, G), w.u8.nf);
+  B2RL_REQUIRE(capacity > 0, "bad capacity");
+  w.rows = w.u8.rows; w.grid_w = w.u8.G; w.D = partials; w.clk = g_k1_clocks;
+  CUtensorMap tg, tr;
+  rc = make_g1_map(&tg, G_rows, w.rows, w.grid_w);
+  if (rc) return rc;
+  rc = make_ring_map(&tr, frames, capacity, row_bytes, frame_w, u8_slots(C1W_BK, w.u8.G), w.u8.nf);
   if (rc) return rc;
   int n = 0;
-  int r2 = launch_wgrad<true>(tg, tr, w, (cudaStream_t)stream, &n);
-  if (r2 > 0) { set_error("b2rl_conv1_u8_wgrad_partials: the slab does not fit in shared memory"); return B2RL_ERR_ARG; }
+  const int r2 = launch_conv1_wgrad<true>(tg, tr, w, (cudaStream_t)stream, &n);
+  if (r2 > 0) { set_error("b2rl_conv1_u8_wgrad_partials: the operand ring does not fit in shared memory"); return B2RL_ERR_ARG; }
+  *n_partials_host = n;
+  return r2;
+}
+
+// The same partials from the materialised bf16 stacks X [rows][64] (conv1's space-to-depth(4) grid matrix, G = grid_w):
+// conv1_taps_conv_wgrad_wgmma_kernel with a TMA-loaded activation block.
+extern "C" int b2rl_conv1_wgrad_partials(const uint16_t* X, int64_t rows, int32_t grid_w, const uint16_t* G_rows, int32_t n_out,
+                                         float* partials, int32_t* n_partials_host, void* stream) {
+  int rc = conv1_wgrad_args(G_rows, n_out, grid_w, partials, n_partials_host);
+  if (rc) return rc;
+  B2RL_REQUIRE(X && reinterpret_cast<uintptr_t>(X) % 16 == 0, "operands must be 16-byte aligned");
+  B2RL_REQUIRE(rows > 0 && rows < (1LL << 31), "bad shape");
+  Conv1WgradParams w = {};
+  w.rows = (int)rows; w.grid_w = grid_w; w.D = partials; w.clk = g_k1_clocks;
+  CUtensorMap tg, tx;
+  rc = make_g1_map(&tg, G_rows, rows, grid_w);
+  if (rc) return rc;
+  rc = make_map(&tx, X, 64, rows, 64, C1W_BK);                       // activation block: box [128 rows][64 c]
+  if (rc) return rc;
+  int n = 0;
+  const int r2 = launch_conv1_wgrad<false>(tg, tx, w, (cudaStream_t)stream, &n);
+  if (r2 > 0) { set_error("b2rl_conv1_wgrad_partials: the operand ring does not fit in shared memory"); return B2RL_ERR_ARG; }
   *n_partials_host = n;
   return r2;
 }

@@ -265,6 +265,10 @@ def wgrad_partials(X, G_rows, n_out, taps, taps_x, grid_w, stream=None):
         return out, 1
     buf = torch.empty((_max_partials(X.device), n_out, taps * C), dtype=_f32, device=X.device)
     n = ctypes.c_int32(0)
+    if (C, n_out, taps, taps_x) == (64, 32, 4, 2):   # conv1: the taps-in-M kernel, the same bits as wgrad_partials_ring
+        _lib.call("b2rl_conv1_wgrad_partials", _lib.ptr(X), int(rows), int(grid_w), _lib.ptr(G_rows), int(n_out), _lib.ptr(buf),
+                  ctypes.byref(n), stream if stream is not None else _lib.stream())
+        return buf, int(n.value)
     _lib.call("b2rl_conv_wgrad_partials", _lib.ptr(X), int(rows), int(C), _lib.ptr(G_rows), int(n_out), int(taps), int(taps_x),
               int(grid_w), _lib.ptr(buf), ctypes.byref(n), stream if stream is not None else _lib.stream())
     return buf, int(n.value)

@@ -320,13 +320,18 @@ int b2rl_conv_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const u
  * exact integers 0..255; ImageNormalizer's 1/255 is folded into W [n_out][4 taps * 64] (b2rl_nature_pack_weights).
  * fwd: D = act(conv1 + bias) over rows (b, gy, gx) of the (frame_w/4)^2 grid, bf16, output row maps of
  * b2rl_conv_gemm_bf16.  wgrad_partials: split-K partials of dW[n][tap*64+c] = sum_r G[r][n] * x[r + shift(tap)][c],
- * contract of b2rl_conv_wgrad_partials. */
+ * contract of b2rl_conv_wgrad_partials; n_out must be 32. */
 int b2rl_conv1_u8_fwd(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first, int64_t row_bytes,
                       int32_t frame_w, int32_t batch, int32_t history, const uint16_t* W, int32_t n_out, void* D, int64_t ldd,
                       const float* bias, int32_t relu, int32_t out_map, int32_t V, void* stream);
 int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first, int64_t row_bytes,
                                  int32_t frame_w, int32_t batch, int32_t history, const uint16_t* G_rows, int32_t n_out, float* partials,
                                  int32_t* n_partials_host, void* stream);
+/* conv1's weight-gradient partials from the materialised bf16 stacks X [rows][64] (the space-to-depth(4) grid matrix,
+ * grid_w x grid_w positions per image), G_rows [rows][32]: the same partition, partials and bits as
+ * b2rl_conv1_u8_wgrad_partials on the ring the stacks came from.  n_out must be 32. */
+int b2rl_conv1_wgrad_partials(const uint16_t* X, int64_t rows, int32_t grid_w, const uint16_t* G_rows, int32_t n_out,
+                              float* partials, int32_t* n_partials_host, void* stream);
 /* The online forward on the state and the target forward on the next state (n_step 1) in ONE launch: D = act(conv1_W(s) +
  * bias) and D2 = act(conv1_W2(s') + bias2), s the stacks idx[b] + first .. + history - 1 and s' the stacks one ring row
  * later, read together from the history + 1 ring rows they span.  W, W2 [32][4 taps * 64]; D, D2 as D of b2rl_conv1_u8_fwd
