@@ -233,6 +233,7 @@ def test_fused_backward_epilogues_match_the_separate_passes(env):
     net = rl.VanillaNet(4, rl.NatureConvBody(in_channels=4))
     s = torch.randint(0, 256, (96, 64, 21, 21), device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
     grads = {}
+    saved = nature_tc.FUSED_BWD          # restored for the tests that follow: their learners' plans read it
     for fused in (False, True):
         nature_tc.FUSED_BWD = fused
         try:
@@ -243,7 +244,7 @@ def test_fused_backward_epilogues_match_the_separate_passes(env):
             torch.cuda.synchronize()
             grads[fused] = {n: p.grad.detach().clone() for n, p in net.named_parameters()}
         finally:
-            nature_tc.FUSED_BWD = False
+            nature_tc.FUSED_BWD = saved
     for n, ref in grads[False].items():
         got = grads[True][n]
         scale = float(ref.abs().max()) + 1e-12
