@@ -39,6 +39,8 @@ SIGNATURES = {
     "b2rl_c51_loss": [c_p, c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_f32, c_i32, c_i32, c_i32, c_p, c_f32, c_f32, c_f32,
                       c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     "b2rl_qr_loss": [c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    "b2rl_nstep_q_loss_ctas": [c_i32],
+    "b2rl_nstep_q_loss": [c_p, c_p, c_p, c_p, c_p, c_f32, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     "b2rl_gae": [c_p, c_p, c_p, c_f32, c_f32, c_i32, c_i32, c_i32, c_i32, c_p, c_p, c_p],
     "b2rl_normalize_advantage": [c_p, c_i32, c_p],
     "b2rl_ppo_loss": [c_p, c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_p, c_p, c_p, c_p, c_p],

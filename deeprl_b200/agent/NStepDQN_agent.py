@@ -14,6 +14,14 @@ csrc/losses.cu).  On ``select_device(-1)`` the same statements run as torch expr
 rollout, the target sync included (csrc/a2c.cu, component/actor.py ``DeviceNStepDQN``).  The epsilon-greedy draws then come from
 the device's Philox stream, not from numpy's.  Configurations the kernels do not cover raise ``NotImplementedError`` naming the
 unmet condition.
+
+``config.cuda_graph = True`` (off by default) runs each ``step()`` of a VanillaNet on a wgmma NatureConvBody at bf16
+(``n_step_dqn_pixel`` with ``Config.COMPUTE_DTYPE = torch.bfloat16``) as captured graphs: one ``GraphedQActor`` replay per env
+step (pinned upload of the frame stacks into the rollout arena, the network, q down to the host; epsilon-greedy stays in numpy
+as in the reference) and one ``GraphedNStepLearner`` replay per rollout (learner.py).  The torch optimizer is replaced by a
+``FlatOptimizer`` with its hyper-parameters; the network's parameters become views into its arena, so ``state_dict()`` is
+always current.  Configurations it does not cover (``component/actor.py nstep_q_graph_unsupported``; the reason is kept in
+``graph_refusal``) keep the eager path; ``config.device_nstep_dqn`` takes precedence.
 """
 import numpy as np
 import torch
@@ -37,6 +45,8 @@ class NStepDQNAgent(BaseAgent):
         self.total_steps = 0
         self.states = self.task.reset()
         self.last_loss = None
+        self._graph = None                                  # (GraphedNStepLearner, GraphedQActor), False: eager; decided once
+        self.graph_refusal = None
         self.device_nstep_dqn = None
         if getattr(config, "device_nstep_dqn", False):
             from ..component.actor import DeviceNStepDQN
@@ -53,9 +63,16 @@ class NStepDQNAgent(BaseAgent):
     def _obs(self, states):
         return self.config.state_normalizer(np.asarray([np.asarray(s) for s in states]))
 
+    def load(self, filename):
+        BaseAgent.load(self, filename)
+        if self._graph:
+            self._graph[0].refresh_packed()                # the next step trains (and acts) from the loaded weights
+
     def step(self):
         if self.device_nstep_dqn is not None:
             return self._step_device()
+        if self._graph_ok():
+            return self._step_graph()
         config = self.config
         T = config.rollout_length
         storage = Storage(T)
@@ -122,3 +139,46 @@ class NStepDQNAgent(BaseAgent):
             sync = sync or self.total_steps // config.num_workers % config.target_network_update_freq == 0
         self.states = states
         self.last_loss = dev.update(self._obs(states), sync)
+
+    # ------------------------------------------------------------------ config.cuda_graph (opt-in)
+    def _graph_ok(self):
+        """Decided on the first step: the captured actor + update serve this configuration (``nstep_q_graph_unsupported``),
+        or the eager path runs (the reason is kept in ``graph_refusal``)."""
+        if self._graph is None:
+            from ..component.actor import GraphedQActor, nstep_q_graph_unsupported
+            from ..learner import GraphedNStepLearner
+            config = self.config
+            self.graph_refusal = nstep_q_graph_unsupported(config, self.network, self.optimizer, self.states)
+            self._graph = False
+            if self.graph_refusal is None:
+                self.optimizer = ops.FlatOptimizer.from_torch(self.optimizer, list(self.network.parameters()))
+                coef = config.state_normalizer.coef
+                lr = GraphedNStepLearner(self.network, self.target_network, self.optimizer, config.rollout_length,
+                                         config.num_workers, config.discount, config.gradient_clip, coef).capture()
+                actor = GraphedQActor(self.network, lambda out: out["q"], config.num_workers, 4, (84, 84), coef, arena=lr.arena)
+                self._graph = (lr, actor)
+        return bool(self._graph)
+
+    def _step_graph(self):
+        """``step()`` with ``config.cuda_graph``: T actor replays, each followed by epsilon-greedy and ``task.step`` on the host,
+        with actions / rewards / masks written into the learner's pinned staging buffer; then one update replay, preceded by
+        the target sync when an env step of this rollout reached its schedule (:48-50; the online network does not change
+        inside the rollout, so syncing at its end is the same)."""
+        config = self.config
+        lr, actor = self._graph
+        states, sync = self.states, False
+        for t in range(config.rollout_length):
+            q = actor.q_values(states, t)
+            epsilon = config.random_action_prob(config.num_workers)
+            actions = epsilon_greedy(epsilon, q)
+            next_states, rewards, terminals, info = self.task.step(actions)
+            self.record_online_return(info)
+            lr.h_action[t].numpy()[...] = actions
+            lr.h_reward[t].numpy()[...] = np.asarray(config.reward_normalizer(rewards), dtype=np.float32)   # tensor(): float32
+            lr.h_mask[t].numpy()[...] = 1 - np.asarray(terminals, dtype=np.float32)
+            states = next_states
+            self.total_steps += config.num_workers
+            sync = sync or self.total_steps // config.num_workers % config.target_network_update_freq == 0
+        self.states = states
+        lr.stage_final(states)
+        self.last_loss = lr.update(sync_target=sync)

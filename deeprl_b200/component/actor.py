@@ -143,25 +143,46 @@ class GraphedQActor:
     epsilon-greedy draw stays on the host (``epsilon_greedy``: the reference's numpy stream, torch_utils.py:51-58).
 
     The eager form of the same step is ~40 kernel / memcpy launches of Python-driven work per env step; this is one launch and
-    one stream synchronise."""
+    one stream synchronise.
 
-    def __init__(self, network, q_fn, num_envs, history, frame_hw, scale):
+    ``arena``: a uint8 device tensor [slots * num_envs * history + 1, H * W] that receives the uploaded stacks instead of the
+    actor's own one-slot buffer: ``q_values(states, slot)`` uploads them into rows ``slot * num_envs * history ...`` and
+    forwards from there (one captured graph per slot), so a learner can read a whole rollout's frame stacks from the arena
+    without uploading them again (learner.GraphedNStepLearner).  The last row is padding the gather stages but never uses."""
+
+    def __init__(self, network, q_fn, num_envs, history, frame_hw, scale, arena=None):
         p = next(network.parameters())
         self.net, self.q_fn, self.dev = network, q_fn, p.device
         self.N, self.hl, self.hw, self.scale = int(num_envs), int(history), tuple(frame_hw), float(scale)
         self.row = self.hw[0] * self.hw[1]
         rows = self.N * self.hl + 1                       # (+1: the gather kernel stages history + n_step rows)
         self.h_frames = torch.zeros((rows, self.row), dtype=torch.uint8, pin_memory=True)
-        self.d_frames = torch.zeros((rows, self.row), dtype=torch.uint8, device=self.dev)
+        if arena is None:
+            self.d_frames = torch.zeros((rows, self.row), dtype=torch.uint8, device=self.dev)
+        else:
+            ok = (arena.dtype == torch.uint8 and arena.device == self.dev and arena.dim() == 2 and arena.shape[1] == self.row
+                  and arena.is_contiguous() and (arena.shape[0] - 1) % (self.N * self.hl) == 0 and arena.shape[0] > 1)
+            if not ok:
+                raise _lib.B2RLError("GraphedQActor: the arena must be a contiguous uint8 tensor [slots * %d + 1, %d] on %s"
+                                     % (self.N * self.hl, self.row, self.dev))
+            self.d_frames = arena
+        self.slots = (self.d_frames.shape[0] - 1) // (self.N * self.hl)
         self._np_frames = self.h_frames.numpy()[:self.N * self.hl].reshape(self.N, self.hl, self.row)
-        self.idx = (torch.arange(self.N, dtype=torch.int64) * self.hl + self.hl - 1).to(self.dev)
-        self.d_action = torch.zeros(rows, dtype=torch.int32, device=self.dev)      # (scalar columns of the ring API: unused)
-        self.d_reward = torch.zeros(rows, dtype=torch.float64, device=self.dev)
-        self.d_mask = torch.ones(rows, dtype=torch.int32, device=self.dev)
+        last = torch.arange(self.N, dtype=torch.int64) * self.hl + self.hl - 1
+        self.idxs = [(last + s * self.N * self.hl).to(self.dev) for s in range(self.slots)]
+        self.idx = self.idxs[0]
+        n = self.d_frames.shape[0]
+        self.d_action = torch.zeros(n, dtype=torch.int32, device=self.dev)         # (scalar columns of the ring API: unused)
+        self.d_reward = torch.zeros(n, dtype=torch.float64, device=self.dev)
+        self.d_mask = torch.ones(n, dtype=torch.int32, device=self.dev)
         self.x = torch.empty((self.N, self.hw[0] // 4, self.hw[1] // 4, 16 * self.hl), dtype=torch.bfloat16, device=self.dev)
         self.d_q = self.h_q = None
-        self.graph, self._sig = None, None
+        self.graphs, self._sig = [None] * self.slots, None
         self.replays = 0
+
+    @property
+    def graph(self):
+        return self.graphs[0]
 
     def _signature(self):
         """What the captured launch sequence depends on besides addresses: who re-packs the body's bf16 operands (the body per
@@ -170,11 +191,12 @@ class GraphedQActor:
         heads = tuple(getattr(m, "_w16", None) is not None for m in self.net.children() if isinstance(m, torch.nn.Linear))
         return (bool(getattr(body, "auto_repack", True)), heads)
 
-    def _forward(self):
+    def _forward(self, slot=0):
         from ..network.fused import frame_scale
-        self.d_frames.copy_(self.h_frames, non_blocking=True)
+        k = self.N * self.hl
+        self.d_frames[slot * k:(slot + 1) * k].copy_(self.h_frames[:k], non_blocking=True)
         _lib.call("b2rl_replay_gather", _lib.ptr(self.d_frames), _lib.ptr(self.d_action), _lib.ptr(self.d_reward),
-                  _lib.ptr(self.d_mask), self.d_frames.shape[0], self.row, _lib.ptr(self.idx), self.N, self.hl, 1, 1.0, None,
+                  _lib.ptr(self.d_mask), self.d_frames.shape[0], self.row, _lib.ptr(self.idxs[slot]), self.N, self.hl, 1, 1.0, None,
                   _lib.DTYPE_CODE[torch.bfloat16], 2, self.hw[1], _lib.ptr(self.x), None, None, None, None, _lib.stream())
         with torch.no_grad(), frame_scale(self.scale):
             q = self.q_fn(self.net(self.x.permute(0, 3, 1, 2))).float()
@@ -184,29 +206,34 @@ class GraphedQActor:
         self.d_q.copy_(q)
         self.h_q.copy_(self.d_q, non_blocking=True)
 
-    def _capture(self):
+    def _capture(self, slot=0):
+        if self._sig != self._signature():               # the launch sequence changed: every slot's graph is stale
+            self.graphs = [None] * self.slots
         cur = torch.cuda.current_stream()
         side = torch.cuda.Stream()
         side.wait_stream(cur)
         with torch.cuda.stream(side):                     # eager warm-up (lazy allocations, cuBLAS workspaces of library heads)
-            self._forward()
+            self._forward(slot)
         cur.wait_stream(side)
         torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._forward()
+        g = torch.cuda.CUDAGraph()
+        pool = next((h.pool() for h in self.graphs if h is not None), None)     # the slots' graphs replay one at a time
+        with torch.cuda.graph(g, pool=pool):
+            self._forward(slot)
+        self.graphs[slot] = g
         self._sig = self._signature()
 
-    def q_values(self, states):
-        """``states``: ``num_envs`` frame stacks (LazyFrames / uint8 arrays [history, H, W]).  Returns float32 [num_envs, A]."""
+    def q_values(self, states, slot=0):
+        """``states``: ``num_envs`` frame stacks (LazyFrames / uint8 arrays [history, H, W]).  Returns float32 [num_envs, A].
+        ``slot``: where in the arena the stacks land (0 without an arena)."""
         for i, s in enumerate(states):
             a = np.asarray(s)
             if a.dtype != np.uint8 or a.size != self.hl * self.row:
                 raise _lib.B2RLError("GraphedQActor expects uint8 frame stacks of %d x %s" % (self.hl, self.hw))
             self._np_frames[i] = a.reshape(self.hl, self.row)
-        if self.graph is None or self._sig != self._signature():
-            self._capture()
-        self.graph.replay()
+        if self.graphs[slot] is None or self._sig != self._signature():
+            self._capture(slot)
+        self.graphs[slot].replay()
         self.replays += 1
         torch.cuda.current_stream().synchronize()
         return self.h_q.numpy().copy()
@@ -224,6 +251,51 @@ def q_actor_supported(config, network):
                 and body.conv1.in_channels == 4
                 and Config.COMPUTE_DTYPE == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
                 and isinstance(config.state_normalizer, RescaleNormalizer))
+
+
+def nstep_q_graph_unsupported(config, network, optimizer, states):
+    """``None`` when ``NStepDQNAgent.step()`` runs as captured graphs under ``config.cuda_graph`` (GraphedQActor per env step,
+    learner.GraphedNStepLearner per rollout), else the unmet condition; the agent then keeps its eager path.  ``states``: the
+    envs' current observations.  (``config.async_actor`` plays no part: this agent steps its envs itself.)"""
+    from ..network import nature_tc
+    from ..network.network_bodies import NatureConvBody
+    from ..network.network_heads import VanillaNet
+    from ..utils import Config
+    from ..utils.normalizer import RescaleNormalizer
+    if not getattr(config, "cuda_graph", False):
+        return "config.cuda_graph is not set"
+    if getattr(config, "device_nstep_dqn", False):
+        return "config.device_nstep_dqn is set; it runs the agent on the device itself"
+    if type(network) is not VanillaNet:
+        return "the network is a %s; the captured update implements VanillaNet" % type(network).__name__
+    body = network.body
+    if not isinstance(body, NatureConvBody):
+        return "the body is a %s; the captured update implements NatureConvBody" % type(body).__name__
+    if body.noisy_linear or config.noisy_linear:
+        return "the network has NoisyLinear layers; the captured update implements nn.Linear"
+    if body.conv1.in_channels != 4:
+        return "the NatureConvBody takes %d channels; the captured update reads stacks of 4 frames" % body.conv1.in_channels
+    if Config.COMPUTE_DTYPE != torch.bfloat16 or Config.DENSE_BACKEND != "tcgen05":
+        return ("the compute dtype is %s with the %r dense backend; the captured update runs bf16 on the wgmma kernels "
+                "(tcgen05)" % (Config.COMPUTE_DTYPE, Config.DENSE_BACKEND))
+    if not (nature_tc.FUSED_BWD and _lib.CONV_SLAB):
+        return "the fused backward epilogues are switched off; the captured update needs the fused update tail"
+    if network.fc_head.out_features >= 32:
+        return "%d actions; the narrow head and loss kernels take fewer than 32" % network.fc_head.out_features
+    if not isinstance(config.state_normalizer, RescaleNormalizer):
+        return "the state normalizer is %s; the captured update folds a RescaleNormalizer into conv1" % type(
+            config.state_normalizer).__name__
+    if not all(np.asarray(s).dtype == np.uint8 and np.asarray(s).shape == (4, 84, 84) for s in states):
+        return "the envs do not return uint8 4 x 84 x 84 frame stacks"
+    # what FlatOptimizer.from_torch turns into a kind the fused tail (NatureTail) takes
+    g = optimizer.param_groups[0]
+    if not ((isinstance(optimizer, torch.optim.RMSprop) and g["momentum"] == 0 and g["weight_decay"] == 0)
+            or (isinstance(optimizer, torch.optim.Adam) and g["weight_decay"] == 0 and not g["amsgrad"])):
+        return ("the optimizer is %s; the fused update tail implements RMSprop (centered or not) and Adam without momentum, "
+                "weight decay or amsgrad" % type(optimizer).__name__)
+    if not body.conv1.weight.is_cuda:
+        return "the network is not on a CUDA device (select_device(0))"
+    return None
 
 
 # ------------------------------------------------------------------------------------------------ A2C on the device

@@ -287,6 +287,67 @@ __global__ void __launch_bounds__(256) qr_loss_kernel(const float* __restrict__ 
   }
 }
 
+// --------------------------------------------------------------------------------------------- n-step Q-learning
+// NStepDQN_agent.py:56-63 for a rollout of T env steps x N workers, q rows t-major (row i = t N + n): bootstrap
+// max_a q_T[n] (:56-57), the backward scan ret_t = r_t + discount * m_t * ret_{t+1} (:58-60, the reference's operation
+// order), delta = ret - q[a], loss = 0.5 * mean(delta^2) over the T N rows (:63) and gq = dloss/dq = -delta / (T N) at the
+// taken action, 0 elsewhere.  One thread per worker column (its scan is sequential in t), NSTEP_THREADS columns per CTA; each
+// CTA's sum of delta^2 is parked in partial[cta] and the last CTA to arrive adds the partials in CTA order, so the loss does
+// not depend on which CTA finishes when.
+constexpr int NSTEP_THREADS = 128;
+constexpr int NSTEP_MAX_A = 32;                 // the narrow heads' action limit (csrc/head.cu)
+constexpr int NSTEP_MAX_ROWS = 1 << 24;         // T N converts to float exactly
+
+__global__ void __launch_bounds__(NSTEP_THREADS) nstep_q_loss_kernel(const float* __restrict__ q,
+                                                                    const float* __restrict__ q_boot,
+                                                                    const int64_t* __restrict__ action,
+                                                                    const float* __restrict__ reward,
+                                                                    const float* __restrict__ mask, float discount, int T,
+                                                                    int N, int A, float* __restrict__ ret_out,
+                                                                    float* __restrict__ delta_out,
+                                                                    float* __restrict__ loss_out, float* __restrict__ gq_out,
+                                                                    float* __restrict__ partial,
+                                                                    int32_t* __restrict__ counter) {
+  pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return
+  __shared__ float red[32];
+  __shared__ bool is_last;
+  const int n = blockIdx.x * NSTEP_THREADS + threadIdx.x;
+  const float rows = (float)(T * N);
+  float acc = 0.0f;
+  if (n < N) {
+    const float* qb = q_boot + (int64_t)n * A;
+    float ret = qb[0];
+    for (int a = 1; a < A; ++a) ret = fmaxf(ret, qb[a]);
+    for (int t = T - 1; t >= 0; --t) {
+      const int64_t i = (int64_t)t * N + n;
+      ret = __fadd_rn(reward[i], __fmul_rn(__fmul_rn(discount, mask[i]), ret));
+      const int a_i = (int)action[i];
+      const float delta = __fsub_rn(ret, q[i * A + a_i]);
+      if (ret_out) ret_out[i] = ret;
+      if (delta_out) delta_out[i] = delta;
+      acc = __fadd_rn(acc, __fmul_rn(delta, delta));
+      if (gq_out) {
+        float* g = gq_out + i * A;
+        for (int a = 0; a < A; ++a) g[a] = a == a_i ? __fdiv_rn(-delta, rows) : 0.0f;
+      }
+    }
+  }
+  const float s = block_reduce(acc, OpAdd(), 0.0f, red);
+  if (threadIdx.x == 0) {
+    partial[blockIdx.x] = s;
+    __threadfence();
+    is_last = atomicAdd(counter, 1) == (int)gridDim.x - 1;
+  }
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {              // deterministic final reduction in CTA order
+    __threadfence();
+    float tot = 0.0f;
+    for (int c = 0; c < (int)gridDim.x; ++c) tot = __fadd_rn(tot, __ldcg(partial + c));
+    if (loss_out) loss_out[0] = __fmul_rn(0.5f, __fdiv_rn(tot, rows));
+    *counter = 0;
+  }
+}
+
 // Shape limits of the C51 / QR entry points.  Their dynamic shared memory is (3N + A) floats: 64 KiB at the limits, past the
 // 48 KiB a launch gets by default and well inside the 227 KiB per block of sm_90.  A request over 48 KiB raises the kernel's
 // limit to the largest accepted request (always the same value, so no call lowers it under a launch a captured graph holds).
@@ -352,4 +413,18 @@ extern "C" int b2rl_qr_loss(const float* quantile, const float* quantile_next, c
                                                          B, A, N, vec_out, loss_out, dquant_out, partial, counter,
                                                          grad_weight);
   return check_launch("b2rl_qr_loss");
+}
+
+extern "C" int b2rl_nstep_q_loss_ctas(int32_t N) { return N > 0 ? (N + NSTEP_THREADS - 1) / NSTEP_THREADS : 0; }
+
+extern "C" int b2rl_nstep_q_loss(const float* q, const float* q_boot, const int64_t* action, const float* reward,
+                                 const float* mask, float discount, int32_t T, int32_t N, int32_t A, float* ret_out,
+                                 float* delta_out, float* loss_out, float* gq_out, float* partial, int32_t* counter,
+                                 void* stream) {
+  B2RL_REQUIRE(q && q_boot && action && reward && mask && partial && counter, "null pointer");
+  B2RL_REQUIRE(T >= 1 && N >= 1 && A >= 1 && A <= NSTEP_MAX_A, "bad shape: needs T >= 1, N >= 1 and 1 <= A <= 32");
+  B2RL_REQUIRE((int64_t)T * N <= NSTEP_MAX_ROWS, "T * N must not exceed 2^24 rows");
+  launch_pdl(nstep_q_loss_kernel, dim3(b2rl_nstep_q_loss_ctas(N)), dim3(NSTEP_THREADS), 0, (cudaStream_t)stream, q, q_boot,
+             action, reward, mask, discount, T, N, A, ret_out, delta_out, loss_out, gq_out, partial, counter);
+  return check_launch("b2rl_nstep_q_loss");
 }

@@ -103,7 +103,85 @@ def update_plan(kind="dqn", per=False, prefetch=False, dual=False, k1_body=True,
                       one_graph=one_graph)
 
 
-class GraphedDQNLearner:
+class _NatureLearner:
+    """What the captured learners of a wgmma NatureConvBody network share: the update plan (decided on first use by the
+    subclass's ``_resolve_plan``), the fused update tail, and the packed bf16 operands of the online (``net``) and target
+    (``tgt``) networks -- re-packed after outside parameter changes and at target sync."""
+
+    @property
+    def plan(self):
+        """The ``UpdatePlan`` of this learner, decided on first use (the module flags the fused tail depends on are read
+        then, as the tail itself is built lazily)."""
+        if self._plan is None:
+            self._plan = self._resolve_plan()
+        return self._plan
+
+    def tail(self):
+        """The two-launch update tail (gradient reduce + clip / optimizer / operand pack) when the online network has a
+        wgmma NatureConvBody and the backward epilogues are fused; None otherwise (generic unpack + FlatOptimizer.step)."""
+        if self._tail is None:
+            from .network.tail import NatureTail
+            if self.plan.tail:
+                self._repack(self.net)
+                self._tail = NatureTail(self.opt, self.net.body, self.scale)
+                self._tail.max_norm, self._tail.grad_scale = self.clip, 1.0 / self.world
+                self._refresh_head_operands(True)
+                if self.world > 1:
+                    # fc4's gradient is reduced into the arena and all-reduced right after its GEMM (beside the convolution
+                    # backward); the small remainder follows the last weight-gradient GEMM
+                    self._tail.split = True
+                    self._tail.early = self._allreduce_early
+            else:
+                self._tail = False
+        return self._tail or None
+
+    def _repack(self, net):
+        """wgmma backend: the learner owns the packed bf16 operands of both networks -- the online body is re-packed
+        once per update (one launch), the target body only when it is synchronised."""
+        body = getattr(net, "body", None)
+        if body is not None and hasattr(body, "repack") and self.dtype == torch.bfloat16:
+            body.auto_repack = False
+            body.repack(self.scale)
+
+    def repack_online(self):
+        """Bring the online network's packed bf16 operands up to date after ``update()``, for a forward outside the learner
+        (the actor).  The fused tail's optimizer kernel writes them itself; without it this is one re-pack launch."""
+        if self.tail() is None:
+            self._repack(self.net)
+
+    def sync_target(self):
+        self.tgt.load_state_dict(self.net.state_dict())        # DQN_agent.py:136-138
+        self._repack(self.tgt)
+        self._refresh_head_operands(False)
+
+    def refresh_packed(self):
+        """Re-derive the packed bf16 operands of both networks from the fp32 parameters (after the parameters were changed
+        from outside: load_state_dict, a broadcast, a copied arena)."""
+        self._repack(self.net)
+        self._repack(self.tgt)
+        self._refresh_head_operands(True)
+
+    def _refresh_head_operands(self, online):
+        """Distributional heads (C51 / QR-DQN) on the wgmma GEMM: the online head reads its bf16 weight from the optimizer's
+        arena-wide bf16 shadow (written by the fused optimizer kernel), the target head from a copy refreshed at target sync."""
+        if not self.plan.dist_head or self.tail() is None:
+            return
+        fa, ft = (getattr(n, "fc_categorical", None) or getattr(n, "fc_quantiles", None) for n in (self.net, self.tgt))
+        if not isinstance(fa, torch.nn.Linear) or not isinstance(ft, torch.nn.Linear) or fa.weight.data_ptr() % 16:
+            return
+        o = self.opt
+        if o.shadow is None:
+            o.shadow = torch.zeros(o.n, dtype=torch.bfloat16, device=o.flat.device)
+        if online:
+            o.shadow.copy_(o.flat)
+            off = (fa.weight.data_ptr() - o.flat.data_ptr()) // 4
+            fa._w16 = o.shadow[off:off + fa.weight.numel()].view_as(fa.weight)
+        if getattr(ft, "_w16", None) is None:
+            ft._w16 = torch.empty_like(ft.weight, dtype=torch.bfloat16)
+        ft._w16.copy_(ft.weight.detach())
+
+
+class GraphedDQNLearner(_NatureLearner):
     def __init__(self, network, target_network, optimizer, replay, kind="dqn", discount=0.99, n_step=1, double_q=False,
                  gradient_clip=5.0, feeds_per_update=4, compute_dtype=torch.bfloat16, state_scale=1.0 / 255,
                  replay_eps=0.01, replay_alpha=0.5, categorical=(-10.0, 10.0), world_size=1, target_sync_every=10000,
@@ -159,14 +237,6 @@ class GraphedDQNLearner:
         self._plan = None
         self.opt.zero_grad()              # the fused tail writes / re-zeroes the gradient arena itself: start from zeros
 
-    @property
-    def plan(self):
-        """The ``UpdatePlan`` of this learner, decided on first use (the module flags the fused tail depends on are read
-        then, as the tail itself is built lazily)."""
-        if self._plan is None:
-            self._plan = self._resolve_plan()
-        return self._plan
-
     def _resolve_plan(self, one_graph=True):
         body, rp = getattr(self.net, "body", None), self.replay
         wgmma = self.dtype == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05" and hasattr(body, "repack")
@@ -181,26 +251,6 @@ class GraphedDQNLearner:
     @property
     def ring(self):
         return self.plan.ring
-
-    # ------------------------------------------------------------------ fused tail / fused head (csrc/tail.cu, csrc/head.cu)
-    def tail(self):
-        """The two-launch update tail (gradient reduce + clip / optimizer / operand pack) when the online network has a
-        wgmma NatureConvBody and the backward epilogues are fused; None otherwise (generic unpack + FlatOptimizer.step)."""
-        if self._tail is None:
-            from .network.tail import NatureTail
-            if self.plan.tail:
-                self._repack(self.net)
-                self._tail = NatureTail(self.opt, self.net.body, self.scale)
-                self._tail.max_norm, self._tail.grad_scale = self.clip, 1.0 / self.world
-                self._refresh_head_operands(True)
-                if self.world > 1:
-                    # fc4's gradient is reduced into the arena and all-reduced right after its GEMM (beside the convolution
-                    # backward); the small remainder follows the last weight-gradient GEMM
-                    self._tail.split = True
-                    self._tail.early = self._allreduce_early
-            else:
-                self._tail = False
-        return self._tail or None
 
     def _heads(self):
         """(online head modules, target head modules) when the heads fit the fused head + loss + backward kernel: narrow,
@@ -377,25 +427,6 @@ class GraphedDQNLearner:
                 self._sampled_ev.record(pre)
                 nature_tc.mark("sampled")
 
-    def _repack(self, net):
-        """wgmma backend: the learner owns the packed bf16 operands of both networks -- the online body is re-packed
-        once per update (one launch), the target body only when it is synchronised."""
-        body = getattr(net, "body", None)
-        if body is not None and hasattr(body, "repack") and self.dtype == torch.bfloat16:
-            body.auto_repack = False
-            body.repack(self.scale)
-
-    def repack_online(self):
-        """Bring the online network's packed bf16 operands up to date after ``update()``, for a forward outside the learner
-        (the actor).  The fused tail's optimizer kernel writes them itself; without it this is one re-pack launch."""
-        if self.tail() is None:
-            self._repack(self.net)
-
-    def sync_target(self):
-        self.tgt.load_state_dict(self.net.state_dict())        # DQN_agent.py:136-138
-        self._repack(self.tgt)
-        self._refresh_head_operands(False)
-
     def _opt(self):
         tail = self.tail()
         if tail is not None:
@@ -405,32 +436,6 @@ class GraphedDQNLearner:
         nature_tc.mark("opt")
         if self.plan.join == "opt":                      # the late prefetch branch ran beside the update tail
             torch.cuda.current_stream().wait_stream(self._pre)
-
-    def refresh_packed(self):
-        """Re-derive the packed bf16 operands of both networks from the fp32 parameters (after the parameters were changed
-        from outside: load_state_dict, a broadcast, a copied arena)."""
-        self._repack(self.net)
-        self._repack(self.tgt)
-        self._refresh_head_operands(True)
-
-    def _refresh_head_operands(self, online):
-        """Distributional heads (C51 / QR-DQN) on the wgmma GEMM: the online head reads its bf16 weight from the optimizer's
-        arena-wide bf16 shadow (written by the fused optimizer kernel), the target head from a copy refreshed at target sync."""
-        if not self.plan.dist_head or self.tail() is None:
-            return
-        fa, ft = (getattr(n, "fc_categorical", None) or getattr(n, "fc_quantiles", None) for n in (self.net, self.tgt))
-        if not isinstance(fa, torch.nn.Linear) or not isinstance(ft, torch.nn.Linear) or fa.weight.data_ptr() % 16:
-            return
-        o = self.opt
-        if o.shadow is None:
-            o.shadow = torch.zeros(o.n, dtype=torch.bfloat16, device=o.flat.device)
-        if online:
-            o.shadow.copy_(o.flat)
-            off = (fa.weight.data_ptr() - o.flat.data_ptr()) // 4
-            fa._w16 = o.shadow[off:off + fa.weight.numel()].view_as(fa.weight)
-        if getattr(ft, "_w16", None) is None:
-            ft._w16 = torch.empty_like(ft.weight, dtype=torch.bfloat16)
-        ft._w16.copy_(ft.weight.detach())
 
     # ------------------------------------------------------------------ capture / replay
     def capture(self, warmup=3, with_h2d=False):
@@ -541,6 +546,140 @@ class GraphedDQNLearner:
     @property
     def h2d_bytes(self):
         return self.h_pack.numel()
+
+
+class GraphedNStepLearner(_NatureLearner):
+    """The update of ``NStepDQNAgent.step()`` (NStepDQN_agent.py:52-67) for a VanillaNet on a wgmma NatureConvBody as ONE
+    captured graph per rollout: the rollout's actions / rewards / masks up in one packed copy and the final states' stacks up
+    into the arena, the online body at batch T N on the rollout's stacks beside the target body at batch N on the final ones
+    (two branches), both heads (``b2rl_head_fwd``), the n-step target and loss (``b2rl_nstep_q_loss``), the head backward
+    with fc4's ReLU (``b2rl_head_bwd_relu``), the fused body backward and the two-launch update tail (gradient reduce,
+    ``clip_grad_norm_``, RMSprop / Adam, bf16 operand writes).
+
+    ``arena`` holds the rollout's uint8 frame stacks: slot t (rows t N 4 .. (t + 1) N 4 - 1) the states of env step t, which
+    the actor's upload writes there (component/actor.py ``GraphedQActor(arena=...)``), slot T the final states, plus one
+    padding row.  Conv1's forward and weight gradient read the stacks from it (K1: ``RingFrames`` with ``idx[i] = 4 i``); no
+    bf16 batch is built.  The online q of the rollout is recomputed rather than kept from the actor: the parameters do not
+    change during a rollout, so it is the q the actor saw.
+
+    The target sync (NStepDQN_agent.py:48-49) is the caller's ``sync_target()`` before ``update()``: the online parameters do
+    not change inside a rollout, so syncing at its end gives the same target."""
+
+    def __init__(self, network, target_network, optimizer, rollout_length, num_envs, discount=0.99, gradient_clip=5.0,
+                 state_scale=1.0 / 255, history=4, frame_hw=(84, 84)):
+        self.net, self.tgt, self.opt = network, target_network, optimizer
+        self.T, self.N, self.hl = int(rollout_length), int(num_envs), int(history)
+        self.discount, self.clip, self.scale = float(discount), float(gradient_clip or 0.0), float(state_scale)
+        self.dtype, self.world = torch.bfloat16, 1
+        self.dev = dev = optimizer.flat.device
+        self._plan, self._tail, self._side = None, None, None
+        if not self.plan.tail:
+            raise _lib.B2RLError("GraphedNStepLearner needs the fused update tail: a wgmma NatureConvBody with the fused "
+                                 "backward epilogues, and RMSprop or Adam")
+        T, N, hl = self.T, self.N, self.hl
+        row = frame_hw[0] * frame_hw[1]
+        k = N * hl
+        self.arena = torch.zeros(((T + 1) * k + 1, row), dtype=torch.uint8, device=dev)
+        idx = torch.arange((T + 1) * N, dtype=torch.int64, device=dev) * hl
+        self.states = nature_tc.RingFrames(self.arena, idx[:T * N], 0, row, frame_hw[1], hl)
+        self.final = nature_tc.RingFrames(self.arena, idx[T * N:], 0, row, frame_hw[1], hl)
+        self.h_final = torch.zeros((k, row), dtype=torch.uint8, pin_memory=True)
+        self._np_final = self.h_final.numpy().reshape(N, hl, row)
+        # ONE packed pinned staging buffer for the rollout's scalars and ONE device mirror -> a single host->device copy node:
+        # [action int64 T*N | reward float32 T*N | mask float32 T*N]
+        rows = T * N
+        self.h_pack = torch.zeros(16 * rows, dtype=torch.uint8, pin_memory=True)
+        self.d_pack = torch.zeros(16 * rows, dtype=torch.uint8, device=dev)
+
+        def views(buf):
+            return (buf[:8 * rows].view(torch.int64).view(T, N), buf[8 * rows:12 * rows].view(torch.float32).view(T, N),
+                    buf[12 * rows:].view(torch.float32).view(T, N))
+
+        self.h_action, self.h_reward, self.h_mask = views(self.h_pack)
+        self.d_action, self.d_reward, self.d_mask = views(self.d_pack)
+        A = network.fc_head.out_features
+        self.out = dict(ret=torch.zeros(rows, dtype=torch.float32, device=dev),
+                        delta=torch.zeros(rows, dtype=torch.float32, device=dev),
+                        loss=torch.zeros(1, dtype=torch.float32, device=dev),
+                        gq=torch.zeros((rows, A), dtype=torch.float32, device=dev))
+        self.loss = self.out["loss"]
+        self.q = None                     # the online q of the last update [T*N, A] (a buffer of the captured graph)
+        self.graph = None
+        self.updates = 0
+        self.opt.zero_grad()              # the fused tail writes / re-zeroes the gradient arena itself: start from zeros
+
+    def _resolve_plan(self):
+        tail = (hasattr(getattr(self.net, "body", None), "repack") and nature_tc.FUSED_BWD and bool(_lib.CONV_SLAB)
+                and self.opt.kind in ("rmsprop", "adam"))
+        return UpdatePlan(ring=True, tail=tail, repack_online=not tail, dist_head=False, head="separate", forward="two-branch",
+                          conv1="separate", single_stream=False, prefetch=None, join=None, one_graph=True)
+
+    def stage_final(self, states):
+        """The final states' frame stacks (uint8 [history, H, W] each) into the pinned buffer the update uploads to slot T."""
+        for i, s in enumerate(states):
+            self._np_final[i] = np.asarray(s).reshape(self.hl, -1)
+
+    def _main(self):
+        cur = torch.cuda.current_stream()
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.dev)
+        side, tail = self._side, self.tail()
+        k = self.N * self.hl
+        self.arena[self.T * k:(self.T + 1) * k].copy_(self.h_final, non_blocking=True)
+        self.d_pack.copy_(self.h_pack, non_blocking=True)
+        # the target forward on the final states and the online forward on the rollout's states: two parallel branches
+        side.wait_stream(cur)
+        with torch.cuda.stream(side), frame_scale(self.scale), torch.no_grad():
+            q_boot = self.tgt(self.final)["q"]
+        with frame_scale(self.scale):
+            q = self.net(self.states)["q"]
+        cur.wait_stream(side)
+        r = ops.nstep_q_loss(q.detach(), q_boot, self.d_action, self.d_reward, self.d_mask, self.discount, out=self.out)
+        with nature_tc.wgrad_stream(side), nature_tc.grad_sink(tail):     # weight-gradient GEMMs on the side branch
+            q.backward(r["gq"])
+        self.q = q.detach()
+
+    def _opt(self):
+        self.tail().step(max_norm=self.clip)
+
+    def _state(self):
+        o = self.opt
+        return [o.flat, o.s1, o.s2, o.step_dev]
+
+    def capture(self, warmup=1):
+        """Warm up eagerly on a side stream (lazy allocations, kernel attributes), then capture.  The warm-up updates are
+        undone: parameters and optimizer state are restored and the online operands re-packed from them."""
+        saved = [t.clone() for t in self._state()]
+        self.refresh_packed()
+        s = torch.cuda.Stream(device=self.dev)
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            for _ in range(warmup):
+                self._main()
+                self._opt()
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self._main()
+            self._opt()
+        for t, v in zip(self._state(), saved):
+            t.copy_(v)
+        self.opt.grad.zero_()
+        self.refresh_packed()
+        torch.cuda.synchronize()
+        return self
+
+    def update(self, sync_target=False):
+        """One rollout's update (graph replay) on what the caller staged: ``h_action`` / ``h_reward`` / ``h_mask`` [T, N],
+        the rollout's stacks in arena slots 0..T-1 and the final states (``stage_final``).  ``sync_target``: an env step of
+        the rollout reached the target sync schedule; the target becomes the online network first.  Returns the device loss
+        tensor (no sync)."""
+        if sync_target:
+            self.sync_target()
+        self.graph.replay()
+        self.updates += 1
+        return self.loss
 
 
 class _PPOLearner:

@@ -97,6 +97,29 @@ def dqn_head_fused(phi, phi_t, phi_o, head, head_t, action, reward, mask, gamma_
     return dict(gphi=gphi, delta=delta, priority=prio, loss=loss, q=q)
 
 
+def nstep_q_loss(q, q_boot, action, reward, mask, discount, out=None):
+    """NStepDQN_agent.py:56-63 in one launch (``b2rl_nstep_q_loss``): ``q`` [T*N, A] of the rollout's states (rows t-major),
+    ``q_boot`` [N, A] of the final states (target network), ``action`` / ``reward`` / ``mask`` [T*N] or [T, N].  Returns
+    dict(ret, delta [T*N], loss [1], gq [T*N, A] = dloss/dq).  ``out``: a dict of preallocated outputs to write instead
+    (persistent buffers of a captured graph)."""
+    q, qb = _c(q, _f32), _c(q_boot, _f32)
+    rows, A = q.shape
+    N = qb.shape[0]
+    if rows % N or qb.shape[1] != A:
+        raise _lib.B2RLError("nstep_q_loss: q has %d rows of %d actions, q_boot %s" % (rows, A, tuple(qb.shape)))
+    dev = q.device
+    o = out if out is not None else {}
+    e = lambda k, *shape: o[k] if k in o else torch.empty(shape, dtype=_f32, device=dev)
+    r = dict(ret=e("ret", rows), delta=e("delta", rows), loss=e("loss", 1), gq=e("gq", rows, A))
+    ctas = int(_lib.lib().b2rl_nstep_q_loss_ctas(N))
+    partial = _Scratch.get(dev, "nstep_q_partial", max(ctas, 1), _f32)
+    counter = _Scratch.get(dev, "nstep_q_counter", 1, torch.int32)
+    _lib.call("b2rl_nstep_q_loss", _lib.ptr(q), _lib.ptr(qb), _lib.ptr(_c(action, torch.int64)), _lib.ptr(_c(reward, _f32)),
+              _lib.ptr(_c(mask, _f32)), float(discount), rows // N, N, A, _lib.ptr(r["ret"]), _lib.ptr(r["delta"]),
+              _lib.ptr(r["loss"]), _lib.ptr(r["gq"]), _lib.ptr(partial), _lib.ptr(counter), _lib.stream())
+    return r
+
+
 class _DQNDelta(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, q_next_target, q_next_online, action, reward, mask, gamma_n):

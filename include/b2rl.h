@@ -138,6 +138,18 @@ int b2rl_dqn_loss(const float* q, const float* q_next_target, const float* q_nex
                   float* delta_out, float* priority_out, float* loss_out, float* dq_out,
                   const float* beta_dev /* optional device scalar overriding beta (CUDA-graph replays) */, void* stream);
 
+/* NStepDQNAgent's target and loss (NStepDQN_agent.py:56-63) in one launch, for a rollout of T env steps x N workers with
+ * rows t-major (row i = t*N + n): q [T*N][A] (online, s_0..s_{T-1}), q_boot [N][A] (target, s_T), action [T*N] int64 in
+ * [0, A), reward / mask [T*N].  ret_t = r_t + discount*m_t*ret_{t+1} from ret_T = max_a q_boot; delta = ret - q[a];
+ * loss_out[0] = 0.5*mean(delta^2); gq_out [T*N][A] = dloss/dq (-delta/(T*N) at the taken action, 0 elsewhere).  ret_out,
+ * delta_out [T*N], loss_out and gq_out may each be NULL.  Limits: T >= 1, N >= 1, 1 <= A <= 32, T*N <= 2^24.  partial:
+ * float [b2rl_nstep_q_loss_ctas(N)] scratch; counter: int32, zero-initialised once (the kernel re-arms it).  The loss is
+ * reduced in a fixed order: the same inputs give the same bits. */
+int b2rl_nstep_q_loss_ctas(int32_t N);
+int b2rl_nstep_q_loss(const float* q, const float* q_boot, const int64_t* action, const float* reward, const float* mask,
+                      float discount, int32_t T, int32_t N, int32_t A, float* ret_out, float* delta_out, float* loss_out,
+                      float* gq_out, float* partial, int32_t* counter, void* stream);
+
 /* CategoricalDQNAgent.compute_loss + reduce_loss (CategoricalDQN_agent.py:60-89).  log_prob [B][A][N] (online, s),
  * prob_next_target / prob_next_online [B][A][N] (online NULL -> not double).  kl_out [B], loss_out [1] = mean,
  * dlogp_out [B][A][N] = dLoss/dlog_prob.  target_prob_out [B][N] optional (NULL to skip). */

@@ -4,8 +4,11 @@ device flag (one actor-step launch per env step, one update launch per rollout o
 (n_step_dqn_feature), ``config.device_dqn`` for DQNAgent (dqn_feature, timed past its exploration steps), ``config.device_c51``
 / ``config.device_qr`` for CategoricalDQNAgent / QuantileRegressionDQNAgent (categorical_dqn_feature,
 quantile_regression_dqn_feature: csrc/dist_dqn.cu, with the launchers' async actor), ``config.device_rainbow`` for
-CategoricalDQNAgent on a noisy RainbowNet (rainbow_feature: csrc/rainbow.cu) -- in one process on one card, the two
-alternated round by round.  Also times the host envs alone (``task.step`` with fixed actions), so the share
+CategoricalDQNAgent on a noisy RainbowNet (rainbow_feature: csrc/rainbow.cu), ``config.cuda_graph`` for NStepDQNAgent on the
+NatureConvBody (n_step_dqn_pixel on SyntheticAtari-v0: one GraphedQActor replay per env step, one GraphedNStepLearner replay per
+rollout; both it and the eager side at bf16, plus the launcher's default fp32 eager side) -- in one process on one card, the
+sides alternated round by round.  For n_step_dqn_pixel the captured update alone is also timed: CUDA events around back-to-back
+replays of its graph.  Also times the host envs alone (``task.step`` with fixed actions), so the share
 left to the learner is visible.  Prints the card's name and power limit with the numbers.
 
     python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--only LAUNCHER[,LAUNCHER]] [--out DIR]
@@ -33,7 +36,10 @@ CONFIGS = [("a2c_feature", "CartPole-v0", "device_a2c", "a2c"), ("a2c_continuous
            ("dqn_feature", "CartPole-v0", "device_dqn", "dqn"),
            ("categorical_dqn_feature", "CartPole-v0", "device_c51", "c51"),
            ("quantile_regression_dqn_feature", "CartPole-v0", "device_qr", "qr"),
-           ("rainbow_feature", "CartPole-v0", "device_rainbow", "rainbow")]
+           ("rainbow_feature", "CartPole-v0", "device_rainbow", "rainbow"),
+           ("n_step_dqn_pixel", "SyntheticAtari-v0", "cuda_graph", "nstep_dqn")]
+# launchers timed at a given Config.COMPUTE_DTYPE per side (set around every step of that side): side -> dtype
+DTYPES = {"n_step_dqn_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32}}
 
 
 def card():
@@ -57,13 +63,35 @@ def make_agent(name, game, flag, on):
     return got[0]
 
 
-def timed(agent, steps):
+def timed(agent, steps, dtype=None):
+    from deeprl_b200 import Config
+    old = Config.COMPUTE_DTYPE
+    Config.COMPUTE_DTYPE = dtype or old
+    try:
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for _ in range(steps):
+            agent.step()
+        torch.cuda.synchronize()
+        return steps / (time.perf_counter() - t0)
+    finally:
+        Config.COMPUTE_DTYPE = old
+
+
+def update_replay_ms(agent, replays=400):
+    """The captured n-step update alone: CUDA events around ``replays`` back-to-back replays of its graph (on the rollout
+    staged last), milliseconds per replay."""
+    g = agent._graph[0].graph
+    for _ in range(20):
+        g.replay()
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        agent.step()
+    start.record()
+    for _ in range(replays):
+        g.replay()
+    end.record()
     torch.cuda.synchronize()
-    return steps / (time.perf_counter() - t0)
+    return start.elapsed_time(end) / replays
 
 
 def env_steps(agent):
@@ -122,32 +150,42 @@ def main():
     for name, game, flag, unit in CONFIGS:
         if only is not None and name not in only:
             continue
+        dtypes = DTYPES.get(name, {})
         agents = {"eager": make_agent(name, game, flag, False), flag: make_agent(name, game, flag, True)}
+        if "eager_fp32" in dtypes:
+            agents["eager_fp32"] = make_agent(name, game, flag, False)
         failed = {}
         for k, ag in agents.items():
             try:
                 past_exploration(ag)
-                timed(ag, args.warmup)
+                timed(ag, args.warmup, dtypes.get(k))
             except RuntimeError as e:
                 failed[k] = "%s: %s" % (type(e).__name__, str(e).split(". Hint")[0])
         timed_agents = {k: ag for k, ag in agents.items() if k not in failed}
         rates = {k: [] for k in timed_agents}
-        for _ in range(args.rounds):                        # alternated: both see the same host / card conditions
+        for _ in range(args.rounds):                        # alternated: all see the same host / card conditions
             for k, ag in timed_agents.items():
-                rates[k].append(timed(ag, args.steps))
+                rates[k].append(timed(ag, args.steps, dtypes.get(k)))
         env = env_only(agents[flag], args.steps)
         c = agents[flag].config
         med = {k: float(np.median(v)) for k, v in rates.items()}
         learner_ms = {k: 1e3 / med[k] - 1e3 / env for k in med}
         row = {"game": game, "num_workers": c.num_workers, "env_steps_per_agent_step": env_steps(agents[flag]), unit + "_steps_per_s": rates,
-               "median_%s_steps_per_s" % unit: med, "speedup": med[flag] / med["eager"] if len(med) == 2 else None,
+               "median_%s_steps_per_s" % unit: med,
+               "speedup": med[flag] / med["eager"] if flag in med and "eager" in med else None,
                "env_only_%s_steps_per_s" % unit: env, "ms_per_step_besides_envs": learner_ms, "failed": failed}
+        if dtypes:
+            row["compute_dtype"] = {k: str(v) for k, v in dtypes.items()}
+        if flag == "cuda_graph" and flag in timed_agents:
+            row["update_replay_ms"] = update_replay_ms(agents[flag])
         result["configs"][name] = row
         print("%-18s %-20s N=%d env steps %d  %s;  envs alone %8.1f steps/s;  ms per step besides the envs: %s%s"
               % (name, game, c.num_workers, env_steps(agents[flag]),
                  "  ".join("%s %8.1f steps/s" % kv for kv in med.items()) + ("  (x%.2f)" % row["speedup"] if row["speedup"] else ""),
                  env, ", ".join("%s %.3f" % kv for kv in learner_ms.items()),
                  "".join(";  %s not timed (%s)" % kv for kv in failed.items())))
+        if "update_replay_ms" in row:
+            print("%-18s captured update alone: %.3f ms per replay" % (name, row["update_replay_ms"]))
         for ag in agents.values():
             ag.close()
     print(json.dumps(result))
