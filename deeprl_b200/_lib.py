@@ -48,6 +48,8 @@ SIGNATURES = {
     "b2rl_bias_act_bf16": [c_p, c_p, c_i64, c_i32, c_i32, c_p],
     "b2rl_bias_act_f32_to_bf16": [c_p, c_p, c_p, c_i64, c_i32, c_i32, c_p],
     "b2rl_act_bwd_bias_grad_bf16": [c_p, c_p, c_i64, c_i32, c_i32, c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p],
+    "b2rl_set_cta_budget": [c_i32],
+    "b2rl_last_grid_ctas": [c_p],
     "b2rl_conv_gemm_bf16": [c_i32, c_p, c_i64, c_i32, c_p, c_i32, c_i32, c_i32, c_i32, c_i32, c_p, c_i64, c_p, c_i32, c_i32,
                             c_i32, c_i32, c_i32, c_i32, c_i32, c_p],
     "b2rl_conv_gemm_dual_bf16": [c_p, c_p, c_i64, c_i32, c_p, c_p, c_i32, c_i32, c_i32, c_i32, c_i32, c_p, c_p, c_i64, c_p, c_p,

@@ -1572,6 +1572,13 @@ static int sm_count() {
   return n;
 }
 
+// CTA budget (b2rl_set_cta_budget): while set, the slab, dense and convolution weight-gradient launchers size their grids to
+// at most this many CTAs instead of one per SM, so that two kernels on parallel graph branches can hold disjoint SMs.
+// 0: every SM.  g_last_ctas: the CTAs of the last such launch (all its kernels), read by b2rl_last_grid_ctas.
+static int g_cta_budget = 0;
+static int g_last_ctas = 0;
+static int grid_cap() { return g_cta_budget > 0 && g_cta_budget < sm_count() ? g_cta_budget : sm_count(); }
+
 // shared memory one CTA may use, static + dynamic (227 KB on sm_90)
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 
@@ -1717,12 +1724,13 @@ static int launch_dense_t(const CUtensorMap& ta, const CUtensorMap& tb, GemmPara
   const int tiles = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + BN - 1) / BN);
   const int kt_total = (p.K + GEMM_BK - 1) / GEMM_BK;
   int S = 1;
-  if (splits == 1) {
+  if (splits == 1 && !g_cta_budget) {                                // a CTA budget launches without clusters
     S = cluster > 0 ? cluster : auto_cluster(tiles, kt_total, cap);
     while (S > 1 && cap[S] <= 0) S >>= 1;
   }
-  int ctas = S > 1 ? tiles * S : (tiles < sm_count() / splits ? tiles : sm_count() / splits);
+  int ctas = S > 1 ? tiles * S : (tiles < grid_cap() / splits ? tiles : grid_cap() / splits);
   if (ctas < 1) ctas = 1;
+  g_last_ctas = ctas * splits;
   if (S > 1) p.k_tiles_per_split = (kt_total + S - 1) / S;   // rank r: k-tiles [r kps, (r + 1) kps); trailing ranks may get none
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(ctas, 1, splits);
@@ -1826,8 +1834,10 @@ static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     attr = smem;
   }
-  int ctas = sp.g.dual ? sm_count() / 2 : sm_count();                 // per operand set
+  int ctas = sp.g.dual ? grid_cap() / 2 : grid_cap();                 // per operand set
   if (ctas > tiles) ctas = tiles;
+  if (ctas < 1) ctas = 1;
+  g_last_ctas = sp.g.dual ? 2 * ctas : ctas;
   launch_pdl(k, dim3(sp.g.dual ? 2 * ctas : ctas), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, ta, tb, ta2, tb2, sp);
   return check_launch("b2rl_conv_gemm_bf16(slab)");
 }
@@ -1900,9 +1910,9 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   w.n_runs = w.ntaps;
   const int groups = (w.ntaps * w.C + 127) / 128;
   const int kt_total = (w.rows + GEMM_BK - 1) / GEMM_BK;
-  // split-K over the SMs (groups x ctas CTAs); every CTA stores (or reduces) its n_out x 128 partial block
+  // split-K over the SMs or the CTA budget (groups x ctas CTAs); every CTA stores (or reduces) its n_out x 128 partial block
   int ctas = kt_total / 4;
-  if (ctas > sm_count() / groups) ctas = sm_count() / groups;
+  if (ctas > grid_cap() / groups) ctas = grid_cap() / groups;
   static int cap = -1;                                               // tunable: B2RL_WGRAD_CTAS caps the split-K width
   if (cap < 0) {
     const char* e = getenv("B2RL_WGRAD_CTAS");
@@ -1913,6 +1923,7 @@ static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParam
   w.k_tiles_per_cta = (kt_total + ctas - 1) / ctas;
   ctas = (kt_total + w.k_tiles_per_cta - 1) / w.k_tiles_per_cta;
   if (n_ctas) *n_ctas = ctas;
+  g_last_ctas = ctas * groups;
   w.win0 = 0;
   if (w.C == 128) {
     launch_wgrad_k<WGRAD_N128>(tg, tx, w, ctas, groups, smem, st);
@@ -1982,6 +1993,18 @@ extern "C" int b2rl_conv1_set_phase_clocks(int64_t* clocks) {
   return B2RL_OK;
 }
 extern "C" void b2rl_set_conv_slab(int32_t on) { g_use_slab = on; }
+
+extern "C" int b2rl_set_cta_budget(int32_t ctas) {
+  B2RL_REQUIRE(ctas >= 0, "the CTA budget is a CTA count (0: every SM)");
+  g_cta_budget = ctas;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_last_grid_ctas(int32_t* ctas) {
+  B2RL_REQUIRE(ctas, "null pointer");
+  *ctas = g_last_ctas;
+  return B2RL_OK;
+}
 
 static int check_common(const void* A, const void* B, const void* D, int64_t lda, int64_t ldb, int M, int N, int K,
                         int out_mode, int splits, int block_n, int b_mn, int relu) {

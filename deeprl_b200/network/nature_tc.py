@@ -168,7 +168,9 @@ def _backward_fused(ctx, gy4):
     else:
         g4, db4 = act_bwd_bias_grad(gy4, y4, True)                                      # fc4's own ReLU / bias gradient
     y3c = y3.view(B, 3136)
-    gw4p = gemm_bf16(g4, y3c, a_major="mn", b_major="mn", out_dtype=_f32, block_n=128, stream=_fork())
+    main, side = _budgets(dev)                                  # CTAs of the dgrad chain and of the weight gradients beside it
+    with _cta_budget(side):
+        gw4p = gemm_bf16(g4, y3c, a_major="mn", b_major="mn", out_dtype=_f32, block_n=128, stream=_fork())
     mark("w_fc4", _WGRAD["stream"])
     if sink is not None and sink.split:
         # multi-GPU: fc4's gradient (95 % of the bytes) goes to the arena NOW, and its all-reduce (sink.early) runs beside the
@@ -188,24 +190,29 @@ def _backward_fused(ctx, gy4):
     # fc4 dgrad -> conv3's output grid (10 x 10 per image), masked by relu(conv3) and summed into db3
     g3 = _zero_grid("g3", (B * 100, 64), dev)
     e3 = _lib.bwd_epilogue(y3c, db3, 64, 64)
-    _lib.call("b2rl_gemm_bwd_bf16", _lib.ptr(g4), g4.stride(0), _lib.ptr(w4p), 1, w4p.stride(0), _lib.ptr(g3), 64, B, 3136,
-              g4.shape[1], 4, 10, 7, ctypes.byref(e3), 128, _lib.stream())
+    with _cta_budget(main):
+        _lib.call("b2rl_gemm_bwd_bf16", _lib.ptr(g4), g4.stride(0), _lib.ptr(w4p), 1, w4p.stride(0), _lib.ptr(g3), 64, B, 3136,
+                  g4.shape[1], 4, 10, 7, ctypes.byref(e3), 128, _lib.stream())
     mark("d_fc4")
-    gw3p, p3 = wgrad_partials(y2, g3, 64, 9, 3, 10, stream=_fork())
+    with _cta_budget(side):
+        gw3p, p3 = wgrad_partials(y2, g3, 64, 9, 3, 10, stream=_fork())
     mark("w_conv3", _WGRAD["stream"])
     # conv3 dgrad on the 10-grid, masked by relu(conv2)
     g2 = torch.empty((B * 100, 64), dtype=_bf16, device=dev)
     e2 = _lib.bwd_epilogue(y2, db2, 64, 0)
-    _lib.call("b2rl_conv_gemm_bwd_bf16", _lib.ptr(g3), B * 100, 64, _lib.ptr(w3d), 64, 9, 3, 10, _lib.ptr(g2), 64, 0, 0, 0,
-              ctypes.byref(e2), 64, _lib.stream())
+    with _cta_budget(main):
+        _lib.call("b2rl_conv_gemm_bwd_bf16", _lib.ptr(g3), B * 100, 64, _lib.ptr(w3d), 64, 9, 3, 10, _lib.ptr(g2), 64, 0, 0, 0,
+                  ctypes.byref(e2), 64, _lib.stream())
     mark("d_conv3")
-    gw2p, p2 = wgrad_partials(x1, g2, 64, 4, 2, 10, stream=_fork())
+    with _cta_budget(side):
+        gw2p, p2 = wgrad_partials(x1, g2, 64, 4, 2, 10, stream=_fork())
     mark("w_conv2", _WGRAD["stream"])
     # conv2 dgrad: space-to-depth(2) rows -> conv1's 21-grid, masked by relu(conv1)
     g1 = _zero_grid("g1", (B * 441, 32), dev)
     e1 = _lib.bwd_epilogue(x1, db1, 32, 32)
-    _lib.call("b2rl_conv_gemm_bwd_bf16", _lib.ptr(g2), B * 100, 64, _lib.ptr(w2d), 128, 4, 2, 10, _lib.ptr(g1), 32, 3, 21, 20,
-              ctypes.byref(e1), 128, _lib.stream())
+    with _cta_budget(main):
+        _lib.call("b2rl_conv_gemm_bwd_bf16", _lib.ptr(g2), B * 100, 64, _lib.ptr(w2d), 128, 4, 2, 10, _lib.ptr(g1), 32, 3, 21,
+                  20, ctypes.byref(e1), 128, _lib.stream())
     mark("d_conv2")
     if AFTER_DGRAD is not None:
         AFTER_DGRAD()
@@ -220,20 +227,55 @@ def _backward_fused(ctx, gy4):
     return (gw1p, p1, gw2p, p2, gw3p, p3, gw4p), (db1, db2, db3, db4)
 
 
-_WGRAD = {"stream": None}
+_WGRAD = {"stream": None, "ctas": 0}
+# CTAs the weight gradients of fc4, conv3 and conv2 hold on the side branch; the dgrad chain gets the other SMs.  Each of these
+# kernels takes a whole SM, so with full grids on both branches the block scheduler interleaves them and the dgrads on the
+# critical path wait for side CTAs to retire.  32 leaves 100 CTAs of the 132 SMs of an H100 SXM: fc4's dgrad is 100 tiles,
+# and the 400-tile convolution dgrads take 4 tiles per CTA on 100 CTAs, as their slowest CTAs already do on 132, so they
+# are as fast alone as on full grids; fewer side CTAs leave the weight gradients too slow to finish beside the chain
+# (scripts/bwd_sm_budget.py, DESIGN section 7).
+SIDE_CTAS = 32
 
 
 @contextlib.contextmanager
-def wgrad_stream(stream):
+def wgrad_stream(stream, side_ctas=None):
     """Inside this context the backward pass launches its weight-gradient GEMMs on ``stream`` (a second branch of the
     captured graph): they only feed the final gradient unpack, so they overlap the dgrad / ReLU-mask chain, which is
     latency-bound with one CTA per SM.  Buffers are allocated on the current stream and the branch is joined before
-    ``backward`` returns, so no allocator bookkeeping is needed."""
-    old, _WGRAD["stream"] = _WGRAD["stream"], stream
+    ``backward`` returns, so no allocator bookkeeping is needed.  With a side stream, the weight gradients of fc4, conv3 and
+    conv2 run on ``side_ctas`` CTAs (default ``SIDE_CTAS``; 0: full grids) and the dgrads beside them on the remaining
+    SMs (``b2rl_set_cta_budget``); conv1's weight gradient, which has nothing beside it, keeps its grid."""
+    old = dict(_WGRAD)
+    _WGRAD["stream"] = stream
+    _WGRAD["ctas"] = 0 if stream is None else (SIDE_CTAS if side_ctas is None else int(side_ctas))
     try:
         yield
     finally:
-        _WGRAD["stream"] = old
+        _WGRAD.update(old)
+
+
+@contextlib.contextmanager
+def _cta_budget(ctas):
+    """Launches inside this context size their grids to at most ``ctas`` CTAs (0: the whole device)."""
+    if not ctas:
+        yield
+        return
+    _lib.call("b2rl_set_cta_budget", int(ctas))
+    try:
+        yield
+    finally:
+        _lib.call("b2rl_set_cta_budget", 0)
+
+
+def _budgets(device):
+    """(dgrad chain, side branch) CTA budgets of the backward pass: (0, 0) without a side-branch budget."""
+    side = _WGRAD["ctas"]
+    if not side:
+        return 0, 0
+    sms = torch.cuda.get_device_properties(device).multi_processor_count
+    if not 0 < side < sms:
+        raise ValueError("side_ctas must leave SMs for the dgrad chain: 0 < %d < %d" % (side, sms))
+    return sms - side, side
 
 
 def _fork():

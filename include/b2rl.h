@@ -253,6 +253,15 @@ int b2rl_gemm_bf16(const uint16_t* A, int32_t a_mn, int64_t lda, const uint16_t*
  *   D fp32 [n_out][taps*C] (out_mode 2, atomic accumulation over `splits` K slices). */
 /* forward / dgrad calls use the slab kernel (one activation slab per tile, resident weights) unless switched off */
 void b2rl_set_conv_slab(int32_t on);
+/* CTA budget of the following launches of the slab convolution kernel (forward / dgrad), the plain GEMM (b2rl_gemm_bf16,
+ * b2rl_gemm_bwd_bf16, b2rl_gemm_splitk_bf16) and the convolution weight gradient (b2rl_conv_wgrad_partials): each sizes its
+ * grid to at most `ctas` CTAs (the persistent kernels loop over more tiles per CTA, the weight gradient writes fewer split-K
+ * partials, the plain GEMM launches without clusters; a weight gradient keeps at least one CTA per 128-column group) instead
+ * of up to one per SM, so that kernels on two parallel graph branches hold disjoint SMs.  0 (the default): up to one CTA per
+ * SM.  The setting is read on the host at launch time; per-tile arithmetic does not depend on it.
+ * b2rl_last_grid_ctas: the CTAs of the last launch of those launchers (summed over the kernels of one call). */
+int b2rl_set_cta_budget(int32_t ctas);
+int b2rl_last_grid_ctas(int32_t* ctas);
 int b2rl_conv_gemm_bf16(int32_t mode, const uint16_t* X, int64_t rows, int32_t C, const uint16_t* W_or_G, int32_t n_out,
                         int32_t taps, int32_t taps_x, int32_t grid_w, int32_t shift_sign, void* D, int64_t ldd,
                         const float* bias, int32_t relu, int32_t out_mode, int32_t out_map, int32_t G, int32_t V,
