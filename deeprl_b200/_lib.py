@@ -45,6 +45,9 @@ SIGNATURES = {
     "b2rl_normalize_advantage": [c_p, c_i32, c_p],
     "b2rl_ppo_loss": [c_p, c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_p, c_p, c_p, c_p, c_p],
     "b2rl_a2c_loss": [c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_p, c_p, c_p, c_p, c_p],
+    "b2rl_a2c_rollout_loss_ctas": [c_i32],
+    "b2rl_a2c_rollout_loss": [c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_f32, c_f32, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p,
+                              c_p, c_p],
     "b2rl_bias_act_bf16": [c_p, c_p, c_i64, c_i32, c_i32, c_p],
     "b2rl_bias_act_f32_to_bf16": [c_p, c_p, c_p, c_i64, c_i32, c_i32, c_p],
     "b2rl_act_bwd_bias_grad_bf16": [c_p, c_p, c_i64, c_i32, c_i32, c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p],
@@ -73,6 +76,8 @@ SIGNATURES = {
     "b2rl_head_fwd": [c_p, c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_p],
     "b2rl_head_bwd": [c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p, c_p],
     "b2rl_head_bwd_relu": [c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
+    "b2rl_ac_head_fwd": [c_p, c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_u64, c_p, c_p, c_p, c_p],
+    "b2rl_head_bwd_geff_relu": [c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     "b2rl_nature_grad_reduce": [c_p, c_i32, c_p, c_i32, c_p, c_i32, c_p, c_i32, c_p, c_p, c_p, c_p, c_p, c_i32, c_i32, c_f32, c_p,
                                 c_p, c_p, c_p, c_f32, c_f32, c_p],
     "b2rl_nature_fused_opt": [c_p, c_i32, c_p, c_p, c_p, c_p, c_i32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_p, c_i32, c_p,

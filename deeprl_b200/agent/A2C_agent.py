@@ -10,6 +10,16 @@ statements run as torch expressions, which is the reference's own path, not a fa
 ``b2rl_a2c_actor_step`` launch per env step and one ``b2rl_a2c_update`` launch per rollout (csrc/a2c.cu, component/actor.py
 ``DeviceA2C``).  The actions are then drawn from the device's Philox stream, not from torch's generator.  Configurations the
 kernels do not cover raise ``NotImplementedError`` naming the unmet condition.
+
+``config.cuda_graph = True`` (off by default) runs each ``step()`` of a CategoricalActorCriticNet on a wgmma NatureConvBody at
+bf16 (``a2c_pixel`` with ``Config.COMPUTE_DTYPE = torch.bfloat16``) as captured graphs: one ``GraphedQActor`` replay per env
+step (pinned upload of the frame stacks into the rollout arena, the body, the actor-critic head with the action drawn on the
+device, the actions down to the host) and one ``GraphedA2CLearner`` replay per rollout (learner.py).  The actions then come
+from the device's Philox stream (keyed from torch's seeded generator, as with ``config.device_a2c``), not from torch's
+``Categorical.sample``.  The torch optimizer is replaced by a ``FlatOptimizer`` with its hyper-parameters; the network's
+parameters become views into its arena, so ``state_dict()`` is always current.  Configurations it does not cover
+(``component/actor.py a2c_graph_unsupported``; the reason is kept in ``graph_refusal``) keep the eager path;
+``config.device_a2c`` takes precedence.
 """
 import numpy as np
 import torch
@@ -61,6 +71,8 @@ class A2CAgent(BaseAgent):
         self.total_steps = 0
         self.states = self.task.reset()
         self.last_loss = None
+        self._graph = None                                  # (GraphedA2CLearner, GraphedQActor), False: eager; decided once
+        self.graph_refusal = None
         self.device_a2c = None
         if getattr(config, "device_a2c", False):
             from ..component.actor import DeviceA2C
@@ -73,9 +85,16 @@ class A2CAgent(BaseAgent):
             prediction = self.network(self.config.state_normalizer(np.asarray([np.asarray(s) for s in state])))
         return to_np(prediction["action"])
 
+    def load(self, filename):
+        BaseAgent.load(self, filename)
+        if self._graph:
+            self._graph[0].refresh_packed()                # the next step trains (and acts) from the loaded weights
+
     def step(self):
         if self.device_a2c is not None:
             return self._step_device()
+        if self._graph_ok():
+            return self._step_graph()
         config = self.config
         storage = Storage(config.rollout_length)
         states = self.states
@@ -130,3 +149,44 @@ class A2CAgent(BaseAgent):
             self.total_steps += config.num_workers
         self.states = states
         self.last_loss = dev.update(config.state_normalizer(np.asarray([np.asarray(s) for s in states])))
+
+    # ------------------------------------------------------------------ config.cuda_graph (opt-in)
+    def _graph_ok(self):
+        """Decided on the first step: the captured actor + update serve this configuration (``a2c_graph_unsupported``), or the
+        eager path runs (the reason is kept in ``graph_refusal``)."""
+        if self._graph is None:
+            from ..component.actor import GraphedQActor, a2c_graph_unsupported
+            from ..learner import GraphedA2CLearner
+            config = self.config
+            self.graph_refusal = a2c_graph_unsupported(config, self.network, self.optimizer, self.states)
+            self._graph = False
+            if self.graph_refusal is None:
+                self.optimizer = ops.FlatOptimizer.from_torch(self.optimizer, list(self.network.parameters()))
+                seed = int(torch.randint(0, 2 ** 62, (1,)).item())      # the Philox key, from torch's (seeded) generator
+                coef = config.state_normalizer.coef
+                lr = GraphedA2CLearner(self.network, self.optimizer, config.rollout_length, config.num_workers, seed,
+                                       config.discount, config.gae_tau, config.use_gae, config.entropy_weight,
+                                       config.value_loss_weight, config.gradient_clip, coef).capture()
+                actor = GraphedQActor(self.network, None, config.num_workers, 4, (84, 84), coef, arena=lr.arena, run=lr.act,
+                                      body=self.network.phi_body)
+                self._graph = (lr, actor)
+        return bool(self._graph)
+
+    def _step_graph(self):
+        """``step()`` with ``config.cuda_graph``: T actor replays (the action drawn on the device into the learner's action row
+        t; its pinned download is the step's only synchronisation), each followed by ``task.step`` on the host, with rewards
+        and masks written into the learner's pinned staging buffer; then the final states and one update replay."""
+        config = self.config
+        lr, actor = self._graph
+        states = self.states
+        for t in range(config.rollout_length):
+            actions = actor.q_values(states, t)
+            next_states, rewards, terminals, info = self.task.step(actions)
+            self.record_online_return(info)
+            lr.h_reward[t].numpy()[...] = np.asarray(config.reward_normalizer(rewards), dtype=np.float32)   # tensor(): float32
+            lr.h_mask[t].numpy()[...] = 1 - np.asarray(terminals, dtype=np.float32)
+            states = next_states
+            self.total_steps += config.num_workers
+        self.states = states
+        lr.stage_final(states)
+        self.last_loss = lr.update()

@@ -148,11 +148,16 @@ class GraphedQActor:
     ``arena``: a uint8 device tensor [slots * num_envs * history + 1, H * W] that receives the uploaded stacks instead of the
     actor's own one-slot buffer: ``q_values(states, slot)`` uploads them into rows ``slot * num_envs * history ...`` and
     forwards from there (one captured graph per slot), so a learner can read a whole rollout's frame stacks from the arena
-    without uploading them again (learner.GraphedNStepLearner).  The last row is padding the gather stages but never uses."""
+    without uploading them again (learner.GraphedNStepLearner).  The last row is padding the gather stages but never uses.
 
-    def __init__(self, network, q_fn, num_envs, history, frame_hw, scale, arena=None):
+    ``run``: what runs on the gathered batch instead of ``q_fn(network(x))``: ``run(x, slot)`` returns the device tensor that
+    ``q_values`` downloads (learner.GraphedA2CLearner.act: the body, the actor-critic head and the action draw, returning the
+    actions).  ``body``: the network's NatureConvBody when it is not ``network.body`` (``phi_body`` of an actor-critic net)."""
+
+    def __init__(self, network, q_fn, num_envs, history, frame_hw, scale, arena=None, run=None, body=None):
         p = next(network.parameters())
-        self.net, self.q_fn, self.dev = network, q_fn, p.device
+        self.net, self.q_fn, self.run, self.dev = network, q_fn, run, p.device
+        self.body = body if body is not None else getattr(network, "body", None)
         self.N, self.hl, self.hw, self.scale = int(num_envs), int(history), tuple(frame_hw), float(scale)
         self.row = self.hw[0] * self.hw[1]
         rows = self.N * self.hl + 1                       # (+1: the gather kernel stages history + n_step rows)
@@ -187,9 +192,8 @@ class GraphedQActor:
     def _signature(self):
         """What the captured launch sequence depends on besides addresses: who re-packs the body's bf16 operands (the body per
         forward, or the learner's optimizer kernel) and whether the distributional heads have their bf16 operand."""
-        body = getattr(self.net, "body", None)
         heads = tuple(getattr(m, "_w16", None) is not None for m in self.net.children() if isinstance(m, torch.nn.Linear))
-        return (bool(getattr(body, "auto_repack", True)), heads)
+        return (bool(getattr(self.body, "auto_repack", True)), heads)
 
     def _forward(self, slot=0):
         from ..network.fused import frame_scale
@@ -199,10 +203,11 @@ class GraphedQActor:
                   _lib.ptr(self.d_mask), self.d_frames.shape[0], self.row, _lib.ptr(self.idxs[slot]), self.N, self.hl, 1, 1.0, None,
                   _lib.DTYPE_CODE[torch.bfloat16], 2, self.hw[1], _lib.ptr(self.x), None, None, None, None, _lib.stream())
         with torch.no_grad(), frame_scale(self.scale):
-            q = self.q_fn(self.net(self.x.permute(0, 3, 1, 2))).float()
+            x = self.x.permute(0, 3, 1, 2)
+            q = self.run(x, slot) if self.run is not None else self.q_fn(self.net(x)).float()
         if self.d_q is None:
             self.d_q = torch.empty_like(q)
-            self.h_q = torch.empty(q.shape, dtype=torch.float32, pin_memory=True)
+            self.h_q = torch.empty(q.shape, dtype=q.dtype, pin_memory=True)
         self.d_q.copy_(q)
         self.h_q.copy_(self.d_q, non_blocking=True)
 
@@ -224,8 +229,8 @@ class GraphedQActor:
         self._sig = self._signature()
 
     def q_values(self, states, slot=0):
-        """``states``: ``num_envs`` frame stacks (LazyFrames / uint8 arrays [history, H, W]).  Returns float32 [num_envs, A].
-        ``slot``: where in the arena the stacks land (0 without an arena)."""
+        """``states``: ``num_envs`` frame stacks (LazyFrames / uint8 arrays [history, H, W]).  Returns float32 [num_envs, A]
+        (with ``run``: what it returns, on the host).  ``slot``: where in the arena the stacks land (0 without an arena)."""
         for i, s in enumerate(states):
             a = np.asarray(s)
             if a.dtype != np.uint8 or a.size != self.hl * self.row:
@@ -282,6 +287,54 @@ def nstep_q_graph_unsupported(config, network, optimizer, states):
         return "the fused backward epilogues are switched off; the captured update needs the fused update tail"
     if network.fc_head.out_features >= 32:
         return "%d actions; the narrow head and loss kernels take fewer than 32" % network.fc_head.out_features
+    if not isinstance(config.state_normalizer, RescaleNormalizer):
+        return "the state normalizer is %s; the captured update folds a RescaleNormalizer into conv1" % type(
+            config.state_normalizer).__name__
+    if not all(np.asarray(s).dtype == np.uint8 and np.asarray(s).shape == (4, 84, 84) for s in states):
+        return "the envs do not return uint8 4 x 84 x 84 frame stacks"
+    # what FlatOptimizer.from_torch turns into a kind the fused tail (NatureTail) takes
+    g = optimizer.param_groups[0]
+    if not ((isinstance(optimizer, torch.optim.RMSprop) and g["momentum"] == 0 and g["weight_decay"] == 0)
+            or (isinstance(optimizer, torch.optim.Adam) and g["weight_decay"] == 0 and not g["amsgrad"])):
+        return ("the optimizer is %s; the fused update tail implements RMSprop (centered or not) and Adam without momentum, "
+                "weight decay or amsgrad" % type(optimizer).__name__)
+    if not body.conv1.weight.is_cuda:
+        return "the network is not on a CUDA device (select_device(0))"
+    return None
+
+
+def a2c_graph_unsupported(config, network, optimizer, states):
+    """``None`` when ``A2CAgent.step()`` runs as captured graphs under ``config.cuda_graph`` (GraphedQActor with
+    learner.GraphedA2CLearner.act per env step, GraphedA2CLearner per rollout), else the unmet condition; the agent then keeps
+    its eager path.  ``states``: the envs' current observations."""
+    from ..network import nature_tc
+    from ..network.network_bodies import NatureConvBody
+    from ..network.network_heads import CategoricalActorCriticNet
+    from ..utils import Config
+    from ..utils.normalizer import RescaleNormalizer
+    if not getattr(config, "cuda_graph", False):
+        return "config.cuda_graph is not set"
+    if getattr(config, "device_a2c", False):
+        return "config.device_a2c is set; it runs the agent on the device itself"
+    if type(network) is not CategoricalActorCriticNet:
+        return "the network is a %s; the captured update implements CategoricalActorCriticNet" % type(network).__name__
+    body = network.phi_body
+    if not isinstance(body, NatureConvBody):
+        return "the phi_body is a %s; the captured update implements NatureConvBody" % type(body).__name__
+    if not (isinstance(network.actor_body, DummyBody) and isinstance(network.critic_body, DummyBody)):
+        return ("the actor / critic bodies are %s / %s; the captured update implements DummyBody for both"
+                % (type(network.actor_body).__name__, type(network.critic_body).__name__))
+    if body.noisy_linear or config.noisy_linear:
+        return "the network has NoisyLinear layers; the captured update implements nn.Linear"
+    if body.conv1.in_channels != 4:
+        return "the NatureConvBody takes %d channels; the captured update reads stacks of 4 frames" % body.conv1.in_channels
+    if Config.COMPUTE_DTYPE != torch.bfloat16 or Config.DENSE_BACKEND != "tcgen05":
+        return ("the compute dtype is %s with the %r dense backend; the captured update runs bf16 on the wgmma kernels "
+                "(tcgen05)" % (Config.COMPUTE_DTYPE, Config.DENSE_BACKEND))
+    if not (nature_tc.FUSED_BWD and _lib.CONV_SLAB):
+        return "the fused backward epilogues are switched off; the captured update needs the fused update tail"
+    if network.fc_action.out_features >= 32:
+        return "%d actions; the actor-critic head and loss kernels take fewer than 32" % network.fc_action.out_features
     if not isinstance(config.state_normalizer, RescaleNormalizer):
         return "the state normalizer is %s; the captured update folds a RescaleNormalizer into conv1" % type(
             config.state_normalizer).__name__

@@ -89,6 +89,69 @@ __global__ void __launch_bounds__(128) head_fwd_kernel(const __nv_bfloat16* __re
   }
 }
 
+// Actor-critic head (CategoricalActorCriticNet with DummyBody actor / critic bodies, network_heads.py:184-194): the A fc_action
+// rows and the fc_critic row of one bf16 feature row, written as out[b] = (logits[0..A-1], v) -- no combine.  With a counter,
+// the same warp draws the action as a2c_actor_kernel does (csrc/a2c.cu): the inverse CDF of softmax(logits) on
+// Philox::u24(seed, ctr0 + b, AC_PHILOX_STREAM), written as int64 to action_out[b].  The counter advances by B; every CTA reads
+// it first and the last CTA to arrive (ticket) writes it, so no CTA can see the advanced value.
+constexpr uint64_t AC_PHILOX_STREAM = 13;      // csrc/a2c.cu A2C_PHILOX_STREAM: one categorical stream for both actors
+
+template <int NB>
+__global__ void __launch_bounds__(128) ac_head_fwd_kernel(const __nv_bfloat16* __restrict__ phi, const float* __restrict__ Wa,
+                                                          const float* __restrict__ ba, const float* __restrict__ Wv,
+                                                          const float* __restrict__ bv, int B, int K, int A,
+                                                          float* __restrict__ out, uint64_t seed, int64_t* __restrict__ counter,
+                                                          int64_t* __restrict__ action_out, int* __restrict__ ticket) {
+  pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return
+  __shared__ int64_t s_ctr0;
+  const int lane = threadIdx.x & 31, b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (counter) {
+    if (threadIdx.x == 0) s_ctr0 = *counter;
+    __syncthreads();
+  }
+  if (b < B) {
+    float acc[NB];
+    head_row_dots<NB>(phi + (int64_t)b * K, Wa, ba, Wv, bv, K, A, lane, acc);
+    if (lane == 0) {
+#pragma unroll
+      for (int n = 0; n < NB; ++n)
+        if (n <= A) out[(int64_t)b * (A + 1) + n] = acc[n];
+      if (counter) {
+        float mx = acc[0];
+#pragma unroll
+        for (int j = 1; j < NB; ++j)
+          if (j < A) mx = fmaxf(mx, acc[j]);
+        float s = 0.0f;
+#pragma unroll
+        for (int j = 0; j < NB; ++j)
+          if (j < A) s += expf(acc[j] - mx);
+        const float target = Philox::u24(seed, (uint64_t)(s_ctr0 + b), AC_PHILOX_STREAM) * s;
+        int pick = A - 1;                         // (rounding may leave the target above the last partial sum)
+        float c = 0.0f;
+        bool found = false;
+#pragma unroll
+        for (int j = 0; j < NB; ++j) {
+          if (j < A && !found) {
+            c += expf(acc[j] - mx);
+            if (target < c) { pick = j; found = true; }
+          }
+        }
+        action_out[b] = pick;
+      }
+    }
+  }
+  if (counter) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence();
+      if (atomicAdd(ticket, 1) == (int)gridDim.x - 1) {   // every CTA has read the counter
+        *counter = s_ctr0 + B;
+        *ticket = 0;
+      }
+    }
+  }
+}
+
 // grid (K/64, ceil(B/HB_ROWS)); block 256 = 64 columns x 4 row groups of HB_ROWS/4 rows (many small CTAs: the kernel is
 // latency-bound, 16 rows per CTA puts 256 CTAs in flight at B = 512)
 constexpr int HB_ROWS = 16;
@@ -483,6 +546,35 @@ extern "C" int b2rl_head_bwd_relu(const float* gq, const uint16_t* phi, const fl
                                   float* relu_colsum, void* stream) {
   B2RL_REQUIRE(relu_colsum, "null relu_colsum");
   return head_bwd_impl(gq, phi, Wa, Wv, B, K, A, gphi, gWa, gba, gWv, gbv, relu_colsum, stream);
+}
+
+// Actor-critic head forward (ac_head_fwd_kernel): out [B][A + 1] = (fc_action logits, fc_critic value).  counter != NULL: also
+// draw the actions into action_out [B] (int64) from Philox(seed, *counter + b) and advance *counter by B; ticket: int32,
+// zero-initialised once (the kernel re-arms it).
+extern "C" int b2rl_ac_head_fwd(const uint16_t* phi, const float* Wa, const float* ba, const float* Wv, const float* bv,
+                                int32_t B, int32_t K, int32_t A, float* out, uint64_t seed, int64_t* counter,
+                                int64_t* action_out, int32_t* ticket, void* stream) {
+  B2RL_REQUIRE(phi && Wa && ba && Wv && bv && out, "null pointer");
+  B2RL_REQUIRE(!counter || (action_out && ticket), "a draw needs action_out and ticket");
+  B2RL_REQUIRE(B > 0 && K > 0 && K % 8 == 0 && A > 0 && A + 1 <= HEAD_MAX_OUT, "need K % 8 == 0 and 0 < A <= 31");
+  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(phi) % 16 == 0 && (reinterpret_cast<uintptr_t>(Wa) | reinterpret_cast<uintptr_t>(Wv)) % 16 == 0,
+               "phi and the weights must be 16-byte aligned");
+  const __nv_bfloat16* x = reinterpret_cast<const __nv_bfloat16*>(phi);
+  const dim3 grid((B + 3) / 4);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (A + 1 <= 8) launch_pdl(ac_head_fwd_kernel<8>, grid, dim3(128), 0, st, x, Wa, ba, Wv, bv, B, K, A, out, seed, counter, action_out, ticket);
+  else if (A + 1 <= 19) launch_pdl(ac_head_fwd_kernel<19>, grid, dim3(128), 0, st, x, Wa, ba, Wv, bv, B, K, A, out, seed, counter, action_out, ticket);
+  else launch_pdl(ac_head_fwd_kernel<HEAD_MAX_OUT>, grid, dim3(128), 0, st, x, Wa, ba, Wv, bv, B, K, A, out, seed, counter, action_out, ticket);
+  return check_launch("b2rl_ac_head_fwd");
+}
+
+// b2rl_head_bwd_relu on effective output gradients already computed: geff [B][HEAD_MAX_OUT + 1], column n < A the gradient of
+// Wa's output n, column A that of Wv's (the actor-critic head: dL/dlogit, then dL/dv; b2rl_a2c_rollout_loss writes this layout)
+extern "C" int b2rl_head_bwd_geff_relu(const float* geff, const uint16_t* phi, const float* Wa, const float* Wv, int32_t B,
+                                       int32_t K, int32_t A, uint16_t* gphi, float* gWa, float* gba, float* gWv, float* gbv,
+                                       float* relu_colsum, void* stream) {
+  B2RL_REQUIRE(geff && relu_colsum, "null pointer");
+  return head_bwd_impl(nullptr, phi, Wa, Wv, B, K, A, gphi, gWa, gba, gWv, gbv, relu_colsum, stream, geff);
 }
 
 

@@ -175,6 +175,109 @@ __global__ void __launch_bounds__(1024) a2c_loss_kernel(const float* __restrict_
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// A2C_agent.py:43-62 for a rollout whose forward is ONE actor-critic head launch over the (T + 1) N rows (b2rl_ac_head_fwd):
+// head [(T+1) N][A + 1] (logits, then v; rows t-major, slot T the final states).  One warp per env column: every lane runs
+// the column's backward GAE scan in gae_seq_kernel's order (mode 0, the same bits as ops.gae(exact=True)) -- the operands are
+// warp-uniform -- and lane j < A then owns logit j of the row: p = softmax(z), lp = log_softmax(z), H = -sum p lp,
+//   geff[i][j] = -(adv / R)(1[j = a] - p_j) + (ew / R) p_j (lp_j + H),   geff[i][A] = (vw / R)(v_i - ret_i)
+// with R = T N, the gradient of  loss = -mean(lp_a adv) - ew mean(H) + vw 0.5 mean((ret - v)^2)  (adv, ret detached) with
+// respect to the head's outputs; the final rows get zero (the reference detaches their values).  geff has the head
+// backward's row stride (HEAD_MAX_OUT + 1 = 33, csrc/head.cu).  Each CTA parks its three sums (lp_a adv, H, (ret - v)^2; per
+// warp in t order, then in warp order) in partial[3 cta ..] and the last CTA adds them in CTA order: two launches on the same
+// inputs give the same loss bits.
+constexpr int A2CR_WARPS = 4;
+constexpr int A2CR_LD = 33;                    // csrc/head.cu HEAD_MAX_OUT + 1
+constexpr int A2CR_MAX_ROWS = 1 << 24;         // (T + 1) N converts to float exactly
+
+__device__ __forceinline__ float a2cr_warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__global__ void __launch_bounds__(A2CR_WARPS * 32) a2c_rollout_loss_kernel(
+    const float* __restrict__ head, const int64_t* __restrict__ action, const float* __restrict__ reward,
+    const float* __restrict__ mask, float discount, float tau, int use_gae, float ew, float vw, int T, int N, int A,
+    float* __restrict__ adv_out, float* __restrict__ ret_out, float* __restrict__ loss_out, float* __restrict__ geff,
+    float* __restrict__ partial, int32_t* __restrict__ counter) {
+  pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return
+  __shared__ float s_sum[3][A2CR_WARPS];
+  __shared__ bool is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int n = blockIdx.x * A2CR_WARPS + warp;
+  const int ld = A + 1;
+  const float R = (float)(T * N);
+  float s_pol = 0.0f, s_ent = 0.0f, s_val = 0.0f;
+  if (n < N) {
+    const int64_t fin = (int64_t)T * N + n;
+    if (lane <= A) geff[fin * A2CR_LD + lane] = 0.0f;
+    float ret = head[fin * ld + A];
+    float adv = 0.0f;
+    float vnext = ret;
+    for (int t = T - 1; t >= 0; --t) {
+      const int64_t i = (int64_t)t * N + n;
+      const float r = reward[i], m = mask[i], v = head[i * ld + A];
+      const float gm = __fmul_rn(discount, m);
+      ret = __fadd_rn(r, __fmul_rn(gm, ret));
+      if (use_gae) {
+        const float td = __fsub_rn(__fadd_rn(r, __fmul_rn(gm, vnext)), v);
+        adv = __fadd_rn(__fmul_rn(__fmul_rn(__fmul_rn(adv, tau), discount), m), td);
+      } else {
+        adv = __fsub_rn(ret, v);
+      }
+      vnext = v;
+      // the row's softmax: lane j < A holds logit j
+      const int a_i = (int)action[i];
+      const float z = lane < A ? head[i * ld + lane] : -INFINITY;
+      float mx = z;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      const float e = lane < A ? expf(z - mx) : 0.0f;
+      const float s = a2cr_warp_sum(e);
+      const float lp = lane < A ? (z - mx) - logf(s) : 0.0f;
+      const float p = e / s;
+      const float H = -a2cr_warp_sum(p * lp);
+      const float lp_a = __shfl_sync(0xffffffffu, lp, a_i & 31);
+      if (lane < A) {
+        const float pol = (lane == a_i ? 1.0f : 0.0f) - p;
+        geff[i * A2CR_LD + lane] = -(adv / R) * pol + (ew / R) * (p * (lp + H));
+      } else if (lane == A) {
+        geff[i * A2CR_LD + A] = (vw / R) * (v - ret);
+      }
+      if (lane == 0) {
+        if (adv_out) adv_out[i] = adv;
+        if (ret_out) ret_out[i] = ret;
+      }
+      s_pol = __fadd_rn(s_pol, __fmul_rn(lp_a, adv));
+      s_ent = __fadd_rn(s_ent, H);
+      const float d = __fsub_rn(ret, v);
+      s_val = __fadd_rn(s_val, __fmul_rn(d, d));
+    }
+  }
+  if (lane == 0) s_sum[0][warp] = s_pol, s_sum[1][warp] = s_ent, s_sum[2][warp] = s_val;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int q = 0; q < 3; ++q) {
+      float c = 0.0f;
+      for (int w = 0; w < A2CR_WARPS; ++w) c = __fadd_rn(c, s_sum[q][w]);
+      partial[3 * blockIdx.x + q] = c;
+    }
+    __threadfence();
+    is_last = atomicAdd(counter, 1) == (int)gridDim.x - 1;
+  }
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {              // deterministic final reduction in CTA order
+    __threadfence();
+    float tot[3] = {0.0f, 0.0f, 0.0f};
+    for (int c = 0; c < (int)gridDim.x; ++c)
+      for (int q = 0; q < 3; ++q) tot[q] = __fadd_rn(tot[q], __ldcg(partial + 3 * c + q));
+    const float pl = -__fdiv_rn(tot[0], R), el = __fdiv_rn(tot[1], R), vl = __fmul_rn(0.5f, __fdiv_rn(tot[2], R));
+    if (loss_out) loss_out[0] = __fadd_rn(__fsub_rn(pl, __fmul_rn(ew, el)), __fmul_rn(vw, vl));
+    *counter = 0;
+  }
+}
+
 }  // namespace b2rl
 
 using namespace b2rl;
@@ -221,4 +324,19 @@ extern "C" int b2rl_a2c_loss(const float* log_pi_a, const float* entropy, const 
                                                                   value_loss_weight, M, out, dlogp_out, dent_out,
                                                                   dv_out);
   return check_launch("b2rl_a2c_loss");
+}
+
+extern "C" int b2rl_a2c_rollout_loss_ctas(int32_t N) { return N > 0 ? (N + A2CR_WARPS - 1) / A2CR_WARPS : 0; }
+
+extern "C" int b2rl_a2c_rollout_loss(const float* head, const int64_t* action, const float* reward, const float* mask,
+                                     float discount, float gae_tau, int32_t use_gae, float entropy_weight,
+                                     float value_loss_weight, int32_t T, int32_t N, int32_t A, float* adv_out, float* ret_out,
+                                     float* loss_out, float* geff_out, float* partial, int32_t* counter, void* stream) {
+  B2RL_REQUIRE(head && action && reward && mask && geff_out && partial && counter, "null pointer");
+  B2RL_REQUIRE(T >= 1 && N >= 1 && A >= 1 && A + 1 <= A2CR_LD - 1, "bad shape: needs T >= 1, N >= 1 and 1 <= A <= 31");
+  B2RL_REQUIRE((int64_t)(T + 1) * N <= A2CR_MAX_ROWS, "(T + 1) * N must not exceed 2^24 rows");
+  launch_pdl(a2c_rollout_loss_kernel, dim3(b2rl_a2c_rollout_loss_ctas(N)), dim3(A2CR_WARPS * 32), 0, (cudaStream_t)stream,
+             head, action, reward, mask, discount, gae_tau, (int)use_gae, entropy_weight, value_loss_weight, (int)T, (int)N,
+             (int)A, adv_out, ret_out, loss_out, geff_out, partial, counter);
+  return check_launch("b2rl_a2c_rollout_loss");
 }

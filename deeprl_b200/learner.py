@@ -18,7 +18,7 @@ import torch
 
 from . import _lib, ops, parallel
 from .component.replay import PrioritizedReplay
-from .network import nature_tc
+from .network import fused, nature_tc
 from .network.fused import frame_scale
 from .utils.config import Config
 
@@ -106,7 +106,14 @@ def update_plan(kind="dqn", per=False, prefetch=False, dual=False, k1_body=True,
 class _NatureLearner:
     """What the captured learners of a wgmma NatureConvBody network share: the update plan (decided on first use by the
     subclass's ``_resolve_plan``), the fused update tail, and the packed bf16 operands of the online (``net``) and target
-    (``tgt``) networks -- re-packed after outside parameter changes and at target sync."""
+    (``tgt``) networks -- re-packed after outside parameter changes and at target sync.
+
+    ``body_attr``: the attribute of the networks that holds the NatureConvBody (``phi_body`` for an actor-critic network)."""
+
+    body_attr = "body"
+
+    def _body(self, net):
+        return getattr(net, self.body_attr, None)
 
     @property
     def plan(self):
@@ -123,7 +130,7 @@ class _NatureLearner:
             from .network.tail import NatureTail
             if self.plan.tail:
                 self._repack(self.net)
-                self._tail = NatureTail(self.opt, self.net.body, self.scale)
+                self._tail = NatureTail(self.opt, self._body(self.net), self.scale)
                 self._tail.max_norm, self._tail.grad_scale = self.clip, 1.0 / self.world
                 self._refresh_head_operands(True)
                 if self.world > 1:
@@ -138,7 +145,7 @@ class _NatureLearner:
     def _repack(self, net):
         """wgmma backend: the learner owns the packed bf16 operands of both networks -- the online body is re-packed
         once per update (one launch), the target body only when it is synchronised."""
-        body = getattr(net, "body", None)
+        body = self._body(net)
         if body is not None and hasattr(body, "repack") and self.dtype == torch.bfloat16:
             body.auto_repack = False
             body.repack(self.scale)
@@ -548,96 +555,42 @@ class GraphedDQNLearner(_NatureLearner):
         return self.h_pack.numel()
 
 
-class GraphedNStepLearner(_NatureLearner):
-    """The update of ``NStepDQNAgent.step()`` (NStepDQN_agent.py:52-67) for a VanillaNet on a wgmma NatureConvBody as ONE
-    captured graph per rollout: the rollout's actions / rewards / masks up in one packed copy and the final states' stacks up
-    into the arena, the online body at batch T N on the rollout's stacks beside the target body at batch N on the final ones
-    (two branches), both heads (``b2rl_head_fwd``), the n-step target and loss (``b2rl_nstep_q_loss``), the head backward
-    with fc4's ReLU (``b2rl_head_bwd_relu``), the fused body backward and the two-launch update tail (gradient reduce,
-    ``clip_grad_norm_``, RMSprop / Adam, bf16 operand writes).
+class _RolloutLearner(_NatureLearner):
+    """What the captured rollout learners (``GraphedNStepLearner``, ``GraphedA2CLearner``) share: the uint8 arena of the
+    rollout's frame stacks -- slot t (rows t N 4 .. (t + 1) N 4 - 1) the states of env step t, which the actor's upload writes
+    there (component/actor.py ``GraphedQActor(arena=...)``), slot T the final states, plus one padding row --, the final states'
+    pinned staging buffer, the fused update tail as the optimizer, and a capture that leaves the parameters untrained."""
 
-    ``arena`` holds the rollout's uint8 frame stacks: slot t (rows t N 4 .. (t + 1) N 4 - 1) the states of env step t, which
-    the actor's upload writes there (component/actor.py ``GraphedQActor(arena=...)``), slot T the final states, plus one
-    padding row.  Conv1's forward and weight gradient read the stacks from it (K1: ``RingFrames`` with ``idx[i] = 4 i``); no
-    bf16 batch is built.  The online q of the rollout is recomputed rather than kept from the actor: the parameters do not
-    change during a rollout, so it is the q the actor saw.
-
-    The target sync (NStepDQN_agent.py:48-49) is the caller's ``sync_target()`` before ``update()``: the online parameters do
-    not change inside a rollout, so syncing at its end gives the same target."""
-
-    def __init__(self, network, target_network, optimizer, rollout_length, num_envs, discount=0.99, gradient_clip=5.0,
-                 state_scale=1.0 / 255, history=4, frame_hw=(84, 84)):
-        self.net, self.tgt, self.opt = network, target_network, optimizer
+    def _init_rollout(self, network, optimizer, rollout_length, num_envs, gradient_clip, state_scale, history, frame_hw):
+        """Common state; returns the arena row of each of the (T + 1) N stacks (``idx[i] = 4 i``, rows t-major)."""
+        self.net, self.opt = network, optimizer
         self.T, self.N, self.hl = int(rollout_length), int(num_envs), int(history)
-        self.discount, self.clip, self.scale = float(discount), float(gradient_clip or 0.0), float(state_scale)
+        self.clip, self.scale = float(gradient_clip or 0.0), float(state_scale)
         self.dtype, self.world = torch.bfloat16, 1
         self.dev = dev = optimizer.flat.device
         self._plan, self._tail, self._side = None, None, None
         if not self.plan.tail:
-            raise _lib.B2RLError("GraphedNStepLearner needs the fused update tail: a wgmma NatureConvBody with the fused "
-                                 "backward epilogues, and RMSprop or Adam")
+            raise _lib.B2RLError("%s needs the fused update tail: a wgmma NatureConvBody with the fused backward epilogues, "
+                                 "and RMSprop or Adam" % type(self).__name__)
         T, N, hl = self.T, self.N, self.hl
         row = frame_hw[0] * frame_hw[1]
         k = N * hl
         self.arena = torch.zeros(((T + 1) * k + 1, row), dtype=torch.uint8, device=dev)
-        idx = torch.arange((T + 1) * N, dtype=torch.int64, device=dev) * hl
-        self.states = nature_tc.RingFrames(self.arena, idx[:T * N], 0, row, frame_hw[1], hl)
-        self.final = nature_tc.RingFrames(self.arena, idx[T * N:], 0, row, frame_hw[1], hl)
         self.h_final = torch.zeros((k, row), dtype=torch.uint8, pin_memory=True)
         self._np_final = self.h_final.numpy().reshape(N, hl, row)
-        # ONE packed pinned staging buffer for the rollout's scalars and ONE device mirror -> a single host->device copy node:
-        # [action int64 T*N | reward float32 T*N | mask float32 T*N]
-        rows = T * N
-        self.h_pack = torch.zeros(16 * rows, dtype=torch.uint8, pin_memory=True)
-        self.d_pack = torch.zeros(16 * rows, dtype=torch.uint8, device=dev)
-
-        def views(buf):
-            return (buf[:8 * rows].view(torch.int64).view(T, N), buf[8 * rows:12 * rows].view(torch.float32).view(T, N),
-                    buf[12 * rows:].view(torch.float32).view(T, N))
-
-        self.h_action, self.h_reward, self.h_mask = views(self.h_pack)
-        self.d_action, self.d_reward, self.d_mask = views(self.d_pack)
-        A = network.fc_head.out_features
-        self.out = dict(ret=torch.zeros(rows, dtype=torch.float32, device=dev),
-                        delta=torch.zeros(rows, dtype=torch.float32, device=dev),
-                        loss=torch.zeros(1, dtype=torch.float32, device=dev),
-                        gq=torch.zeros((rows, A), dtype=torch.float32, device=dev))
-        self.loss = self.out["loss"]
-        self.q = None                     # the online q of the last update [T*N, A] (a buffer of the captured graph)
         self.graph = None
         self.updates = 0
         self.opt.zero_grad()              # the fused tail writes / re-zeroes the gradient arena itself: start from zeros
+        return torch.arange((T + 1) * N, dtype=torch.int64, device=dev) * hl
 
-    def _resolve_plan(self):
-        tail = (hasattr(getattr(self.net, "body", None), "repack") and nature_tc.FUSED_BWD and bool(_lib.CONV_SLAB)
+    def _tail_applies(self):
+        return (hasattr(self._body(self.net), "repack") and nature_tc.FUSED_BWD and bool(_lib.CONV_SLAB)
                 and self.opt.kind in ("rmsprop", "adam"))
-        return UpdatePlan(ring=True, tail=tail, repack_online=not tail, dist_head=False, head="separate", forward="two-branch",
-                          conv1="separate", single_stream=False, prefetch=None, join=None, one_graph=True)
 
     def stage_final(self, states):
         """The final states' frame stacks (uint8 [history, H, W] each) into the pinned buffer the update uploads to slot T."""
         for i, s in enumerate(states):
             self._np_final[i] = np.asarray(s).reshape(self.hl, -1)
-
-    def _main(self):
-        cur = torch.cuda.current_stream()
-        if self._side is None:
-            self._side = torch.cuda.Stream(device=self.dev)
-        side, tail = self._side, self.tail()
-        k = self.N * self.hl
-        self.arena[self.T * k:(self.T + 1) * k].copy_(self.h_final, non_blocking=True)
-        self.d_pack.copy_(self.h_pack, non_blocking=True)
-        # the target forward on the final states and the online forward on the rollout's states: two parallel branches
-        side.wait_stream(cur)
-        with torch.cuda.stream(side), frame_scale(self.scale), torch.no_grad():
-            q_boot = self.tgt(self.final)["q"]
-        with frame_scale(self.scale):
-            q = self.net(self.states)["q"]
-        cur.wait_stream(side)
-        r = ops.nstep_q_loss(q.detach(), q_boot, self.d_action, self.d_reward, self.d_mask, self.discount, out=self.out)
-        with nature_tc.wgrad_stream(side), nature_tc.grad_sink(tail):     # weight-gradient GEMMs on the side branch
-            q.backward(r["gq"])
-        self.q = q.detach()
 
     def _opt(self):
         self.tail().step(max_norm=self.clip)
@@ -670,6 +623,77 @@ class GraphedNStepLearner(_NatureLearner):
         torch.cuda.synchronize()
         return self
 
+
+class GraphedNStepLearner(_RolloutLearner):
+    """The update of ``NStepDQNAgent.step()`` (NStepDQN_agent.py:52-67) for a VanillaNet on a wgmma NatureConvBody as ONE
+    captured graph per rollout: the rollout's actions / rewards / masks up in one packed copy and the final states' stacks up
+    into the arena, the online body at batch T N on the rollout's stacks beside the target body at batch N on the final ones
+    (two branches), both heads (``b2rl_head_fwd``), the n-step target and loss (``b2rl_nstep_q_loss``), the head backward
+    with fc4's ReLU (``b2rl_head_bwd_relu``), the fused body backward and the two-launch update tail (gradient reduce,
+    ``clip_grad_norm_``, RMSprop / Adam, bf16 operand writes).
+
+    ``arena`` holds the rollout's uint8 frame stacks: slot t (rows t N 4 .. (t + 1) N 4 - 1) the states of env step t, which
+    the actor's upload writes there (component/actor.py ``GraphedQActor(arena=...)``), slot T the final states, plus one
+    padding row.  Conv1's forward and weight gradient read the stacks from it (K1: ``RingFrames`` with ``idx[i] = 4 i``); no
+    bf16 batch is built.  The online q of the rollout is recomputed rather than kept from the actor: the parameters do not
+    change during a rollout, so it is the q the actor saw.
+
+    The target sync (NStepDQN_agent.py:48-49) is the caller's ``sync_target()`` before ``update()``: the online parameters do
+    not change inside a rollout, so syncing at its end gives the same target."""
+
+    def __init__(self, network, target_network, optimizer, rollout_length, num_envs, discount=0.99, gradient_clip=5.0,
+                 state_scale=1.0 / 255, history=4, frame_hw=(84, 84)):
+        self.tgt, self.discount = target_network, float(discount)
+        idx = self._init_rollout(network, optimizer, rollout_length, num_envs, gradient_clip, state_scale, history, frame_hw)
+        T, N, dev = self.T, self.N, self.dev
+        row = frame_hw[0] * frame_hw[1]
+        self.states = nature_tc.RingFrames(self.arena, idx[:T * N], 0, row, frame_hw[1], self.hl)
+        self.final = nature_tc.RingFrames(self.arena, idx[T * N:], 0, row, frame_hw[1], self.hl)
+        # ONE packed pinned staging buffer for the rollout's scalars and ONE device mirror -> a single host->device copy node:
+        # [action int64 T*N | reward float32 T*N | mask float32 T*N]
+        rows = T * N
+        self.h_pack = torch.zeros(16 * rows, dtype=torch.uint8, pin_memory=True)
+        self.d_pack = torch.zeros(16 * rows, dtype=torch.uint8, device=dev)
+
+        def views(buf):
+            return (buf[:8 * rows].view(torch.int64).view(T, N), buf[8 * rows:12 * rows].view(torch.float32).view(T, N),
+                    buf[12 * rows:].view(torch.float32).view(T, N))
+
+        self.h_action, self.h_reward, self.h_mask = views(self.h_pack)
+        self.d_action, self.d_reward, self.d_mask = views(self.d_pack)
+        A = network.fc_head.out_features
+        self.out = dict(ret=torch.zeros(rows, dtype=torch.float32, device=dev),
+                        delta=torch.zeros(rows, dtype=torch.float32, device=dev),
+                        loss=torch.zeros(1, dtype=torch.float32, device=dev),
+                        gq=torch.zeros((rows, A), dtype=torch.float32, device=dev))
+        self.loss = self.out["loss"]
+        self.q = None                     # the online q of the last update [T*N, A] (a buffer of the captured graph)
+
+    def _resolve_plan(self):
+        tail = self._tail_applies()
+        return UpdatePlan(ring=True, tail=tail, repack_online=not tail, dist_head=False, head="separate", forward="two-branch",
+                          conv1="separate", single_stream=False, prefetch=None, join=None, one_graph=True)
+
+    def _main(self):
+        cur = torch.cuda.current_stream()
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.dev)
+        side, tail = self._side, self.tail()
+        k = self.N * self.hl
+        self.arena[self.T * k:(self.T + 1) * k].copy_(self.h_final, non_blocking=True)
+        self.d_pack.copy_(self.h_pack, non_blocking=True)
+        # the target forward on the final states and the online forward on the rollout's states: two parallel branches
+        side.wait_stream(cur)
+        with torch.cuda.stream(side), frame_scale(self.scale), torch.no_grad():
+            q_boot = self.tgt(self.final)["q"]
+        with frame_scale(self.scale):
+            q = self.net(self.states)["q"]
+        cur.wait_stream(side)
+        r = ops.nstep_q_loss(q.detach(), q_boot, self.d_action, self.d_reward, self.d_mask, self.discount, out=self.out)
+        with nature_tc.wgrad_stream(side), nature_tc.grad_sink(tail):     # weight-gradient GEMMs on the side branch
+            q.backward(r["gq"])
+        self.q = q.detach()
+
     def update(self, sync_target=False):
         """One rollout's update (graph replay) on what the caller staged: ``h_action`` / ``h_reward`` / ``h_mask`` [T, N],
         the rollout's stacks in arena slots 0..T-1 and the final states (``stage_final``).  ``sync_target``: an env step of
@@ -677,6 +701,90 @@ class GraphedNStepLearner(_NatureLearner):
         tensor (no sync)."""
         if sync_target:
             self.sync_target()
+        self.graph.replay()
+        self.updates += 1
+        return self.loss
+
+
+class GraphedA2CLearner(_RolloutLearner):
+    """The update of ``A2CAgent.step()`` (A2C_agent.py:92-115) for a CategoricalActorCriticNet whose ``phi_body`` is a wgmma
+    NatureConvBody (DummyBody actor / critic bodies) as ONE captured graph per rollout: the rollout's rewards / masks up in one
+    packed copy and the final states' stacks up into arena slot T; the body at batch (T + 1) N on every stack of the arena
+    (K1); the actor-critic head (``b2rl_ac_head_fwd``: logits and v); GAE, the objective and its gradient with respect to the
+    head's outputs (``b2rl_a2c_rollout_loss``); the head backward with fc4's ReLU (``b2rl_head_bwd_geff_relu``); the fused
+    body backward with its weight gradients on the side branch; and the two-launch update tail (gradient reduce,
+    ``clip_grad_norm_``, RMSprop / Adam, bf16 operand writes, which the next actor replay reads).
+
+    One forward covers the final states too: the reference's bootstrap value comes from the same (online) network
+    (A2C_agent.py:93-96), and the final rows' zero gradient costs about 1 / (T + 1) of the backward.  The rollout's logits and
+    values are recomputed rather than kept from the actor: the parameters do not change during a rollout.
+
+    The actions are drawn on the device by the actor's replays (``act``, run by ``GraphedQActor(run=...)``) straight into
+    ``d_action`` row t: the inverse CDF of the softmax on Philox ``u24(seed, counter + n, 13)`` with a device-resident counter,
+    the stream ``config.device_a2c`` uses -- not torch's ``Categorical.sample``."""
+
+    body_attr = "phi_body"
+
+    def __init__(self, network, optimizer, rollout_length, num_envs, seed, discount=0.99, gae_tau=1.0, use_gae=True,
+                 entropy_weight=0.01, value_loss_weight=1.0, gradient_clip=5.0, state_scale=1.0 / 255, history=4,
+                 frame_hw=(84, 84)):
+        self.tgt = None
+        self.discount, self.gae_tau, self.use_gae = float(discount), float(gae_tau), bool(use_gae)
+        self.ew, self.vw = float(entropy_weight), float(value_loss_weight)
+        idx = self._init_rollout(network, optimizer, rollout_length, num_envs, gradient_clip, state_scale, history, frame_hw)
+        T, N, dev = self.T, self.N, self.dev
+        self.states = nature_tc.RingFrames(self.arena, idx, 0, frame_hw[0] * frame_hw[1], frame_hw[1], self.hl)
+        # ONE packed pinned staging buffer for the rollout's scalars and ONE device mirror: [reward float32 T*N | mask float32 T*N]
+        rows = T * N
+        self.h_pack = torch.zeros(2 * rows, dtype=torch.float32, pin_memory=True)
+        self.d_pack = torch.zeros(2 * rows, dtype=torch.float32, device=dev)
+        self.h_reward, self.h_mask = self.h_pack[:rows].view(T, N), self.h_pack[rows:].view(T, N)
+        self.d_reward, self.d_mask = self.d_pack[:rows].view(T, N), self.d_pack[rows:].view(T, N)
+        A = network.fc_action.out_features
+        self.d_action = torch.zeros((T, N), dtype=torch.int64, device=dev)          # row t: the actor replay of env step t
+        self.seed = int(seed)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=dev)               # Philox position of the next draw
+        self.ticket = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.act_out = torch.zeros((T, N, A + 1), dtype=torch.float32, device=dev)  # the actor's (logits, v) per slot
+        self.head_out = torch.zeros(((T + 1) * N, A + 1), dtype=torch.float32, device=dev)
+        self.out = dict(adv=torch.zeros(rows, dtype=torch.float32, device=dev),
+                        ret=torch.zeros(rows, dtype=torch.float32, device=dev),
+                        loss=torch.zeros(1, dtype=torch.float32, device=dev),
+                        geff=torch.zeros(((T + 1) * N, ops.AC_GEFF_LD), dtype=torch.float32, device=dev))
+        self.loss = self.out["loss"]
+
+    def _resolve_plan(self):
+        tail = self._tail_applies()
+        return UpdatePlan(ring=True, tail=tail, repack_online=not tail, dist_head=False, head="separate", forward="one-stream",
+                          conv1="separate", single_stream=False, prefetch=None, join=None, one_graph=True)
+
+    def act(self, x, slot):
+        """The actor's work on its gathered batch ``x`` (bf16 space-to-depth stacks of env step ``slot``; run by GraphedQActor
+        under no_grad and the frame scale): the body, then the head with the draw into ``d_action[slot]``.  Returns that row."""
+        net = self.net
+        fused.ac_head(self._body(net)(x), net.fc_action, net.fc_critic, out=self.act_out[slot],
+                      draw=(self.seed, self.counter, self.d_action[slot], self.ticket))
+        return self.d_action[slot]
+
+    def _main(self):
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.dev)
+        side, tail, net = self._side, self.tail(), self.net
+        k = self.N * self.hl
+        self.arena[self.T * k:(self.T + 1) * k].copy_(self.h_final, non_blocking=True)
+        self.d_pack.copy_(self.h_pack, non_blocking=True)
+        with frame_scale(self.scale):
+            phi = self._body(net)(self.states)
+        fused.ac_head(phi.detach(), net.fc_action, net.fc_critic, out=self.head_out)
+        r = ops.a2c_rollout_loss(self.head_out, self.d_action, self.d_reward, self.d_mask, self.discount, self.gae_tau,
+                                 self.use_gae, self.ew, self.vw, out=self.out)
+        with nature_tc.wgrad_stream(side), nature_tc.grad_sink(tail):     # weight-gradient GEMMs on the side branch
+            phi.backward(fused.ac_head_backward(phi, r["geff"], net.fc_action, net.fc_critic))
+
+    def update(self):
+        """One rollout's update (graph replay) on what the caller staged: ``h_reward`` / ``h_mask`` [T, N], the rollout's stacks
+        in arena slots 0..T-1 and its actions in ``d_action`` (the actor replays), and the final states (``stage_final``).
+        Returns the device loss tensor (no sync)."""
         self.graph.replay()
         self.updates += 1
         return self.loss

@@ -209,6 +209,46 @@ def narrow_head_ok(phi, fc_action, fc_value=None):
             and isinstance(fc_action, torch.nn.Linear) and fc_action.out_features < 32)
 
 
+def ac_head(phi, fc_action, fc_critic, out=None, draw=None):
+    """CategoricalActorCriticNet's head on bf16 features (DummyBody actor / critic bodies, network_heads.py:184-188) in one
+    launch (``b2rl_ac_head_fwd``): returns ``out`` [B, A+1] fp32 = (logits, v), no autograd.  ``draw``: (seed, counter int64
+    [1], action_out int64 [B], ticket int32 [1]) -- the action of each row is also drawn from softmax(logits) on the device's
+    Philox stream into ``action_out``, and the device counter advances by B."""
+    B, K = phi.shape
+    A = fc_action.out_features
+    if out is None:
+        out = torch.empty((B, A + 1), dtype=torch.float32, device=phi.device)
+    seed, counter, action, ticket = draw if draw is not None else (0, None, None, None)
+    _lib.call("b2rl_ac_head_fwd", _lib.ptr(phi), _lib.ptr(fc_action.weight.detach()), _lib.ptr(fc_action.bias.detach()),
+              _lib.ptr(fc_critic.weight.detach()), _lib.ptr(fc_critic.bias.detach()), B, K, A, _lib.ptr(out), int(seed),
+              _lib.ptr(counter), _lib.ptr(action), _lib.ptr(ticket), _lib.stream())
+    return out
+
+
+def ac_head_backward(phi, geff, fc_action, fc_critic):
+    """The backward of ``ac_head`` from the effective output gradients ``geff`` [B, 33] (``ops.a2c_rollout_loss``) on features
+    ``phi`` = relu(fc4(.)) of a wgmma NatureConvBody (``b2rl_head_bwd_geff_relu``): the head's weight and bias gradients are
+    accumulated into their ``.grad`` (the optimizer arena), fc4's ReLU mask and bias gradient ride along as in
+    ``_NarrowHead.backward``.  Returns the bf16 feature gradient, for ``phi.backward``."""
+    from . import nature_tc
+    if not _fc4_relu_features(phi):
+        raise _lib.B2RLError("ac_head_backward: phi must be the live fc4 output of a wgmma NatureConvBody with the fused "
+                             "backward epilogues")
+    params = (fc_action.weight, fc_action.bias, fc_critic.weight, fc_critic.bias)
+    if not all(p.grad is not None and p.grad.dtype == torch.float32 and p.grad.is_contiguous() for p in params):
+        raise _lib.B2RLError("ac_head_backward: the head's gradients must be fp32 buffers (a FlatOptimizer arena)")
+    B, K = phi.shape
+    gphi = torch.empty_like(phi)
+    sink = nature_tc.SINK
+    colsum = sink.db4 if (sink is not None and sink.db4.numel() == K) else torch.zeros(K, dtype=torch.float32, device=phi.device)
+    _lib.call("b2rl_head_bwd_geff_relu", _lib.ptr(geff), _lib.ptr(phi), _lib.ptr(fc_action.weight.detach()),
+              _lib.ptr(fc_critic.weight.detach()), B, K, fc_action.out_features, _lib.ptr(gphi),
+              *[_lib.ptr(p.grad) for p in params], _lib.ptr(colsum), _lib.stream())
+    nature_tc.premask(gphi, colsum)
+    nature_tc.mark("head_bwd")
+    return gphi
+
+
 class _DistHead(torch.autograd.Function):
     """Distributional head (CategoricalNet / QuantileNet, network_heads.py:40-55, 89-102) on bf16 features with no cuBLAS / ATen
     kernel: logits = phi W^T + b on the wgmma GEMM, softmax + log_softmax in one launch (csrc/disthead.cu), and in the backward

@@ -120,6 +120,36 @@ def nstep_q_loss(q, q_boot, action, reward, mask, discount, out=None):
     return r
 
 
+AC_GEFF_LD = 33                              # row stride of the head backward's effective gradients (csrc/head.cu HEAD_MAX_OUT + 1)
+
+
+def a2c_rollout_loss(head, action, reward, mask, discount, gae_tau, use_gae, entropy_weight, value_loss_weight, out=None):
+    """A2C_agent.py:43-62 in one launch (``b2rl_a2c_rollout_loss``): ``head`` [(T+1)*N, A+1] = (logits, v) of the rollout's
+    states and, in rows T*N.., the final states (rows t-major); ``action`` int64 / ``reward`` / ``mask`` [T*N] or [T, N].
+    Returns dict(adv, ret [T*N] (the bits of ``gae(exact=True)``), loss [1], geff [(T+1)*N, 33] = dloss / d(head outputs) in
+    columns 0..A, the final rows zero).  ``out``: a dict of preallocated outputs to write instead (persistent buffers of a
+    captured graph)."""
+    head = _c(head, _f32)
+    T, N = reward.shape[0], reward.numel() // reward.shape[0]
+    A = head.shape[1] - 1
+    if head.shape[0] != (T + 1) * N or reward.numel() != T * N:
+        raise _lib.B2RLError("a2c_rollout_loss: head has %d rows, reward %s" % (head.shape[0], tuple(reward.shape)))
+    dev = head.device
+    o = out if out is not None else {}
+    e = lambda k, *shape: o[k] if k in o else torch.empty(shape, dtype=_f32, device=dev)
+    r = dict(adv=e("adv", T * N), ret=e("ret", T * N), loss=e("loss", 1))
+    # (the kernel writes geff's columns 0..A; the rest stay zero)
+    r["geff"] = o["geff"] if "geff" in o else torch.zeros(((T + 1) * N, AC_GEFF_LD), dtype=_f32, device=dev)
+    ctas = int(_lib.lib().b2rl_a2c_rollout_loss_ctas(N))
+    partial = _Scratch.get(dev, "a2c_rollout_partial", max(3 * ctas, 1), _f32)
+    counter = _Scratch.get(dev, "a2c_rollout_counter", 1, torch.int32)
+    _lib.call("b2rl_a2c_rollout_loss", _lib.ptr(head), _lib.ptr(_c(action, torch.int64)), _lib.ptr(_c(reward, _f32)),
+              _lib.ptr(_c(mask, _f32)), float(discount), float(gae_tau), int(bool(use_gae)), float(entropy_weight),
+              float(value_loss_weight), T, N, A, _lib.ptr(r["adv"]), _lib.ptr(r["ret"]), _lib.ptr(r["loss"]),
+              _lib.ptr(r["geff"]), _lib.ptr(partial), _lib.ptr(counter), _lib.stream())
+    return r
+
+
 class _DQNDelta(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, q_next_target, q_next_online, action, reward, mask, gamma_n):

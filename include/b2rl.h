@@ -194,6 +194,20 @@ int b2rl_a2c_loss(const float* log_pi_a, const float* entropy, const float* v, c
                   const float* ret, float entropy_weight, float value_loss_weight, int32_t M, float* out,
                   float* dlogp_out, float* dent_out, float* dv_out, void* stream);
 
+/* A2CAgent's GAE and objective (A2C_agent.py:43-62) with the gradient to the actor-critic head, in one launch, for a rollout of
+ * T env steps x N workers: head [(T+1)*N][A+1] = (logits, v) rows t-major (b2rl_ac_head_fwd; rows T*N.. the final states),
+ * action [T*N] int64 in [0, A), reward / mask [T*N].  adv_out / ret_out [T*N] (may be NULL) are the bits of b2rl_gae mode 0.
+ * loss_out[0] = -mean(lp_a*adv) - ew*mean(H) + vw*0.5*mean((ret-v)^2) (may be NULL).  geff_out [(T+1)*N][33] = the loss's
+ * gradient with respect to the head's outputs in b2rl_head_bwd_geff_relu's layout (columns 0..A; the final rows zero).
+ * Limits: T >= 1, N >= 1, 1 <= A <= 31, (T+1)*N <= 2^24.  partial: float [3 * b2rl_a2c_rollout_loss_ctas(N)] scratch; counter:
+ * int32, zero-initialised once (the kernel re-arms it).  The loss is reduced in a fixed order: the same inputs give the same
+ * bits. */
+int b2rl_a2c_rollout_loss_ctas(int32_t N);
+int b2rl_a2c_rollout_loss(const float* head, const int64_t* action, const float* reward, const float* mask, float discount,
+                          float gae_tau, int32_t use_gae, float entropy_weight, float value_loss_weight, int32_t T, int32_t N,
+                          int32_t A, float* adv_out, float* ret_out, float* loss_out, float* geff_out, float* partial,
+                          int32_t* counter, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Multi-tensor optimizer step with global-norm clip (DQN_agent.py:132-134; examples.py:67-68,139,204):
  * flat float32 views of all parameters / gradients (one contiguous arena, n elements).
@@ -327,6 +341,19 @@ int b2rl_head_bwd(const float* gq, const uint16_t* phi, const float* Wa, const f
  * relu_colsum[K] (fp32, zero it first) receives the column sums of the masked gphi = that layer's bias gradient. */
 int b2rl_head_bwd_relu(const float* gq, const uint16_t* phi, const float* Wa, const float* Wv, int32_t B, int32_t K, int32_t A,
                        uint16_t* gphi, float* gWa, float* gba, float* gWv, float* gbv, float* relu_colsum, void* stream);
+/* Actor-critic head (CategoricalActorCriticNet with DummyBody actor / critic bodies): out [B][A+1] (fp32) = (phi Wa^T + ba,
+ * phi Wv^T + bv), Wa = fc_action [A][K], Wv = fc_critic [1][K].  counter != NULL: the action of row b is also drawn into
+ * action_out[b] (int64) -- the inverse CDF of softmax(logits) on Philox u24(seed, *counter + b, stream 13), as
+ * b2rl_a2c_actor_step draws it -- and *counter advances by B once every CTA has read it (ticket: int32, zero-initialised once;
+ * the kernel re-arms it).  0 < A <= 31, K % 8 == 0, phi and the weights 16-byte aligned. */
+int b2rl_ac_head_fwd(const uint16_t* phi, const float* Wa, const float* ba, const float* Wv, const float* bv, int32_t B,
+                     int32_t K, int32_t A, float* out, uint64_t seed, int64_t* counter, int64_t* action_out, int32_t* ticket,
+                     void* stream);
+/* b2rl_head_bwd_relu from effective output gradients geff [B][33] (column n < A: output n of Wa; column A: Wv's output when
+ * Wv != NULL) instead of gq -- the actor-critic head's backward from b2rl_a2c_rollout_loss's geff_out. */
+int b2rl_head_bwd_geff_relu(const float* geff, const uint16_t* phi, const float* Wa, const float* Wv, int32_t B, int32_t K,
+                            int32_t A, uint16_t* gphi, float* gWa, float* gba, float* gWv, float* gbv, float* relu_colsum,
+                            void* stream);
 
 /* Convolution weight gradient as split-K partials (no atomics): partial i of *n_partials_host (<= one per SM, written on the
  * HOST, deterministic for given shapes) is stored at partials + i * n_out*taps*C floats. */

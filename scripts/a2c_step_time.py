@@ -6,9 +6,10 @@ device flag (one actor-step launch per env step, one update launch per rollout o
 quantile_regression_dqn_feature: csrc/dist_dqn.cu, with the launchers' async actor), ``config.device_rainbow`` for
 CategoricalDQNAgent on a noisy RainbowNet (rainbow_feature: csrc/rainbow.cu), ``config.cuda_graph`` for NStepDQNAgent on the
 NatureConvBody (n_step_dqn_pixel on SyntheticAtari-v0: one GraphedQActor replay per env step, one GraphedNStepLearner replay per
-rollout; both it and the eager side at bf16, plus the launcher's default fp32 eager side) -- in one process on one card, the
-sides alternated round by round.  For n_step_dqn_pixel the captured update alone is also timed: CUDA events around back-to-back
-replays of its graph.  Also times the host envs alone (``task.step`` with fixed actions), so the share
+rollout; both it and the eager side at bf16, plus the launcher's default fp32 eager side), and ``config.cuda_graph`` for A2CAgent
+on the NatureConvBody the same way (a2c_pixel on SyntheticAtari-v0: one GraphedQActor replay per env step with the action drawn
+on the device, one GraphedA2CLearner replay per rollout) -- in one process on one card, the sides alternated round by round.
+For the pixel launchers the captured update alone is also timed: CUDA events around back-to-back replays of its graph.  Also times the host envs alone (``task.step`` with fixed actions), so the share
 left to the learner is visible.  Prints the card's name and power limit with the numbers.
 
     python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--only LAUNCHER[,LAUNCHER]] [--out DIR]
@@ -37,9 +38,11 @@ CONFIGS = [("a2c_feature", "CartPole-v0", "device_a2c", "a2c"), ("a2c_continuous
            ("categorical_dqn_feature", "CartPole-v0", "device_c51", "c51"),
            ("quantile_regression_dqn_feature", "CartPole-v0", "device_qr", "qr"),
            ("rainbow_feature", "CartPole-v0", "device_rainbow", "rainbow"),
-           ("n_step_dqn_pixel", "SyntheticAtari-v0", "cuda_graph", "nstep_dqn")]
+           ("n_step_dqn_pixel", "SyntheticAtari-v0", "cuda_graph", "nstep_dqn"),
+           ("a2c_pixel", "SyntheticAtari-v0", "cuda_graph", "a2c")]
 # launchers timed at a given Config.COMPUTE_DTYPE per side (set around every step of that side): side -> dtype
-DTYPES = {"n_step_dqn_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32}}
+DTYPES = {"n_step_dqn_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32},
+          "a2c_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32}}
 
 
 def card():
@@ -79,7 +82,7 @@ def timed(agent, steps, dtype=None):
 
 
 def update_replay_ms(agent, replays=400):
-    """The captured n-step update alone: CUDA events around ``replays`` back-to-back replays of its graph (on the rollout
+    """The captured rollout update alone: CUDA events around ``replays`` back-to-back replays of its graph (on the rollout
     staged last), milliseconds per replay."""
     g = agent._graph[0].graph
     for _ in range(20):
