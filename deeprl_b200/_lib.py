@@ -45,6 +45,9 @@ SIGNATURES = {
     "b2rl_normalize_advantage": [c_p, c_i32, c_p],
     "b2rl_ppo_loss": [c_p, c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_p, c_p, c_p, c_p, c_p],
     "b2rl_a2c_loss": [c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_p, c_p, c_p, c_p, c_p],
+    "b2rl_ppo_rollout_prep": [c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p],
+    "b2rl_ppo_cat_loss_ctas": [c_i32],
+    "b2rl_ppo_cat_loss": [c_p, c_p, c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p],
     "b2rl_a2c_rollout_loss_ctas": [c_i32],
     "b2rl_a2c_rollout_loss": [c_p, c_p, c_p, c_p, c_f32, c_f32, c_i32, c_f32, c_f32, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p,
                               c_p, c_p],
@@ -82,6 +85,8 @@ SIGNATURES = {
                                 c_p, c_p, c_p, c_f32, c_f32, c_p],
     "b2rl_nature_fused_opt": [c_p, c_i32, c_p, c_p, c_p, c_p, c_i32, c_f32, c_f32, c_f32, c_f32, c_f32, c_f32, c_p, c_i32, c_p,
                               c_p, c_i32, c_i32, c_f32, c_p, c_p, c_p, c_p, c_p, c_p, c_i32, c_p, c_p],
+    "b2rl_nature_fused_opt_lr": [c_p, c_i32, c_p, c_p, c_p, c_p, c_i32, c_f32, c_p, c_f32, c_f32, c_f32, c_f32, c_f32, c_p, c_i32,
+                                 c_p, c_p, c_i32, c_i32, c_f32, c_p, c_p, c_p, c_p, c_p, c_p, c_i32, c_p, c_p],
     "b2rl_gaussian_actor_step": [c_p, c_p, c_p, c_p, c_i32, c_f64, c_f64] + [c_p] * 13 + [c_i32] * 5 + [c_p, c_u64, c_p, c_p] + [c_p] * 6 + [c_p],
     "b2rl_ppo_set_phase_clocks": [c_p],
     "b2rl_ppo_minibatch_updates": [c_p] * 5 + [c_i32] * 5 + [c_p, c_i32] + [c_p] * 10 + [c_f32] * 11 + [c_p, c_p],

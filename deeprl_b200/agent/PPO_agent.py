@@ -5,6 +5,18 @@ representation) or one clipped optimizer step (shared representation).
 CUDA device: GAE = ``b2rl_gae``, advantage normalisation = ``b2rl_normalize_advantage``, each minibatch's surrogate /
 value loss / approx-KL and their gradients = one ``b2rl_ppo_loss`` launch.  ``select_device(-1)``: torch statements
 (the reference's own CPU path; see A2C_agent.py docstring).
+
+``config.cuda_graph = True`` (off by default) runs each ``step()`` of a shared-representation CategoricalActorCriticNet on a
+wgmma NatureConvBody at bf16 (``ppo_pixel`` with ``Config.COMPUTE_DTYPE = torch.bfloat16``) as captured graphs: one
+``GraphedQActor`` replay per env step (pinned upload of the frame stacks into the rollout arena, the body, the actor-critic
+head with the action drawn on the device, the actions down to the host) and one ``GraphedPPOPixelLearner`` replay per rollout
+(learner.py: the final states' value, GAE and the old log-probabilities from the actor's outputs, advantage normalisation,
+then every epoch's minibatch updates unrolled).  The actions then come from the device's Philox stream (keyed from torch's
+seeded generator, as in ``a2c_pixel``), not from torch's ``Categorical.sample``; the minibatches are still drawn by
+``random_sample`` on the host.  A ``FlatOptimizer`` built from ``self.opt`` takes over the Adam state; ``self.opt`` stays as
+the holder of ``lr_scheduler``'s learning rate, which each update reads from the device.  The network's parameters become
+views into the optimizer's arena, so ``state_dict()`` is always current.  Configurations it does not cover
+(``component/actor.py ppo_graph_unsupported``; the reason is kept in ``graph_refusal``) keep the eager path.
 """
 import numpy as np
 import torch
@@ -36,6 +48,8 @@ class PPOAgent(BaseAgent):
             self.lr_scheduler = torch.optim.lr_scheduler.LambdaLR(self.opt, lambda step: 1 - step / config.max_steps)
         self.gae_exact = True
         self.last_stats = None
+        self._graph = None                                 # cuda_graph: (GraphedPPOPixelLearner, GraphedQActor)
+        self._graph_checked, self.graph_refusal = False, None
         # data parallel under torchrun (parallel.init(), world > 1): rank-local rollout / GAE / advantage normalisation /
         # permutations / state normaliser; every minibatch update is one step on the union of the ranks' minibatches, with the
         # gradients exchanged inside the persistent PPO kernel.  Parameters start as rank 0's.
@@ -48,6 +62,11 @@ class PPOAgent(BaseAgent):
             with torch.no_grad():
                 for p in self.network.parameters():
                     dist.broadcast(p.data, 0)
+
+    def load(self, filename):
+        BaseAgent.load(self, filename)
+        if self._graph_checked and self.graph_refusal is None:
+            self._graph[0].refresh_packed()                # the next step trains (and acts) from the loaded weights
 
     def eval_step(self, state):
         with torch.no_grad():
@@ -202,6 +221,8 @@ class PPOAgent(BaseAgent):
             self.critic_opt.step()
 
     def step(self):
+        if self._graph_ok():
+            return self._step_graph()
         config = self.config
         entries = self._rollout()
         self._normalize(entries)
@@ -255,3 +276,57 @@ class PPOAgent(BaseAgent):
         batches = [b for _ in range(config.optimization_epochs) for b in random_sample(np.arange(rows), mb)]
         g.run(g.set_batches(batches))
         self.last_stats = g.stats
+
+    # ------------------------------------------------------------------ config.cuda_graph (opt-in)
+    def _graph_ok(self):
+        """Decided on the first step: the captured actor + update serve this configuration (``ppo_graph_unsupported``), or the
+        eager path runs (the reason is kept in ``graph_refusal``)."""
+        if not self._graph_checked:
+            from ..component.actor import GraphedQActor, ppo_graph_unsupported
+            from ..learner import GraphedPPOPixelLearner
+            config = self.config
+            self._graph_checked = True
+            self.graph_refusal = ppo_graph_unsupported(config, self.network, getattr(self, "opt", None), self._raw_states)
+            if self.graph_refusal is None:
+                self.flat_opt = ops.FlatOptimizer.from_torch(self.opt, list(self.network.parameters()))
+                seed = int(torch.randint(0, 2 ** 62, (1,)).item())      # the Philox key, from torch's (seeded) generator
+                coef = config.state_normalizer.coef
+                lr = GraphedPPOPixelLearner(self.network, self.flat_opt, config.rollout_length, config.num_workers, seed,
+                                            config.mini_batch_size, config.optimization_epochs, config.discount,
+                                            config.gae_tau, config.use_gae, config.ppo_ratio_clip, config.entropy_weight,
+                                            config.gradient_clip, coef).capture()
+                actor = GraphedQActor(self.network, None, config.num_workers, 4, (84, 84), coef, arena=lr.arena, run=lr.act,
+                                      body=self.network.phi_body)
+                self._graph = (lr, actor)
+        return self.graph_refusal is None
+
+    def graph_lr(self):
+        """``lr_scheduler.step(self.total_steps)`` (PPO_agent.py:67) and the learning rate it leaves on ``self.opt``: what the
+        update graph's Adam uses for this rollout."""
+        self.lr_scheduler.step(self.total_steps)
+        return float(self.opt.param_groups[0]["lr"])
+
+    def _step_graph(self):
+        """``step()`` with ``config.cuda_graph``: T actor replays (the action drawn on the device into the learner's action row
+        t; its pinned download is the step's only synchronisation), each followed by ``task.step`` on the host, with rewards
+        and masks written into the learner's pinned staging buffer; then the final states, the learning rate, the minibatches
+        of every epoch (``random_sample``, as the eager loop draws them) and one update replay."""
+        config = self.config
+        lr, actor = self._graph
+        states = self._raw_states
+        for t in range(config.rollout_length):
+            actions = actor.q_values(states, t)
+            next_states, rewards, terminals, info = self.task.step(actions)
+            self.record_online_return(info)
+            lr.h_reward[t].numpy()[...] = np.asarray(config.reward_normalizer(rewards), dtype=np.float32)   # tensor(): float32
+            lr.h_mask[t].numpy()[...] = 1 - np.asarray(terminals, dtype=np.float32)
+            states = next_states
+            self.total_steps += config.num_workers
+        self._raw_states = states
+        self.states = config.state_normalizer(states)
+        lr.stage_final(states)
+        rows = config.rollout_length * config.num_workers
+        step_lr = self.graph_lr()
+        batches = [b for _ in range(config.optimization_epochs) for b in random_sample(np.arange(rows), config.mini_batch_size)]
+        lr.stage_batches(batches, step_lr)
+        self.last_stats = lr.update()

@@ -2,7 +2,9 @@
 two ``task.step()`` calls (PPO_agent.py:45-50) -- ``MeanStdNormalizer`` (normalizer.py:36-51), the ``GaussianActorCriticNet``
 forward (network_heads.py:173-214) and the Normal sample / log-prob / entropy -- as ONE launch of ``b2rl_gaussian_actor_step``
 (csrc/actor.cu) on a pinned, double-buffered observation upload.  The envs stay on the host (north_star)."""
+import contextlib
 import ctypes
+import gc
 
 import numpy as np
 import torch
@@ -223,7 +225,7 @@ class GraphedQActor:
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         pool = next((h.pool() for h in self.graphs if h is not None), None)     # the slots' graphs replay one at a time
-        with torch.cuda.graph(g, pool=pool):
+        with no_gc(), torch.cuda.graph(g, pool=pool):
             self._forward(slot)
         self.graphs[slot] = g
         self._sig = self._signature()
@@ -256,6 +258,19 @@ def q_actor_supported(config, network):
                 and body.conv1.in_channels == 4
                 and Config.COMPUTE_DTYPE == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
                 and isinstance(config.state_normalizer, RescaleNormalizer))
+
+
+@contextlib.contextmanager
+def no_gc():
+    """No garbage collection inside a graph capture: collecting unreachable objects that own CUDA resources (pinned buffers,
+    graphs, streams of an agent dropped earlier) frees them mid-capture, which invalidates the capture."""
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 def nstep_q_graph_unsupported(config, network, optimizer, states):
@@ -349,6 +364,23 @@ def a2c_graph_unsupported(config, network, optimizer, states):
     if not body.conv1.weight.is_cuda:
         return "the network is not on a CUDA device (select_device(0))"
     return None
+
+
+def ppo_graph_unsupported(config, network, optimizer, states):
+    """``None`` when ``PPOAgent.step()`` runs as captured graphs under ``config.cuda_graph`` (GraphedQActor with
+    learner.GraphedPPOPixelLearner.act per env step, GraphedPPOPixelLearner per rollout), else the unmet condition; the agent
+    then keeps its eager path.  The conditions of ``a2c_graph_unsupported`` (the same network, optimizer and frames), plus a
+    shared representation (one optimizer over the whole network) and rollouts of whole minibatches.  ``states``: the envs'
+    current raw observations."""
+    if not getattr(config, "cuda_graph", False):
+        return "config.cuda_graph is not set"
+    if not config.shared_repr:
+        return "config.shared_repr is not set; the captured update implements one optimizer over the shared network"
+    rows = config.rollout_length * config.num_workers
+    if rows < 2 or rows % config.mini_batch_size:
+        return ("the rollout's %d rows are not a multiple of mini_batch_size %d; random_sample would yield a short last "
+                "minibatch" % (rows, config.mini_batch_size))
+    return a2c_graph_unsupported(config, network, optimizer, states)
 
 
 # ------------------------------------------------------------------------------------------------ A2C on the device

@@ -1,4 +1,5 @@
-// onpolicy.cu -- GAE backward recurrence, advantage normalisation, PPO clipped surrogate, A2C objective.
+// onpolicy.cu -- GAE backward recurrence, advantage normalisation, PPO clipped surrogate, A2C objective, and the rollout
+// launches of the captured pixel learners (A2C rollout loss, PPO rollout prep and categorical minibatch loss).
 // Reference: deep_rl/agent/A2C_agent.py:43-64, deep_rl/agent/PPO_agent.py:51-86.  sm_90a only.
 #include "common.cuh"
 
@@ -278,6 +279,138 @@ __global__ void __launch_bounds__(A2CR_WARPS * 32) a2c_rollout_loss_kernel(
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// PPO_agent.py:44-66 (shared_repr) for a rollout whose (logits, v) rows the actor's head launches stored: head
+// [(T+1) N][A + 1] (rows t-major, slot T the final states).  One warp per env column: every lane runs the column's backward
+// GAE scan in gae_seq_kernel's order (the bits of ops.gae(exact=True)) and the warp takes the log-softmax of each row at its
+// action (Categorical.log_prob: the pre-update log pi(a|s) the ratio needs).  adv_out is normalised afterwards by
+// b2rl_normalize_advantage.
+__global__ void __launch_bounds__(A2CR_WARPS * 32) ppo_rollout_prep_kernel(
+    const float* __restrict__ head, const int64_t* __restrict__ action, const float* __restrict__ reward,
+    const float* __restrict__ mask, float discount, float tau, int use_gae, int T, int N, int A,
+    float* __restrict__ logp_out, float* __restrict__ adv_out, float* __restrict__ ret_out) {
+  pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int n = blockIdx.x * A2CR_WARPS + warp;
+  if (n >= N) return;
+  const int ld = A + 1;
+  float ret = head[((int64_t)T * N + n) * ld + A];
+  float adv = 0.0f;
+  float vnext = ret;
+  for (int t = T - 1; t >= 0; --t) {
+    const int64_t i = (int64_t)t * N + n;
+    const float r = reward[i], m = mask[i], v = head[i * ld + A];
+    const float gm = __fmul_rn(discount, m);
+    ret = __fadd_rn(r, __fmul_rn(gm, ret));
+    if (use_gae) {
+      const float td = __fsub_rn(__fadd_rn(r, __fmul_rn(gm, vnext)), v);
+      adv = __fadd_rn(__fmul_rn(__fmul_rn(__fmul_rn(adv, tau), discount), m), td);
+    } else {
+      adv = __fsub_rn(ret, v);
+    }
+    vnext = v;
+    const float z = lane < A ? head[i * ld + lane] : -INFINITY;
+    float mx = z;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const float s = a2cr_warp_sum(lane < A ? expf(z - mx) : 0.0f);
+    const float lp = (z - mx) - logf(s);
+    const float lp_a = __shfl_sync(0xffffffffu, lp, (int)action[i] & 31);
+    if (lane == 0) {
+      logp_out[i] = lp_a;
+      adv_out[i] = adv;
+      ret_out[i] = ret;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// PPO_agent.py:77-92 (shared_repr) for one minibatch of a categorical actor-critic head: head [B][A + 1] = (logits, v) of the
+// minibatch's rows, idx [B] their rows in the rollout, through which action / old_logp / adv (normalised) / ret are read.
+// One warp per row, lane j < A owning logit j: p = softmax(z), lp = log_softmax(z), H = -sum p lp, r = exp(lp_a - old_lp_a),
+//   policy_loss = -mean(min(r A, clamp(r, 1 - c, 1 + c) A)) - ew mean(H),   value_loss = 0.5 mean((ret - v)^2)
+//   geff[b][j] = g_b (1[j = a] - p_j) + (ew / B) p_j (lp_j + H),   geff[b][A] = (v - ret) / B
+// with g_b = d policy_loss / d lp_a under ppo_loss_kernel's tie and boundary rules (torch.min splits a tie evenly; clamp
+// passes the gradient on the closed interval).  Each CTA parks its four sums (min-objective, H, (ret - v)^2, old_lp - lp_a;
+// per warp in row order, then in warp order) in partial[4 cta ..] and the last CTA adds them in CTA order: two launches on
+// the same inputs give the same bits of stats = [policy_loss, value_loss, approx_kl].
+constexpr int PPOC_WARPS = 8;
+
+__global__ void __launch_bounds__(PPOC_WARPS * 32) ppo_cat_loss_kernel(
+    const float* __restrict__ head, const int64_t* __restrict__ idx, const int64_t* __restrict__ action,
+    const float* __restrict__ old_logp, const float* __restrict__ adv, const float* __restrict__ ret, float clip, float ew,
+    int B, int A, float* __restrict__ geff, float* __restrict__ stats, float* __restrict__ partial,
+    int32_t* __restrict__ counter) {
+  pdl_sync();   // PDL contract (common.cuh): before any global-memory access or return
+  __shared__ float s_sum[4][PPOC_WARPS];
+  __shared__ bool is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int b = blockIdx.x * PPOC_WARPS + warp;
+  const float invB = 1.0f / (float)B;
+  float s_obj = 0.0f, s_ent = 0.0f, s_val = 0.0f, s_kl = 0.0f;
+  if (b < B) {
+    const int ld = A + 1;
+    const int64_t i = idx[b];
+    const int a_i = (int)action[i];
+    const float z = lane < A ? head[(int64_t)b * ld + lane] : -INFINITY;
+    const float v = head[(int64_t)b * ld + A];
+    float mx = z;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const float e = lane < A ? expf(z - mx) : 0.0f;
+    const float s = a2cr_warp_sum(e);
+    const float lp = lane < A ? (z - mx) - logf(s) : 0.0f;
+    const float p = e / s;
+    const float H = -a2cr_warp_sum(p * lp);
+    const float lp_a = __shfl_sync(0xffffffffu, lp, a_i & 31);
+    const float olp = old_logp[i], A_i = adv[i], R_i = ret[i];
+    // ppo_loss_kernel's statements for this row
+    const float ratio = expf(__fsub_rn(lp_a, olp));
+    const float obj = __fmul_rn(ratio, A_i);
+    const float rc = fminf(fmaxf(ratio, 1.0f - clip), 1.0f + clip);
+    const float objc = __fmul_rn(rc, A_i);
+    const bool inside = ratio >= 1.0f - clip && ratio <= 1.0f + clip;
+    float g;
+    if (obj < objc) g = A_i * ratio;
+    else if (obj > objc) g = inside ? A_i * ratio : 0.0f;
+    else g = 0.5f * A_i * ratio + (inside ? 0.5f * A_i * ratio : 0.0f);
+    const float dlogp = -g * invB;
+    const float d = __fsub_rn(R_i, v);
+    if (lane < A) {
+      geff[(int64_t)b * A2CR_LD + lane] = dlogp * ((lane == a_i ? 1.0f : 0.0f) - p) + (ew * invB) * (p * (lp + H));
+    } else if (lane == A) {
+      geff[(int64_t)b * A2CR_LD + A] = -d * invB;
+    }
+    s_obj = fminf(obj, objc);
+    s_ent = H;
+    s_val = __fmul_rn(d, d);
+    s_kl = __fsub_rn(olp, lp_a);
+  }
+  if (lane == 0) s_sum[0][warp] = s_obj, s_sum[1][warp] = s_ent, s_sum[2][warp] = s_val, s_sum[3][warp] = s_kl;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int q = 0; q < 4; ++q) {
+      float c = 0.0f;
+      for (int w = 0; w < PPOC_WARPS; ++w) c = __fadd_rn(c, s_sum[q][w]);
+      partial[4 * blockIdx.x + q] = c;
+    }
+    __threadfence();
+    is_last = atomicAdd(counter, 1) == (int)gridDim.x - 1;
+  }
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {              // deterministic final reduction in CTA order
+    __threadfence();
+    float tot[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    for (int c = 0; c < (int)gridDim.x; ++c)
+      for (int q = 0; q < 4; ++q) tot[q] = __fadd_rn(tot[q], __ldcg(partial + 4 * c + q));
+    const float Bf = (float)B;
+    stats[0] = __fsub_rn(-__fdiv_rn(tot[0], Bf), __fmul_rn(ew, __fdiv_rn(tot[1], Bf)));
+    stats[1] = __fmul_rn(0.5f, __fdiv_rn(tot[2], Bf));
+    stats[2] = __fdiv_rn(tot[3], Bf);
+    *counter = 0;
+  }
+}
+
 }  // namespace b2rl
 
 using namespace b2rl;
@@ -339,4 +472,28 @@ extern "C" int b2rl_a2c_rollout_loss(const float* head, const int64_t* action, c
              head, action, reward, mask, discount, gae_tau, (int)use_gae, entropy_weight, value_loss_weight, (int)T, (int)N,
              (int)A, adv_out, ret_out, loss_out, geff_out, partial, counter);
   return check_launch("b2rl_a2c_rollout_loss");
+}
+
+extern "C" int b2rl_ppo_rollout_prep(const float* head, const int64_t* action, const float* reward, const float* mask,
+                                     float discount, float gae_tau, int32_t use_gae, int32_t T, int32_t N, int32_t A,
+                                     float* logp_out, float* adv_out, float* ret_out, void* stream) {
+  B2RL_REQUIRE(head && action && reward && mask && logp_out && adv_out && ret_out, "null pointer");
+  B2RL_REQUIRE(T >= 1 && N >= 1 && A >= 1 && A + 1 <= A2CR_LD - 1, "bad shape: needs T >= 1, N >= 1 and 1 <= A <= 31");
+  B2RL_REQUIRE((int64_t)(T + 1) * N <= A2CR_MAX_ROWS, "(T + 1) * N must not exceed 2^24 rows");
+  launch_pdl(ppo_rollout_prep_kernel, dim3((N + A2CR_WARPS - 1) / A2CR_WARPS), dim3(A2CR_WARPS * 32), 0,
+             (cudaStream_t)stream, head, action, reward, mask, discount, gae_tau, (int)use_gae, (int)T, (int)N, (int)A,
+             logp_out, adv_out, ret_out);
+  return check_launch("b2rl_ppo_rollout_prep");
+}
+
+extern "C" int b2rl_ppo_cat_loss_ctas(int32_t B) { return B > 0 ? (B + PPOC_WARPS - 1) / PPOC_WARPS : 0; }
+
+extern "C" int b2rl_ppo_cat_loss(const float* head, const int64_t* idx, const int64_t* action, const float* old_logp,
+                                 const float* adv, const float* ret, float clip, float entropy_weight, int32_t B, int32_t A,
+                                 float* geff_out, float* stats_out, float* partial, int32_t* counter, void* stream) {
+  B2RL_REQUIRE(head && idx && action && old_logp && adv && ret && geff_out && stats_out && partial && counter, "null pointer");
+  B2RL_REQUIRE(B >= 1 && B <= A2CR_MAX_ROWS && A >= 1 && A + 1 <= A2CR_LD - 1, "bad shape: needs 1 <= B <= 2^24 and 1 <= A <= 31");
+  launch_pdl(ppo_cat_loss_kernel, dim3(b2rl_ppo_cat_loss_ctas(B)), dim3(PPOC_WARPS * 32), 0, (cudaStream_t)stream, head, idx,
+             action, old_logp, adv, ret, clip, entropy_weight, (int)B, (int)A, geff_out, stats_out, partial, counter);
+  return check_launch("b2rl_ppo_cat_loss");
 }

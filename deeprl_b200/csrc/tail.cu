@@ -193,6 +193,7 @@ struct OptArgs {
   __nv_bfloat16* w1f; __nv_bfloat16* w2f; __nv_bfloat16* w2d; __nv_bfloat16* w3f; __nv_bfloat16* w3d; __nv_bfloat16* w4p;
   int zero_grad;
   __nv_bfloat16* shadow;        // bf16 copy of the whole arena at the same offsets, or null (the GEMM operands of the heads)
+  const float* lr_dev;          // the learning rate on the device (a schedule stepped between graph replays), or null: lr
 };
 
 __global__ void __launch_bounds__(TAIL_THREADS) nature_fused_opt_kernel(const OptArgs a) {
@@ -214,11 +215,12 @@ __global__ void __launch_bounds__(TAIL_THREADS) nature_fused_opt_kernel(const Op
   } else {
     coef = a.sc->coef;
   }
-  float step_size = a.lr, bc2s = 1.0f;
+  const float lr = a.lr_dev ? *a.lr_dev : a.lr;
+  float step_size = lr, bc2s = 1.0f;
   if (a.opt == 2) {
     const float t = (float)(*a.step_dev);
     const float bc1 = 1.0f - powf(a.a, t), bc2 = 1.0f - powf(a.b, t);
-    step_size = a.lr / bc1;
+    step_size = lr / bc1;
     bc2s = sqrtf(bc2);
   }
   const bool packs = kind >= U_W1 && kind <= U_W4 && a.w4p != nullptr;
@@ -265,7 +267,7 @@ __global__ void __launch_bounds__(TAIL_THREADS) nature_fused_opt_kernel(const Op
         } else {
           avg = sqrtf(s) + a.eps;
         }
-        p[j] = p[j] - a.lr * (gr / avg);
+        p[j] = p[j] - lr * (gr / avg);
       }
     }
     p4[v] = make_float4(p[0], p[1], p[2], p[3]);
@@ -337,12 +339,14 @@ extern "C" int b2rl_nature_grad_reduce(const int32_t* units, int32_t n_units, co
   return check_launch("b2rl_nature_grad_reduce");
 }
 
-extern "C" int b2rl_nature_fused_opt(const int32_t* units, int32_t n_units, float* param, float* grad, float* s1, float* s2,
-                                     int32_t opt, float lr, float a_, float b_, float eps, float max_norm, float grad_scale,
-                                     const float* unit_sumsq, int32_t n_sumsq, void* norm_scratch, const int64_t* step_dev,
-                                     int32_t c1, int32_t n4, float scale, uint16_t* w1f, uint16_t* w2f, uint16_t* w2d,
-                                     uint16_t* w3f, uint16_t* w3d, uint16_t* w4p, int32_t zero_grad, uint16_t* bf16_shadow,
-                                     void* stream) {
+// b2rl_nature_fused_opt with the learning rate read from the device: lr_dev != NULL replaces lr (a float32 the host writes
+// between replays of a captured graph, e.g. a decaying schedule); lr_dev == NULL is b2rl_nature_fused_opt.
+extern "C" int b2rl_nature_fused_opt_lr(const int32_t* units, int32_t n_units, float* param, float* grad, float* s1, float* s2,
+                                        int32_t opt, float lr, const float* lr_dev, float a_, float b_, float eps,
+                                        float max_norm, float grad_scale, const float* unit_sumsq, int32_t n_sumsq,
+                                        void* norm_scratch, const int64_t* step_dev, int32_t c1, int32_t n4, float scale,
+                                        uint16_t* w1f, uint16_t* w2f, uint16_t* w2d, uint16_t* w3f, uint16_t* w3d, uint16_t* w4p,
+                                        int32_t zero_grad, uint16_t* bf16_shadow, void* stream) {
   B2RL_REQUIRE(units && param && grad && s1 && norm_scratch, "null pointer");
   B2RL_REQUIRE(opt >= 0 && opt <= 2 && (opt == 0 || s2) && (opt != 2 || step_dev), "bad optimizer description");
   B2RL_REQUIRE(n_units > 0 && (!unit_sumsq || n_sumsq > 0), "bad counts");
@@ -360,6 +364,18 @@ extern "C" int b2rl_nature_fused_opt(const int32_t* units, int32_t n_units, floa
   a.w3d = reinterpret_cast<__nv_bfloat16*>(w3d); a.w4p = reinterpret_cast<__nv_bfloat16*>(w4p);
   a.zero_grad = zero_grad;
   a.shadow = reinterpret_cast<__nv_bfloat16*>(bf16_shadow);
+  a.lr_dev = lr_dev;
   launch_pdl(nature_fused_opt_kernel, dim3(n_units), dim3(TAIL_THREADS), 0, (cudaStream_t)stream, a);
   return check_launch("b2rl_nature_fused_opt");
+}
+
+extern "C" int b2rl_nature_fused_opt(const int32_t* units, int32_t n_units, float* param, float* grad, float* s1, float* s2,
+                                     int32_t opt, float lr, float a_, float b_, float eps, float max_norm, float grad_scale,
+                                     const float* unit_sumsq, int32_t n_sumsq, void* norm_scratch, const int64_t* step_dev,
+                                     int32_t c1, int32_t n4, float scale, uint16_t* w1f, uint16_t* w2f, uint16_t* w2d,
+                                     uint16_t* w3f, uint16_t* w3d, uint16_t* w4p, int32_t zero_grad, uint16_t* bf16_shadow,
+                                     void* stream) {
+  return b2rl_nature_fused_opt_lr(units, n_units, param, grad, s1, s2, opt, lr, nullptr, a_, b_, eps, max_norm, grad_scale,
+                                  unit_sumsq, n_sumsq, norm_scratch, step_dev, c1, n4, scale, w1f, w2f, w2d, w3f, w3d, w4p,
+                                  zero_grad, bf16_shadow, stream);
 }

@@ -613,7 +613,8 @@ class _RolloutLearner(_NatureLearner):
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        from .component.actor import no_gc
+        with no_gc(), torch.cuda.graph(self.graph):
             self._main()
             self._opt()
         for t, v in zip(self._state(), saved):
@@ -788,6 +789,125 @@ class GraphedA2CLearner(_RolloutLearner):
         self.graph.replay()
         self.updates += 1
         return self.loss
+
+
+class GraphedPPOPixelLearner(_RolloutLearner):
+    """The update of ``PPOAgent.step()`` with ``config.shared_repr`` (PPO_agent.py:44-99) for a CategoricalActorCriticNet whose
+    ``phi_body`` is a wgmma NatureConvBody (DummyBody actor / critic bodies) as ONE captured graph per rollout, in order:
+
+    * one packed upload: the minibatch rows of all E epochs x M minibatches (drawn on the host by ``random_sample``, so numpy's
+      stream is consumed as on the eager path), the rollout's rewards / masks, and this rollout's learning rate; and the final
+      states' stacks up into arena slot T;
+    * the body at batch N on the final states (K1) and the head without a draw -> ``act_out[T]`` (the reference's
+      ``self.network(states)`` after the loop);
+    * ``b2rl_ppo_rollout_prep``: the old log-probabilities at the taken actions, and ``ret`` / ``adv`` by GAE, from the
+      (logits, v) rows the actor's replays stored in ``act_out`` -- the pre-update policy, not recomputed; then
+      ``b2rl_normalize_advantage``;
+    * E M minibatch updates, unrolled: the body at batch ``mini_batch_size`` on the minibatch's arena rows (K1: conv1's
+      forward and weight gradient read the uint8 frames), the head, ``b2rl_ppo_cat_loss``, the head backward with fc4's ReLU,
+      the fused body backward (weight gradients on the side branch) and the update tail (gradient reduce,
+      ``clip_grad_norm_``, Adam at the device learning rate, bf16 operand writes that the next minibatch and the next actor
+      replay read).
+
+    The actions are drawn by the actor's replays (``act``, as ``GraphedA2CLearner``) into ``d_action`` row t: the inverse CDF
+    of the softmax on Philox ``u24(seed, counter + n, 13)`` -- not torch's ``Categorical.sample``."""
+
+    body_attr = "phi_body"
+    act = GraphedA2CLearner.act
+
+    def __init__(self, network, optimizer, rollout_length, num_envs, seed, mini_batch_size, optimization_epochs,
+                 discount=0.99, gae_tau=0.95, use_gae=True, ppo_ratio_clip=0.1, entropy_weight=0.01, gradient_clip=0.5,
+                 state_scale=1.0 / 255, history=4, frame_hw=(84, 84)):
+        self.tgt = None
+        self.discount, self.gae_tau, self.use_gae = float(discount), float(gae_tau), bool(use_gae)
+        self.ratio_clip, self.ew = float(ppo_ratio_clip), float(entropy_weight)
+        idx = self._init_rollout(network, optimizer, rollout_length, num_envs, gradient_clip, state_scale, history, frame_hw)
+        T, N, hl, dev = self.T, self.N, self.hl, self.dev
+        rows = T * N
+        self.mb, self.epochs = int(mini_batch_size), int(optimization_epochs)
+        if rows % self.mb or rows < 2:
+            raise _lib.B2RLError("GraphedPPOPixelLearner: the rollout's %d rows must be at least 2 and a multiple of "
+                                 "mini_batch_size %d" % (rows, self.mb))
+        self.n_batches = self.epochs * (rows // self.mb)
+        K = self.n_batches * self.mb
+        row = frame_hw[0] * frame_hw[1]
+        self.final = nature_tc.RingFrames(self.arena, idx[T * N:], 0, row, frame_hw[1], hl)
+        # ONE packed pinned staging buffer and ONE device mirror -> a single host->device copy node:
+        # [rollout row int64 K | arena row int64 K | reward float32 T*N | mask float32 T*N | lr float32 (+ pad)]
+        nbytes = 16 * K + 8 * rows + 8
+        self.h_pack = torch.zeros(nbytes, dtype=torch.uint8, pin_memory=True)
+        self.d_pack = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+
+        def views(buf):
+            o = [0, 8 * K, 16 * K, 16 * K + 4 * rows, 16 * K + 8 * rows]
+            return (buf[o[0]:o[1]].view(torch.int64).view(self.n_batches, self.mb),
+                    buf[o[1]:o[2]].view(torch.int64).view(self.n_batches, self.mb),
+                    buf[o[2]:o[3]].view(torch.float32).view(T, N), buf[o[3]:o[4]].view(torch.float32).view(T, N),
+                    buf[o[4]:o[4] + 4].view(torch.float32))
+
+        self.h_idx, self.h_arow, self.h_reward, self.h_mask, self.h_lr = views(self.h_pack)
+        self.d_idx, self.d_arow, self.d_reward, self.d_mask, self.d_lr = views(self.d_pack)
+        self.batches = [nature_tc.RingFrames(self.arena, self.d_arow[j], 0, row, frame_hw[1], hl) for j in range(self.n_batches)]
+        A = network.fc_action.out_features
+        self.d_action = torch.zeros((T, N), dtype=torch.int64, device=dev)          # row t: the actor replay of env step t
+        self.seed = int(seed)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=dev)               # Philox position of the next draw
+        self.ticket = torch.zeros(1, dtype=torch.int32, device=dev)
+        # the actor's (logits, v) per slot; slot T: the final states' (written by the update)
+        self.act_out = torch.zeros((T + 1, N, A + 1), dtype=torch.float32, device=dev)
+        self.roll = {k: torch.zeros(rows, dtype=torch.float32, device=dev) for k in ("logp", "adv", "ret")}
+        self.head_mb = torch.zeros((self.mb, A + 1), dtype=torch.float32, device=dev)
+        self.geff = torch.zeros((self.mb, ops.AC_GEFF_LD), dtype=torch.float32, device=dev)
+        self.stats = torch.zeros((self.n_batches, 3), dtype=torch.float32, device=dev)    # per minibatch: [pl, vl, kl]
+        self.tail().lr_dev = self.d_lr
+
+    def _resolve_plan(self):
+        tail = self._tail_applies()
+        return UpdatePlan(ring=True, tail=tail, repack_online=not tail, dist_head=False, head="separate", forward="one-stream",
+                          conv1="separate", single_stream=False, prefetch=None, join=None, one_graph=True)
+
+    def stage_batches(self, batches, lr):
+        """The E M minibatches' rollout rows (``random_sample``'s arrays, in order) and this rollout's learning rate into the
+        pinned buffer the update uploads."""
+        b = np.asarray(batches, dtype=np.int64).reshape(self.n_batches, self.mb)
+        self.h_idx.numpy()[...] = b
+        self.h_arow.numpy()[...] = b * self.hl
+        self.h_lr.numpy()[0] = lr
+
+    def _main(self):
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.dev)
+        side, tail, net = self._side, self.tail(), self.net
+        body = self._body(net)
+        T, k = self.T, self.N * self.hl
+        self.arena[T * k:(T + 1) * k].copy_(self.h_final, non_blocking=True)
+        self.d_pack.copy_(self.h_pack, non_blocking=True)
+        with torch.no_grad(), frame_scale(self.scale):
+            fused.ac_head(body(self.final), net.fc_action, net.fc_critic, out=self.act_out[T])
+        r = ops.ppo_rollout_prep(self.act_out.view((T + 1) * self.N, -1), self.d_action, self.d_reward, self.d_mask,
+                                 self.discount, self.gae_tau, self.use_gae, out=self.roll)
+        ops.normalize_advantage_(r["adv"])
+        for j in range(self.n_batches):
+            with frame_scale(self.scale):
+                phi = body(self.batches[j])
+            fused.ac_head(phi.detach(), net.fc_action, net.fc_critic, out=self.head_mb)
+            ops.ppo_cat_loss(self.head_mb, self.d_idx[j], self.d_action, r["logp"], r["adv"], r["ret"], self.ratio_clip,
+                             self.ew, geff=self.geff, stats=self.stats[j])
+            with nature_tc.wgrad_stream(side), nature_tc.grad_sink(tail):     # weight-gradient GEMMs on the side branch
+                phi.backward(fused.ac_head_backward(phi, self.geff, net.fc_action, net.fc_critic))
+            tail.step(max_norm=self.clip)
+
+    def _opt(self):
+        """(The optimizer steps run inside ``_main``, one per minibatch.)"""
+
+    def update(self):
+        """One rollout's update (graph replay) on what the caller staged: ``h_reward`` / ``h_mask`` [T, N], the rollout's stacks
+        in arena slots 0..T-1 with their actions in ``d_action`` and (logits, v) in ``act_out`` (the actor replays), the final
+        states (``stage_final``), and the minibatches and learning rate (``stage_batches``).  Returns the device statistics
+        [policy_loss, value_loss, approx_kl] of the last minibatch (no sync)."""
+        self.graph.replay()
+        self.updates += 1
+        return self.stats[-1]
 
 
 class _PPOLearner:

@@ -7,7 +7,8 @@
   partials summed, GEMM layouts -> reference layouts, written into the ``.grad`` arena, bias gradients moved, sum of
   squares per unit.
 * ``step(max_norm, grad_scale)`` -- kernel B: clip coefficient, RMSprop / Adam, gradient re-zeroed, updated weights written
-  into the packed bf16 operands (no separate pack launch, no ``zero_grad`` memset).
+  into the packed bf16 operands (no separate pack launch, no ``zero_grad`` memset).  With ``lr_dev`` set (a float32 device
+  scalar) the kernel reads the learning rate there instead of ``opt.lr``.
 
 The unit tables (int32 x 4 per unit, see the header of csrc/tail.cu) are built here once.
 """
@@ -98,6 +99,8 @@ class NatureTail:
         # clip_grad_norm_'s arguments of the NEXT step(): kernel A's last CTA already turns its unit partials into the
         # coefficient, so kernel B starts with one scalar load (set by the owner before the backward pass)
         self.max_norm, self.grad_scale = 0.0, 1.0
+        # a float32 device scalar that replaces opt.lr in step() (a schedule the owner writes between graph replays), or None
+        self.lr_dev = None
 
     def packed(self):
         from . import nature_tc
@@ -145,9 +148,9 @@ class NatureTail:
             _lib.call("b2rl_grad_norm", _lib.ptr(o.grad), o.n, float(grad_scale), float(max_norm or 0.0), _lib.ptr(o.scratch),
                       _lib.stream())
         a, b = (o.betas if o.kind == "adam" else (o.alpha, 0.0))
-        _lib.call("b2rl_nature_fused_opt", _lib.ptr(self.b_units), self.n_b, _lib.ptr(o.flat), _lib.ptr(o.grad), _lib.ptr(o.s1),
-                  _lib.ptr(o.s2), self.kind, float(o.lr), float(a), float(b), float(o.eps), float(max_norm or 0.0),
-                  float(grad_scale), None, self.n_a, _lib.ptr(o.scratch),
+        _lib.call("b2rl_nature_fused_opt_lr", _lib.ptr(self.b_units), self.n_b, _lib.ptr(o.flat), _lib.ptr(o.grad),
+                  _lib.ptr(o.s1), _lib.ptr(o.s2), self.kind, float(o.lr), _lib.ptr(self.lr_dev), float(a), float(b),
+                  float(o.eps), float(max_norm or 0.0), float(grad_scale), None, self.n_a, _lib.ptr(o.scratch),
                   _lib.ptr(o.step_dev), self.c1, self.n4, self.scale, _lib.ptr(pk.w1f), _lib.ptr(pk.w2f), _lib.ptr(pk.w2d),
                   _lib.ptr(pk.w3f), _lib.ptr(pk.w3d), _lib.ptr(pk.w4p), 1, _lib.ptr(o.shadow), _lib.stream())
         pk.scale = self.scale

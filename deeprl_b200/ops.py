@@ -150,6 +150,44 @@ def a2c_rollout_loss(head, action, reward, mask, discount, gae_tau, use_gae, ent
     return r
 
 
+def ppo_rollout_prep(head, action, reward, mask, discount, gae_tau, use_gae, out=None):
+    """PPO_agent.py:44-61 (shared_repr) from the actor's stored head outputs in one launch (``b2rl_ppo_rollout_prep``):
+    ``head`` [(T+1)*N, A+1] = (logits, v) of the rollout's states and, in rows T*N.., the final states (rows t-major);
+    ``action`` int64 / ``reward`` / ``mask`` [T*N] or [T, N].  Returns dict(logp = log pi(action) [T*N], adv, ret [T*N] (the
+    bits of ``gae(exact=True)``, adv not yet normalised)).  ``out``: preallocated outputs to write instead."""
+    head = _c(head, _f32)
+    T, N = reward.shape[0], reward.numel() // reward.shape[0]
+    A = head.shape[1] - 1
+    if head.shape[0] != (T + 1) * N or reward.numel() != T * N:
+        raise _lib.B2RLError("ppo_rollout_prep: head has %d rows, reward %s" % (head.shape[0], tuple(reward.shape)))
+    o = out if out is not None else {}
+    r = {k: o[k] if k in o else torch.empty(T * N, dtype=_f32, device=head.device) for k in ("logp", "adv", "ret")}
+    _lib.call("b2rl_ppo_rollout_prep", _lib.ptr(head), _lib.ptr(_c(action, torch.int64)), _lib.ptr(_c(reward, _f32)),
+              _lib.ptr(_c(mask, _f32)), float(discount), float(gae_tau), int(bool(use_gae)), T, N, A, _lib.ptr(r["logp"]),
+              _lib.ptr(r["adv"]), _lib.ptr(r["ret"]), _lib.stream())
+    return r
+
+
+def ppo_cat_loss(head, idx, action, old_logp, adv, ret, clip, entropy_weight, geff=None, stats=None):
+    """PPO_agent.py:77-92 (shared_repr) for one minibatch of a categorical actor-critic head in one launch
+    (``b2rl_ppo_cat_loss``): ``head`` [B, A+1] = (logits, v) of the minibatch, ``idx`` int64 [B] its rows of the rollout
+    arrays ``action`` / ``old_logp`` / ``adv`` / ``ret``.  Returns dict(geff [B, 33] = d(policy_loss + value_loss) /
+    d(head outputs) in columns 0..A, stats [3] = policy_loss, value_loss, approx_kl).  ``geff`` / ``stats``: preallocated
+    outputs (persistent buffers of a captured graph)."""
+    head = _c(head, _f32)
+    B, A = head.shape[0], head.shape[1] - 1
+    dev = head.device
+    geff = geff if geff is not None else torch.zeros((B, AC_GEFF_LD), dtype=_f32, device=dev)
+    stats = stats if stats is not None else torch.empty(3, dtype=_f32, device=dev)
+    ctas = int(_lib.lib().b2rl_ppo_cat_loss_ctas(B))
+    partial = _Scratch.get(dev, "ppo_cat_partial", max(4 * ctas, 1), _f32)
+    counter = _Scratch.get(dev, "ppo_cat_counter", 1, torch.int32)
+    _lib.call("b2rl_ppo_cat_loss", _lib.ptr(head), _lib.ptr(_c(idx, torch.int64)), _lib.ptr(_c(action, torch.int64)),
+              _lib.ptr(_c(old_logp, _f32)), _lib.ptr(_c(adv, _f32)), _lib.ptr(_c(ret, _f32)), float(clip),
+              float(entropy_weight), B, A, _lib.ptr(geff), _lib.ptr(stats), _lib.ptr(partial), _lib.ptr(counter), _lib.stream())
+    return dict(geff=geff, stats=stats)
+
+
 class _DQNDelta(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, q_next_target, q_next_online, action, reward, mask, gamma_n):

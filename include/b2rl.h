@@ -208,6 +208,25 @@ int b2rl_a2c_rollout_loss(const float* head, const int64_t* action, const float*
                           int32_t A, float* adv_out, float* ret_out, float* loss_out, float* geff_out, float* partial,
                           int32_t* counter, void* stream);
 
+/* PPOAgent's rollout statistics (PPO_agent.py:44-61, shared_repr) from the (logits, v) rows the actor's head launches stored:
+ * head [(T+1)*N][A+1] rows t-major (rows T*N.. the final states), action [T*N] int64, reward / mask [T*N].  logp_out [T*N] =
+ * log_softmax(logits)[action] (the old log-probabilities), adv_out / ret_out [T*N] the bits of b2rl_gae mode 0 (before
+ * b2rl_normalize_advantage).  Limits: T >= 1, N >= 1, 1 <= A <= 31, (T+1)*N <= 2^24. */
+int b2rl_ppo_rollout_prep(const float* head, const int64_t* action, const float* reward, const float* mask, float discount,
+                          float gae_tau, int32_t use_gae, int32_t T, int32_t N, int32_t A, float* logp_out, float* adv_out,
+                          float* ret_out, void* stream);
+
+/* PPO's clipped surrogate for one minibatch of a categorical actor-critic head (PPO_agent.py:77-92, shared_repr): head [B][A+1]
+ * = (logits, v) of the minibatch, idx [B] int64 its rows of the rollout arrays action (int64) / old_logp / adv / ret.
+ * geff_out [B][33] = d(policy_loss + value_loss) / d(head outputs) in b2rl_head_bwd_geff_relu's layout (columns 0..A), with
+ * b2rl_ppo_loss's tie and boundary rules; stats_out[0..2] = policy_loss, value_loss, approx_kl.  partial: float
+ * [4 * b2rl_ppo_cat_loss_ctas(B)] scratch; counter: int32, zero-initialised once (the kernel re-arms it).  The statistics are
+ * reduced in a fixed order: the same inputs give the same bits.  Limits: 1 <= B <= 2^24, 1 <= A <= 31. */
+int b2rl_ppo_cat_loss_ctas(int32_t B);
+int b2rl_ppo_cat_loss(const float* head, const int64_t* idx, const int64_t* action, const float* old_logp, const float* adv,
+                      const float* ret, float clip, float entropy_weight, int32_t B, int32_t A, float* geff_out,
+                      float* stats_out, float* partial, int32_t* counter, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Multi-tensor optimizer step with global-norm clip (DQN_agent.py:132-134; examples.py:67-68,139,204):
  * flat float32 views of all parameters / gradients (one contiguous arena, n elements).
@@ -428,6 +447,13 @@ int b2rl_nature_fused_opt(const int32_t* units, int32_t n_units, float* param, f
                           int32_t n_sumsq, void* norm_scratch, const int64_t* step_dev, int32_t c1, int32_t n4, float scale,
                           uint16_t* w1f, uint16_t* w2f, uint16_t* w2d, uint16_t* w3f, uint16_t* w3d, uint16_t* w4p,
                           int32_t zero_grad, uint16_t* bf16_shadow, void* stream);
+/* b2rl_nature_fused_opt with the learning rate on the device: lr_dev (float32) != NULL replaces lr, so a captured graph
+ * follows a schedule the host writes between replays; lr_dev == NULL is b2rl_nature_fused_opt. */
+int b2rl_nature_fused_opt_lr(const int32_t* units, int32_t n_units, float* param, float* grad, float* s1, float* s2, int32_t opt,
+                             float lr, const float* lr_dev, float a_, float b_, float eps, float max_norm, float grad_scale,
+                             const float* unit_sumsq, int32_t n_sumsq, void* norm_scratch, const int64_t* step_dev, int32_t c1,
+                             int32_t n4, float scale, uint16_t* w1f, uint16_t* w2f, uint16_t* w2d, uint16_t* w3f, uint16_t* w3d,
+                             uint16_t* w4p, int32_t zero_grad, uint16_t* bf16_shadow, void* stream);
 /* clip_grad_norm_'s coefficient alone (torch.nn.utils.clip_grad_norm_): norm_scratch[0] = ||grad * grad_scale||,
  * norm_scratch[1] = min(max_norm / (norm + 1e-6), 1) * grad_scale. */
 int b2rl_grad_norm(const float* grad, int64_t n, float grad_scale, float max_norm, void* norm_scratch, void* stream);

@@ -8,8 +8,11 @@ CategoricalDQNAgent on a noisy RainbowNet (rainbow_feature: csrc/rainbow.cu), ``
 NatureConvBody (n_step_dqn_pixel on SyntheticAtari-v0: one GraphedQActor replay per env step, one GraphedNStepLearner replay per
 rollout; both it and the eager side at bf16, plus the launcher's default fp32 eager side), and ``config.cuda_graph`` for A2CAgent
 on the NatureConvBody the same way (a2c_pixel on SyntheticAtari-v0: one GraphedQActor replay per env step with the action drawn
-on the device, one GraphedA2CLearner replay per rollout) -- in one process on one card, the sides alternated round by round.
-For the pixel launchers the captured update alone is also timed: CUDA events around back-to-back replays of its graph.  Also times the host envs alone (``task.step`` with fixed actions), so the share
+on the device, one GraphedA2CLearner replay per rollout), and ``config.cuda_graph`` for PPOAgent on the NatureConvBody
+(ppo_pixel: the same actor, one GraphedPPOPixelLearner replay per rollout for all its minibatch updates) -- in one process on one card, the sides alternated round by round.
+For the pixel launchers the captured update alone is also timed: CUDA events around back-to-back replays of its graph; and the
+first step of the graph side (which captures the actor's per-slot graphs) is timed alone, with the memory the caching
+allocator reserved during it.  Also times the host envs alone (``task.step`` with fixed actions), so the share
 left to the learner is visible.  Prints the card's name and power limit with the numbers.
 
     python scripts/a2c_step_time.py [--steps 300] [--rounds 5] [--only LAUNCHER[,LAUNCHER]] [--out DIR]
@@ -39,10 +42,12 @@ CONFIGS = [("a2c_feature", "CartPole-v0", "device_a2c", "a2c"), ("a2c_continuous
            ("quantile_regression_dqn_feature", "CartPole-v0", "device_qr", "qr"),
            ("rainbow_feature", "CartPole-v0", "device_rainbow", "rainbow"),
            ("n_step_dqn_pixel", "SyntheticAtari-v0", "cuda_graph", "nstep_dqn"),
-           ("a2c_pixel", "SyntheticAtari-v0", "cuda_graph", "a2c")]
+           ("a2c_pixel", "SyntheticAtari-v0", "cuda_graph", "a2c"),
+           ("ppo_pixel", "SyntheticAtari-v0", "cuda_graph", "ppo")]
 # launchers timed at a given Config.COMPUTE_DTYPE per side (set around every step of that side): side -> dtype
 DTYPES = {"n_step_dqn_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32},
-          "a2c_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32}}
+          "a2c_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32},
+          "ppo_pixel": {"eager": torch.bfloat16, "cuda_graph": torch.bfloat16, "eager_fp32": torch.float32}}
 
 
 def card():
@@ -157,10 +162,16 @@ def main():
         agents = {"eager": make_agent(name, game, flag, False), flag: make_agent(name, game, flag, True)}
         if "eager_fp32" in dtypes:
             agents["eager_fp32"] = make_agent(name, game, flag, False)
-        failed = {}
+        failed, first = {}, {}
         for k, ag in agents.items():
             try:
                 past_exploration(ag)
+                if k == "cuda_graph":                       # the first step captures the graphs
+                    torch.cuda.synchronize()
+                    torch.cuda.empty_cache()                # (graph capture empties the cache too)
+                    m0 = torch.cuda.memory_reserved()
+                    first = {"first_step_s": 1.0 / timed(ag, 1, dtypes.get(k)),
+                             "first_step_reserved_mb": (torch.cuda.memory_reserved() - m0) / 2 ** 20}
                 timed(ag, args.warmup, dtypes.get(k))
             except RuntimeError as e:
                 failed[k] = "%s: %s" % (type(e).__name__, str(e).split(". Hint")[0])
@@ -181,6 +192,7 @@ def main():
             row["compute_dtype"] = {k: str(v) for k, v in dtypes.items()}
         if flag == "cuda_graph" and flag in timed_agents:
             row["update_replay_ms"] = update_replay_ms(agents[flag])
+            row.update(first)
         result["configs"][name] = row
         print("%-18s %-20s N=%d env steps %d  %s;  envs alone %8.1f steps/s;  ms per step besides the envs: %s%s"
               % (name, game, c.num_workers, env_steps(agents[flag]),
@@ -189,6 +201,8 @@ def main():
                  "".join(";  %s not timed (%s)" % kv for kv in failed.items())))
         if "update_replay_ms" in row:
             print("%-18s captured update alone: %.3f ms per replay" % (name, row["update_replay_ms"]))
+            print("%-18s first step (captures): %.2f s, %.0f MB reserved" % (name, row["first_step_s"],
+                                                                           row["first_step_reserved_mb"]))
         for ag in agents.values():
             ag.close()
     print(json.dumps(result))
