@@ -19,6 +19,13 @@ condition.  ``CategoricalDQNAgent`` / ``QuantileRegressionDQNAgent`` have their 
 ``async_actor``, the actor thread launching its actor steps under ``config.lock``.  ``config.device_rainbow`` does the same for
 a ``CategoricalDQNAgent`` on a RainbowNet (``DeviceRainbow``, csrc/rainbow.cu): the NoisyLinear noise is drawn in the kernels,
 so the ``reset_noise()`` calls of the eager path do not run.
+
+``config.cuda_graph = True`` with ``ReplayWrapper(..., async_=True)`` over 84x84 uint8 frames (``dqn_pixel``,
+``categorical_dqn_pixel``, ``quantile_regression_dqn_pixel`` as written, at ``Config.COMPUTE_DTYPE = torch.bfloat16``): past
+exploration each step's transitions are staged in the learner's pinned buffer and fed inside ONE update replay
+(``_async_graph_update``; learner.GraphedDQNLearner with ``prefetch`` and ``wrapper_order``), the actor's forward is a
+GraphedQActor replay, on the actor thread with ``async_actor`` (component/actor.py ``ParameterOrder``).  Configurations it
+does not cover (``component/actor.py dqn_graph_unsupported``; the reason is kept in ``graph_refusal``) keep their path.
 """
 import threading
 
@@ -46,17 +53,40 @@ class DQNActor(BaseActor):
     def compute_q(self, prediction):
         return to_np(self._q_tensor(prediction))
 
+    _order = None                                          # component/actor.py ParameterOrder: the agent's async captured path
+
     def _graphed(self):
         """``config.cuda_graph``: the forward pass below as one captured launch sequence (component/actor.py GraphedQActor).
         Not for subclasses that redefine ``compute_q`` itself (they get the statements of the reference)."""
         ga = getattr(self, "_graph_actor", None)
         if ga is None:
             from ..component import actor as device_actor
-            ok = (type(self).compute_q is DQNActor.compute_q and device_actor.q_actor_supported(self.config, self._network)
+            order = self._order
+            ok = (type(self).compute_q is DQNActor.compute_q
+                  and device_actor.q_actor_supported(self.config, self._network, async_ok=order is not None)
                   and all(np.asarray(s).dtype == np.uint8 and np.asarray(s).shape == (4, 84, 84) for s in self._state))
             ga = self._graph_actor = device_actor.GraphedQActor(
                 self._network, self._q_tensor, len(self._state), 4, (84, 84), self.config.state_normalizer.coef) if ok else False
+            if ga and order is not None and self.config.async_actor:
+                ga.capture_error_mode = "thread_local"     # the learner thread may synchronise while this thread captures
         return ga or None
+
+    def _ordered_q_values(self, order):
+        """``async_actor`` on the agent's captured path: the GraphedQActor replay on this thread's stream, after the latest
+        update replay and before the next one (``ParameterOrder``); ``config.lock`` is held to enqueue (and to capture), not
+        while this thread waits for its q values."""
+        stream = order.actor_stream()
+        with torch.cuda.stream(stream):
+            with order.lock:
+                ga = self._graphed()
+                stream.wait_event(order.updated)
+                if ga is None:                             # (a subclass's own compute_q): the eager forward, same order
+                    with torch.no_grad():
+                        prediction = self._network(self.config.state_normalizer(np.asarray([np.asarray(s) for s in self._state])))
+                else:
+                    ga.enqueue(self._state)
+                order.acted.record(stream)
+            return ga.result() if ga is not None else self.compute_q(prediction)
 
     def _transition(self):
         """DQN_agent.py:24-45: epsilon-greedy on a forward pass of the shared network, one env step."""
@@ -74,8 +104,11 @@ class DQNActor(BaseActor):
             return self._env_step(action)
         if config.noisy_linear:
             self._network.reset_noise()
-        ga = self._graphed() if getattr(config, "cuda_graph", False) else None
-        if ga is not None:
+        order = self._order if config.async_actor else None
+        ga = self._graphed() if getattr(config, "cuda_graph", False) and order is None else None
+        if order is not None:
+            q_values = self._ordered_q_values(order)
+        elif ga is not None:
             with config.lock:
                 q_values = ga.q_values(self._state)
         else:
@@ -133,6 +166,7 @@ class DQNAgent(BaseAgent):
         self.total_steps = 0
         self.last_loss = None
         self.device_dqn = None
+        self._learner = None
         flag = self._device_flag
         if getattr(config, "device_rainbow", False):
             for other in ("device_dqn", flag):
@@ -153,6 +187,13 @@ class DQNAgent(BaseAgent):
             from ..component.actor import DeviceDQN
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
             self.device_dqn = self.actor._device_dqn = DeviceDQN(self, seed)
+        # config.cuda_graph with async replay: decided once, here, before the actor thread starts
+        from ..component.actor import ParameterOrder, dqn_graph_unsupported
+        self.graph_refusal = dqn_graph_unsupported(config, self)
+        self._async_graph = self.graph_refusal is None
+        if self._async_graph:
+            self._order = ParameterOrder(config.lock)
+            self.actor._order = self._order if config.async_actor else None
 
     def close(self):
         close_obj(self.replay)
@@ -288,18 +329,24 @@ class DQNAgent(BaseAgent):
                 action=actions,
                 reward=[config.reward_normalizer(r) for r in rewards],
                 mask=1 - np.asarray(dones, dtype=np.int32)))
-        feed_many = getattr(self.replay, "feed_many", None)
-        if feed_many is not None:                          # one staging upload for the env steps of this agent step;
-            feed_many(feeds)                               # ring / tree state as after feed(d) for d in feeds (replay.py:75-90)
+        if self._async_graph and self.total_steps > config.exploration_steps:
+            # config.cuda_graph with async replay: the feeds are staged for the learner and fed inside its update graph
+            self._async_graph_update(feeds)
         else:
-            for d in feeds:
-                self.replay.feed(d)
+            feed_many = getattr(self.replay, "feed_many", None)
+            if feed_many is not None:                      # one staging upload for the env steps of this agent step;
+                feed_many(feeds)                           # ring / tree state as after feed(d) for d in feeds (replay.py:75-90)
+            else:
+                for d in feeds:
+                    self.replay.feed(d)
 
-        if self.total_steps > config.exploration_steps and self.device_dqn is not None:
+        if self.total_steps <= config.exploration_steps or self._async_graph:
+            pass
+        elif self.device_dqn is not None:
             self._device_update()                          # config.device_dqn: the whole update is one launch
-        elif self.total_steps > config.exploration_steps and self._graph_ok():
+        elif self._graph_ok():
             self._graph_update()                           # config.cuda_graph: the whole update is one graph replay
-        elif self.total_steps > config.exploration_steps:
+        else:
             transitions = self._sample()
             if config.noisy_linear:
                 self.target_network.reset_noise()
@@ -368,3 +415,57 @@ class DQNAgent(BaseAgent):
             lr.update()
             lr.repack_online()                             # the actor's next forward sees theta_k
         self.last_loss = lr.loss
+
+    # ------------------------------------------------------------------ config.cuda_graph with async replay (opt-in)
+    def _async_graph_update(self, feeds):
+        """``step()`` on the captured path with async replay (``component/actor.py dqn_graph_unsupported``): this step's
+        transitions -- frame ``s[-1]``, action, ``reward_normalizer(r)``, mask -- and PER's ``replay_beta()`` go into the
+        learner's pinned staging buffer, then ONE update replay copies them up, trains on the batch the previous replay drew,
+        feeds them after that batch's last ring read and draws the next batch (learner.GraphedDQNLearner with ``prefetch``
+        and ``wrapper_order``: the graph form of ReplayWrapper(async_=True)).  The first call builds the learner; its eager
+        warm-up is this step's own update and its capture executes nothing (``first_update``)."""
+        config = self.config
+        lr, first = self._learner, self._learner is None
+        if first:
+            lr = self._learner = self._async_learner(feeds)
+        else:
+            lr.staged.synchronize()                        # the previous replay's copy node has read the staging buffer
+        n = sum(len(d["state"]) for d in feeds)
+        if n != lr.feeds:
+            raise RuntimeError("%d transitions in this step; the captured update feeds %d" % (n, lr.feeds))
+        cat = lambda key, dt: np.concatenate([np.asarray(d[key], dtype=dt).reshape(len(d["state"]), -1) for d in feeds])
+        lr.h_frames.numpy()[...] = cat("state", np.uint8)
+        lr.h_action.numpy()[...] = cat("action", np.int64).reshape(-1)
+        lr.h_reward.numpy()[...] = cat("reward", np.float64).reshape(-1)
+        lr.h_mask.numpy()[...] = cat("mask", np.int64).reshape(-1)
+        if lr.per:
+            lr.h_beta[0] = float(config.replay_beta())     # once per update, as _per_args calls it on the eager path
+        order = self._order
+        with order.lock:                                   # held to enqueue (and to capture), not across a synchronise
+            cur = torch.cuda.current_stream()
+            cur.wait_event(order.acted)                    # the actor's latest forward has read (and, before the learner
+            if first:                                      # existed, re-packed) the packed operands
+                cur.wait_stream(self.replay._side)         # after the feeds the wrapper ran during exploration
+                lr.first_update()                          # (its re-pack and warm-up start from this stream)
+            else:
+                lr.update()
+            order.updated.record(cur)
+        self.last_loss = lr.loss
+
+    def _async_learner(self, feeds):
+        from ..learner import GraphedDQNLearner
+        config = self.config
+        inner = self.replay.replay
+        inner.allocate(np.asarray(feeds[0]["state"][0]))   # (the ring exists once the wrapper has fed it)
+        with config.lock:
+            lr = GraphedDQNLearner(
+                self.network, self.target_network, self._flat, inner, kind=self._graph_kind, discount=config.discount,
+                n_step=config.n_step, double_q=bool(config.double_q), gradient_clip=config.gradient_clip or 0.0,
+                feeds_per_update=sum(len(d["state"]) for d in feeds), compute_dtype=Config.COMPUTE_DTYPE,
+                state_scale=config.state_normalizer.coef, replay_eps=getattr(config, "replay_eps", 0.01),
+                replay_alpha=getattr(config, "replay_alpha", 0.5),
+                categorical=(getattr(config, "categorical_v_min", -10.0), getattr(config, "categorical_v_max", 10.0)),
+                target_sync_every=0, prefetch=True, wrapper_order=True)
+        if config.async_actor:
+            lr.capture_error_mode = "thread_local"         # the actor thread may synchronise its stream during the capture
+        return lr

@@ -186,6 +186,7 @@ class GraphedQActor:
         self.d_q = self.h_q = None
         self.graphs, self._sig = [None] * self.slots, None
         self.replays = 0
+        self.capture_error_mode = "global"                # "thread_local": captured on an actor thread (ParameterOrder)
 
     @property
     def graph(self):
@@ -225,7 +226,7 @@ class GraphedQActor:
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         pool = next((h.pool() for h in self.graphs if h is not None), None)     # the slots' graphs replay one at a time
-        with no_gc(), torch.cuda.graph(g, pool=pool):
+        with no_gc(), torch.cuda.graph(g, pool=pool, capture_error_mode=self.capture_error_mode):
             self._forward(slot)
         self.graphs[slot] = g
         self._sig = self._signature()
@@ -233,6 +234,11 @@ class GraphedQActor:
     def q_values(self, states, slot=0):
         """``states``: ``num_envs`` frame stacks (LazyFrames / uint8 arrays [history, H, W]).  Returns float32 [num_envs, A]
         (with ``run``: what it returns, on the host).  ``slot``: where in the arena the stacks land (0 without an arena)."""
+        self.enqueue(states, slot)
+        return self.result()
+
+    def enqueue(self, states, slot=0):
+        """The first half of ``q_values``: stage the stacks, capture if needed and replay, on the current stream."""
         for i, s in enumerate(states):
             a = np.asarray(s)
             if a.dtype != np.uint8 or a.size != self.hl * self.row:
@@ -242,18 +248,42 @@ class GraphedQActor:
             self._capture(slot)
         self.graphs[slot].replay()
         self.replays += 1
+
+    def result(self):
+        """The second half of ``q_values``: wait for the replay (on the current stream) and return its download."""
         torch.cuda.current_stream().synchronize()
         return self.h_q.numpy().copy()
 
 
-def q_actor_supported(config, network):
+class ParameterOrder:
+    """What ``config.lock`` guarantees between the DQN agent's actor thread and its learner (DQN_agent.py:30,133: a forward
+    reads one whole parameter version), moved onto the device for the captured path with ``async_actor``.  The actor replays
+    on a stream of its own; each actor replay waits for the event recorded after the latest update replay (``updated``) and
+    each update replay waits for the one recorded after the latest actor replay (``acted``), so a forward never runs while an
+    update's tail rewrites the packed bf16 operands, nor an update while a forward reads them.  The host holds ``lock`` only
+    while it enqueues the wait, the replay and the record (and while it captures), never across a synchronise: the learner
+    does not wait on the host for the actor's forward, and the actor's wait for its own q values leaves the learner free."""
+
+    def __init__(self, lock):
+        self.lock = lock
+        self.updated, self.acted = torch.cuda.Event(), torch.cuda.Event()
+        self.stream = None                                # the actor's stream, made on the actor thread
+
+    def actor_stream(self):
+        if self.stream is None:
+            self.stream = torch.cuda.Stream()
+        return self.stream
+
+
+def q_actor_supported(config, network, async_ok=False):
     """``config.cuda_graph`` + synchronous actor + bf16 wgmma NatureConvBody on a CUDA device + ImageNormalizer-style rescale
-    of uint8 frames: the conditions under which the actor's forward is the captured device path."""
+    of uint8 frames: the conditions under which the actor's forward is the captured device path.  ``async_ok``: the agent
+    orders an actor thread's replays against its updates (``ParameterOrder``), so ``async_actor`` is no obstacle."""
     from ..network.network_bodies import NatureConvBody
     from ..utils import Config
     from ..utils.normalizer import RescaleNormalizer
     body = getattr(network, "body", None)
-    return bool(getattr(config, "cuda_graph", False) and not config.async_actor and not config.noisy_linear
+    return bool(getattr(config, "cuda_graph", False) and (async_ok or not config.async_actor) and not config.noisy_linear
                 and isinstance(body, NatureConvBody) and not body.noisy_linear and body.conv1.weight.is_cuda
                 and body.conv1.in_channels == 4
                 and Config.COMPUTE_DTYPE == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
@@ -381,6 +411,76 @@ def ppo_graph_unsupported(config, network, optimizer, states):
         return ("the rollout's %d rows are not a multiple of mini_batch_size %d; random_sample would yield a short last "
                 "minibatch" % (rows, config.mini_batch_size))
     return a2c_graph_unsupported(config, network, optimizer, states)
+
+
+def dqn_graph_unsupported(config, agent):
+    """``None`` when ``DQNAgent.step()`` (or the C51 / QR-DQN agent's) runs on the captured path with async replay under
+    ``config.cuda_graph``: the env transitions staged in learner.GraphedDQNLearner's pinned buffer and one update replay per
+    step (``prefetch`` = the graph form of ``ReplayWrapper(async_=True)``, ``wrapper_order``), the actor's forward a
+    GraphedQActor replay (on its own thread with ``async_actor``, ordered by ``ParameterOrder``).  Else the unmet condition;
+    the agent then keeps its eager path.  Reads ``agent.network``, ``agent.optimizer`` (the torch optimizer), ``agent.replay``
+    (the wrapper: its class and keyword arguments) and the agent's class."""
+    from ..network import nature_tc
+    from ..network.network_bodies import NatureConvBody
+    from ..network.network_heads import CategoricalNet, DuelingNet, QuantileNet, VanillaNet
+    from ..utils import Config
+    from ..utils.normalizer import RescaleNormalizer
+    from .replay import PrioritizedReplay, ReplayWrapper, UniformReplay
+    if not getattr(config, "cuda_graph", False):
+        return "config.cuda_graph is not set"
+    for flag in ("device_dqn", "device_c51", "device_qr", "device_rainbow"):
+        if getattr(config, flag, False):
+            return "config.%s is set; it runs the agent on the device itself" % flag
+    rp = agent.replay
+    if not isinstance(rp, ReplayWrapper) or not rp.async_:
+        return ("the replay is not ReplayWrapper(..., async_=True); the captured update with async replay implements its "
+                "double buffer")
+    if rp.replay_cls not in (UniformReplay, PrioritizedReplay):
+        return "the replay is a %s; the captured update implements UniformReplay and PrioritizedReplay" % rp.replay_cls.__name__
+    kind = agent._graph_kind
+    if kind == "qr" and rp.replay_cls is PrioritizedReplay:
+        return "QR-DQN with prioritized replay is undefined in the reference (its loss is per target quantile)"
+    net = agent.network
+    if type(net).__name__ == "RainbowNet" or config.noisy_linear:
+        return "the network is a RainbowNet or has NoisyLinear layers; the captured update implements nn.Linear heads"
+    want = {"dqn": (VanillaNet, DuelingNet), "c51": (CategoricalNet,), "qr": (QuantileNet,)}[kind]
+    if type(net) not in want:
+        return "the network is a %s; the captured update implements %s for %s" % (
+            type(net).__name__, " / ".join(c.__name__ for c in want), type(agent).__name__)
+    body = net.body
+    if not isinstance(body, NatureConvBody):
+        return "the body is a %s; the captured update implements NatureConvBody" % type(body).__name__
+    if body.noisy_linear:
+        return "the network has NoisyLinear layers; the captured update implements nn.Linear"
+    if Config.COMPUTE_DTYPE != torch.bfloat16 or Config.DENSE_BACKEND != "tcgen05":
+        return ("the compute dtype is %s with the %r dense backend; the captured update runs bf16 on the wgmma kernels "
+                "(tcgen05)" % (Config.COMPUTE_DTYPE, Config.DENSE_BACKEND))
+    if not (nature_tc.FUSED_BWD and _lib.CONV_SLAB):
+        return "the fused backward epilogues are switched off; the captured update needs the fused update tail"
+    if not isinstance(config.state_normalizer, RescaleNormalizer):
+        return "the state normalizer is %s; the captured update folds a RescaleNormalizer into conv1" % type(
+            config.state_normalizer).__name__
+    space = getattr(getattr(config, "eval_env", None), "observation_space", None)
+    shape = tuple(getattr(space, "shape", ()) or ())
+    dtype = np.dtype(getattr(space, "dtype", None) or np.float64)
+    hl = int(rp.replay_kwargs.get("history_length", 1))
+    if body.conv1.in_channels != 4 or hl != 4 or shape != (4, 84, 84) or dtype != np.uint8:
+        return ("the frames are %s %s with history_length %d into %d channels; the captured update reads 84 x 84 uint8 frames "
+                "with a history of 4" % (dtype, shape or "unknown", hl, body.conv1.in_channels))
+    if config.num_workers != 1:
+        return "%d envs per actor step; the staged feeds follow the reference's one-transition feed() calls" % config.num_workers
+    g = agent.optimizer.param_groups[0]
+    if not ((isinstance(agent.optimizer, torch.optim.RMSprop) and g["momentum"] == 0 and g["weight_decay"] == 0)
+            or (isinstance(agent.optimizer, torch.optim.Adam) and g["weight_decay"] == 0 and not g["amsgrad"])):
+        return ("the optimizer is %s; the fused update tail implements RMSprop (centered or not) and Adam without momentum, "
+                "weight decay or amsgrad" % type(agent.optimizer).__name__)
+    if agent._uses_reference_hooks():
+        return "%s overrides compute_loss / reduce_loss; the captured update runs the stock loss" % type(agent).__name__
+    if getattr(rp, "_primed", False):
+        return "the replay wrapper has already handed out an eager batch; its pending batch is not handed to the learner"
+    if not body.conv1.weight.is_cuda:
+        return "the network is not on a CUDA device (select_device(0))"
+    return None
 
 
 # ------------------------------------------------------------------------------------------------ A2C on the device

@@ -192,7 +192,7 @@ class GraphedDQNLearner(_NatureLearner):
     def __init__(self, network, target_network, optimizer, replay, kind="dqn", discount=0.99, n_step=1, double_q=False,
                  gradient_clip=5.0, feeds_per_update=4, compute_dtype=torch.bfloat16, state_scale=1.0 / 255,
                  replay_eps=0.01, replay_alpha=0.5, categorical=(-10.0, 10.0), world_size=1, target_sync_every=10000,
-                 prefetch=False, dual=False):
+                 prefetch=False, dual=False, wrapper_order=False):
         self.net, self.tgt, self.opt, self.replay = network, target_network, optimizer, replay
         self.kind, self.gamma_n, self.double_q = kind, discount ** n_step, double_q
         self.clip, self.feeds = gradient_clip, feeds_per_update
@@ -233,6 +233,13 @@ class GraphedDQNLearner(_NatureLearner):
         # dual: one launch per body layer for online(s) + target(s') (nature_tc.forward_dual): 27 instead of 33 launches per
         # update; off by default (the two-stream fork of the prefetch branch already hides the per-launch fixed cost).
         self.dual = bool(dual)
+        # wrapper_order (async replay with feeds, for an agent): the first update feeds ONCE and draws the batch it trains on
+        # and the one the next update trains on after those feeds, like ReplayWrapper's first sample() (three draws: both
+        # buffers, then the refill of the second); the h2d copy node is followed by ``staged``, an event the host waits on
+        # before it rewrites the pinned staging buffer (no synchronise per update)
+        self.wrapper_order = bool(wrapper_order)
+        self.staged = torch.cuda.Event(external=True) if self.wrapper_order else None
+        self.capture_error_mode = "global"
         self._batch = [None, None]
         self._parity = 0
         self.updates = 0
@@ -276,14 +283,16 @@ class GraphedDQNLearner(_NatureLearner):
     # ------------------------------------------------------------------ the update, as eager code
     def _h2d(self):
         self.d_pack.copy_(self.h_pack, non_blocking=True)
+        if self.staged is not None:
+            self.staged.record()
 
-    def _sample(self, tag=0, phase=None):
+    def _sample(self, tag=0, phase=None, feed=True):
         """feeds of this update + one sampled batch into buffer set ``tag`` (on the current stream).  ``phase`` "select" =
         feed + index draw only, "gather" = the batch from those indices (uniform replay), None = everything."""
         rp = self.replay
         # DQN_agent.py:104-112 calls feed() once per env transition; `feeds` single-item calls are exactly one multi-item
         # call with each item in its own slot (reference_feed_quirk off) plus `feeds` tree.add(max_priority) -- one launch
-        if self.feeds and phase != "gather":
+        if self.feeds and feed and phase != "gather":
             quirk, rp.quirk = rp.quirk, False
             rp._device_cursor = True                     # (a captured feed advances the device cursor only)
             if self.per:
@@ -323,17 +332,21 @@ class GraphedDQNLearner(_NatureLearner):
         # update's feeds, the index draw and the action / reward / mask gather of the next batch into the other buffer set --
         # forks after that last read, so every batch sees the ring exactly as the materialising form gathers it (after the
         # previous update's feeds, before this update's)
+        feed = True
         if self.prefetch:
             eager = parity is None
             if eager:
                 parity = self._parity
             if self._batch[parity] is None:                              # very first update: nothing prefetched yet
                 self._batch[parity] = self._sample(parity)
+                if self.wrapper_order:
+                    self._sample(1 - parity, feed=False)                 # the wrapper's first fill of its second buffer
+                    feed = False                                         # this update's feeds ran above
             t = self._batch[parity]
             if plan.prefetch == "start":
-                self._prefetch_branch(parity)
+                self._prefetch_branch(parity, feed=feed)
             elif plan.prefetch != "after-ring-read":
-                self._prefetch_branch(parity, "select")  # feed + index draw now (two one-CTA kernels), the gather later
+                self._prefetch_branch(parity, "select", feed=feed)  # feed + index draw now (two one-CTA kernels), the gather later
             if eager:
                 self._parity = 1 - parity
         else:
@@ -406,7 +419,7 @@ class GraphedDQNLearner(_NatureLearner):
         # the late prefetch fork: after conv1's weight gradient from the ring (beside the rest of the backward pass and the
         # update tail), after the last dgrad GEMM, or -- the fallback when neither fired -- after the backward pass
         fired, phase = [], None if plan.prefetch == "after-ring-read" else "gather"
-        fork = lambda after=None: fired or (self._prefetch_branch(parity, phase, after), fired.append(1))
+        fork = lambda after=None: fired or (self._prefetch_branch(parity, phase, after, feed), fired.append(1))
         nature_tc.AFTER_RING_READ = fork if plan.prefetch == "after-ring-read" else None
         nature_tc.AFTER_DGRAD = fork if plan.prefetch == "gather-after-dgrad" else None
         try:
@@ -422,13 +435,13 @@ class GraphedDQNLearner(_NatureLearner):
         if plan.join == "main":
             cur.wait_stream(pre)
 
-    def _prefetch_branch(self, parity, phase=None, after=None):
+    def _prefetch_branch(self, parity, phase=None, after=None, feed=True):
         cur, pre = torch.cuda.current_stream(), self._pre
         pre.wait_stream(cur)                                             # after the host->device copy of this update's feeds
         if after is not None:
             pre.wait_stream(after)                                       # and after the ring read launched there
         with torch.cuda.stream(pre):
-            b = self._sample(1 - parity, phase)
+            b = self._sample(1 - parity, phase, feed)
             if phase != "select":
                 self._batch[1 - parity] = b
                 self._sampled_ev.record(pre)
@@ -490,7 +503,8 @@ class GraphedDQNLearner(_NatureLearner):
     def _capture_main(self, with_h2d):
         for parity in ((0, 1) if self.prefetch else (None,)):
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, pool=self.g_main[0].pool() if self.g_main else None):
+            with torch.cuda.graph(g, pool=self.g_main[0].pool() if self.g_main else None,
+                                  capture_error_mode=self.capture_error_mode):
                 if with_h2d:
                     self._h2d()
                 self._main(parity)
@@ -533,6 +547,18 @@ class GraphedDQNLearner(_NatureLearner):
         self.updates += 1
         if self.sync_every and self.updates % self.sync_every == 0:
             self.sync_target()
+        return self.loss
+
+    def first_update(self):
+        """An agent's first update, then the capture (``wrapper_order``; the caller has staged this update's feeds and beta):
+        the eager warm-up of ``capture(warmup=1, with_h2d=True)`` IS this update -- its own feeds, both batches drawn after
+        them (ReplayWrapper's first sample), one optimizer step -- and the capture that follows executes nothing, so the
+        agent ends exactly one update further on.  The next ``update()`` replays the other parity.  Returns the loss."""
+        assert self.wrapper_order and self.prefetch and self.feeds and self.updates == 0
+        self.capture(warmup=1, with_h2d=True)
+        if self.per:                                     # (the captured feeds' host bookkeeping ran at capture, not on the device)
+            self.replay.tree.n_entries = self.replay._size
+        self.updates = 1
         return self.loss
 
     def update_from_host(self, frames, action, reward, mask, beta=None):
