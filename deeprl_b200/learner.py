@@ -479,6 +479,8 @@ class GraphedDQNLearner(_NatureLearner):
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         self.g_main, self.g_opt = [], None
+        tree = getattr(self.replay, "tree", None)
+        n_entries = tree.n_entries if tree is not None else None     # a capture's tree.add_n adds no leaf on the device
         try:
             self._capture_main(with_h2d)
         except Exception as e:                            # noqa: BLE001 -- any capture error: use the split form
@@ -497,6 +499,8 @@ class GraphedDQNLearner(_NatureLearner):
         # host mirrors of the ring cursor advanced during warm-up / capture calls; re-derive from the device
         st = self.replay.ring_state.cpu()
         self.replay.pos, self.replay._size = int(st[0]), int(st[1])
+        if tree is not None:
+            tree.n_entries = n_entries
         self.launches_per_update = None
         return self
 
@@ -544,6 +548,9 @@ class GraphedDQNLearner(_NatureLearner):
         if self.g_opt is not None:
             self._allreduce()
             self.g_opt.replay()
+        if self.per and self.feeds:                      # the replay's tree.add_n: its host count (state_dict saves it)
+            tree = self.replay.tree
+            tree.n_entries = min(tree.n_entries + self.feeds, tree.capacity)
         self.updates += 1
         if self.sync_every and self.updates % self.sync_every == 0:
             self.sync_target()
@@ -556,8 +563,6 @@ class GraphedDQNLearner(_NatureLearner):
         agent ends exactly one update further on.  The next ``update()`` replays the other parity.  Returns the loss."""
         assert self.wrapper_order and self.prefetch and self.feeds and self.updates == 0
         self.capture(warmup=1, with_h2d=True)
-        if self.per:                                     # (the captured feeds' host bookkeeping ran at capture, not on the device)
-            self.replay.tree.n_entries = self.replay._size
         self.updates = 1
         return self.loss
 

@@ -465,11 +465,9 @@ def test_launchers_end_to_end(rl, monkeypatch, name, game):
     assert all(bool(torch.isfinite(x)) for x in losses_) and ag.total_steps == 30 * c.num_workers * c.rollout_length
     assert len(set(float(x) for x in losses_)) > 1
     torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        ag.step()
-        torch.cuda.synchronize()
-    kernels = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-               and not e.name.startswith(("Memcpy", "Memset"))]
+    from _kernel_trace import profiled_kernels
+    kernels = profiled_kernels(lambda: (ag.step(), torch.cuda.synchronize()),
+                               {"a2c_actor_kernel": c.rollout_length, "a2c_update_kernel": 1}, warmup=False)
     assert sum("a2c_actor_kernel" in k for k in kernels) == c.rollout_length, kernels
     assert sum("a2c_update_kernel" in k for k in kernels) == 1, kernels
     assert len(kernels) == c.rollout_length + 1, kernels

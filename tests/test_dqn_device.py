@@ -588,14 +588,10 @@ def test_launcher_end_to_end(rl, monkeypatch, replay_cls):
         if ag.last_loss is not None:
             losses_.append(float(ag.last_loss))
     assert syncs >= 2 and len(losses_) > 10 and all(np.isfinite(losses_)) and len(set(losses_)) > 1
-    sched = torch.profiler.schedule(wait=0, warmup=1, active=1, repeat=1)
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA], schedule=sched) as prof:
-        for _ in range(2):
-            ag.step()
-            torch.cuda.synchronize()
-            prof.step()
-    kernels = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-               and not e.name.startswith(("Memcpy", "Memset"))]
+    from _kernel_trace import profiled_kernels
+    kernels = profiled_kernels(lambda: (ag.step(), torch.cuda.synchronize()), dict(
+        {"dqn_actor_kernel": c.sgd_update_frequency, "dqn_replay_update_kernel": 1, "feed_kernel": 1, "gather": 1},
+        **({"direct_copy": 1, "sumtree_sample": 1} if replay_cls == "PrioritizedReplay" else {})))
     assert sum("dqn_actor_kernel" in k for k in kernels) == c.sgd_update_frequency, kernels
     assert sum("dqn_replay_update_kernel" in k for k in kernels) == 1, kernels
     others = [k for k in kernels if "dqn_actor_kernel" not in k and "dqn_replay_update_kernel" not in k]

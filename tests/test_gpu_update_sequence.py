@@ -205,17 +205,21 @@ def seed_optimizer(orc, lr, s1, s2, step):
         orc.opt.state[orc.sd[n]] = st
 
 
+def oracle_batch(frames, bufs, hl, n_step):
+    """The batch of ``bufs`` (indices, action, reward, mask) with its state / next-state stacks read from ``frames``."""
+    idx = bufs["idx"]
+    rows = idx.view(-1, 1) + torch.arange(-(hl - 1), 1, device=idx.device).view(1, -1)
+    fr = frames.view(-1, 84, 84)
+    return types.SimpleNamespace(state=fr[rows.view(-1)].view(-1, hl, 84, 84).cpu().numpy(),
+                                 next_state=fr[(rows + n_step).view(-1)].view(-1, hl, 84, 84).cpu().numpy(),
+                                 action=bufs["action"].cpu().numpy(), reward=bufs["reward"].cpu().numpy(),
+                                 mask=bufs["mask"].cpu().numpy())
+
+
 def teacher_forced(bench, lr, workload, snap, frames, bufs, spied, loss_dev, beta, what):
     """One oracle update from the snapshot taken before the replay, on the batch it trained on, against the device."""
     from oracle import agents
-    idx = bufs["idx"]
-    hl = lr.replay.history_length
-    rows = idx.view(-1, 1) + torch.arange(-(hl - 1), 1, device=idx.device).view(1, -1)
-    fr = frames.view(-1, 84, 84)
-    tr = types.SimpleNamespace(state=fr[rows.view(-1)].view(-1, hl, 84, 84).cpu().numpy(),
-                               next_state=fr[(rows + lr.replay.n_step).view(-1)].view(-1, hl, 84, 84).cpu().numpy(),
-                               action=bufs["action"].cpu().numpy(), reward=bufs["reward"].cpu().numpy(),
-                               mask=bufs["mask"].cpu().numpy())
+    tr = oracle_batch(frames, bufs, lr.replay.history_length, lr.replay.n_step)
     head = {"dqn": "vanilla", "per": "dueling", "c51": "categorical", "qr": "quantile"}[workload]
     if workload in ("dqn", "per"):
         opt_fn = lambda p: torch.optim.RMSprop(p, lr=0.00025, alpha=0.95, eps=0.01, centered=True)
@@ -232,8 +236,19 @@ def teacher_forced(bench, lr, workload, snap, frames, bufs, spied, loss_dev, bet
     seed_optimizer(orc, lr, snap["s1"], snap["s2"], snap["step"])
     if workload == "per":
         tr.sampling_prob = bufs["prob"].cpu().numpy()
-    # ---- the forwards the loss kernel read: online on s, target (and double-Q online) on s'
-    key = {"dqn": ("q", "q"), "per": ("q", "q"), "c51": ("log_prob", "prob"), "qr": ("quantile", "quantile")}[workload]
+    check_oracle_step(orc, lr, tr, snap, spied, loss_dev, what)
+
+
+OUTPUT_KEYS = {"vanilla": ("q", "q"), "dueling": ("q", "q"), "categorical": ("log_prob", "prob"),
+               "quantile": ("quantile", "quantile")}
+
+
+def check_oracle_step(orc, lr, tr, snap, spied, loss_dev, what, grad_cos=0.995, delta_per_tensor=True):
+    """The device's update from ``snap`` against ``orc`` (a DQNFamilyOracle seeded with the same parameters, target and
+    optimizer state) on the batch ``tr``: the forwards the loss kernel read, the loss, the clipped gradient recovered from
+    the optimizer moments (``grad_cos``: the bound of its global cosine) and the parameter delta (``delta_per_tensor``:
+    its direction per tensor too, not only globally)."""
+    key = OUTPUT_KEYS[orc.head]
     with torch.no_grad():
         s, s2 = orc.normalize(tr.state), orc.normalize(tr.next_state)
         pairs = [(spied["out"], orc.forward(orc.sd, s)[key[0]], "online(s)"),
@@ -267,11 +282,11 @@ def teacher_forced(bench, lr, workload, snap, frames, bufs, spied, loss_dev, bet
         do = (orc.sd[n].detach() - before[n]).flatten()
         if go.norm() > 1e-8 and cosine(gd, go) <= 0.98:
             bad.append("gradient direction of %s: %.5f" % (n, cosine(gd, go)))
-        if do.norm() > 0 and cosine(dd, do) <= 0.98:
+        if delta_per_tensor and do.norm() > 0 and cosine(dd, do) <= 0.98:
             bad.append("parameter-delta direction of %s: %.5f" % (n, cosine(dd, do)))
         g_dev.append(gd), g_orc.append(go), d_dev.append(dd), d_orc.append(do)
     g_dev, g_orc, d_dev, d_orc = (torch.cat(x) for x in (g_dev, g_orc, d_dev, d_orc))
-    if cosine(g_dev, g_orc) <= 0.995:
+    if cosine(g_dev, g_orc) <= grad_cos:
         bad.append("gradient direction %.5f" % cosine(g_dev, g_orc))
     if cosine(d_dev, d_orc) <= 0.98:
         bad.append("parameter-delta direction %.5f" % cosine(d_dev, d_orc))

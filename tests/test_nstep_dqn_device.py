@@ -429,14 +429,9 @@ def test_launcher_end_to_end(rl, monkeypatch):
     assert len(set(float(x) for x in losses_)) > 1
     torch.cuda.synchronize()
     # one warm-up cycle of the profiler, then the recorded step (events launched as the tracer starts can be missed)
-    sched = torch.profiler.schedule(wait=0, warmup=1, active=1, repeat=1)
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA], schedule=sched) as prof:
-        for _ in range(2):
-            ag.step()
-            torch.cuda.synchronize()
-            prof.step()
-    kernels = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-               and not e.name.startswith(("Memcpy", "Memset"))]
+    from _kernel_trace import profiled_kernels
+    kernels = profiled_kernels(lambda: (ag.step(), torch.cuda.synchronize()),
+                               {"nstep_dqn_actor_kernel": T, "nstep_dqn_update_kernel": 1})
     assert sum("nstep_dqn_actor_kernel" in k for k in kernels) == T, kernels
     assert sum("nstep_dqn_update_kernel" in k for k in kernels) == 1, kernels
     assert len(kernels) == T + 1, kernels

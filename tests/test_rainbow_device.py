@@ -855,13 +855,9 @@ def test_launcher_end_to_end(rl, monkeypatch):
         torch.cuda.synchronize()
 
     step()
-    sched = torch.profiler.schedule(wait=0, warmup=1, active=1, repeat=1)
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA], schedule=sched) as prof:
-        for _ in range(2):
-            step()
-            prof.step()
-    kernels = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-               and not e.name.startswith(("Memcpy", "Memset"))]
+    from _kernel_trace import profiled_kernels
+    kernels = profiled_kernels(step, {"rainbow_actor_kernel": c.sgd_update_frequency, "rainbow_replay_update_kernel": 1,
+                                     "feed_kernel": 1, "gather": 1, "sumtree_sample": 1, "direct_copy": 1})
     assert sum("rainbow_actor_kernel" in k for k in kernels) == c.sgd_update_frequency, kernels
     assert sum("rainbow_replay_update_kernel" in k for k in kernels) == 1, kernels
     others = [k for k in kernels if "rainbow_actor_kernel" not in k and "rainbow_replay_update_kernel" not in k]
