@@ -22,6 +22,8 @@
 //   warpgroups 1, 2  rows 0-63 / 64-127 of the tile: wgmma.mma_async m64nBNk16 (fp32 accumulators in registers), then the
 //                    epilogue: accumulators -> shared staging tile -> 8 columns x BN/16 rows per thread, whole rows
 //                    per warp instruction (epi_col / epi_row) -> bias / ReLU -> bf16 | fp32 | atomic fp32
+// (the convolution slab kernel instead gives the MMAs to one warpgroup and the two halves' epilogues to two more: see
+// conv_slab_body)
 // Every kernel runs its prologue (barrier init, tensor-map prefetch) before pdl_sync(): under programmatic dependent launch
 // that part overlaps the tail of the previous kernel (common.cuh).
 // sm_90a only.
@@ -87,7 +89,7 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 // named barriers: 0 = __syncthreads, 1 = the 256 MMA threads, 2 / 3 = MMA warpgroup 1 / 2, 4 = uint8 converters,
-// 5 / 6 = "MMA turn" of warpgroup 1 / 2 (slab kernel)
+// 5 / 6 = half 0 / 1 of the slab kernel's staging tile written, 7 / 8 = half 0 / 1 read (SLAB_BAR_STAGED / SLAB_BAR_FREE)
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
@@ -930,19 +932,32 @@ struct SlabParams {
   int stages;
   int base_offset_mode;    // 1: descriptor base_offset = (window start >> 7) & 7; 2: base_offset = 0 (address-based swizzle)
   U8Src u8;                // U8 kernels: the activation slabs are built from the uint8 frame ring (K1), tmA is unused
-  unsigned long long* clk; // U8 kernels, profiling hook (normally null): cycles per role summed over the CTAs, K1_CLK_*
+  unsigned long long* clk; // profiling hook (normally null): cycles per role summed over the CTAs, K1_CLK_*
 };
 
-// slots of the K1 phase probe (b2rl_conv1_set_phase_clocks): clock64() cycles summed over all CTAs -- the CTA's whole run
-// (thread 0), the producer's waits for a free uint8 stage, the converters' (thread 0 of warp 12) waits for a free slab and for
-// the pixels and their conversion, the MMA warpgroups' (thread 0 of each) waits for the MMA turn and the slab, their chain
-// from the first issue to its retirement, their whole epilogue and its accumulator staging part (stage_acc + barrier); the
-// last slot counts the tiles the MMA warpgroups took.
+// slots of the phase probe of the slab and K1 kernels (b2rl_conv1_set_phase_clocks): clock64() cycles summed over all CTAs,
+// each role timed by its thread 0 -- the CTA's whole run (thread 0), the producer's waits for a free stage, the converters'
+// waits for a free slab and for the pixels and their conversion; the MMA warpgroup's waits for the slab, its chain from the
+// first issue to its retirement, its waits for the epilogue warpgroups to free the staging tile and its accumulator staging;
+// the epilogue warpgroups' (both summed) waits for a staged half and their work on it; the tiles the MMA warpgroup took.
 enum { K1_CLK_CTA, K1_CLK_PRODUCER_WAIT, K1_CLK_CONVERT_WAIT_SLAB, K1_CLK_CONVERT_WAIT_PIXELS, K1_CLK_CONVERT, K1_CLK_MMA_WAIT,
-       K1_CLK_MMA, K1_CLK_EPILOGUE, K1_CLK_EPILOGUE_STAGE, K1_CLK_TILES, K1_CLK_SLOTS };
+       K1_CLK_MMA, K1_CLK_MMA_WAIT_FREE, K1_CLK_MMA_STAGE, K1_CLK_EPILOGUE_WAIT, K1_CLK_EPILOGUE, K1_CLK_TILES, K1_CLK_SLOTS };
 __device__ __forceinline__ long long clk_now(const unsigned long long* clk) { return clk ? clock64() : 0; }
 
-constexpr int SLAB_U8_THREADS = GEMM_THREADS + 128;   // K1: a fourth warpgroup (warps 12-15) converts the uint8 pixels
+constexpr int SLAB_U8_THREADS = GEMM_THREADS + 128;   // K1 weight gradient: a fourth warpgroup (warps 12-15) converts the pixels
+// The slab kernel: warpgroup 0 TMA producer, 1 MMA, 2 / 3 epilogue of rows 0-63 / 64-127 of each tile; K1: warpgroup 4
+// converts the uint8 pixels
+constexpr int SLAB_THREADS = 512;
+constexpr int SLAB_K1_THREADS = SLAB_THREADS + 128;
+constexpr int SLAB_BAR_STAGED = 5, SLAB_BAR_FREE = 7;  // + half: named barriers of the staging-tile hand-off (256 threads)
+// register split (setmaxnreg, per thread) per role: the launch gives every thread 65536 / threads (128 at 512 threads, 96 at
+// 640), and the roles' shares add up to at most that sum.  The MMA warpgroup holds both m64 x BN accumulator halves (BN 128:
+// 128 registers); an epilogue warpgroup one half's mask (BN 128: 32 registers) and its per-row work.
+template <bool U8> struct SlabRegs;
+template <> struct SlabRegs<false> { static constexpr int producer = 40, mma = 232, epilogue = 120, convert = 0; };   // 512
+template <> struct SlabRegs<true> { static constexpr int producer = 64, mma = 136, epilogue = 88, convert = 104; };    // 480
+template <int R> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Paired conv1 forward (PAIR: U8, BN 64, 2 x 2 taps, one column block): x1 = conv1_online(s) and z1 = conv1_target(s') in ONE
 // launch from the five-frame ring window idx-3 .. idx+1 shared by s (frames 0-3) and s' (frames 1-4, n_step 1).
@@ -961,10 +976,11 @@ __device__ __forceinline__ uint64_t make_desc_sw32(uint32_t smem_addr) {
 }
 // The tap grid (TX x TY taps) and the column blocks (CB = channels / 64) are template parameters: a tile's 2 x TX x TY x CB
 // k-tiles are then one unrolled chain of wgmmas in ONE commit group (a chain carried through runtime loops makes ptxas
-// serialize every wgmma).  The two MMA warpgroups ping-pong: warpgroup g takes every other tile of the CTA (the CTA's
-// i-th tile goes to warpgroup i % 2), whole 128-row tiles as two m64 accumulator halves, and "MMA turn" named barriers
-// let a warpgroup issue its tile's MMAs only after the other one has issued the previous tile's -- so one warpgroup's
-// epilogue runs while the other's MMAs keep the tensor cores busy.
+// serialize every wgmma).  One MMA warpgroup issues every tile of the CTA, whole 128-row tiles as two m64 accumulator
+// halves, and stages them into the fp32 staging tile; two epilogue warpgroups finish one 64-row half each, side by side.
+// Per half, named barriers hand the staging tile over (SLAB_BAR_STAGED: written, SLAB_BAR_FREE: read): the MMAs of the
+// next tile run during the epilogue of this one, so the CTA's period per tile is about the longest of MMA chain + staging,
+// one half's epilogue and (K1) one slab's conversion, not MMA chain + both halves' epilogue over two warpgroups.
 // The body of conv_slab_wgmma_kernel and of its paired conv1 instantiation conv1_pair_wgmma_kernel (below); the tensor maps
 // are the kernels' __grid_constant__ parameters.  PAIR: tmA = ring, tmB = online weights (box [32 n][1 tap][64 k]),
 // tmA2 / tmB2 = target weights (boxes [32][1][64] / [32][1][16]).
@@ -1009,7 +1025,7 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
   __shared__ float s_dbias[128];                    // per-CTA bias-gradient accumulator (backward extras)
   if (threadIdx.x < 128) s_dbias[threadIdx.x] = 0.0f;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS / 2); }   // one warpgroup per slab
+    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS / 2); }   // the MMA warpgroup
     mb_init(w_full, 1);
     if (U8) {
       for (int s = 0; s < U8_STAGES; ++s) { mb_init(&u8_full[s], 1); mb_init(&u8_empty[s], 1); }
@@ -1030,13 +1046,15 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
   }
   __syncthreads();
   pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
-  unsigned long long* const clk = U8 ? sp.clk : nullptr;
+  unsigned long long* const clk = sp.clk;
   const long long t_start = clk_now(clk);
-  long long c_wait = 0, c_wait2 = 0, c_work = 0, c_epi = 0, c_stage = 0;   // per-role sums of the probe (thread 0 of its role)
-  // register file split of the 384-thread kernel (setmaxnreg): the producer warpgroup needs few, the MMA warpgroups hold two
-  // m64 x BN accumulator halves across the epilogue of the first (BN 128: 128 registers); 128 x 56 + 256 x 224 <= 64K
+  long long c_wait = 0, c_wait2 = 0, c_work = 0, c_stage = 0;   // per-role sums of the probe (thread 0 of its role)
+  using R = SlabRegs<U8>;
+  constexpr int launch_regs = 65536 / (U8 ? SLAB_K1_THREADS : SLAB_THREADS) / 8 * 8;   // per thread
+  static_assert(R::producer + R::mma + 2 * R::epilogue + R::convert <= (U8 ? 5 : 4) * launch_regs,
+                "the roles' register shares exceed what the launch allocates");
   if (warp < 4) {
-    if constexpr (!U8) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+    reg_dec<R::producer>();
     if (warp == 0 && elect_one()) {
     if constexpr (PAIR) {
       mb_expect_tx(w_full, (uint32_t)k_tiles * (W_TILE + WB_TILE / 2));
@@ -1076,7 +1094,9 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
       uint32_t it = 0;
       for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
         const int s = it % sp.stages;
+        const long long t0 = clk_now(clk);
         mb_wait(&empty[s], ((it / sp.stages) & 1) ^ 1);
+        c_wait += clk_now(clk) - t0;
         mb_expect_tx(&full[s], slab_bytes);
         for (int cb = 0; cb < CB; ++cb)
           tma_load_2d(sS + (size_t)s * slab_bytes + (size_t)cb * slab_block, mA, &full[s], cb * GEMM_BK,
@@ -1088,11 +1108,13 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
           prefetch_l2_bulk(p.mask + (int64_t)r0 * p.mask_ld, (uint32_t)(((int64_t)(nr - 1) * p.mask_ld + p.N) * 2));
         }
       }
+      if (clk) atomicAdd(clk + K1_CLK_PRODUCER_WAIT, (unsigned long long)c_wait);
     }
     }
-  } else if (U8 && warp >= 12) {
-    // ---------------------------------------------------------------------- K1 converters (warps 12-15): staged uint8 -> slab
-    const int tid = (int)threadIdx.x - GEMM_THREADS;
+  } else if (U8 && warp >= 16) {
+    // ---------------------------------------------------------------------- K1 converters (warps 16-19): staged uint8 -> slab
+    reg_inc<R::convert>();
+    const int tid = (int)threadIdx.x - SLAB_THREADS;
     uint32_t it = 0;
     for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
       const int s = it % sp.stages, us = it % U8_STAGES;
@@ -1112,22 +1134,19 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
       atomicAdd(clk + K1_CLK_CONVERT_WAIT_PIXELS, (unsigned long long)c_wait2);
       atomicAdd(clk + K1_CLK_CONVERT, (unsigned long long)c_work);
     }
-  } else {
-    // ---------------------------------------------------------------------- MMA + epilogue, warpgroup g: tiles i = g, g + 2, ...
-    // of this CTA, rows 0-63 / 64-127 of a tile in accumulator halves d[0] / d[1]; the epilogue stages one half at a time
-    // through the warpgroup's own 64-row part of sAcc
-    if constexpr (!U8) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
-    const int t = wl * 32 + lane;                                   // epilogue_half's thread index in the warpgroup
-    float* sAcc_g = sAcc + g * 64 * ACC_LD;
+  } else if (warp < 8) {
+    // ---------------------------------------------------------------------- MMA (warps 4-7): every tile of this CTA, rows
+    // 0-63 / 64-127 in accumulator halves d[0] / d[1], each staged into its half of sAcc once its epilogue warpgroup has
+    // read the previous tile's
+    reg_inc<R::mma>();
+    const int wl = warp - 4;
     const uint32_t w0 = s2u(sW), wb0 = s2u(sWB);
     mb_wait(w_full, 0);
-    uint32_t it = g;
-    int n_tiles_g = 0;
-    for (int tile = cta + g * n_cta; tile < tiles; tile += 2 * n_cta, it += 2) {
+    long long c_free = 0;
+    uint32_t it = 0;
+    for (int tile = cta; tile < tiles; tile += n_cta, ++it) {
       const int s = it % sp.stages;
       const long long t0 = clk_now(clk);
-      if (it > 0) named_sync(5 + g, 256);                           // the other warpgroup has issued tile it - 1
       mb_wait(&full[s], (it / sp.stages) & 1);
       const long long t1 = clk_now(clk);
       float d[2][BN / 2];
@@ -1159,36 +1178,50 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
         }
       }
       wg_commit();
-      if (tile + n_cta < tiles) named_arrive(5 + (g ^ 1), 256);      // MMA turn to the other warpgroup
-      // first half's mask: in flight while the MMAs run, the second half's during the first half's epilogue -- at BN 128
-      // each only once the registers it needs are free (128 accumulator and 32 mask registers together spill)
-      int4 mk[2][BN / 16];
-      if constexpr (BN <= 64) epi_mask_load<BN, EXT>(p, tile * GEMM_BM, 0, t, mk[0]);
       wg_wait0();
       acc_fence<BN>(d[0]);
       acc_fence<BN>(d[1]);
       if (lane == 0) mb_arrive(&empty[s]);
       const long long t2 = clk_now(clk);
-      if constexpr (BN > 64) epi_mask_load<BN, EXT>(p, tile * GEMM_BM, 0, t, mk[0]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (BN > 64 && h == 1) epi_mask_load<BN, EXT>(p, tile * GEMM_BM + 64, 0, t, mk[1]);
         const long long t3 = clk_now(clk);
-        stage_acc<BN>(d[h], sAcc_g, ACC_LD, wl, lane);
-        named_sync(2 + g, 128);
-        c_stage += clk_now(clk) - t3;
-        if (BN <= 64 && h == 0) epi_mask_load<BN, EXT>(p, tile * GEMM_BM + 64, 0, t, mk[1]);   // in flight during the first half
-        epilogue_half<BN, EXT, PAIR>(p, tile * GEMM_BM + 64 * h, 0, t, sAcc_g, mk[h], s_dbias);
-        named_sync(2 + g, 128);
+        if (it > 0) named_sync(SLAB_BAR_FREE + h, 256);              // epilogue warpgroup h has read the previous tile's half
+        const long long t4 = clk_now(clk);
+        stage_acc<BN>(d[h], sAcc + h * 64 * ACC_LD, ACC_LD, wl, lane);
+        named_arrive(SLAB_BAR_STAGED + h, 256);
+        c_free += t4 - t3, c_stage += clk_now(clk) - t4;
       }
-      c_wait += t1 - t0, c_work += t2 - t1, c_epi += clk_now(clk) - t2, ++n_tiles_g;
+      c_wait += t1 - t0, c_work += t2 - t1;
     }
-    if (clk && t == 0) {
+    if (clk && wl == 0 && lane == 0) {
       atomicAdd(clk + K1_CLK_MMA_WAIT, (unsigned long long)c_wait);
       atomicAdd(clk + K1_CLK_MMA, (unsigned long long)c_work);
-      atomicAdd(clk + K1_CLK_EPILOGUE, (unsigned long long)c_epi);
-      atomicAdd(clk + K1_CLK_EPILOGUE_STAGE, (unsigned long long)c_stage);
-      atomicAdd(clk + K1_CLK_TILES, (unsigned long long)n_tiles_g);
+      atomicAdd(clk + K1_CLK_MMA_WAIT_FREE, (unsigned long long)c_free);
+      atomicAdd(clk + K1_CLK_MMA_STAGE, (unsigned long long)c_stage);
+      atomicAdd(clk + K1_CLK_TILES, (unsigned long long)it);
+    }
+  } else {
+    // ---------------------------------------------------------------------- epilogue, warpgroup 2 + e (warps 8-15): rows
+    // 64 e .. 64 e + 63 of every tile of this CTA; the tile's mask is requested before the wait for its staged half, so that
+    // it is in flight during the tile's MMAs
+    reg_dec<R::epilogue>();
+    const int e = (warp - 8) >> 2, wl = (warp - 8) & 3;
+    const int t = wl * 32 + lane;                                   // epilogue_half's thread index in the warpgroup
+    const float* sAcc_e = sAcc + e * 64 * ACC_LD;
+    for (int tile = cta; tile < tiles; tile += n_cta) {
+      int4 mk[BN / 16];
+      epi_mask_load<BN, EXT>(p, tile * GEMM_BM + 64 * e, 0, t, mk);
+      const long long t0 = clk_now(clk);
+      named_sync(SLAB_BAR_STAGED + e, 256);
+      const long long t1 = clk_now(clk);
+      epilogue_half<BN, EXT, PAIR>(p, tile * GEMM_BM + 64 * e, 0, t, sAcc_e, mk, s_dbias);
+      if (tile + n_cta < tiles) named_arrive(SLAB_BAR_FREE + e, 256);   // the MMA warpgroup waits only for a next tile
+      c_wait += t1 - t0, c_work += clk_now(clk) - t1;
+    }
+    if (clk && t == 0) {
+      atomicAdd(clk + K1_CLK_EPILOGUE_WAIT, (unsigned long long)c_wait);
+      atomicAdd(clk + K1_CLK_EPILOGUE, (unsigned long long)c_work);
     }
   }
   __syncthreads();
@@ -1197,7 +1230,7 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
 }
 
 template <int BN, bool EXT, bool U8, int TX, int TY, int CB>
-__global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_slab_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+__global__ void __launch_bounds__(U8 ? SLAB_K1_THREADS : SLAB_THREADS, 1) conv_slab_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                           const __grid_constant__ CUtensorMap tmB,
                                                                           const __grid_constant__ CUtensorMap tmA2,
                                                                           const __grid_constant__ CUtensorMap tmB2,
@@ -1205,7 +1238,7 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv_s
   conv_slab_body<BN, EXT, U8, TX, TY, CB, false>(tmA, tmB, tmA2, tmB2, sp);
 }
 // conv1's K1 instantiation with the PAIR flag: b2rl_conv1_u8_fwd_pair
-__global__ void __launch_bounds__(SLAB_U8_THREADS, 1) conv1_pair_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+__global__ void __launch_bounds__(SLAB_K1_THREADS, 1) conv1_pair_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                              const __grid_constant__ CUtensorMap tmB,
                                                                              const __grid_constant__ CUtensorMap tmA2,
                                                                              const __grid_constant__ CUtensorMap tmB2,
@@ -1838,7 +1871,7 @@ static int launch_slab_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   if (ctas > tiles) ctas = tiles;
   if (ctas < 1) ctas = 1;
   g_last_ctas = sp.g.dual ? 2 * ctas : ctas;
-  launch_pdl(k, dim3(sp.g.dual ? 2 * ctas : ctas), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, ta, tb, ta2, tb2, sp);
+  launch_pdl(k, dim3(sp.g.dual ? 2 * ctas : ctas), dim3(U8 ? SLAB_K1_THREADS : SLAB_THREADS), smem, st, ta, tb, ta2, tb2, sp);
   return check_launch("b2rl_conv_gemm_bf16(slab)");
 }
 
@@ -1985,9 +2018,10 @@ static int64_t g_partial_stride = 0;
 static int g_partial_count = 0;
 static int g_use_slab = 2;   // 2: shifted windows with base_offset 0 -- the 128B swizzle is a pure function of the smem address
 static unsigned long long* g_k1_clocks = nullptr;
-// Profiling hook of the K1 conv1 forwards (b2rl_conv1_u8_fwd, b2rl_conv1_u8_fwd_pair) and of conv1's weight gradient
-// (b2rl_conv1_u8_wgrad_partials, b2rl_conv1_wgrad_partials): while set, every launch adds its K1_CLK_SLOTS phase-cycle sums
-// to clocks[] (scripts/conv1_pair_time.py --phases, scripts/conv1_wgrad_time.py --phases).  Null (the default): no probe.
+// Profiling hook of every slab launch (the K1 conv1 forwards b2rl_conv1_u8_fwd / b2rl_conv1_u8_fwd_pair, the slab forwards
+// and dgrads of b2rl_conv_gemm_*) and of conv1's weight gradient (b2rl_conv1_u8_wgrad_partials, b2rl_conv1_wgrad_partials):
+// while set, every launch adds its K1_CLK_SLOTS phase-cycle sums to clocks[] (scripts/slab_phase_time.py --phases,
+// scripts/conv1_pair_time.py --phases, scripts/conv1_wgrad_time.py --phases).  Null (the default): no probe.
 extern "C" int b2rl_conv1_set_phase_clocks(int64_t* clocks) {
   g_k1_clocks = reinterpret_cast<unsigned long long*>(clocks);
   return B2RL_OK;
@@ -2084,6 +2118,7 @@ static int conv_gemm_impl(int32_t mode, const uint16_t* X, int64_t rows, int32_t
       sp.slab_rows = (GEMM_BM + max_shift + 7) / 8 * 8;
       sp.min_shift = shift_sign > 0 ? 0 : -max_shift;
       sp.base_offset_mode = g_use_slab;
+      sp.clk = g_k1_clocks;
       if (sp.slab_rows <= 256) {
         CUtensorMap ta, tb, ta2, tb2;
         rc = make_map(&ta, X, C, rows, C, sp.slab_rows);            // box [slab_rows][64]

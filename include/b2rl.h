@@ -408,9 +408,11 @@ int b2rl_conv1_u8_fwd_pair(const uint8_t* frames, int64_t capacity, const int64_
                            int32_t frame_w, int32_t batch, int32_t history, const uint16_t* W, const uint16_t* W2, void* D,
                            void* D2, int64_t ldd, const float* bias, const float* bias2, int32_t relu, int32_t out_map, int32_t V,
                            void* stream);
-/* Profiling hook of the two conv1 forwards above: while `clocks` (device, 10 int64, zeroed by the caller) is set, every launch
- * adds per-role clock64() cycle sums to it -- CTA run, producer waits, converter waits (slab, pixels) and conversion, MMA waits,
- * MMA chain, epilogue and its staging part, tiles (csrc/gemm.cu K1_CLK_*).  NULL (the default) turns it off. */
+/* Profiling hook of every convolution slab launch (the two conv1 forwards above, the conv_gemm forwards and dgrads) and of
+ * conv1's weight gradient: while `clocks` (device, 12 int64, zeroed by the caller) is set, every launch adds per-role clock64()
+ * cycle sums to it -- CTA run, producer waits, converter waits (slab, pixels) and conversion, MMA waits for the slab, MMA
+ * chain, MMA waits for a free staging tile, accumulator staging, epilogue waits for a staged half, epilogue work, tiles
+ * (csrc/gemm.cu K1_CLK_*).  NULL (the default) turns it off. */
 int b2rl_conv1_set_phase_clocks(int64_t* clocks);
 
 /* D = act(A B^T + bias) (bf16 out) in one launch: K split over the `splits` CTAs (1, 2, 4 or 8; 0: chosen from the shape) of

@@ -2,7 +2,7 @@
 window) against the two b2rl_conv1_u8_fwd launches it replaces, at the bench's batch: each form timed alone in a CUDA
 graph of back-to-back calls (bench.time_kernel_graph, best of 5 replays), beside its HBM and MMA floors.  Prints the card's
 name and power limit first.  --phases: the K1 kernels' clock64 probe (b2rl_conv1_set_phase_clocks) -- cycles per tile of
-each role (producer, converters, MMA warpgroups, epilogue) -- for the single launch and the pair.
+each role (producer, converters, MMA warpgroup, epilogue warpgroups) -- for the single launch and the pair.
 Usage: python scripts/conv1_pair_time.py [--batch 512] [--iters 50] [--phases]"""
 import argparse
 import os
@@ -19,8 +19,9 @@ from deeprl_b200.network.nature_tc import RingFrames  # noqa: E402
 
 PEAK, HBM = 989e12, 3.35e12          # H100 SXM data sheet: dense bf16 FLOP/s, HBM3 bytes/s
 CLK = ["CTA run", "producer: wait for a free uint8 stage", "converters: wait for a free slab", "converters: wait for pixels",
-       "converters: convert", "MMA: wait for turn + slab", "MMA: chain issue -> retire", "epilogue",
-       "epilogue: of it, accumulator staging", "tiles"]
+       "converters: convert", "MMA: wait for the slab", "MMA: chain issue -> retire", "MMA: wait for a free staging half",
+       "MMA: accumulator staging", "epilogue: wait for a staged half (2 warpgroups)",
+       "epilogue: work (2 warpgroups)", "tiles"]
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--batch", type=int, default=512)

@@ -22,7 +22,7 @@ from deeprl_b200.network.nature_tc import RingFrames  # noqa: E402
 
 PEAK, HBM = 989e12, 3.35e12          # H100 SXM data sheet: dense bf16 FLOP/s, HBM3 bytes/s
 CLK = ["CTA run", "producer: wait for free stages", "converters: wait for a free stage", "converters: wait for pixels",
-       "converters: convert", "MMA: wait for a full stage", "MMA: issue + retire-one wait", "", "", "k-blocks"]
+       "converters: convert", "MMA: wait for a full stage", "MMA: issue + retire-one wait", "", "", "", "", "k-blocks"]
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--batch", type=int, default=512)
