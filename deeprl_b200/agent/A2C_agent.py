@@ -18,7 +18,7 @@ device, the actions down to the host) and one ``GraphedA2CLearner`` replay per r
 from the device's Philox stream (keyed from torch's seeded generator, as with ``config.device_a2c``), not from torch's
 ``Categorical.sample``.  The torch optimizer is replaced by a ``FlatOptimizer`` with its hyper-parameters; the network's
 parameters become views into its arena, so ``state_dict()`` is always current.  Configurations it does not cover
-(``component/actor.py a2c_graph_unsupported``; the reason is kept in ``graph_refusal``) keep the eager path;
+(``component/coverage.py a2c_graph_unsupported``; the reason is kept in ``graph_refusal``) keep the eager path;
 ``config.device_a2c`` takes precedence.
 """
 import numpy as np
@@ -27,7 +27,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..component import Storage
-from ..utils import tensor, to_np
+from ..utils import philox_seed, tensor, to_np
 from .BaseAgent import BaseAgent
 
 
@@ -76,8 +76,7 @@ class A2CAgent(BaseAgent):
         self.device_a2c = None
         if getattr(config, "device_a2c", False):
             from ..component.actor import DeviceA2C
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
-            self.device_a2c = DeviceA2C(self.network, self.optimizer, config, seed)
+            self.device_a2c = DeviceA2C(self.network, self.optimizer, config, philox_seed())
             self.optimizer = self.device_a2c.opt
 
     def eval_step(self, state):
@@ -155,16 +154,16 @@ class A2CAgent(BaseAgent):
         """Decided on the first step: the captured actor + update serve this configuration (``a2c_graph_unsupported``), or the
         eager path runs (the reason is kept in ``graph_refusal``)."""
         if self._graph is None:
-            from ..component.actor import GraphedQActor, a2c_graph_unsupported
+            from ..component.actor import GraphedQActor
+            from ..component.coverage import a2c_graph_unsupported
             from ..learner import GraphedA2CLearner
             config = self.config
             self.graph_refusal = a2c_graph_unsupported(config, self.network, self.optimizer, self.states)
             self._graph = False
             if self.graph_refusal is None:
                 self.optimizer = ops.FlatOptimizer.from_torch(self.optimizer, list(self.network.parameters()))
-                seed = int(torch.randint(0, 2 ** 62, (1,)).item())      # the Philox key, from torch's (seeded) generator
                 coef = config.state_normalizer.coef
-                lr = GraphedA2CLearner(self.network, self.optimizer, config.rollout_length, config.num_workers, seed,
+                lr = GraphedA2CLearner(self.network, self.optimizer, config.rollout_length, config.num_workers, philox_seed(),
                                        config.discount, config.gae_tau, config.use_gae, config.entropy_weight,
                                        config.value_loss_weight, config.gradient_clip, coef).capture()
                 actor = GraphedQActor(self.network, None, config.num_workers, 4, (84, 84), coef, arena=lr.arena, run=lr.act,

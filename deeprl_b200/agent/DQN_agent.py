@@ -25,7 +25,7 @@ so the ``reset_noise()`` calls of the eager path do not run.
 exploration each step's transitions are staged in the learner's pinned buffer and fed inside ONE update replay
 (``_async_graph_update``; learner.GraphedDQNLearner with ``prefetch`` and ``wrapper_order``), the actor's forward is a
 GraphedQActor replay, on the actor thread with ``async_actor`` (component/actor.py ``ParameterOrder``).  Configurations it
-does not cover (``component/actor.py dqn_graph_unsupported``; the reason is kept in ``graph_refusal``) keep their path.
+does not cover (``component/coverage.py dqn_graph_unsupported``; the reason is kept in ``graph_refusal``) keep their path.
 """
 import threading
 
@@ -36,7 +36,7 @@ import torch.nn as nn
 from .. import ops
 from ..component import LazyFrames, PrioritizedTransition
 from ..network.fused import frame_scale
-from ..utils import Config, RescaleNormalizer, close_obj, epsilon_greedy, tensor, to_np
+from ..utils import Config, RescaleNormalizer, close_obj, epsilon_greedy, philox_seed, tensor, to_np
 from .BaseAgent import BaseActor, BaseAgent
 
 
@@ -60,12 +60,12 @@ class DQNActor(BaseActor):
         Not for subclasses that redefine ``compute_q`` itself (they get the statements of the reference)."""
         ga = getattr(self, "_graph_actor", None)
         if ga is None:
-            from ..component import actor as device_actor
+            from ..component.actor import GraphedQActor
+            from ..component.coverage import q_actor_unsupported
             order = self._order
             ok = (type(self).compute_q is DQNActor.compute_q
-                  and device_actor.q_actor_supported(self.config, self._network, async_ok=order is not None)
-                  and all(np.asarray(s).dtype == np.uint8 and np.asarray(s).shape == (4, 84, 84) for s in self._state))
-            ga = self._graph_actor = device_actor.GraphedQActor(
+                  and q_actor_unsupported(self.config, self._network, self._state, async_ok=order is not None) is None)
+            ga = self._graph_actor = GraphedQActor(
                 self._network, self._q_tensor, len(self._state), 4, (84, 84), self.config.state_normalizer.coef) if ok else False
             if ga and order is not None and self.config.async_actor:
                 ga.capture_error_mode = "thread_local"     # the learner thread may synchronise while this thread captures
@@ -167,28 +167,25 @@ class DQNAgent(BaseAgent):
         self.last_loss = None
         self.device_dqn = None
         self._learner = None
-        flag = self._device_flag
+        from ..component.actor import DeviceDistDQN, DeviceDQN, DeviceRainbow, ParameterOrder
+        flag, device = self._device_flag, None
         if getattr(config, "device_rainbow", False):
             for other in ("device_dqn", flag):
                 if other is not None and getattr(config, other, False):
                     raise NotImplementedError("config.device_rainbow and config.%s are both set; a RainbowNet runs on the "
                                               "device with config.device_rainbow alone" % other)
-            from ..component.actor import DeviceRainbow
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
-            self.device_dqn = self.actor._device_dqn = DeviceRainbow(self, seed)
+            device = DeviceRainbow
         elif flag is not None and getattr(config, flag, False):
             if getattr(config, "device_dqn", False):
                 raise NotImplementedError("config.device_dqn and config.%s are both set; %s runs on the device with "
                                           "config.%s alone" % (flag, type(self).__name__, flag))
-            from ..component.actor import DeviceDistDQN
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
-            self.device_dqn = self.actor._device_dqn = DeviceDistDQN(self, seed)
+            device = DeviceDistDQN
         elif getattr(config, "device_dqn", False):
-            from ..component.actor import DeviceDQN
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
-            self.device_dqn = self.actor._device_dqn = DeviceDQN(self, seed)
+            device = DeviceDQN
+        if device is not None:
+            self.device_dqn = self.actor._device_dqn = device(self, philox_seed())
         # config.cuda_graph with async replay: decided once, here, before the actor thread starts
-        from ..component.actor import ParameterOrder, dqn_graph_unsupported
+        from ..component.coverage import dqn_graph_unsupported
         self.graph_refusal = dqn_graph_unsupported(config, self)
         self._async_graph = self.graph_refusal is None
         if self._async_graph:
@@ -394,19 +391,25 @@ class DQNAgent(BaseAgent):
         inner = getattr(self.replay, "replay", self.replay)
         return len(getattr(inner, "item_shape", ())) == 2 and inner.size() >= inner.batch_size + 64
 
-    def _graph_update(self):
+    def _graphed_learner(self, replay, **schedule):
+        """The learner.GraphedDQNLearner of ``_graph_update`` and ``_async_learner``, which differ only in ``schedule``:
+        ``feeds_per_update``, ``prefetch`` and ``wrapper_order``."""
         from ..learner import GraphedDQNLearner
+        config = self.config
+        return GraphedDQNLearner(
+            self.network, self.target_network, self._flat, replay, kind=self._graph_kind, discount=config.discount,
+            n_step=config.n_step, double_q=bool(config.double_q), gradient_clip=config.gradient_clip or 0.0,
+            compute_dtype=Config.COMPUTE_DTYPE, state_scale=config.state_normalizer.coef,
+            replay_eps=getattr(config, "replay_eps", 0.01), replay_alpha=getattr(config, "replay_alpha", 0.5),
+            categorical=(getattr(config, "categorical_v_min", -10.0), getattr(config, "categorical_v_max", 10.0)),
+            target_sync_every=0, **schedule)
+
+    def _graph_update(self):
         config = self.config
         lr = getattr(self, "_learner", None)
         if lr is None:
-            inner = getattr(self.replay, "replay", self.replay)
-            lr = self._learner = GraphedDQNLearner(
-                self.network, self.target_network, self._flat, inner, kind=self._graph_kind, discount=config.discount,
-                n_step=config.n_step, double_q=bool(config.double_q), gradient_clip=config.gradient_clip or 0.0,
-                feeds_per_update=0, compute_dtype=Config.COMPUTE_DTYPE, state_scale=config.state_normalizer.coef,
-                replay_eps=getattr(config, "replay_eps", 0.01), replay_alpha=getattr(config, "replay_alpha", 0.5),
-                categorical=(getattr(config, "categorical_v_min", -10.0), getattr(config, "categorical_v_max", 10.0)),
-                target_sync_every=0, prefetch=False)
+            lr = self._learner = self._graphed_learner(getattr(self.replay, "replay", self.replay), feeds_per_update=0,
+                                                       prefetch=False)
             with config.lock:
                 lr.capture(warmup=1)                       # NOTE: the warm-up is one real (extra) gradient update
         if lr.per:
@@ -418,7 +421,7 @@ class DQNAgent(BaseAgent):
 
     # ------------------------------------------------------------------ config.cuda_graph with async replay (opt-in)
     def _async_graph_update(self, feeds):
-        """``step()`` on the captured path with async replay (``component/actor.py dqn_graph_unsupported``): this step's
+        """``step()`` on the captured path with async replay (``component/coverage.py dqn_graph_unsupported``): this step's
         transitions -- frame ``s[-1]``, action, ``reward_normalizer(r)``, mask -- and PER's ``replay_beta()`` go into the
         learner's pinned staging buffer, then ONE update replay copies them up, trains on the batch the previous replay drew,
         feeds them after that batch's last ring read and draws the next batch (learner.GraphedDQNLearner with ``prefetch``
@@ -453,19 +456,12 @@ class DQNAgent(BaseAgent):
         self.last_loss = lr.loss
 
     def _async_learner(self, feeds):
-        from ..learner import GraphedDQNLearner
         config = self.config
         inner = self.replay.replay
         inner.allocate(np.asarray(feeds[0]["state"][0]))   # (the ring exists once the wrapper has fed it)
         with config.lock:
-            lr = GraphedDQNLearner(
-                self.network, self.target_network, self._flat, inner, kind=self._graph_kind, discount=config.discount,
-                n_step=config.n_step, double_q=bool(config.double_q), gradient_clip=config.gradient_clip or 0.0,
-                feeds_per_update=sum(len(d["state"]) for d in feeds), compute_dtype=Config.COMPUTE_DTYPE,
-                state_scale=config.state_normalizer.coef, replay_eps=getattr(config, "replay_eps", 0.01),
-                replay_alpha=getattr(config, "replay_alpha", 0.5),
-                categorical=(getattr(config, "categorical_v_min", -10.0), getattr(config, "categorical_v_max", 10.0)),
-                target_sync_every=0, prefetch=True, wrapper_order=True)
+            lr = self._graphed_learner(inner, feeds_per_update=sum(len(d["state"]) for d in feeds), prefetch=True,
+                                       wrapper_order=True)
         if config.async_actor:
             lr.capture_error_mode = "thread_local"         # the actor thread may synchronise its stream during the capture
         return lr

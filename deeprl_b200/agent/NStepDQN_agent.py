@@ -20,7 +20,7 @@ unmet condition.
 step (pinned upload of the frame stacks into the rollout arena, the network, q down to the host; epsilon-greedy stays in numpy
 as in the reference) and one ``GraphedNStepLearner`` replay per rollout (learner.py).  The torch optimizer is replaced by a
 ``FlatOptimizer`` with its hyper-parameters; the network's parameters become views into its arena, so ``state_dict()`` is
-always current.  Configurations it does not cover (``component/actor.py nstep_q_graph_unsupported``; the reason is kept in
+always current.  Configurations it does not cover (``component/coverage.py nstep_q_graph_unsupported``; the reason is kept in
 ``graph_refusal``) keep the eager path; ``config.device_nstep_dqn`` takes precedence.
 """
 import numpy as np
@@ -29,7 +29,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..component import Storage
-from ..utils import epsilon_greedy, tensor, to_np
+from ..utils import epsilon_greedy, philox_seed, tensor, to_np
 from .BaseAgent import BaseAgent
 
 
@@ -50,8 +50,7 @@ class NStepDQNAgent(BaseAgent):
         self.device_nstep_dqn = None
         if getattr(config, "device_nstep_dqn", False):
             from ..component.actor import DeviceNStepDQN
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the Philox key, from torch's (seeded) generator
-            self.device_nstep_dqn = DeviceNStepDQN(self.network, self.target_network, self.optimizer, config, seed)
+            self.device_nstep_dqn = DeviceNStepDQN(self.network, self.target_network, self.optimizer, config, philox_seed())
             self.optimizer = self.device_nstep_dqn.opt
 
     def eval_step(self, state):
@@ -145,7 +144,8 @@ class NStepDQNAgent(BaseAgent):
         """Decided on the first step: the captured actor + update serve this configuration (``nstep_q_graph_unsupported``),
         or the eager path runs (the reason is kept in ``graph_refusal``)."""
         if self._graph is None:
-            from ..component.actor import GraphedQActor, nstep_q_graph_unsupported
+            from ..component.actor import GraphedQActor
+            from ..component.coverage import nstep_q_graph_unsupported
             from ..learner import GraphedNStepLearner
             config = self.config
             self.graph_refusal = nstep_q_graph_unsupported(config, self.network, self.optimizer, self.states)

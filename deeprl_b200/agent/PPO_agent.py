@@ -16,7 +16,7 @@ seeded generator, as in ``a2c_pixel``), not from torch's ``Categorical.sample``;
 ``random_sample`` on the host.  A ``FlatOptimizer`` built from ``self.opt`` takes over the Adam state; ``self.opt`` stays as
 the holder of ``lr_scheduler``'s learning rate, which each update reads from the device.  The network's parameters become
 views into the optimizer's arena, so ``state_dict()`` is always current.  Configurations it does not cover
-(``component/actor.py ppo_graph_unsupported``; the reason is kept in ``graph_refusal``) keep the eager path.
+(``component/coverage.py ppo_graph_unsupported``; the reason is kept in ``graph_refusal``) keep the eager path.
 """
 import numpy as np
 import torch
@@ -24,7 +24,7 @@ import torch.nn as nn
 
 from .. import ops
 from ..component import Storage
-from ..utils import random_sample, tensor, to_np
+from ..utils import philox_seed, random_sample, tensor, to_np
 from .A2C_agent import compute_advantages
 from .BaseAgent import BaseAgent
 
@@ -282,19 +282,19 @@ class PPOAgent(BaseAgent):
         """Decided on the first step: the captured actor + update serve this configuration (``ppo_graph_unsupported``), or the
         eager path runs (the reason is kept in ``graph_refusal``)."""
         if not self._graph_checked:
-            from ..component.actor import GraphedQActor, ppo_graph_unsupported
+            from ..component.actor import GraphedQActor
+            from ..component.coverage import ppo_graph_unsupported
             from ..learner import GraphedPPOPixelLearner
             config = self.config
             self._graph_checked = True
             self.graph_refusal = ppo_graph_unsupported(config, self.network, getattr(self, "opt", None), self._raw_states)
             if self.graph_refusal is None:
                 self.flat_opt = ops.FlatOptimizer.from_torch(self.opt, list(self.network.parameters()))
-                seed = int(torch.randint(0, 2 ** 62, (1,)).item())      # the Philox key, from torch's (seeded) generator
                 coef = config.state_normalizer.coef
-                lr = GraphedPPOPixelLearner(self.network, self.flat_opt, config.rollout_length, config.num_workers, seed,
-                                            config.mini_batch_size, config.optimization_epochs, config.discount,
-                                            config.gae_tau, config.use_gae, config.ppo_ratio_clip, config.entropy_weight,
-                                            config.gradient_clip, coef).capture()
+                lr = GraphedPPOPixelLearner(self.network, self.flat_opt, config.rollout_length, config.num_workers,
+                                            philox_seed(), config.mini_batch_size, config.optimization_epochs,
+                                            config.discount, config.gae_tau, config.use_gae, config.ppo_ratio_clip,
+                                            config.entropy_weight, config.gradient_clip, coef).capture()
                 actor = GraphedQActor(self.network, None, config.num_workers, 4, (84, 84), coef, arena=lr.arena, run=lr.act,
                                       body=self.network.phi_body)
                 self._graph = (lr, actor)

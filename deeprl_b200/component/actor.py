@@ -12,6 +12,9 @@ import torch
 from .. import _lib
 from ..network.network_bodies import DummyBody, FCBody
 from ..utils.normalizer import MeanStdNormalizer, RunningMoments
+from .coverage import a2c_unsupported, dist_dqn_unsupported, dqn_unsupported, nstep_dqn_unsupported, rainbow_unsupported
+# the captured paths' predicates stay importable from here, where callers have always found them
+from .coverage import a2c_graph_unsupported, dqn_graph_unsupported, nstep_q_graph_unsupported, ppo_graph_unsupported  # noqa: F401
 
 _f32, _f64 = torch.float32, torch.float64
 
@@ -275,21 +278,6 @@ class ParameterOrder:
         return self.stream
 
 
-def q_actor_supported(config, network, async_ok=False):
-    """``config.cuda_graph`` + synchronous actor + bf16 wgmma NatureConvBody on a CUDA device + ImageNormalizer-style rescale
-    of uint8 frames: the conditions under which the actor's forward is the captured device path.  ``async_ok``: the agent
-    orders an actor thread's replays against its updates (``ParameterOrder``), so ``async_actor`` is no obstacle."""
-    from ..network.network_bodies import NatureConvBody
-    from ..utils import Config
-    from ..utils.normalizer import RescaleNormalizer
-    body = getattr(network, "body", None)
-    return bool(getattr(config, "cuda_graph", False) and (async_ok or not config.async_actor) and not config.noisy_linear
-                and isinstance(body, NatureConvBody) and not body.noisy_linear and body.conv1.weight.is_cuda
-                and body.conv1.in_channels == 4
-                and Config.COMPUTE_DTYPE == torch.bfloat16 and Config.DENSE_BACKEND == "tcgen05"
-                and isinstance(config.state_normalizer, RescaleNormalizer))
-
-
 @contextlib.contextmanager
 def no_gc():
     """No garbage collection inside a graph capture: collecting unreachable objects that own CUDA resources (pinned buffers,
@@ -303,237 +291,29 @@ def no_gc():
             gc.enable()
 
 
-def nstep_q_graph_unsupported(config, network, optimizer, states):
-    """``None`` when ``NStepDQNAgent.step()`` runs as captured graphs under ``config.cuda_graph`` (GraphedQActor per env step,
-    learner.GraphedNStepLearner per rollout), else the unmet condition; the agent then keeps its eager path.  ``states``: the
-    envs' current observations.  (``config.async_actor`` plays no part: this agent steps its envs itself.)"""
-    from ..network import nature_tc
-    from ..network.network_bodies import NatureConvBody
-    from ..network.network_heads import VanillaNet
-    from ..utils import Config
-    from ..utils.normalizer import RescaleNormalizer
-    if not getattr(config, "cuda_graph", False):
-        return "config.cuda_graph is not set"
-    if getattr(config, "device_nstep_dqn", False):
-        return "config.device_nstep_dqn is set; it runs the agent on the device itself"
-    if type(network) is not VanillaNet:
-        return "the network is a %s; the captured update implements VanillaNet" % type(network).__name__
-    body = network.body
-    if not isinstance(body, NatureConvBody):
-        return "the body is a %s; the captured update implements NatureConvBody" % type(body).__name__
-    if body.noisy_linear or config.noisy_linear:
-        return "the network has NoisyLinear layers; the captured update implements nn.Linear"
-    if body.conv1.in_channels != 4:
-        return "the NatureConvBody takes %d channels; the captured update reads stacks of 4 frames" % body.conv1.in_channels
-    if Config.COMPUTE_DTYPE != torch.bfloat16 or Config.DENSE_BACKEND != "tcgen05":
-        return ("the compute dtype is %s with the %r dense backend; the captured update runs bf16 on the wgmma kernels "
-                "(tcgen05)" % (Config.COMPUTE_DTYPE, Config.DENSE_BACKEND))
-    if not (nature_tc.FUSED_BWD and _lib.CONV_SLAB):
-        return "the fused backward epilogues are switched off; the captured update needs the fused update tail"
-    if network.fc_head.out_features >= 32:
-        return "%d actions; the narrow head and loss kernels take fewer than 32" % network.fc_head.out_features
-    if not isinstance(config.state_normalizer, RescaleNormalizer):
-        return "the state normalizer is %s; the captured update folds a RescaleNormalizer into conv1" % type(
-            config.state_normalizer).__name__
-    if not all(np.asarray(s).dtype == np.uint8 and np.asarray(s).shape == (4, 84, 84) for s in states):
-        return "the envs do not return uint8 4 x 84 x 84 frame stacks"
-    # what FlatOptimizer.from_torch turns into a kind the fused tail (NatureTail) takes
-    g = optimizer.param_groups[0]
-    if not ((isinstance(optimizer, torch.optim.RMSprop) and g["momentum"] == 0 and g["weight_decay"] == 0)
-            or (isinstance(optimizer, torch.optim.Adam) and g["weight_decay"] == 0 and not g["amsgrad"])):
-        return ("the optimizer is %s; the fused update tail implements RMSprop (centered or not) and Adam without momentum, "
-                "weight decay or amsgrad" % type(optimizer).__name__)
-    if not body.conv1.weight.is_cuda:
-        return "the network is not on a CUDA device (select_device(0))"
-    return None
-
-
-def a2c_graph_unsupported(config, network, optimizer, states):
-    """``None`` when ``A2CAgent.step()`` runs as captured graphs under ``config.cuda_graph`` (GraphedQActor with
-    learner.GraphedA2CLearner.act per env step, GraphedA2CLearner per rollout), else the unmet condition; the agent then keeps
-    its eager path.  ``states``: the envs' current observations."""
-    from ..network import nature_tc
-    from ..network.network_bodies import NatureConvBody
-    from ..network.network_heads import CategoricalActorCriticNet
-    from ..utils import Config
-    from ..utils.normalizer import RescaleNormalizer
-    if not getattr(config, "cuda_graph", False):
-        return "config.cuda_graph is not set"
-    if getattr(config, "device_a2c", False):
-        return "config.device_a2c is set; it runs the agent on the device itself"
-    if type(network) is not CategoricalActorCriticNet:
-        return "the network is a %s; the captured update implements CategoricalActorCriticNet" % type(network).__name__
-    body = network.phi_body
-    if not isinstance(body, NatureConvBody):
-        return "the phi_body is a %s; the captured update implements NatureConvBody" % type(body).__name__
-    if not (isinstance(network.actor_body, DummyBody) and isinstance(network.critic_body, DummyBody)):
-        return ("the actor / critic bodies are %s / %s; the captured update implements DummyBody for both"
-                % (type(network.actor_body).__name__, type(network.critic_body).__name__))
-    if body.noisy_linear or config.noisy_linear:
-        return "the network has NoisyLinear layers; the captured update implements nn.Linear"
-    if body.conv1.in_channels != 4:
-        return "the NatureConvBody takes %d channels; the captured update reads stacks of 4 frames" % body.conv1.in_channels
-    if Config.COMPUTE_DTYPE != torch.bfloat16 or Config.DENSE_BACKEND != "tcgen05":
-        return ("the compute dtype is %s with the %r dense backend; the captured update runs bf16 on the wgmma kernels "
-                "(tcgen05)" % (Config.COMPUTE_DTYPE, Config.DENSE_BACKEND))
-    if not (nature_tc.FUSED_BWD and _lib.CONV_SLAB):
-        return "the fused backward epilogues are switched off; the captured update needs the fused update tail"
-    if network.fc_action.out_features >= 32:
-        return "%d actions; the actor-critic head and loss kernels take fewer than 32" % network.fc_action.out_features
-    if not isinstance(config.state_normalizer, RescaleNormalizer):
-        return "the state normalizer is %s; the captured update folds a RescaleNormalizer into conv1" % type(
-            config.state_normalizer).__name__
-    if not all(np.asarray(s).dtype == np.uint8 and np.asarray(s).shape == (4, 84, 84) for s in states):
-        return "the envs do not return uint8 4 x 84 x 84 frame stacks"
-    # what FlatOptimizer.from_torch turns into a kind the fused tail (NatureTail) takes
-    g = optimizer.param_groups[0]
-    if not ((isinstance(optimizer, torch.optim.RMSprop) and g["momentum"] == 0 and g["weight_decay"] == 0)
-            or (isinstance(optimizer, torch.optim.Adam) and g["weight_decay"] == 0 and not g["amsgrad"])):
-        return ("the optimizer is %s; the fused update tail implements RMSprop (centered or not) and Adam without momentum, "
-                "weight decay or amsgrad" % type(optimizer).__name__)
-    if not body.conv1.weight.is_cuda:
-        return "the network is not on a CUDA device (select_device(0))"
-    return None
-
-
-def ppo_graph_unsupported(config, network, optimizer, states):
-    """``None`` when ``PPOAgent.step()`` runs as captured graphs under ``config.cuda_graph`` (GraphedQActor with
-    learner.GraphedPPOPixelLearner.act per env step, GraphedPPOPixelLearner per rollout), else the unmet condition; the agent
-    then keeps its eager path.  The conditions of ``a2c_graph_unsupported`` (the same network, optimizer and frames), plus a
-    shared representation (one optimizer over the whole network) and rollouts of whole minibatches.  ``states``: the envs'
-    current raw observations."""
-    if not getattr(config, "cuda_graph", False):
-        return "config.cuda_graph is not set"
-    if not config.shared_repr:
-        return "config.shared_repr is not set; the captured update implements one optimizer over the shared network"
-    rows = config.rollout_length * config.num_workers
-    if rows < 2 or rows % config.mini_batch_size:
-        return ("the rollout's %d rows are not a multiple of mini_batch_size %d; random_sample would yield a short last "
-                "minibatch" % (rows, config.mini_batch_size))
-    return a2c_graph_unsupported(config, network, optimizer, states)
-
-
-def dqn_graph_unsupported(config, agent):
-    """``None`` when ``DQNAgent.step()`` (or the C51 / QR-DQN agent's) runs on the captured path with async replay under
-    ``config.cuda_graph``: the env transitions staged in learner.GraphedDQNLearner's pinned buffer and one update replay per
-    step (``prefetch`` = the graph form of ``ReplayWrapper(async_=True)``, ``wrapper_order``), the actor's forward a
-    GraphedQActor replay (on its own thread with ``async_actor``, ordered by ``ParameterOrder``).  Else the unmet condition;
-    the agent then keeps its eager path.  Reads ``agent.network``, ``agent.optimizer`` (the torch optimizer), ``agent.replay``
-    (the wrapper: its class and keyword arguments) and the agent's class."""
-    from ..network import nature_tc
-    from ..network.network_bodies import NatureConvBody
-    from ..network.network_heads import CategoricalNet, DuelingNet, QuantileNet, VanillaNet
-    from ..utils import Config
-    from ..utils.normalizer import RescaleNormalizer
-    from .replay import PrioritizedReplay, ReplayWrapper, UniformReplay
-    if not getattr(config, "cuda_graph", False):
-        return "config.cuda_graph is not set"
-    for flag in ("device_dqn", "device_c51", "device_qr", "device_rainbow"):
-        if getattr(config, flag, False):
-            return "config.%s is set; it runs the agent on the device itself" % flag
-    rp = agent.replay
-    if not isinstance(rp, ReplayWrapper) or not rp.async_:
-        return ("the replay is not ReplayWrapper(..., async_=True); the captured update with async replay implements its "
-                "double buffer")
-    if rp.replay_cls not in (UniformReplay, PrioritizedReplay):
-        return "the replay is a %s; the captured update implements UniformReplay and PrioritizedReplay" % rp.replay_cls.__name__
-    kind = agent._graph_kind
-    if kind == "qr" and rp.replay_cls is PrioritizedReplay:
-        return "QR-DQN with prioritized replay is undefined in the reference (its loss is per target quantile)"
-    net = agent.network
-    if type(net).__name__ == "RainbowNet" or config.noisy_linear:
-        return "the network is a RainbowNet or has NoisyLinear layers; the captured update implements nn.Linear heads"
-    want = {"dqn": (VanillaNet, DuelingNet), "c51": (CategoricalNet,), "qr": (QuantileNet,)}[kind]
-    if type(net) not in want:
-        return "the network is a %s; the captured update implements %s for %s" % (
-            type(net).__name__, " / ".join(c.__name__ for c in want), type(agent).__name__)
-    body = net.body
-    if not isinstance(body, NatureConvBody):
-        return "the body is a %s; the captured update implements NatureConvBody" % type(body).__name__
-    if body.noisy_linear:
-        return "the network has NoisyLinear layers; the captured update implements nn.Linear"
-    if Config.COMPUTE_DTYPE != torch.bfloat16 or Config.DENSE_BACKEND != "tcgen05":
-        return ("the compute dtype is %s with the %r dense backend; the captured update runs bf16 on the wgmma kernels "
-                "(tcgen05)" % (Config.COMPUTE_DTYPE, Config.DENSE_BACKEND))
-    if not (nature_tc.FUSED_BWD and _lib.CONV_SLAB):
-        return "the fused backward epilogues are switched off; the captured update needs the fused update tail"
-    if not isinstance(config.state_normalizer, RescaleNormalizer):
-        return "the state normalizer is %s; the captured update folds a RescaleNormalizer into conv1" % type(
-            config.state_normalizer).__name__
-    space = getattr(getattr(config, "eval_env", None), "observation_space", None)
-    shape = tuple(getattr(space, "shape", ()) or ())
-    dtype = np.dtype(getattr(space, "dtype", None) or np.float64)
-    hl = int(rp.replay_kwargs.get("history_length", 1))
-    if body.conv1.in_channels != 4 or hl != 4 or shape != (4, 84, 84) or dtype != np.uint8:
-        return ("the frames are %s %s with history_length %d into %d channels; the captured update reads 84 x 84 uint8 frames "
-                "with a history of 4" % (dtype, shape or "unknown", hl, body.conv1.in_channels))
-    if config.num_workers != 1:
-        return "%d envs per actor step; the staged feeds follow the reference's one-transition feed() calls" % config.num_workers
-    g = agent.optimizer.param_groups[0]
-    if not ((isinstance(agent.optimizer, torch.optim.RMSprop) and g["momentum"] == 0 and g["weight_decay"] == 0)
-            or (isinstance(agent.optimizer, torch.optim.Adam) and g["weight_decay"] == 0 and not g["amsgrad"])):
-        return ("the optimizer is %s; the fused update tail implements RMSprop (centered or not) and Adam without momentum, "
-                "weight decay or amsgrad" % type(agent.optimizer).__name__)
-    if agent._uses_reference_hooks():
-        return "%s overrides compute_loss / reduce_loss; the captured update runs the stock loss" % type(agent).__name__
-    if getattr(rp, "_primed", False):
-        return "the replay wrapper has already handed out an eager batch; its pending batch is not handed to the learner"
-    if not body.conv1.weight.is_cuda:
-        return "the network is not on a CUDA device (select_device(0))"
-    return None
-
-
 # ------------------------------------------------------------------------------------------------ A2C on the device
-def a2c_unsupported(network, optimizer, config):
-    """``None`` when ``config.device_a2c``'s kernels (csrc/a2c.cu) cover this agent, else the unmet condition."""
-    import torch.nn.functional as F
-
-    from ..network.network_heads import CategoricalActorCriticNet, GaussianActorCriticNet
-    from ..utils.normalizer import RescaleNormalizer
-    fc2 = lambda b: isinstance(b, FCBody) and len(b.layers) == 2 and not b.noisy_linear
-    if isinstance(network, CategoricalActorCriticNet):
-        if not (fc2(network.phi_body) and isinstance(network.actor_body, DummyBody)
-                and isinstance(network.critic_body, DummyBody)):
-            return ("a CategoricalActorCriticNet needs a two-layer FCBody phi_body and DummyBody actor / critic bodies "
-                    "(got %s / %s / %s)" % tuple(type(b).__name__ for b in (network.phi_body, network.actor_body,
-                                                                              network.critic_body)))
-        trunks = [network.phi_body]
-    elif isinstance(network, GaussianActorCriticNet):
-        if not (isinstance(network.phi_body, DummyBody) and fc2(network.actor_body) and fc2(network.critic_body)):
-            return ("a GaussianActorCriticNet needs a DummyBody phi_body and two-layer FCBody actor / critic bodies "
-                    "(got %s / %s / %s)" % tuple(type(b).__name__ for b in (network.phi_body, network.actor_body,
-                                                                              network.critic_body)))
-        trunks = [network.actor_body, network.critic_body]
-    else:
-        return "the network is a %s, not a CategoricalActorCriticNet or GaussianActorCriticNet" % type(network).__name__
-    widths = [(b.layers[0].in_features, b.layers[0].out_features, b.layers[1].out_features) for b in trunks]
-    if len(set(widths)) != 1 or len(set(id(b.gate) for b in trunks)) != 1:
-        return "the actor and critic bodies must have the same widths and gate"
-    D, H1, H2 = widths[0]
-    A = network.fc_action.out_features
-    if trunks[0].gate not in (torch.tanh, F.relu):
-        return "the FCBody gate must be torch.tanh or F.relu"
-    if not network.fc_action.weight.is_cuda:
-        return "the network is not on a CUDA device (select_device(0))"
-    if D > 256 or H1 > 128 or H2 > 128 or A > 32:
-        return "sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, actions %d <= 32" % (D, H1, H2, A)
-    if not isinstance(optimizer, torch.optim.RMSprop):
-        return "the optimizer is %s; the device update implements RMSprop" % type(optimizer).__name__
-    if type(config.state_normalizer) is not RescaleNormalizer:
-        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
-    head = 0 if isinstance(network, CategoricalActorCriticNet) else 1
-    smem = _lib.lib().b2rl_a2c_smem_bytes(head, int(head == 0), D, H1, H2, A, config.num_workers, config.rollout_length)
-    if not 0 < smem <= 227 * 1024:
-        return ("a rollout of %d x %d rows needs %d bytes of shared memory, more than one SM has (b2rl_a2c_smem_bytes)"
-                % (config.rollout_length + 1, config.num_workers, smem))
-    return None
-
-
 class _DeviceRollout:
-    """What ``DeviceA2C`` and ``DeviceNStepDQN`` share: the rollout arenas, the pinned double-buffered float64 observation
-    upload, rewards / masks (uploaded once per rollout), the action download, the parity-mode actions, the Philox counter and
-    the check that the parameters still live in the optimizer's arena.  The subclass sets ``opt``, ``dev``, ``tensors`` (kernel
-    order), ``cfg``, ``N``, ``T``, ``D`` and ``acols`` first."""
+    """What ``DeviceA2C``, ``DeviceNStepDQN`` and ``DeviceDQN`` share: the rollout arenas, the pinned double-buffered float64
+    observation upload, rewards / masks (uploaded once per rollout), the action download, the parity-mode actions, the Philox
+    counter, the check that the parameters still live in the optimizer's arena and, for the Q agents, the target arena.  The
+    subclass sets ``opt``, ``dev``, ``tensors`` (kernel order), ``cfg``, ``N``, ``T``, ``D`` and ``acols`` first."""
+
+    def _adopt_target(self, target_network):
+        """The target network's parameters become views into ``target``, a second arena of the online arena's layout (their
+        values kept), so the target sync is one device copy and the module's ``state_dict()`` is always current."""
+        self.target = torch.zeros_like(self.opt.flat)
+        with torch.no_grad():
+            for p, o in zip(target_network.parameters(), self.opt.offsets):
+                k = p.numel()
+                self.target[o:o + k].copy_(p.detach().reshape(-1))
+                p.data = self.target[o:o + k].view_as(p)
+
+    def _check_target(self, tensors, owner):
+        """``tensors``: the target network's parameters in kernel order, each at its online twin's offset in ``target``."""
+        base = self.target.data_ptr()
+        for t, o in zip(tensors, self.off.tolist()):
+            if t.data_ptr() != base + 4 * o:
+                raise _lib.B2RLError("%s: a target parameter no longer lives in the target arena" % owner)
 
     def _buffers(self, seed):
         N, T, D, acols = self.N, self.T, self.D, self.acols
@@ -667,40 +447,6 @@ class DeviceA2C(_DeviceRollout):
 
 
 # ------------------------------------------------------------------------------------------------ n-step Q on the device
-def nstep_dqn_unsupported(network, optimizer, config):
-    """``None`` when ``config.device_nstep_dqn``'s kernels (csrc/a2c.cu, b2rl_nstep_dqn_*) cover this agent, else the unmet
-    condition."""
-    import torch.nn.functional as F
-
-    from ..network.network_heads import VanillaNet
-    from ..utils.normalizer import RescaleNormalizer
-    if not isinstance(network, VanillaNet):
-        return "the network is a %s, not a VanillaNet" % type(network).__name__
-    body = network.body
-    if not isinstance(body, FCBody):
-        return "a VanillaNet needs an FCBody body (got %s)" % type(body).__name__
-    if body.noisy_linear:
-        return "the FCBody has NoisyLinear layers; the device kernels implement nn.Linear"
-    if len(body.layers) != 2:
-        return "the device kernels implement a two-layer FCBody (got %d layers)" % len(body.layers)
-    if body.gate not in (torch.tanh, F.relu):
-        return "the FCBody gate must be torch.tanh or F.relu"
-    if not network.fc_head.weight.is_cuda:
-        return "the network is not on a CUDA device (select_device(0))"
-    D, H1, H2, A = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features, network.fc_head.out_features
-    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32:
-        return "sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32" % (D, H1, H2, A)
-    if not isinstance(optimizer, torch.optim.RMSprop):
-        return "the optimizer is %s; the device update implements RMSprop" % type(optimizer).__name__
-    if type(config.state_normalizer) is not RescaleNormalizer:
-        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
-    smem = _lib.lib().b2rl_nstep_dqn_smem_bytes(D, H1, H2, A, config.num_workers, config.rollout_length)
-    if not 0 < smem <= 227 * 1024:
-        return ("a rollout of %d x %d rows needs %d bytes of shared memory, more than one SM has (b2rl_nstep_dqn_smem_bytes)"
-                % (config.rollout_length + 1, config.num_workers, smem))
-    return None
-
-
 class DeviceNStepDQN(_DeviceRollout):
     """``NStepDQNAgent.step()`` on the device (``config.device_nstep_dqn``): one ``b2rl_nstep_dqn_actor_step`` launch per env
     step (epsilon-greedy on the device's Philox stream) and one ``b2rl_nstep_dqn_update`` launch per rollout, which also does the
@@ -722,12 +468,7 @@ class DeviceNStepDQN(_DeviceRollout):
         self.tensors = self.kernel_order(network)
         self.opt = ops.FlatOptimizer.from_torch(optimizer, list(network.parameters()))
         self.dev = self.opt.flat.device
-        self.target = torch.zeros_like(self.opt.flat)
-        with torch.no_grad():
-            for p, o in zip(target_network.parameters(), self.opt.offsets):
-                k = p.numel()
-                self.target[o:o + k].copy_(p.detach().reshape(-1))
-                p.data = self.target[o:o + k].view_as(p)
+        self._adopt_target(target_network)
         self.N, self.T = int(config.num_workers), int(config.rollout_length)
         self.D, self.H1, self.H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
         self.A = network.fc_head.out_features
@@ -741,10 +482,7 @@ class DeviceNStepDQN(_DeviceRollout):
 
     def begin_rollout(self):
         self._arena_offsets()
-        base = self.target.data_ptr()
-        for t, o in zip(self.kernel_order(self.target_net), self.off.tolist()):
-            if t.data_ptr() != base + 4 * o:
-                raise _lib.B2RLError("DeviceNStepDQN: a target parameter no longer lives in the target arena")
+        self._check_target(self.kernel_order(self.target_net), "DeviceNStepDQN")
         self._dims = (self.D, self.H1, self.H2, self.A)
 
     def act(self, t, raw_obs, epsilon):
@@ -781,63 +519,6 @@ def dqn_kernel_order(net):
     return body + [head.weight, head.bias]
 
 
-def _fc_body_unsupported(network, config):
-    """The body checks of ``dqn_unsupported`` and ``dist_dqn_unsupported``: a two-layer, non-noisy FCBody with tanh or ReLU on
-    a CUDA device."""
-    import torch.nn.functional as F
-
-    from ..network.network_bodies import NatureConvBody
-    body = network.body
-    if isinstance(body, NatureConvBody):
-        return "the body is a NatureConvBody; the device kernels implement a two-layer FCBody"
-    if not isinstance(body, FCBody):
-        return "the network needs an FCBody body (got %s)" % type(body).__name__
-    if body.noisy_linear or config.noisy_linear:
-        return "the network has NoisyLinear layers; the device kernels implement nn.Linear"
-    if len(body.layers) != 2:
-        return "the device kernels implement a two-layer FCBody (got %d layers)" % len(body.layers)
-    if body.gate not in (torch.tanh, F.relu):
-        return "the FCBody gate must be torch.tanh or F.relu"
-    if not body.layers[0].weight.is_cuda:
-        return "the network is not on a CUDA device (select_device(0))"
-    return None
-
-
-def dqn_unsupported(agent):
-    """``None`` when ``config.device_dqn``'s kernels (csrc/a2c.cu: b2rl_nstep_dqn_actor_step, b2rl_dqn_replay_update) cover
-    this ``DQNAgent``, else the unmet condition."""
-    from ..network.network_heads import DuelingNet, VanillaNet
-    from ..utils.normalizer import RescaleNormalizer
-    config, network = agent.config, agent.network
-    if type(network) not in (VanillaNet, DuelingNet):
-        return ("the network is a %s; the device kernels implement VanillaNet and DuelingNet (C51, QR and Rainbow heads are "
-                "not covered)" % type(network).__name__)
-    if agent._uses_reference_hooks():
-        return "%s overrides compute_loss / reduce_loss; the device update implements DQNAgent's" % type(agent).__name__
-    why = _fc_body_unsupported(network, config)
-    if why is not None:
-        return why
-    body = network.body
-    head = network.fc_advantage if isinstance(network, DuelingNet) else network.fc_head
-    D, H1, H2, A = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features, head.out_features
-    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32:
-        return "sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32" % (D, H1, H2, A)
-    if not isinstance(agent.optimizer, torch.optim.RMSprop) or agent._flat is None:
-        return "the optimizer is %s; the device update implements RMSprop" % type(agent.optimizer).__name__
-    if type(config.state_normalizer) is not RescaleNormalizer:
-        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
-    if config.async_actor:
-        return "async_actor is set; the device actor runs in the agent's thread (async_actor=False)"
-    if config.history_length != 1:
-        return "history_length is %d; the device kernels read single 1-D states, not frame stacks" % config.history_length
-    smem = _lib.lib().b2rl_dqn_replay_smem_bytes(int(isinstance(network, DuelingNet)), D, H1, H2, A, int(config.batch_size),
-                                                 int(bool(config.double_q)))
-    if not 0 < smem <= 227 * 1024:
-        return ("a batch of %d needs %d bytes of shared memory, more than one SM has (b2rl_dqn_replay_smem_bytes)"
-                % (config.batch_size, smem))
-    return None
-
-
 class DeviceDQN(_DeviceRollout):
     """``DQNAgent.step()`` on the device (``config.device_dqn``): one ``b2rl_nstep_dqn_actor_step`` launch per env step
     (rescale, forward, epsilon-greedy on the device's Philox stream) and one ``b2rl_dqn_replay_update`` launch per gradient
@@ -850,9 +531,7 @@ class DeviceDQN(_DeviceRollout):
 
     flag = "config.device_dqn"
 
-    @staticmethod
-    def unsupported(agent):
-        return dqn_unsupported(agent)
+    unsupported = staticmethod(dqn_unsupported)
 
     def __init__(self, agent, seed):
         from ..network.network_heads import DuelingNet
@@ -867,12 +546,7 @@ class DeviceDQN(_DeviceRollout):
         self.tensors = self._tensors(network)
         self.opt = agent._flat
         self.dev = self.opt.flat.device
-        self.target = torch.zeros_like(self.opt.flat)
-        with torch.no_grad():
-            for p, o in zip(agent.target_network.parameters(), self.opt.offsets):
-                k = p.numel()
-                self.target[o:o + k].copy_(p.detach().reshape(-1))
-                p.data = self.target[o:o + k].view_as(p)
+        self._adopt_target(agent.target_network)
         self.N, self.T = int(config.num_workers), 1
         self.D, self.H1, self.H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
         self.A = self.tensors[4].shape[0]
@@ -888,10 +562,7 @@ class DeviceDQN(_DeviceRollout):
     def _offsets(self):
         """``_arena_offsets``, and the check that the target parameters still live in the target arena."""
         self._arena_offsets()
-        base = self.target.data_ptr()
-        for t, o in zip(self._tensors(self.target_net), self.off.tolist()):
-            if t.data_ptr() != base + 4 * o:
-                raise _lib.B2RLError("DeviceDQN: a target parameter no longer lives in the target arena")
+        self._check_target(self._tensors(self.target_net), "DeviceDQN")
 
     def act(self, raw_obs, epsilon):
         """One env step's actions: rescale + forward + epsilon-greedy in one launch, downloaded for ``task.step``."""
@@ -931,51 +602,6 @@ class DeviceDQN(_DeviceRollout):
 
 
 # ------------------------------------------------------------------------------------------------ C51 / QR-DQN on the device
-def dist_dqn_unsupported(agent):
-    """``None`` when ``config.device_c51`` / ``config.device_qr``'s kernels (csrc/dist_dqn.cu: b2rl_dist_dqn_actor_step,
-    b2rl_dist_dqn_replay_update) cover this ``CategoricalDQNAgent`` / ``QuantileRegressionDQNAgent``, else the unmet
-    condition."""
-    from ..agent.CategoricalDQN_agent import CategoricalDQNAgent
-    from ..component.replay import PrioritizedReplay
-    from ..network.network_heads import CategoricalNet, QuantileNet, RainbowNet
-    from ..utils.normalizer import RescaleNormalizer
-    config, network = agent.config, agent.network
-    c51 = isinstance(agent, CategoricalDQNAgent)
-    want = CategoricalNet if c51 else QuantileNet
-    if isinstance(network, RainbowNet):
-        return "the network is a RainbowNet; the device kernels implement CategoricalNet (RainbowNet / NoisyLinear is not covered)"
-    if type(network) is not want:
-        return "the network is a %s; the device kernels implement %s" % (type(network).__name__, want.__name__)
-    if agent._uses_reference_hooks():
-        return "%s overrides compute_loss / reduce_loss; the device update implements %s's" % (
-            type(agent).__name__, agent._fused_owner().__name__)
-    why = _fc_body_unsupported(network, config)
-    if why is not None:
-        return why
-    body = network.body
-    D, H1, H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
-    A, K = network.action_dim, network.num_atoms if c51 else network.num_quantiles
-    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32 or not 2 <= K <= 256:
-        return ("sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32, "
-                "2 <= %s %d <= 256" % (D, H1, H2, A, "atoms" if c51 else "quantiles", K))
-    if not isinstance(agent.optimizer, torch.optim.RMSprop) or agent._flat is None:
-        return "the optimizer is %s; the device update implements RMSprop" % type(agent.optimizer).__name__
-    if type(config.state_normalizer) is not RescaleNormalizer:
-        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
-    if config.history_length not in (None, 1):
-        return "history_length is %d; the device kernels read single 1-D states, not frame stacks" % config.history_length
-    replay_cls = getattr(agent.replay, "replay_cls", type(agent.replay))
-    if not c51 and issubclass(replay_cls, PrioritizedReplay):
-        return ("QR-DQN with prioritized replay is undefined in the reference: its loss is per target quantile, not per sample "
-                "(QuantileRegressionDQN_agent.py:74)")
-    smem = _lib.lib().b2rl_dist_dqn_smem_bytes(int(not c51), D, H1, H2, A, K, int(config.batch_size),
-                                               int(bool(config.double_q)))
-    if not 0 < smem <= 227 * 1024:
-        return ("a batch of %d needs %d bytes of shared memory, more than one SM has (b2rl_dist_dqn_smem_bytes)"
-                % (config.batch_size, smem))
-    return None
-
-
 class DeviceDistDQN(DeviceDQN):
     """``CategoricalDQNAgent.step()`` / ``QuantileRegressionDQNAgent.step()`` on the device (``config.device_c51`` /
     ``config.device_qr``): one ``b2rl_dist_dqn_actor_step`` launch per env step (rescale, forward, the action values,
@@ -991,9 +617,7 @@ class DeviceDistDQN(DeviceDQN):
     def flag(self):
         return "config.device_c51" if self.kind == 0 else "config.device_qr"
 
-    @staticmethod
-    def unsupported(agent):
-        return dist_dqn_unsupported(agent)
+    unsupported = staticmethod(dist_dqn_unsupported)
 
     def __init__(self, agent, seed):
         from ..agent.CategoricalDQN_agent import CategoricalDQNAgent
@@ -1058,56 +682,6 @@ def rainbow_kernel_order(net):
     return [getattr(m, k) for m in rainbow_layers(net) for k in names]
 
 
-def rainbow_unsupported(agent):
-    """``None`` when ``config.device_rainbow``'s kernels (csrc/rainbow.cu: b2rl_rainbow_actor_step, b2rl_rainbow_replay_update)
-    cover this agent, else the unmet condition."""
-    import torch.nn.functional as F
-
-    from ..agent.CategoricalDQN_agent import CategoricalDQNAgent
-    from ..network.network_bodies import NatureConvBody
-    from ..network.network_heads import RainbowNet
-    from ..network.network_utils import NoisyLinear
-    from ..utils.normalizer import RescaleNormalizer
-    config, network = agent.config, agent.network
-    if not isinstance(agent, CategoricalDQNAgent):
-        return "the agent is a %s; Rainbow is a CategoricalDQNAgent on a RainbowNet" % type(agent).__name__
-    if type(network) is not RainbowNet:
-        return "the network is a %s; the device kernels implement RainbowNet" % type(network).__name__
-    if agent._uses_reference_hooks():
-        return "%s overrides compute_loss / reduce_loss; the device update implements CategoricalDQNAgent's" % type(agent).__name__
-    body = network.body
-    if isinstance(body, NatureConvBody):
-        return "the body is a NatureConvBody; the device kernels implement a two-layer FCBody"
-    if not isinstance(body, FCBody):
-        return "the network needs an FCBody body (got %s)" % type(body).__name__
-    if len(body.layers) != 2:
-        return "the device kernels implement a two-layer FCBody (got %d layers)" % len(body.layers)
-    noisy = [isinstance(m, NoisyLinear) for m in rainbow_layers(network)]
-    if len(set(noisy + [bool(network.noisy_linear), bool(body.noisy_linear), bool(config.noisy_linear)])) != 1:
-        return ("the body, the head and config.noisy_linear disagree: the device kernels implement all four layers NoisyLinear "
-                "or all four nn.Linear, not a mix")
-    if body.gate not in (torch.tanh, F.relu):
-        return "the FCBody gate must be torch.tanh or F.relu"
-    if not next(network.parameters()).is_cuda:
-        return "the network is not on a CUDA device (select_device(0))"
-    D, H1, H2 = body.layers[0].in_features, body.layers[0].out_features, body.layers[1].out_features
-    A, K = network.action_dim, network.num_atoms
-    if D > 256 or H1 > 128 or H2 > 128 or not 2 <= A <= 32 or not 2 <= K <= 256:
-        return ("sizes beyond the kernels' limits: state_dim %d <= 256, hidden %d / %d <= 128, 2 <= actions %d <= 32, "
-                "2 <= atoms %d <= 256" % (D, H1, H2, A, K))
-    if not isinstance(agent.optimizer, torch.optim.RMSprop) or agent._flat is None:
-        return "the optimizer is %s; the device update implements RMSprop" % type(agent.optimizer).__name__
-    if type(config.state_normalizer) is not RescaleNormalizer:
-        return "the state normalizer is %s; the device actor applies RescaleNormalizer" % type(config.state_normalizer).__name__
-    if config.history_length not in (None, 1):
-        return "history_length is %d; the device kernels read single 1-D states, not frame stacks" % config.history_length
-    smem = _lib.lib().b2rl_rainbow_smem_bytes(int(noisy[0]), D, H1, H2, A, K, int(config.batch_size), int(bool(config.double_q)))
-    if not 0 < smem <= 227 * 1024:
-        return ("a batch of %d needs %d bytes of shared memory, more than one SM has (b2rl_rainbow_smem_bytes)"
-                % (config.batch_size, smem))
-    return None
-
-
 class DeviceRainbow(DeviceDistDQN):
     """``CategoricalDQNAgent.step()`` for a RainbowNet on the device (``config.device_rainbow``): one ``b2rl_rainbow_actor_step``
     launch per env step and one ``b2rl_rainbow_replay_update`` launch per gradient update (csrc/rainbow.cu).  The arenas, the
@@ -1127,9 +701,7 @@ class DeviceRainbow(DeviceDistDQN):
 
     flag = "config.device_rainbow"
 
-    @staticmethod
-    def unsupported(agent):
-        return rainbow_unsupported(agent)
+    unsupported = staticmethod(rainbow_unsupported)
 
     def __init__(self, agent, seed):
         from ..utils import Config

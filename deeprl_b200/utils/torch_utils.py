@@ -37,6 +37,11 @@ def random_seed(seed=None):
     torch.manual_seed(np.random.randint(int(1e6)))
 
 
+def philox_seed():
+    """The key of a device Philox stream, drawn from torch's (seeded) generator: one draw per call."""
+    return int(torch.randint(0, 2 ** 62, (1,)).item())
+
+
 def set_one_thread():
     os.environ["OMP_NUM_THREADS"] = "1"
     os.environ["MKL_NUM_THREADS"] = "1"

@@ -196,7 +196,7 @@ def _refusals(rl):
 
 
 def _predicate(rl, cfg, net):
-    from deeprl_b200.component.actor import a2c_graph_unsupported
+    from deeprl_b200.component.coverage import a2c_graph_unsupported
     opt = cfg.optimizer_fn(net.parameters())
     states = cfg.task_fn().reset()
     return a2c_graph_unsupported(cfg, net, opt, states)

@@ -80,7 +80,7 @@ def _stub_agent(cls, config, network=None, optimizer_fn=None):
 
 
 def _predicate(cls, config, **kw):
-    from deeprl_b200.component.actor import dqn_graph_unsupported
+    from deeprl_b200.component.coverage import dqn_graph_unsupported
     return dqn_graph_unsupported(config, _stub_agent(cls, config, **kw))
 
 
@@ -160,7 +160,7 @@ def test_every_refusal_names_its_condition(host_bf16):
     assert "overrides compute_loss / reduce_loss" in _predicate(Hooked, cfg)
     ag = _stub_agent(cls, cfg)
     ag.replay._primed = True
-    from deeprl_b200.component.actor import dqn_graph_unsupported
+    from deeprl_b200.component.coverage import dqn_graph_unsupported
     assert "already handed out an eager batch" in dqn_graph_unsupported(cfg, ag)
     qcls, qcfg = _launch("quantile_regression_dqn_pixel")
     examples._replay(qcfg, examples.PrioritizedReplay, True, memory_size=100, history_length=4)

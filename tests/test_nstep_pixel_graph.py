@@ -176,7 +176,7 @@ def _refusals(rl):
 
 
 def _predicate(rl, cfg, net, opt_fn=None):
-    from deeprl_b200.component.actor import nstep_q_graph_unsupported
+    from deeprl_b200.component.coverage import nstep_q_graph_unsupported
     opt = (opt_fn or cfg.optimizer_fn)(net.parameters())
     states = cfg.task_fn().reset()
     return nstep_q_graph_unsupported(cfg, net, opt, states)

@@ -292,7 +292,7 @@ def _refusals(rl):
 
 
 def _predicate(rl, cfg, net):
-    from deeprl_b200.component.actor import ppo_graph_unsupported
+    from deeprl_b200.component.coverage import ppo_graph_unsupported
     opt = cfg.optimizer_fn(net.parameters())
     states = cfg.task_fn().reset()
     return ppo_graph_unsupported(cfg, net, opt, states)
