@@ -1563,6 +1563,153 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv1_
   if (clk && threadIdx.x == 0) atomicAdd(clk + K1_CLK_CTA, (unsigned long long)(clock64() - t_start));
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// conv2's and conv3's weight gradients with every tap of a k-block in one CTA.  n_out = 64 output channels, C input channels
+// and TAPS_X x TAPS_X taps on the G x G grid, tap t = (dy, dx) at row shift s_t = dy G + dx: conv3 C 64, 3 x 3 taps; conv2
+// C 128 (its space-to-depth(2) input), 2 x 2 taps.  As in conv1's kernel the gradient rows carry the shift:
+//   dW[n][t*C + c] = sum_r' G[r' - s_t][n] x[r'][c]
+// Per 128-row k-block the producer loads ONE gradient box, rows [k0 - halo, k0 + BK) with halo = s_max = (TAPS_X - 1)(G + 1),
+// 64 channels = one 128-byte row each, 128B-swizzled MN-major, and ONE activation block, rows [k0, k0 + BK) of C channels
+// (C / 64 boxes of [128 rows][64 c], no halo).  Every tap's MMAs read these two: the A descriptor of tap t starts halo - s_t
+// rows into the gradient box (a 128-byte step; the swizzle is a function of the address, as in the slab kernels), B is the
+// activation block for all taps.  Tap t has its own m64 x C accumulator (output channels x input channels), so each
+// accumulator row is a result; MMA warpgroup g holds taps g*TPW .. g*TPW + TPW - 1: conv3 3 warpgroups x 3 taps of m64n64
+// (96 registers), conv2 2 x 2 taps of m64n128 (128 registers).  Loads per k-block: (BK + halo) * 128 + BK * 2C bytes for
+// 2 * BK * 64 * taps * C FLOP -- every operand once, against one fetch per 128-column tap group of conv_wgrad_wgmma_kernel.
+// A CTA takes a contiguous range of k-blocks (equal ranges, at most one CTA per SM or per CTA of the budget) and stores its
+// [64][taps * C] fp32 partial block at D + blockIdx.x * 64 * taps * C; the consumer sums the partials (deterministic).
+// Each k-block is one commit group per warpgroup, retired (its stage released) after the next one has been issued.
+// Phase probe slots: K1_CLK_CTA, K1_CLK_PRODUCER_WAIT (waits for a free stage), K1_CLK_MMA_WAIT (MMA warpgroups' waits for a
+// full stage, summed over them), K1_CLK_MMA (their issue, retire-one wait and release), K1_CLK_TILES (k-blocks).
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int CTW_BK = 128;                           // rows of one k-block
+struct TapsWgradParams {
+  int rows, grid_w;             // batch * G * G rows of the G x G grid; G
+  int blocks, blocks_per_cta;   // 128-row k-blocks in all / per CTA
+  int stages;                   // operand stages (gradient box + activation block)
+  float* D;                     // partials: CTA i at D + i * 64 * taps * C
+  unsigned long long* clk;      // profiling hook (normally null), K1_CLK_* slots
+};
+// bytes of one gradient box: rows [k0 - halo, k0 + BK) of 128 bytes, padded to the 1024-byte alignment of the stage ring
+__host__ __device__ inline uint32_t ctw_g_bytes(int halo) { return ((uint32_t)(CTW_BK + halo) * 128 + 1023) & ~1023u; }
+template <int WGS> __host__ __device__ constexpr int ctw_threads() { return 128 * (WGS + 1); }
+
+template <int C, int TAPS_X, int WGS>
+__global__ void __launch_bounds__(ctw_threads<WGS>(), 1) conv_taps_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmG,
+                                                                                     const __grid_constant__ CUtensorMap tmX,
+                                                                                     const TapsWgradParams w) {
+  constexpr int MAX_STAGES = 6, TAPS = TAPS_X * TAPS_X, TPW = TAPS / WGS, CB = C / 64;
+  constexpr uint32_t X_BOX = CTW_BK * 128, X_BYTES = X_BOX * CB;
+  static_assert(TPW * WGS == TAPS && (C == 64 || C == 128), "taps split evenly over the MMA warpgroups; C 64 or 128");
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int halo = (TAPS_X - 1) * (w.grid_w + 1);
+  const uint32_t g_bytes = ctw_g_bytes(halo), stage_bytes = g_bytes + X_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)w.stages * stage_bytes);
+  uint64_t* empty = full + MAX_STAGES;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
+  const int blk0 = (int)blockIdx.x * w.blocks_per_cta;
+  const int n_blk = max(min(w.blocks, blk0 + w.blocks_per_cta) - blk0, 0);
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], 4 * WGS); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
+  }
+  __syncthreads();
+  pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
+  unsigned long long* const clk = w.clk;
+  const long long t_start = clk_now(clk);
+  long long c_wait = 0, c_work = 0;                              // per-role sums of the probe (one thread per role)
+  // register split (setmaxnreg): the producer warpgroup gives its share to the MMA warpgroups (conv3: 96 accumulator
+  // registers of 128 per thread at 512 threads)
+  constexpr int launch_regs = 65536 / ctw_threads<WGS>() / 8 * 8, producer_regs = 40;
+  constexpr int mma_regs = ((WGS + 1) * launch_regs - producer_regs) / WGS / 8 * 8;
+
+  if (warp < 4) {
+    reg_dec<producer_regs>();
+    if (warp == 0 && elect_one()) {
+    // ------------------------------------------------------------------------ producer: per k-block the gradient box and the
+    // activation block
+    for (int i = 0; i < n_blk; ++i) {
+      const int s = i % w.stages, k0 = (blk0 + i) * CTW_BK;
+      uint8_t* st = smem + (size_t)s * stage_bytes;
+      const long long t0 = clk_now(clk);
+      mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
+      c_wait += clk_now(clk) - t0;
+      mb_expect_tx(&full[s], (uint32_t)(CTW_BK + halo) * 128 + X_BYTES);
+      tma_load_2d(st, &tmG, &full[s], 0, k0 - halo);                                     // [BK + halo rows][64 n]
+#pragma unroll
+      for (int cb = 0; cb < CB; ++cb) tma_load_2d(st + g_bytes + cb * X_BOX, &tmX, &full[s], cb * 64, k0);   // [BK][64 c]
+    }
+    if (clk) atomicAdd(clk + K1_CLK_PRODUCER_WAIT, (unsigned long long)c_wait);
+    }
+  } else {
+    reg_inc<mma_regs>();
+    if (n_blk > 0) {
+    // ------------------------------------------------------------------------ MMA, warpgroup g: taps g*TPW + j
+    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
+    uint32_t a0[TPW];
+#pragma unroll
+    for (int j = 0; j < TPW; ++j) {
+      const int t = g * TPW + j;
+      a0[j] = s2u(smem) + (uint32_t)(halo - (t / TAPS_X) * w.grid_w - t % TAPS_X) * 128;
+    }
+    const uint32_t b0 = s2u(smem) + g_bytes;
+    float d[TPW][C / 2];
+#pragma unroll
+    for (int j = 0; j < TPW; ++j) acc_zero<C>(d[j]);
+    for (int i = 0; i < n_blk; ++i) {
+      const int s = i % w.stages;
+      const long long t0 = clk_now(clk);
+      mb_wait(&full[s], (i / w.stages) & 1);
+      const long long t1 = clk_now(clk);
+      const uint32_t st = (uint32_t)s * stage_bytes;
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < CTW_BK / 16; ++k) {                       // k16 step: 16 rows = 2048 bytes of every operand
+        const uint64_t b = make_desc(b0 + st + k * 2048, X_BOX);     // C 128: the second 64-channel box X_BOX bytes on
+#pragma unroll
+        for (int j = 0; j < TPW; ++j) {
+          const uint64_t a = make_desc(a0[j] + st + k * 2048, 8192);
+          if constexpr (C == 64) wgmma_n64<1, 1>(d[j], a, b);
+          else wgmma_n128<1, 1>(d[j], a, b);
+        }
+      }
+      wg_commit();
+      wg_wait1();                                                    // k-block i - 1 has retired: release its stage
+      if (i > 0 && lane == 0) mb_arrive(&empty[(i - 1) % w.stages]);
+      c_wait += t1 - t0, c_work += clk_now(clk) - t1;
+    }
+    wg_wait0();
+#pragma unroll
+    for (int j = 0; j < TPW; ++j) acc_fence<C>(d[j]);
+    if (lane == 0) mb_arrive(&empty[(n_blk - 1) % w.stages]);
+    // accumulator element d[j][4 jj + 2 h + e]: output channel 16 wl + lane / 4 + 8 h, input channel 8 jj + 2 (lane % 4) + e
+    float* base = w.D + (int64_t)blockIdx.x * (64 * TAPS * C) + 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int n = 16 * wl + (lane >> 2) + 8 * h;
+#pragma unroll
+      for (int j = 0; j < TPW; ++j) {
+        float* dst = base + n * (TAPS * C) + (g * TPW + j) * C;
+#pragma unroll
+        for (int jj = 0; jj < C / 8; ++jj)
+          *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(d[j][4 * jj + 2 * h], d[j][4 * jj + 2 * h + 1]);
+      }
+    }
+    if (clk && (threadIdx.x & 127) == 0) {
+      atomicAdd(clk + K1_CLK_MMA_WAIT, (unsigned long long)c_wait);
+      atomicAdd(clk + K1_CLK_MMA, (unsigned long long)c_work);
+      if (g == 0) atomicAdd(clk + K1_CLK_TILES, (unsigned long long)n_blk);
+    }
+    }
+  }
+  __syncthreads();
+  if (clk && threadIdx.x == 0) atomicAdd(clk + K1_CLK_CTA, (unsigned long long)(clock64() - t_start));
+}
+
 // ------------------------------------------------------------------------------------------------- host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -2006,6 +2153,34 @@ static int launch_conv1_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, Conv
   *n_ctas = (w.blocks + w.blocks_per_cta - 1) / w.blocks_per_cta;
   launch_pdl(k, dim3(*n_ctas), dim3(U8 ? SLAB_U8_THREADS : GEMM_THREADS), smem, st, tg, tx, w);
   return check_launch("conv1 weight gradient");
+}
+
+// conv_taps_wgrad_wgmma_kernel: the 128-row k-blocks in equal contiguous ranges over at most grid_cap() CTAs; returns the
+// CTA count (= partial blocks written) through n_ctas, or 1 when the operand ring does not fit in shared memory
+template <int C, int TAPS_X, int WGS>
+static int launch_taps_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, TapsWgradParams w, cudaStream_t st, int* n_ctas) {
+  auto k = conv_taps_wgrad_wgmma_kernel<C, TAPS_X, WGS>;
+  static const size_t limit = dyn_smem_limit(k);
+  const size_t stage = ctw_g_bytes((TAPS_X - 1) * (w.grid_w + 1)) + (size_t)CTW_BK * 2 * C;
+  const size_t fixed = 1024 + 2 * 6 * 8;                             // alignment of the ring + its barriers
+  if (limit <= fixed) return 1;
+  int stages = (int)((limit - fixed) / stage);
+  if (stages > 6) stages = 6;
+  if (stages < 2) return 1;
+  w.stages = stages;
+  const size_t smem = fixed + stages * stage;
+  static size_t attr = 0;
+  if (attr < smem) {
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    attr = smem;
+  }
+  w.blocks = (w.rows + CTW_BK - 1) / CTW_BK;
+  const int ctas = w.blocks < grid_cap() ? w.blocks : grid_cap();
+  w.blocks_per_cta = (w.blocks + ctas - 1) / ctas;
+  *n_ctas = (w.blocks + w.blocks_per_cta - 1) / w.blocks_per_cta;
+  g_last_ctas = *n_ctas;
+  launch_pdl(k, dim3(*n_ctas), dim3(ctw_threads<WGS>()), smem, st, tg, tx, w);
+  return check_launch("conv2 / conv3 weight gradient");
 }
 
 }  // namespace b2rl
@@ -2489,6 +2664,34 @@ extern "C" int b2rl_conv1_wgrad_partials(const uint16_t* X, int64_t rows, int32_
   int n = 0;
   const int r2 = launch_conv1_wgrad<false>(tg, tx, w, (cudaStream_t)stream, &n);
   if (r2 > 0) { set_error("b2rl_conv1_wgrad_partials: the operand ring does not fit in shared memory"); return B2RL_ERR_ARG; }
+  *n_partials_host = n;
+  return r2;
+}
+
+// conv2's and conv3's weight-gradient partials, every tap of a k-block in one CTA (conv_taps_wgrad_wgmma_kernel): the
+// arguments and the output layout of b2rl_conv_wgrad_partials, one partial per CTA (at most one per SM, or the CTA budget).
+extern "C" int b2rl_conv_taps_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out,
+                                             int32_t taps, int32_t taps_x, int32_t grid_w, float* partials,
+                                             int32_t* n_partials_host, void* stream) {
+  B2RL_REQUIRE(X && G && partials && n_partials_host, "null pointer");
+  B2RL_REQUIRE(n_out == 64 && ((C == 64 && taps == 9 && taps_x == 3) || (C == 128 && taps == 4 && taps_x == 2)),
+               "the taps weight gradient serves n_out 64 with C 64 and 3 x 3 taps (conv3) or C 128 and 2 x 2 taps (conv2)");
+  const int halo = (taps_x - 1) * (grid_w + 1);
+  B2RL_REQUIRE(grid_w > 0 && CTW_BK + halo <= 256, "grid too wide for one gradient box");
+  B2RL_REQUIRE(rows > 0 && rows < (1LL << 31), "bad shape");
+  B2RL_REQUIRE((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(G)) % 16 == 0, "operands must be 16-byte aligned");
+  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(partials) % 8 == 0, "partials must be 8-byte aligned");
+  TapsWgradParams w = {};
+  w.rows = (int)rows; w.grid_w = grid_w; w.D = partials; w.clk = g_k1_clocks;
+  CUtensorMap tg, tx;
+  int rc = make_map(&tg, G, 64, rows, 64, CTW_BK + halo);             // gradient box: [BK + halo rows][64 n]
+  if (rc) return rc;
+  rc = make_map(&tx, X, C, rows, C, CTW_BK);                         // activation block: C / 64 boxes [128 rows][64 c]
+  if (rc) return rc;
+  int n = 0;
+  const int r2 = C == 64 ? launch_taps_wgrad<64, 3, 3>(tg, tx, w, (cudaStream_t)stream, &n)
+                         : launch_taps_wgrad<128, 2, 2>(tg, tx, w, (cudaStream_t)stream, &n);
+  if (r2 > 0) { set_error("b2rl_conv_taps_wgrad_partials: the operand ring does not fit in shared memory"); return B2RL_ERR_ARG; }
   *n_partials_host = n;
   return r2;
 }

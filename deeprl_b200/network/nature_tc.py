@@ -311,6 +311,10 @@ def wgrad_partials(X, G_rows, n_out, taps, taps_x, grid_w, stream=None):
         _lib.call("b2rl_conv1_wgrad_partials", _lib.ptr(X), int(rows), int(grid_w), _lib.ptr(G_rows), int(n_out), _lib.ptr(buf),
                   ctypes.byref(n), stream if stream is not None else _lib.stream())
         return buf, int(n.value)
+    if n_out == 64 and (C, taps, taps_x) in ((64, 9, 3), (128, 4, 2)):   # conv3 / conv2: every tap of a k-block in one CTA
+        _lib.call("b2rl_conv_taps_wgrad_partials", _lib.ptr(X), int(rows), int(C), _lib.ptr(G_rows), int(n_out), int(taps),
+                  int(taps_x), int(grid_w), _lib.ptr(buf), ctypes.byref(n), stream if stream is not None else _lib.stream())
+        return buf, int(n.value)
     _lib.call("b2rl_conv_wgrad_partials", _lib.ptr(X), int(rows), int(C), _lib.ptr(G_rows), int(n_out), int(taps), int(taps_x),
               int(grid_w), _lib.ptr(buf), ctypes.byref(n), stream if stream is not None else _lib.stream())
     return buf, int(n.value)

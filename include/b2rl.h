@@ -378,6 +378,10 @@ int b2rl_head_bwd_geff_relu(const float* geff, const uint16_t* phi, const float*
  * HOST, deterministic for given shapes) is stored at partials + i * n_out*taps*C floats. */
 int b2rl_conv_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out, int32_t taps,
                              int32_t taps_x, int32_t grid_w, float* partials, int32_t* n_partials_host, void* stream);
+/* The same partials for conv2 (C 128, 2 x 2 taps) and conv3 (C 64, 3 x 3 taps), n_out 64: one CTA computes every tap of its
+ * 128-row k-blocks from one load of each operand.  One partial per CTA: at most one per SM, or the CTA budget. */
+int b2rl_conv_taps_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out, int32_t taps,
+                                  int32_t taps_x, int32_t grid_w, float* partials, int32_t* n_partials_host, void* stream);
 
 /* K1 -- conv1 of NatureConvBody straight from the uint8 replay ring: the fused gather -> normalize -> conv1 of the
  * reference chain replay.py:124-134 (frame-stack gather) -> normalizer.py:58-61 -> network_bodies.py:27, with no
