@@ -218,9 +218,18 @@ __device__ __forceinline__ int4 ldg_v4_here(const void* ptr) {
   asm volatile("ld.global.nc.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(ptr));
   return v;
 }
-// 16-byte global store of a 16-byte aligned address
-__device__ __forceinline__ void stg128(void* ptr, const int4 v) {
-  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(ptr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+// 8 floats rounded to bf16 (round to nearest even, as __floats2bfloat162_rn) and stored as one 16-byte group
+__device__ __forceinline__ void stg_bf16x8(__nv_bfloat16* ptr, const float (&v)[8]) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 h<4>;\n"
+      "cvt.rn.bf16x2.f32 h0, %2, %1;\n"
+      "cvt.rn.bf16x2.f32 h1, %4, %3;\n"
+      "cvt.rn.bf16x2.f32 h2, %6, %5;\n"
+      "cvt.rn.bf16x2.f32 h3, %8, %7;\n"
+      "st.global.v4.b32 [%0], {h0, h1, h2, h3};\n"
+      "}\n" ::"l"(ptr), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
+      : "memory");
 }
 template <int BN, bool EXT>
 __device__ __forceinline__ void epi_mask_load(const GemmParams& p, int row0, int n0, int t, int4 (&m)[BN / 16]) {
@@ -309,18 +318,17 @@ __device__ __forceinline__ int64_t epi_col_off(const GemmParams& p, int n) {
 
 // Epilogue of one 64-row half of a 128 x BN tile (first row row0, first column n0) for warpgroup thread t: `s` is the
 // half's fp32 staging tile, `m` its mask (epi_mask_load).  The bias-gradient column sums of the half stay in registers
-// (dsum: the thread's 8 columns over its BN/16 rows) until one dbias_flush at the end.  PAIR (paired conv1 forward, n0 = 0):
-// tile columns 0 .. BN/2 - 1 are columns of (D, bias), columns BN/2 .. BN - 1 those of (D2, bias2); p.N = BN / 2.
-template <int BN, bool EXT, bool PAIR = false>
+// (dsum: the thread's 8 columns over its BN/16 rows) until one dbias_flush at the end.  The general form of the plain and
+// tap-addressing GEMMs (every output mode and column count); the convolution slab kernels use slab_epilogue_half.
+template <int BN, bool EXT>
 __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int n0, int t, const float* s,
                                               const int4 (&m)[BN / 16], float* s_dbias) {
   constexpr int ACC_LD = acc_ld(BN);
   float dsum[8] = {};
   const int c = epi_col<BN>(t);
-  const bool second = PAIR && c >= BN / 2;                    // the thread's 8 columns all lie in one half
-  const int n = n0 + c - (second ? BN / 2 : 0);
-  const float* bias = second ? p.bias2 : p.bias;
-  void* D = second ? p.D2 : p.D;
+  const int n = n0 + c;
+  const float* bias = p.bias;
+  void* D = p.D;
   const bool cols = n < p.N, full = n + 8 <= p.N;
   const bool add_bias = bias && blockIdx.z == 0 && cols;
   float b[8];
@@ -384,16 +392,7 @@ __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int
           if (full || n + j < p.N) dsum[j] += v[j];
       }
     }
-    if constexpr (PAIR) {
-      // bf16, whole 16-byte column groups (b2rl_conv1_u8_fwd_pair): the one store form, which keeps the code of this
-      // epilogue small beside the converters' and the producer's (explicit store: through the selected pointer the compiler
-      // splits it)
-      int4 o;
-      __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&o);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
-      stg128(reinterpret_cast<__nv_bfloat16*>(D) + off, o);
-    } else if (p.out_mode == 0) {
+    if (p.out_mode == 0) {
       __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(D) + off;
       if (full && off % 8 == 0) {
         int4 o;
@@ -429,6 +428,101 @@ __device__ __forceinline__ void epilogue_half(const GemmParams& p, int row0, int
     }
   }
   if (EXT && p.dbias) dbias_flush<BN>(p, n0, t, dsum, s_dbias);
+}
+
+// Rows of one pass of slab_epilogue_half: all of a thread's BN/16 rows, except where their staged values and masks do
+// not fit beside the rest in the epilogue warpgroup's registers (BN 128 with the mask: 32 registers of mask) -- two passes
+template <int BN, bool EXT>
+__host__ __device__ constexpr int slab_epi_pass_rows() { return EXT && BN == 128 ? BN / 32 : BN / 16; }
+
+// The epilogue of the convolution slab kernels (conv_slab_body), on the same thread mapping as epilogue_half.  The launchers
+// give these kernels one output form (conv_gemm_impl, b2rl_conv1_u8_fwd / _pair): bf16 in whole 16-byte column groups (N and
+// ldd multiples of 8, D and D2 16-byte aligned, columns 0 .. N - 1 from n0 = 0), forwards with ReLU (bias optional) and no
+// extras, EXT dgrads with mask and bias gradient, no bias, no ReLU.  So each row is one 16-byte store and the per-row tests
+// of epilogue_half are gone.  Every staged value of a pass (two 16-byte loads per row) and every row base is requested
+// before the first is used: a pass waits for one shared-memory round trip, not one per row.  The arithmetic of each element
+// and the order of the dsum additions (rows k = 0, 1, ...) are those of epilogue_half, so every output has the same bits.
+// PAIR (paired conv1 forward): tile columns 0 .. BN/2 - 1 are columns of (D, bias), BN/2 .. BN - 1 those of (D2, bias2);
+// p.N = BN / 2.
+template <int BN, bool EXT, bool PAIR>
+__device__ __forceinline__ void slab_epilogue_half(const GemmParams& p, int row0, int t, const float* s,
+                                                   const int4 (&m)[BN / 16], float* s_dbias) {
+  constexpr int ACC_LD = acc_ld(BN);
+  constexpr int ROWS = BN / 16, PASS = slab_epi_pass_rows<BN, EXT>();
+  float dsum[8] = {};
+  const int c = epi_col<BN>(t);
+  const bool second = PAIR && c >= BN / 2;                    // the thread's 8 columns all lie in one half
+  const int n = c - (second ? BN / 2 : 0);
+  __nv_bfloat16* D = reinterpret_cast<__nv_bfloat16*>(second ? p.D2 : p.D);
+  const bool cols = n < p.N;
+  const float* bias = second ? p.bias2 : p.bias;
+  const bool add_bias = !EXT && bias && cols;
+  float b[8];
+  if (add_bias) {
+    const float* bp = bias + n;
+    if ((reinterpret_cast<uintptr_t>(bp) & 15) == 0) {
+      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bp)), b1 = __ldg(reinterpret_cast<const float4*>(bp + 4));
+      b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) b[j] = __ldg(bp + j);
+    }
+  }
+  // bank-conflict-free order of the two 16-byte reads and the row bases handed over by lane: as in epilogue_half
+  const int h0 = ((c >> 5) ^ epi_row<BN>(t, 0)) & 1;
+  const uint32_t s_base = s2u(s);
+  const int64_t coff = epi_col_off<EXT>(p, n);
+  int64_t rbase = -1;
+  if ((t & 31) < 16) {
+    constexpr int RPW = 256 / BN;
+    const int q = t & 31;
+    rbase = epi_row_base<EXT>(p, row0 + (t >> 5) * RPW + q % RPW + (q / RPW) * 4 * RPW);
+  }
+#pragma unroll
+  for (int k0 = 0; k0 < ROWS; k0 += PASS) {
+    float4 x[PASS], y[PASS];
+    int64_t base[PASS];
+#pragma unroll
+    for (int i = 0; i < PASS; ++i) {
+      const uint32_t sp = s_base + (uint32_t)(epi_row<BN>(t, k0 + i) * ACC_LD + c) * 4;
+      x[i] = lds128(sp + 16 * h0);
+      y[i] = lds128(sp + 16 * (h0 ^ 1));
+    }
+#pragma unroll
+    for (int i = 0; i < PASS; ++i) base[i] = __shfl_sync(0xffffffffu, rbase, (k0 + i) * (256 / BN) + (t & 31) / (BN / 8));
+    // a warp barrier between the requests and their first use: without it the compiler hoists a row's stores above the
+    // loads of the rows after it (forward kernels), and the pass waits for the shared-memory round trip more than once
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < PASS; ++i) {
+      const int k = k0 + i;
+      const float4 lo = h0 ? y[i] : x[i], hi = h0 ? x[i] : y[i];
+      float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+      // rows that are not stored are computed too and only their store and sum are dropped: a branch around the row would
+      // let the compiler sink its shared-memory loads into it, back behind the previous row's store
+      const bool store = base[i] >= 0 && cols;
+      if constexpr (EXT) {
+        const __nv_bfloat162* mh = reinterpret_cast<const __nv_bfloat162*>(&m[k]);   // ReLU gradient
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 mf = __bfloat1622float2(mh[q]);
+          if (!(mf.x > 0.0f)) v[2 * q] = 0.0f;
+          if (!(mf.y > 0.0f)) v[2 * q + 1] = 0.0f;
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) dsum[j] = store ? dsum[j] + v[j] : dsum[j];
+      } else {
+        if (add_bias) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[j] += b[j];
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.0f);
+      }
+      if (store) stg_bf16x8(D + base[i] + coff, v);
+    }
+  }
+  if constexpr (EXT) dbias_flush<BN>(p, 0, t, dsum, s_dbias);
 }
 
 template <int BN, int STAGES, bool EXT>
@@ -1215,7 +1309,7 @@ __device__ __forceinline__ void conv_slab_body(const CUtensorMap& tmA, const CUt
       const long long t0 = clk_now(clk);
       named_sync(SLAB_BAR_STAGED + e, 256);
       const long long t1 = clk_now(clk);
-      epilogue_half<BN, EXT, PAIR>(p, tile * GEMM_BM + 64 * e, 0, t, sAcc_e, mk, s_dbias);
+      slab_epilogue_half<BN, EXT, PAIR>(p, tile * GEMM_BM + 64 * e, t, sAcc_e, mk, s_dbias);
       if (tile + n_cta < tiles) named_arrive(SLAB_BAR_FREE + e, 256);   // the MMA warpgroup waits only for a next tile
       c_wait += t1 - t0, c_work += clk_now(clk) - t1;
     }
@@ -2286,7 +2380,12 @@ static int conv_gemm_impl(int32_t mode, const uint16_t* X, int64_t rows, int32_t
     int rc = check_common(X, W_or_G, D, C, K, (int)rows, n_out, K, out_mode, splits, block_n, 0, relu);
     if (rc) return rc;
     p.M = (int)rows; p.N = n_out; p.K = K; p.a_mn = 0; p.b_mn = 0; p.a_tap_tiles = C / 64;
-    if (g_use_slab && splits == 1 && n_out <= block_n && out_mode != 2) {
+    // the slab kernels' one output form (slab_epilogue_half): bf16 in whole 16-byte column groups; forwards with ReLU,
+    // dgrads with mask and bias gradient.  Every other call goes to the tap-addressing kernel.
+    const bool bf16_groups = out_mode == 0 && n_out % 8 == 0 && ldd % 8 == 0 &&
+                             (reinterpret_cast<uintptr_t>(D) | reinterpret_cast<uintptr_t>(D2)) % 16 == 0;
+    const bool slab_epilogue = ext ? (p.mask && p.dbias && !relu && !bias) : relu != 0;
+    if (g_use_slab && splits == 1 && n_out <= block_n && bf16_groups && slab_epilogue) {
       const int max_shift = ((taps - 1) / taps_x) * grid_w + (taps - 1) % taps_x;
       SlabParams sp = {};
       sp.g = p; sp.taps = taps; sp.col_blocks = C / 64;
@@ -2510,8 +2609,10 @@ extern "C" int b2rl_conv1_u8_fwd(const uint8_t* frames, int64_t capacity, const 
   int rc = u8_src(sp.u8, frames, idx, first, row_bytes, frame_w, batch, history);
   if (rc) return rc;
   B2RL_REQUIRE(W && D, "null pointer");
-  B2RL_REQUIRE(n_out > 0 && n_out <= 32 && out_map >= 0 && out_map <= 2, "n_out <= 32, out_map 0..2");
-  B2RL_REQUIRE(reinterpret_cast<uintptr_t>(W) % 16 == 0, "operands must be 16-byte aligned");
+  B2RL_REQUIRE(n_out > 0 && n_out <= 32 && n_out % 8 == 0 && out_map >= 0 && out_map <= 2, "n_out 8, 16, 24 or 32, out_map 0..2");
+  B2RL_REQUIRE((reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(D)) % 16 == 0 && ldd % 8 == 0,
+               "operands and output must be 16-byte aligned, ldd a multiple of 8");
+  B2RL_REQUIRE(relu, "the slab forward applies ReLU (conv1 of NatureConvBody)");
   const int G = sp.u8.G, C = 64, taps = 4, K = taps * C;
   GemmParams p = {};
   p.M = sp.u8.rows; p.N = n_out; p.K = K; p.ldd = (int)ldd;
@@ -2570,6 +2671,7 @@ extern "C" int b2rl_conv1_u8_fwd_pair(const uint8_t* frames, int64_t capacity, c
   B2RL_REQUIRE((reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(W2) | reinterpret_cast<uintptr_t>(D) |
                 reinterpret_cast<uintptr_t>(D2)) % 16 == 0, "operands and outputs must be 16-byte aligned");
   B2RL_REQUIRE(capacity >= history + 1, "bad capacity");
+  B2RL_REQUIRE(relu, "the slab forward applies ReLU (conv1 of NatureConvBody)");
   sp.u8.nf = history + 1;                                  // the window of s and s'
   const int G = sp.u8.G;
   GemmParams p = {};

@@ -389,8 +389,9 @@ int b2rl_conv_taps_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, co
  * the oldest stacked frame relative to idx[b] (-(history-1) for the state, n_step-(history-1) for the next state);
  * history must be 4 (4 frames x 16 pixels = the 64 channels of one space-to-depth(4) position).  The pixels enter as
  * exact integers 0..255; ImageNormalizer's 1/255 is folded into W [n_out][4 taps * 64] (b2rl_nature_pack_weights).
- * fwd: D = act(conv1 + bias) over rows (b, gy, gx) of the (frame_w/4)^2 grid, bf16, output row maps of
- * b2rl_conv_gemm_bf16.  wgrad_partials: split-K partials of dW[n][tap*64+c] = sum_r G[r][n] * x[r + shift(tap)][c],
+ * fwd: D = relu(conv1 + bias) over rows (b, gy, gx) of the (frame_w/4)^2 grid, bf16, output row maps of
+ * b2rl_conv_gemm_bf16; relu must be 1, n_out a multiple of 8, D 16-byte aligned and ldd a multiple of 8 (the slab
+ * kernel's one store form: whole 16-byte column groups).  wgrad_partials: split-K partials of dW[n][tap*64+c] = sum_r G[r][n] * x[r + shift(tap)][c],
  * contract of b2rl_conv_wgrad_partials; n_out must be 32. */
 int b2rl_conv1_u8_fwd(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first, int64_t row_bytes,
                       int32_t frame_w, int32_t batch, int32_t history, const uint16_t* W, int32_t n_out, void* D, int64_t ldd,
@@ -406,7 +407,7 @@ int b2rl_conv1_wgrad_partials(const uint16_t* X, int64_t rows, int32_t grid_w, c
 /* The online forward on the state and the target forward on the next state (n_step 1) in ONE launch: D = act(conv1_W(s) +
  * bias) and D2 = act(conv1_W2(s') + bias2), s the stacks idx[b] + first .. + history - 1 and s' the stacks one ring row
  * later, read together from the history + 1 ring rows they span.  W, W2 [32][4 taps * 64]; D, D2 as D of b2rl_conv1_u8_fwd
- * with n_out 32 (row stride ldd).  Bit-identical to b2rl_conv1_u8_fwd(first, W, D, bias) and (first + 1, W2, D2, bias2).
+ * with n_out 32 (row stride ldd); relu must be 1.  Bit-identical to b2rl_conv1_u8_fwd(first, W, D, bias) and (first + 1, W2, D2, bias2).
  * history 4 and 84 x 84 frames only. */
 int b2rl_conv1_u8_fwd_pair(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first, int64_t row_bytes,
                            int32_t frame_w, int32_t batch, int32_t history, const uint16_t* W, const uint16_t* W2, void* D,
