@@ -75,7 +75,6 @@ SIGNATURES = {
     "b2rl_gemm_splitk_bf16": [c_p, c_i64, c_p, c_i64, c_p, c_i64, c_i32, c_i32, c_i32, c_p, c_i32, c_i32, c_i32, c_p],
     "b2rl_nature_pack_weights": [c_p, c_p, c_p, c_p, c_i32, c_i32, c_f32, c_p, c_p, c_p, c_p, c_p, c_p, c_p],
     "b2rl_nature_unpack_grads": [c_p] * 8 + [c_i32, c_i32, c_f32] + [c_p] * 8 + [c_i32, c_i32, c_i32, c_p],
-    "b2rl_conv_wgrad_partials": [c_p, c_i64, c_i32, c_p, c_i32, c_i32, c_i32, c_i32, c_p, c_p, c_p],
     "b2rl_conv_taps_wgrad_partials": [c_p, c_i64, c_i32, c_p, c_i32, c_i32, c_i32, c_i32, c_p, c_p, c_p],
     "b2rl_head_fwd": [c_p, c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_p],
     "b2rl_head_bwd": [c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_p, c_p, c_p, c_p, c_p],

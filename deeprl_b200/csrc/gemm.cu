@@ -28,7 +28,6 @@
 // that part overlaps the tail of the previous kernel (common.cuh).
 // sm_90a only.
 #include <cuda.h>
-#include <cstdlib>
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -1342,148 +1341,11 @@ __global__ void __launch_bounds__(SLAB_K1_THREADS, 1) conv1_pair_wgmma_kernel(co
 
 
 // ---------------------------------------------------------------------------------------------------------------
-// Slab variant of the convolution weight gradient:  D[n, tap*C + c] += sum_r G[r, n] * X[r + shift(tap), c].
-// Both operands are read as stored (MN-major, K = rows).  A CTA owns a contiguous range of 64-row k-tiles (blockIdx.x) and
-// one group of taps (blockIdx.y: 128 output columns, two taps of 64 channels or one of 128); per k-tile it loads the
-// gradient rows ONCE and ONE slab of 64 + max_shift activation rows, and issues every tap's MMAs on windows of that slab (a
-// K-row shift is a 128-byte step in the MN-major swizzled layout, address-based swizzle as above) into register
-// accumulators.  At the end each CTA stores its partial sums plainly at D + blockIdx.x * partial_stride (the consumer sums
-// them: deterministic), or adds them to D with fp32 vector atomics when partial_stride == 0.
-// ---------------------------------------------------------------------------------------------------------------
-struct WgradParams {
-  int rows, n_out, C, col_blocks;
-  int tap0, ntaps, taps_x, grid_w;
-  int slab_rows, stages, k_tiles_per_cta, a_boxes;
-  float* D;
-  int ldd;
-  int64_t partial_stride;   // 0: atomically accumulate into D; > 0: CTA i stores its partial sums at D + i*partial_stride
-  // one window per tap, built on the host (launch_wgrad): slab window offset (16-byte units) and accumulator column
-  int n_runs;
-  int win0;                 // window of blockIdx.y == 0 (the one-window instantiation serves the last of an odd count)
-  uint32_t run_off[9], run_acc[9];
-  // M-stacking (n_out <= 64): warpgroup 2's A operand holds the SAME gradient columns read `stack_delta` rows away (a second
-  // TMA box), so its accumulator rows of a window at shift s hold the tap at shift s - stack_delta: with stack_delta = -grid_w
-  // the windows of tap row dy also produce tap row dy + 1 -- the last tap row costs no MMAs at all (conv2 / conv1: half the
-  // MMAs; conv3: 6 windows instead of 9 taps).
-  // run_low[j] = first output column of the lower half of run j, or -1 (a duplicate of an upper tap: dropped).
-  int stack_delta, stack_rows;
-  int run_low[9];
-};
-
-// The windows of a CTA are a compile-time shape WIN: WGRAD_N128 (one n128 window, C = 128), WGRAD_2X64 (two n64 windows) or
-// WGRAD_1X64 (one n64 window: the last group of an odd window count).  With no runtime choice of MMA shape in the
-// accumulator chain, ptxas keeps the wgmmas asynchronous: every k-tile is one commit group, and the group of k-tile i - 1 is
-// retired (its stage released) only after k-tile i has been issued.
-constexpr int WGRAD_N128 = 0, WGRAD_2X64 = 1, WGRAD_1X64 = 2;
-template <int WIN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) conv_wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmG,
-                                                                          const __grid_constant__ CUtensorMap tmX,
-                                                                          const WgradParams w) {
-  constexpr int MAX_STAGES = 6;
-  constexpr uint32_t A_BYTES = 2 * 8192;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t slab_block = (uint32_t)w.slab_rows * 128, slab_bytes = slab_block * w.col_blocks;
-  const uint32_t stage_bytes = A_BYTES + slab_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)w.stages * stage_bytes);
-  uint64_t* empty = full + MAX_STAGES;
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
-  const int kt_total = (w.rows + GEMM_BK - 1) / GEMM_BK;
-  const int kt_begin = blockIdx.x * w.k_tiles_per_cta;
-  const int n_kt = max(min(kt_total, kt_begin + w.k_tiles_per_cta) - kt_begin, 0);
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) { mb_init(&full[s], 1); mb_init(&empty[s], MMA_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmG) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
-  }
-  __syncthreads();
-  pdl_sync();   // everything above (barriers, tensor-map prefetch) overlaps the previous kernel's tail
-
-  if (warp == 0 && elect_one()) {
-    for (int i = 0; i < n_kt; ++i) {
-      const int s = i % w.stages;
-      mb_wait(&empty[s], ((i / w.stages) & 1) ^ 1);
-      mb_expect_tx(&full[s], (uint32_t)w.a_boxes * 8192 + slab_bytes);
-      uint8_t* st = smem + (size_t)s * stage_bytes;
-      const int k0 = (kt_begin + i) * GEMM_BK;
-      for (int g = 0; g < w.a_boxes; ++g)                                                                 // [64 k][64 n]
-        tma_load_2d(st + g * 8192, &tmG, &full[s], w.stack_delta ? 0 : g * 64, k0 + (g ? w.stack_delta : 0));
-      for (int cb = 0; cb < w.col_blocks; ++cb)
-        tma_load_2d(st + A_BYTES + (size_t)cb * slab_block, &tmX, &full[s], cb * GEMM_BK, k0);           // [slab_rows][64 c]
-    }
-  } else if (warp >= 4 && n_kt > 0 && (warp - 4) / 4 >= w.a_boxes) {
-    // one A box (n_out <= 64, not stacked): warpgroup 2 only releases the stages
-    for (int i = 0; i < n_kt; ++i) {
-      mb_wait(&full[i % w.stages], (i / w.stages) & 1);
-      if (lane == 0) mb_arrive(&empty[i % w.stages]);
-    }
-  } else if (warp >= 4 && n_kt > 0) {
-    // ---------------------------------------------------------------------- MMA, warpgroup g: accumulator rows (output
-    // channels) 64 g .. 64 g + 63 from A box g -- or, M-stacked, the same channels one tap row further down
-    constexpr int NJ = WIN == WGRAD_2X64 ? 2 : 1, WC = WIN == WGRAD_N128 ? 128 : 64;   // windows, columns per window
-    const int cw = warp - 4, g = cw >> 2, wl = cw & 3;
-    const int j0 = w.win0 + (int)blockIdx.y * NJ;                                      // this CTA's first window
-    const uint64_t a0 = make_desc(s2u(smem) + g * 8192, 8192);
-    const uint32_t b0 = s2u(smem) + A_BYTES + w.run_off[j0] * 16;
-    const uint32_t b1 = s2u(smem) + A_BYTES + w.run_off[NJ > 1 ? j0 + 1 : j0] * 16;
-    float d[NJ * WC / 2];
-    acc_zero<NJ * WC>(d);
-    for (int i = 0; i < n_kt; ++i) {
-      const int s = i % w.stages;
-      mb_wait(&full[s], (i / w.stages) & 1);
-      const uint32_t st = (uint32_t)s * stage_bytes;
-      const uint64_t a = a0 + (st >> 4);
-      wg_fence();
-      if constexpr (WIN == WGRAD_N128) {
-        mma_ktile<128, 1, 1>(d, a, make_desc(b0 + st, slab_block));
-      } else {
-        mma_ktile<64, 1, 1>(d, a, make_desc(b0 + st, 8192));
-        if constexpr (NJ > 1) mma_ktile<64, 1, 1>(d + 32, a, make_desc(b1 + st, 8192));
-      }
-      wg_commit();
-      wg_wait1();                                                      // k-tile i - 1 has retired: release its stage
-      if (i > 0 && lane == 0) mb_arrive(&empty[(i - 1) % w.stages]);
-    }
-    wg_wait0();
-    acc_fence<NJ * WC>(d);
-    if (lane == 0) mb_arrive(&empty[(n_kt - 1) % w.stages]);
-    // accumulator element d[32 sl + 4 jj + 2 h + e]: channel 16 wl + lane / 4 + 8 h, column 64 sl + 8 jj + 2 (lane % 4) + e
-    const bool low = w.stack_delta != 0 && g == 1;
-    float* base = w.D + (int64_t)blockIdx.x * w.partial_stride + 2 * (lane & 3);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int n = 16 * wl + (lane >> 2) + 8 * h;
-      const int nn = low ? n : g * 64 + n;
-      if (nn >= w.n_out) continue;
-#pragma unroll
-      for (int sl = 0; sl < NJ; ++sl) {
-        const int j = j0 + sl;
-        int oc = w.tap0 * w.C + (int)w.run_acc[j];
-        if (low) {
-          if (w.run_low[j] < 0) continue;                              // duplicate of a tap the upper half already holds
-          oc = w.run_low[j];
-        }
-        float* dst = base + (int64_t)nn * w.ldd + oc;
-#pragma unroll
-        for (int jj = 0; jj < WC / 8; ++jj) {
-          const float2 v = make_float2(d[32 * sl + 4 * jj + 2 * h], d[32 * sl + 4 * jj + 2 * h + 1]);
-          if (w.partial_stride > 0) *reinterpret_cast<float2*>(dst + 8 * jj) = v;   // split-K partials: summed by the consumer
-          else atomicAdd(reinterpret_cast<float2*>(dst + 8 * jj), v);
-        }
-      }
-    }
-  }
-  __syncthreads();
-}
-
-// ---------------------------------------------------------------------------------------------------------------
 // conv1's weight gradient with the taps in the MMA rows.  conv1 has n_out = 32 channels and 2 x 2 taps at row shifts
 // s_t = 0, 1, G, G + 1 of the G x G grid.  The sum is written with the activations unshifted and the gradient rows carrying
 // the shift:
 //   dW[n][t*64 + c] = sum_r G[r][n] x[r + s_t][c] = sum_r' G[r' - s_t][n] x[r'][c]
-// (r' - s_t < 0: the TMA's out-of-bounds zero fill; r' >= rows: x is zero there -- the same products as the slab form).
+// (r' - s_t < 0: the TMA's out-of-bounds zero fill; r' >= rows: x is zero there -- the same products as the first sum).
 // Each MMA warpgroup g holds ONE m64n64 accumulator over two taps: rows 0-31 are tap 2g + 1, rows 32-63 tap 2g, so every
 // accumulator row is a result.  The A operand (MN-major, K = rows r') is one TMA box of the gradient rows [k0 - G - 1,
 // k0 + BK) stored with the 64-byte swizzle (one 64-byte row per grid row = 32 channels = one swizzle atom column): the
@@ -1669,7 +1531,7 @@ __global__ void __launch_bounds__(U8 ? SLAB_U8_THREADS : GEMM_THREADS, 1) conv1_
 // activation block for all taps.  Tap t has its own m64 x C accumulator (output channels x input channels), so each
 // accumulator row is a result; MMA warpgroup g holds taps g*TPW .. g*TPW + TPW - 1: conv3 3 warpgroups x 3 taps of m64n64
 // (96 registers), conv2 2 x 2 taps of m64n128 (128 registers).  Loads per k-block: (BK + halo) * 128 + BK * 2C bytes for
-// 2 * BK * 64 * taps * C FLOP -- every operand once, against one fetch per 128-column tap group of conv_wgrad_wgmma_kernel.
+// 2 * BK * 64 * taps * C FLOP: every operand is loaded once, whatever the number of taps.
 // A CTA takes a contiguous range of k-blocks (equal ranges, at most one CTA per SM or per CTA of the budget) and stores its
 // [64][taps * C] fp32 partial block at D + blockIdx.x * 64 * taps * C; the consumer sums the partials (deterministic).
 // Each k-block is one commit group per warpgroup, retired (its stage released) after the next one has been issued.
@@ -2150,67 +2012,6 @@ static int launch_slab(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
                        : launch_slab_shape<BN, false>(ta, tb, ta2, tb2, sp, st);
 }
 
-// one launch of the weight-gradient instantiation for window shape WIN over `groups` tap groups from window w.win0 on
-template <int WIN>
-static void launch_wgrad_k(const CUtensorMap& tg, const CUtensorMap& tx, const WgradParams& w, int ctas, int groups,
-                           size_t smem, cudaStream_t st) {
-  auto k = conv_wgrad_wgmma_kernel<WIN>;
-  static size_t attr = 0;
-  if (attr < smem) {
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    attr = smem;
-  }
-  launch_pdl(k, dim3(ctas, groups), dim3(GEMM_THREADS), smem, st, tg, tx, w);
-}
-
-static int launch_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, WgradParams w, cudaStream_t st, int* n_ctas = nullptr) {
-  const size_t slab_bytes = (size_t)w.slab_rows * 128 * w.col_blocks, stage = 16384 + slab_bytes;
-  static const size_t limit = dyn_smem_limit(conv_wgrad_wgmma_kernel<WGRAD_2X64>);
-  const size_t fixed = 1024 + 2 * 6 * 8 + 16;
-  const size_t budget = limit > fixed + 200 * 1024 ? 200 * 1024 : (limit > fixed ? limit - fixed : 0);
-  int stages = (int)(budget / stage);
-  if (stages > 6) stages = 6;
-  if (stages < 2) return 1;
-  w.stages = stages;
-  const size_t smem = 1024 + stages * stage + 2 * 6 * 8 + 16;
-  // one window per tap; a CTA accumulates the taps of one 128-column group (blockIdx.y)
-  if (w.ntaps > 9 || (w.C != 64 && w.C != 128)) return 1;
-  for (int n = 0; n < w.ntaps; ++n) {
-    const int tap = w.tap0 + n, dy = tap / w.taps_x, dx = tap - dy * w.taps_x;
-    w.run_off[n] = (uint32_t)(dy * w.grid_w + dx) * 8;
-    w.run_acc[n] = (uint32_t)(n * w.C);
-    w.run_low[n] = (w.stack_delta && dy == w.stack_rows - 2) ? ((dy + 1) * w.taps_x + dx) * w.C : -1;
-  }
-  w.n_runs = w.ntaps;
-  const int groups = (w.ntaps * w.C + 127) / 128;
-  const int kt_total = (w.rows + GEMM_BK - 1) / GEMM_BK;
-  // split-K over the SMs or the CTA budget (groups x ctas CTAs); every CTA stores (or reduces) its n_out x 128 partial block
-  int ctas = kt_total / 4;
-  if (ctas > grid_cap() / groups) ctas = grid_cap() / groups;
-  static int cap = -1;                                               // tunable: B2RL_WGRAD_CTAS caps the split-K width
-  if (cap < 0) {
-    const char* e = getenv("B2RL_WGRAD_CTAS");
-    cap = e ? atoi(e) : 0;
-  }
-  if (cap > 0 && ctas > cap) ctas = cap;
-  if (ctas < 1) ctas = 1;
-  w.k_tiles_per_cta = (kt_total + ctas - 1) / ctas;
-  ctas = (kt_total + w.k_tiles_per_cta - 1) / w.k_tiles_per_cta;
-  if (n_ctas) *n_ctas = ctas;
-  g_last_ctas = ctas * groups;
-  w.win0 = 0;
-  if (w.C == 128) {
-    launch_wgrad_k<WGRAD_N128>(tg, tx, w, ctas, groups, smem, st);
-  } else {                                                           // pairs of windows, then the odd one out on its own
-    if (w.ntaps >= 2) launch_wgrad_k<WGRAD_2X64>(tg, tx, w, ctas, w.ntaps / 2, smem, st);
-    if (w.ntaps % 2) {
-      w.win0 = w.ntaps - 1;
-      launch_wgrad_k<WGRAD_1X64>(tg, tx, w, ctas, 1, smem, st);
-    }
-  }
-  return check_launch("b2rl_conv_gemm_bf16(wgrad slab)");
-}
-
 // conv1_taps_conv_wgrad_wgmma_kernel: the 128-row k-blocks in equal contiguous ranges over at most one CTA per SM; returns
 // the CTA count (= partial blocks written) through n_ctas, or 1 when the operand ring does not fit in shared memory
 template <bool U8>
@@ -2281,10 +2082,6 @@ static int launch_taps_wgrad(const CUtensorMap& tg, const CUtensorMap& tx, TapsW
 
 using namespace b2rl;
 
-static int g_wgrad_partials = 0;          // set by b2rl_conv_wgrad_partials for the duration of one call
-static float* g_partial_buf = nullptr;
-static int64_t g_partial_stride = 0;
-static int g_partial_count = 0;
 static int g_use_slab = 2;   // 2: shifted windows with base_offset 0 -- the 128B swizzle is a pure function of the smem address
 static unsigned long long* g_k1_clocks = nullptr;
 // Profiling hook of every slab launch (the K1 conv1 forwards b2rl_conv1_u8_fwd / b2rl_conv1_u8_fwd_pair, the slab forwards
@@ -2420,40 +2217,6 @@ static int conv_gemm_impl(int32_t mode, const uint16_t* X, int64_t rows, int32_t
   int rc = check_common(W_or_G, X, D, n_out, C, n_out, taps * C, (int)rows, out_mode, splits, block_n, 1, relu);
   if (rc) return rc;
   B2RL_REQUIRE(out_mode == 2, "wgrad accumulates with out_mode 2");
-  // (the slab kernel stores / reduces float2 pairs: D and its rows must be 8-byte aligned)
-  if (g_use_slab && C % 64 == 0 && C <= 128 && n_out <= 128 && shift_sign > 0 && ldd % 2 == 0 &&
-      reinterpret_cast<uintptr_t>(g_wgrad_partials ? g_partial_buf : D) % 8 == 0) {
-    int max_shift = ((taps - 1) / taps_x) * grid_w + (taps - 1) % taps_x;
-    WgradParams w = {};
-    w.rows = (int)rows; w.n_out = n_out; w.C = C; w.col_blocks = C / 64; w.taps_x = taps_x; w.grid_w = grid_w;
-    w.a_boxes = n_out > 64 ? 2 : 1;
-    // M-stacking (see WgradParams): with at most 64 output channels the second half of the 128 accumulator lanes computes the
-    // last tap row from the windows of the row before it (B2RL_WGRAD_STACK=0: every tap its own window)
-    static int stack_on = -1;
-    if (stack_on < 0) {
-      const char* e = getenv("B2RL_WGRAD_STACK");
-      stack_on = (e && atoi(e) == 0) ? 0 : 1;
-    }
-    const int taps_y = taps / taps_x;
-    int win_taps = taps;
-    if (stack_on && n_out <= 64 && taps_y >= 2 && taps_y * taps_x == taps) {
-      w.stack_delta = -grid_w; w.stack_rows = taps_y; w.a_boxes = 2;
-      win_taps = (taps_y - 1) * taps_x;
-      max_shift = (taps_y - 2) * grid_w + taps_x - 1;
-    }
-    w.slab_rows = (GEMM_BK + max_shift + 7) / 8 * 8;
-    w.D = reinterpret_cast<float*>(D); w.ldd = (int)ldd;
-    if (g_wgrad_partials) { w.D = g_partial_buf; w.partial_stride = g_partial_stride; }
-    CUtensorMap tg, tx;
-    rc = make_map(&tg, W_or_G, n_out, rows, n_out, 64);             // gradient rows: box [64 k][64 n]
-    if (rc) return rc;
-    rc = make_map(&tx, X, C, rows, C, w.slab_rows);                 // activation slab: box [slab_rows][64 c]
-    if (rc) return rc;
-    w.tap0 = 0;
-    w.ntaps = win_taps;
-    const int r2 = launch_wgrad(tg, tx, w, (cudaStream_t)stream, &g_partial_count);
-    if (r2 <= 0) return r2;
-  }
   p.M = n_out; p.N = taps * C; p.K = (int)rows; p.a_mn = 1; p.b_mn = 1; p.b_tap_tiles = C / block_n;
   return gemm_dispatch(W_or_G, 1, n_out, rows, n_out, X, 1, C, rows, C, p, splits, block_n, (cudaStream_t)stream);
 }
@@ -2526,22 +2289,6 @@ extern "C" int b2rl_gemm_bwd_bf16(const uint16_t* A, int64_t lda, const uint16_t
   rc = apply_ext(p, ext, N);
   if (rc) return rc;
   return dense_dispatch(A, 0, lda, M, K, B, b_mn, ldb, b_mn ? K : N, b_mn ? N : K, p, 1, block_n, 0, (cudaStream_t)stream);
-}
-
-// Weight gradient as split-K PARTIALS: partial i (one per CTA, n_partials_host of them, at most one per SM) is stored at
-// partials + i * n_out * taps * C; the consumer (b2rl_nature_unpack_grads) sums them.  Replaces ~1M fp32 atomics per
-// layer by coalesced stores.
-extern "C" int b2rl_conv_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out,
-                                        int32_t taps, int32_t taps_x, int32_t grid_w, float* partials,
-                                        int32_t* n_partials_host, void* stream) {
-  B2RL_REQUIRE(partials && n_partials_host, "null pointer");
-  B2RL_REQUIRE(g_use_slab && C % 64 == 0 && C <= 128 && n_out <= 128, "partials need the slab wgrad kernel");
-  g_wgrad_partials = 1; g_partial_buf = partials; g_partial_stride = (int64_t)n_out * taps * C; g_partial_count = 0;
-  int rc = b2rl_conv_gemm_bf16(1, X, rows, C, G, n_out, taps, taps_x, grid_w, 1, partials, (int64_t)taps * C, nullptr, 0, 2,
-                               0, 0, 0, 1, C == 128 ? 128 : 64, stream);
-  g_wgrad_partials = 0;
-  *n_partials_host = g_partial_count;
-  return rc;
 }
 
 // D = act(A B^T + bias) in bf16, K split over the `splits` CTAs of a cluster per output tile and the partials summed in
@@ -2723,9 +2470,9 @@ static int conv1_wgrad_args(const uint16_t* G_rows, int32_t n_out, int grid_w, c
 }
 
 // split-K partials of conv1's weight gradient dW[n][tap*64 + c] = sum_r G[r][n] * x[r + shift(tap)][c] with x read from the
-// ring as above (G_rows: bf16 [batch*G*G][32], the masked output gradient on conv1's grid; n_out must be 32).  Same output
-// contract as b2rl_conv_wgrad_partials (partial i at partials + i * 32 * 256, at most one per SM), same bits as
-// b2rl_conv1_wgrad_partials on the materialised stacks.
+// ring as above (G_rows: bf16 [batch*G*G][32], the masked output gradient on conv1's grid; n_out must be 32).  One partial
+// per CTA, at most one per SM: partial i at partials + i * 32 * 256, *n_partials_host of them; the consumer sums them.  Same
+// bits as b2rl_conv1_wgrad_partials on the materialised stacks.
 extern "C" int b2rl_conv1_u8_wgrad_partials(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first,
                                             int64_t row_bytes, int32_t frame_w, int32_t batch, int32_t history, const uint16_t* G_rows,
                                             int32_t n_out, float* partials, int32_t* n_partials_host, void* stream) {
@@ -2770,8 +2517,9 @@ extern "C" int b2rl_conv1_wgrad_partials(const uint16_t* X, int64_t rows, int32_
   return r2;
 }
 
-// conv2's and conv3's weight-gradient partials, every tap of a k-block in one CTA (conv_taps_wgrad_wgmma_kernel): the
-// arguments and the output layout of b2rl_conv_wgrad_partials, one partial per CTA (at most one per SM, or the CTA budget).
+// conv2's and conv3's weight-gradient partials, every tap of a k-block in one CTA (conv_taps_wgrad_wgmma_kernel): one
+// partial per CTA (at most one per SM, or the CTA budget), partial i at partials + i * n_out * taps * C, *n_partials_host
+// of them; the consumer (b2rl_nature_unpack_grads, b2rl_nature_grad_reduce) sums them.
 extern "C" int b2rl_conv_taps_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out,
                                              int32_t taps, int32_t taps_x, int32_t grid_w, float* partials,
                                              int32_t* n_partials_host, void* stream) {

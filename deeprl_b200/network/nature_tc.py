@@ -299,24 +299,27 @@ def _max_partials(device):
 
 
 def wgrad_partials(X, G_rows, n_out, taps, taps_x, grid_w, stream=None):
-    """Split-K partial weight gradients (one per CTA, no atomics): returns (partials [P_max, n_out, taps*C] fp32, P)."""
+    """Split-K partial weight gradients: returns (partials [P_max, n_out, taps*C] fp32, P); the caller sums partials[:P].
+    conv1 (C 64, n_out 32, 2 x 2 taps) goes to conv1's taps kernel, conv2 and conv3 to theirs: one partial per CTA, no
+    atomics, the same bits on every call.  Every other geometry (conv1 of a NatureConvBody with in_channels other than 4)
+    and every call with the slab kernels switched off (``set_conv_slab(0)``) runs the tap-addressing GEMM, which adds into
+    one partial (P = 1) with fp32 atomics: exact on integer data, but slower and not bit-reproducible from run to run."""
     rows, C = X.shape
-    if not _lib.CONV_SLAB:                       # tap-addressing mode (tests): atomic accumulation into one "partial"
+    conv1 = (C, n_out, taps, taps_x) == (64, 32, 4, 2)
+    conv23 = n_out == 64 and (C, taps, taps_x) in ((64, 9, 3), (128, 4, 2))
+    if not (_lib.CONV_SLAB and (conv1 or conv23)):
         out = torch.zeros((1, n_out, taps * C), dtype=_f32, device=X.device)
         conv_gemm(1, X, G_rows, n_out, taps, taps_x, grid_w, 1, out[0], splits=16, block_n=128 if C == 128 else 64)
         return out, 1
     buf = torch.empty((_max_partials(X.device), n_out, taps * C), dtype=_f32, device=X.device)
     n = ctypes.c_int32(0)
-    if (C, n_out, taps, taps_x) == (64, 32, 4, 2):   # conv1: the taps-in-M kernel, the same bits as wgrad_partials_ring
+    s = stream if stream is not None else _lib.stream()
+    if conv1:                                    # the same bits as wgrad_partials_ring
         _lib.call("b2rl_conv1_wgrad_partials", _lib.ptr(X), int(rows), int(grid_w), _lib.ptr(G_rows), int(n_out), _lib.ptr(buf),
-                  ctypes.byref(n), stream if stream is not None else _lib.stream())
-        return buf, int(n.value)
-    if n_out == 64 and (C, taps, taps_x) in ((64, 9, 3), (128, 4, 2)):   # conv3 / conv2: every tap of a k-block in one CTA
+                  ctypes.byref(n), s)
+    else:
         _lib.call("b2rl_conv_taps_wgrad_partials", _lib.ptr(X), int(rows), int(C), _lib.ptr(G_rows), int(n_out), int(taps),
-                  int(taps_x), int(grid_w), _lib.ptr(buf), ctypes.byref(n), stream if stream is not None else _lib.stream())
-        return buf, int(n.value)
-    _lib.call("b2rl_conv_wgrad_partials", _lib.ptr(X), int(rows), int(C), _lib.ptr(G_rows), int(n_out), int(taps), int(taps_x),
-              int(grid_w), _lib.ptr(buf), ctypes.byref(n), stream if stream is not None else _lib.stream())
+                  int(taps_x), int(grid_w), _lib.ptr(buf), ctypes.byref(n), s)
     return buf, int(n.value)
 
 

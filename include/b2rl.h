@@ -287,11 +287,11 @@ int b2rl_gemm_bf16(const uint16_t* A, int32_t a_mn, int64_t lda, const uint16_t*
 /* forward / dgrad calls use the slab kernel (one activation slab per tile, resident weights) unless switched off */
 void b2rl_set_conv_slab(int32_t on);
 /* CTA budget of the following launches of the slab convolution kernel (forward / dgrad), the plain GEMM (b2rl_gemm_bf16,
- * b2rl_gemm_bwd_bf16, b2rl_gemm_splitk_bf16) and the convolution weight gradient (b2rl_conv_wgrad_partials): each sizes its
- * grid to at most `ctas` CTAs (the persistent kernels loop over more tiles per CTA, the weight gradient writes fewer split-K
- * partials, the plain GEMM launches without clusters; a weight gradient keeps at least one CTA per 128-column group) instead
- * of up to one per SM, so that kernels on two parallel graph branches hold disjoint SMs.  0 (the default): up to one CTA per
- * SM.  The setting is read on the host at launch time; per-tile arithmetic does not depend on it.
+ * b2rl_gemm_bwd_bf16, b2rl_gemm_splitk_bf16) and conv2's / conv3's weight gradient (b2rl_conv_taps_wgrad_partials): each
+ * sizes its grid to at most `ctas` CTAs (the persistent kernels loop over more tiles per CTA, the weight gradient writes
+ * fewer split-K partials, the plain GEMM launches without clusters) instead of up to one per SM, so that kernels on two
+ * parallel graph branches hold disjoint SMs.  0 (the default): up to one CTA per SM.  The setting is read on the host at
+ * launch time; per-tile arithmetic does not depend on it.
  * b2rl_last_grid_ctas: the CTAs of the last launch of those launchers (summed over the kernels of one call). */
 int b2rl_set_cta_budget(int32_t ctas);
 int b2rl_last_grid_ctas(int32_t* ctas);
@@ -346,7 +346,7 @@ int b2rl_nature_unpack_grads(const float* g1f, const float* g2f, const float* g3
                              const float* db2, const float* db3, const float* db4, int32_t c1, int32_t n4, float scale,
                              float* gw1, float* gw2, float* gw3, float* gw4, float* gb1, float* gb2, float* gb3,
                              float* gb4, int32_t p1, int32_t p2, int32_t p3 /* split-K partial counts of g1f/g2f/g3f, stored
-                             n_out*K floats apart (b2rl_conv_wgrad_partials); 1 = plain */, void* stream);
+                             n_out*K floats apart (the *_wgrad_partials entries); 1 = plain */, void* stream);
 
 /* Narrow value heads (VanillaNet / DuelingNet, network_heads.py:11-37) on the bf16 features phi [B][K] of the fused body:
  * forward q [B][A] (fp32) = phi Wa^T + ba, or with Wv/bv != NULL the dueling combine q = v + adv - mean(adv);
@@ -374,12 +374,10 @@ int b2rl_head_bwd_geff_relu(const float* geff, const uint16_t* phi, const float*
                             int32_t A, uint16_t* gphi, float* gWa, float* gba, float* gWv, float* gbv, float* relu_colsum,
                             void* stream);
 
-/* Convolution weight gradient as split-K partials (no atomics): partial i of *n_partials_host (<= one per SM, written on the
- * HOST, deterministic for given shapes) is stored at partials + i * n_out*taps*C floats. */
-int b2rl_conv_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out, int32_t taps,
-                             int32_t taps_x, int32_t grid_w, float* partials, int32_t* n_partials_host, void* stream);
-/* The same partials for conv2 (C 128, 2 x 2 taps) and conv3 (C 64, 3 x 3 taps), n_out 64: one CTA computes every tap of its
- * 128-row k-blocks from one load of each operand.  One partial per CTA: at most one per SM, or the CTA budget. */
+/* Convolution weight gradient as split-K partials (no atomics) for conv2 (C 128, 2 x 2 taps) and conv3 (C 64, 3 x 3 taps),
+ * n_out 64: one CTA computes every tap of its 128-row k-blocks from one load of each operand.  One partial per CTA (at most
+ * one per SM, or the CTA budget): partial i of *n_partials_host (written on the HOST, deterministic for given shapes) is
+ * stored at partials + i * n_out*taps*C floats. */
 int b2rl_conv_taps_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, const uint16_t* G, int32_t n_out, int32_t taps,
                                   int32_t taps_x, int32_t grid_w, float* partials, int32_t* n_partials_host, void* stream);
 
@@ -392,7 +390,7 @@ int b2rl_conv_taps_wgrad_partials(const uint16_t* X, int64_t rows, int32_t C, co
  * fwd: D = relu(conv1 + bias) over rows (b, gy, gx) of the (frame_w/4)^2 grid, bf16, output row maps of
  * b2rl_conv_gemm_bf16; relu must be 1, n_out a multiple of 8, D 16-byte aligned and ldd a multiple of 8 (the slab
  * kernel's one store form: whole 16-byte column groups).  wgrad_partials: split-K partials of dW[n][tap*64+c] = sum_r G[r][n] * x[r + shift(tap)][c],
- * contract of b2rl_conv_wgrad_partials; n_out must be 32. */
+ * partial i of *n_partials_host (at most one per SM) at partials + i * 32 * 256 floats; n_out must be 32. */
 int b2rl_conv1_u8_fwd(const uint8_t* frames, int64_t capacity, const int64_t* idx, int32_t first, int64_t row_bytes,
                       int32_t frame_w, int32_t batch, int32_t history, const uint16_t* W, int32_t n_out, void* D, int64_t ldd,
                       const float* bias, int32_t relu, int32_t out_map, int32_t V, void* stream);

@@ -2,7 +2,6 @@
 (bench.time_kernel_graph, best of 5 replays), beside its MMA and byte floors:
   * b2rl_conv1_u8_wgrad_partials  -- conv1_taps_conv_wgrad_wgmma_kernel<true>, activations built from the uint8 ring (K1)
   * b2rl_conv1_wgrad_partials     -- conv1_taps_conv_wgrad_wgmma_kernel<false>, activations from the bf16 stacks
-  * b2rl_conv_wgrad_partials      -- the general slab weight-gradient kernel at conv1's geometry (C 64, 4 taps, grid 21)
 Prints the card's name and power limit first.  --phases: the clock64 probe (b2rl_conv1_set_phase_clocks) of the two taps
 kernels -- cycles per k-block of each role.
 Usage: python scripts/conv1_wgrad_time.py [--batch 512] [--iters 50] [--phases]"""
@@ -43,7 +42,7 @@ s = RingFrames(ring, idx, -3, 84 * 84, 84, 4)
 x0m = s.materialize().permute(0, 2, 3, 1).reshape(rows, 64).contiguous()
 g1 = torch.randn((rows, 32), generator=gen, device=dev).to(torch.bfloat16)
 sms = torch.cuda.get_device_properties(0).multi_processor_count
-bufs = {name: torch.empty((sms, 32, 256), device=dev) for name in ("ring", "bf16", "slab")}
+bufs = {name: torch.empty((sms, 32, 256), device=dev) for name in ("ring", "bf16")}
 n = ctypes.c_int32(0)
 
 
@@ -56,11 +55,6 @@ def bf16_form():
               _lib.stream())
 
 
-def slab_form():
-    _lib.call("b2rl_conv_wgrad_partials", _lib.ptr(x0m), rows, 64, _lib.ptr(g1), 32, 4, 2, 21, _lib.ptr(bufs["slab"]),
-              ctypes.byref(n), _lib.stream())
-
-
 # floors: the useful MMAs (2 rows x 32 x 256 per grid row) and the bytes of four frames per sample (ring) or the bf16
 # stacks, plus the output gradient read once
 flops = 2 * rows * 32 * 256
@@ -69,8 +63,7 @@ bytes_bf16 = rows * 64 * 2 + rows * 32 * 2
 print("# batch %d, %d back-to-back calls per graph, best of 5 replays; floors: MMA %.1f us, bytes %.1f us (ring) / %.1f us "
       "(bf16)" % (B, a.iters, flops / PEAK * 1e6, bytes_ring / HBM * 1e6, bytes_bf16 / HBM * 1e6))
 times = {}
-for name, fn in (("b2rl_conv_wgrad_partials (slab kernel, bf16)", slab_form),
-                 ("b2rl_conv1_wgrad_partials (taps kernel, bf16)", bf16_form),
+for name, fn in (("b2rl_conv1_wgrad_partials (taps kernel, bf16)", bf16_form),
                  ("b2rl_conv1_u8_wgrad_partials (taps kernel, ring)", ring_form)):
     times[name] = bench.time_kernel_graph(fn, iters=a.iters) * 1e3
     print("%-52s %9.2f us" % (name, times[name]))

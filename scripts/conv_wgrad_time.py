@@ -1,8 +1,7 @@
-"""conv2's and conv3's weight gradients at the bench's batch, each entry timed alone in a CUDA graph of back-to-back calls
-(bench.time_kernel_graph, best of 5 replays), with the full grid and with the side branch's CTA budget:
-  * b2rl_conv_wgrad_partials       -- conv_wgrad_wgmma_kernel: 64-row k-tiles, one CTA per 128-column group of taps
-  * b2rl_conv_taps_wgrad_partials  -- conv_taps_wgrad_wgmma_kernel: 128-row k-blocks, every tap in one CTA
-beside the MMA floor on the SMs the launch may use (dense bf16 data-sheet rate x SMs / all SMs) and the share of it reached.
+"""conv2's and conv3's weight gradients at the bench's batch (b2rl_conv_taps_wgrad_partials, conv_taps_wgrad_wgmma_kernel:
+128-row k-blocks, every tap in one CTA), timed alone in a CUDA graph of back-to-back calls (bench.time_kernel_graph, best
+of 5 replays), with the full grid and with the side branch's CTA budget, beside the MMA floor on the SMs the launch may
+use (dense bf16 data-sheet rate x SMs / all SMs) and the share of it reached.
 Prints the card's name, power limit and clocks first.  --phases: the clock64 probe (b2rl_conv1_set_phase_clocks) of the
 taps kernel -- cycles per k-block of each role.
 Usage: python scripts/conv_wgrad_time.py [--batch 512] [--iters 50] [--budgets 0,32] [--phases]"""
@@ -41,47 +40,39 @@ gen = torch.Generator(device=dev).manual_seed(0)
 n = ctypes.c_int32(0)
 
 
-def entry(name, X, G, geo, buf):
+def entry(X, G, geo, buf):
     C, n_out, taps, tx, gw = geo
-    return lambda: _lib.call(name, _lib.ptr(X), X.shape[0], C, _lib.ptr(G), n_out, taps, tx, gw, _lib.ptr(buf), ctypes.byref(n),
-                             _lib.stream())
+    return lambda: _lib.call("b2rl_conv_taps_wgrad_partials", _lib.ptr(X), X.shape[0], C, _lib.ptr(G), n_out, taps, tx, gw,
+                             _lib.ptr(buf), ctypes.byref(n), _lib.stream())
 
 
 print("# batch %d, %d back-to-back calls per graph, best of 5 replays; floor = MMA FLOP / (%.0f TFLOP/s x SMs usable / %d)"
       % (a.batch, a.iters, PEAK / 1e12, SMS))
-print("%-6s %-32s %8s %10s %10s %8s %8s" % ("layer", "entry", "budget", "us", "floor us", "share", "CTAs"))
-news = {}
+print("%-6s %8s %10s %10s %8s %8s" % ("layer", "budget", "us", "floor us", "share", "CTAs"))
+runs = {}
 for layer, geo in LAYERS.items():
     C, n_out, taps, tx, gw = geo
     rows = a.batch * gw * gw
     X = (torch.randn((rows, C), generator=gen, device=dev) * 0.1).relu_().to(torch.bfloat16)
     G = (torch.randn((rows, n_out), generator=gen, device=dev) * 0.1).to(torch.bfloat16)
     flops = 2 * rows * n_out * taps * C
-    bufs, cnt = {}, {}
+    buf = torch.empty((SMS, n_out, taps * C), device=dev)
+    fn = entry(X, G, geo, buf)
     for budget in [int(x) for x in a.budgets.split(",")]:
         usable = budget if 0 < budget < SMS else SMS
         floor = flops / (PEAK * usable / SMS) * 1e6
-        for name in ("b2rl_conv_wgrad_partials", "b2rl_conv_taps_wgrad_partials"):
-            buf = bufs.setdefault(name, torch.empty((SMS, n_out, taps * C), device=dev))
-            fn = entry(name, X, G, geo, buf)
-            with nature_tc._cta_budget(budget):
-                t = bench.time_kernel_graph(fn, iters=a.iters) * 1e3
-                fn()
-            ctas = ctypes.c_int32(0)
-            _lib.call("b2rl_last_grid_ctas", ctypes.byref(ctas))
-            torch.cuda.synchronize()
-            cnt[name] = n.value
-            print("%-6s %-32s %8s %10.2f %10.2f %7.0f%% %8d" % (layer, name, budget or "full", t, floor, 100 * floor / t,
-                                                                ctas.value))
-            if name.startswith("b2rl_conv_taps"):
-                news[(layer, budget)] = (fn, n.value)
-        old, new = (bufs[k][:cnt[k]].double().sum(0) for k in ("b2rl_conv_wgrad_partials", "b2rl_conv_taps_wgrad_partials"))
-        print("# %s, budget %s: the two entries' summed partials differ by %.1e normwise" % (
-            layer, budget or "full", float((new - old).norm() / old.norm())))
+        with nature_tc._cta_budget(budget):
+            t = bench.time_kernel_graph(fn, iters=a.iters) * 1e3
+            fn()
+        ctas = ctypes.c_int32(0)
+        _lib.call("b2rl_last_grid_ctas", ctypes.byref(ctas))
+        torch.cuda.synchronize()
+        print("%-6s %8s %10.2f %10.2f %7.0f%% %8d" % (layer, budget or "full", t, floor, 100 * floor / t, ctas.value))
+        runs[(layer, budget)] = (fn, n.value)
 
 if a.phases:
     clocks = torch.zeros(len(CLK), dtype=torch.int64, device=dev)
-    for (layer, budget), (fn, parts) in news.items():
+    for (layer, budget), (fn, parts) in runs.items():
         reps = 20
         with nature_tc._cta_budget(budget):
             fn()

@@ -223,13 +223,12 @@ def slab_schedule(rows, n_cta):
     return per, per // 2
 
 
-def wgrad_k_tiles(rows, n_windows, C, sms):
-    """conv_wgrad_wgmma_kernel: (CTAs = partials, k-tiles per CTA) by the formula of launch_wgrad."""
-    kt = -(-rows // 64)
-    groups = -(-(n_windows * C) // 128)
-    ctas = max(min(kt // 4, sms // groups), 1)
-    per = -(-kt // ctas)
-    return -(-kt // per), per
+def taps_schedule(rows, ctas):
+    """The weight-gradient taps kernels (conv1's, conv2 / conv3's): (CTAs = partials, 128-row k-blocks per CTA) on at most
+    `ctas` CTAs, equal contiguous ranges."""
+    from test_gpu_conv_taps_wgrad import BK, partition      # imported here: that module imports this one
+    blocks = -(-rows // BK)
+    return partition(rows, ctas), -(-blocks // min(blocks, ctas))
 
 
 def gemm_k_tiles(M, N, K, block_n, sms):
@@ -441,41 +440,52 @@ def test_conv3_dgrad_per_column_bias_gradient(k, B):
 
 
 # ================================================================================================= 4. weight gradients
-WGRAD = {   # layer: (geometry of the layer, as _backward_fused calls wgrad_partials); windows after M-stacking
-    "conv1": (CONV1, 2),    # 2X64, stacked
-    "conv2": (CONV2, 2),    # N128, stacked
-    "conv3": (CONV3, 6),    # 2X64 x 3, stacked
-    "odd96": ((64, 96, 9, 3, 10), 9),     # unstacked: 2X64 x 4 + 1X64
-    "odd128": ((64, 128, 9, 3, 10), 9),
+WGRAD = {   # layer: geometry (conv1-3 as _backward_fused calls wgrad_partials)
+    "conv1": CONV1, "conv2": CONV2, "conv3": CONV3,                 # the taps kernels: one partial per CTA
+    "odd96": (64, 96, 9, 3, 10), "odd128": (64, 128, 9, 3, 10),     # the tap-addressing GEMM: one atomic partial
+    "conv1_c8": (128, 32, 4, 2, 21),                                # conv1 of NatureConvBody(in_channels=8): likewise
 }
+TAPS_WGRAD = ("conv1", "conv2", "conv3")
 
 
 def wgrad_case(k, layer, B, kind, gen):
-    (C, n, taps, tx, gw), _ = WGRAD[layer]
+    """nature_tc.wgrad_partials on the layer's geometry, its partial buffer NaN-filled before the kernel runs."""
+    C, n, taps, tx, gw = WGRAD[layer]
     rows = B * gw * gw
     X = draw(gen, (rows, C), kind, 0, 7)
     Gr = draw(gen, (rows, n), kind, -1, 1)
-    buf = nan_partials(k, n, taps * C)
-    cnt = ctypes.c_int32(0)
-    k.lib.call("b2rl_conv_wgrad_partials", k.lib.ptr(X), rows, C, k.lib.ptr(Gr), n, taps, tx, gw, k.lib.ptr(buf),
-               ctypes.byref(cnt), k.lib.stream())
+    empty = torch.empty
+    with pytest.MonkeyPatch.context() as mp:
+        mp.setattr(torch, "empty", lambda *a, **kw: empty(*a, **kw).fill_(float("nan")))
+        buf, cnt = k.tc.wgrad_partials(X, Gr, n, taps, tx, gw)
     torch.cuda.synchronize()
     ref = row_wgrad(X.double(), Gr.double(), taps, tx, gw)
     S = row_wgrad(X.double().abs(), Gr.double().abs(), taps, tx, gw)
-    return buf, int(cnt.value), ref, S
+    return buf, cnt, ref, S
 
 
 @gpu
 @pytest.mark.parametrize("B", BATCHES)
 @pytest.mark.parametrize("layer", list(WGRAD))
-def test_wgrad_partials_exact(k, layer, B):
-    """Split-K partials of conv_wgrad_wgmma_kernel (M-stacked 2X64 / N128 windows, and the unstacked odd window count with its
-    one-window launch), summed in fp64, equal the reference; the partial count is the launcher's."""
+def test_wgrad_dispatch_exact(k, layer, B):
+    """nature_tc.wgrad_partials, the dispatch the backward pass calls: conv1-3 on their taps kernels, every other geometry on
+    the tap-addressing GEMM.  The partials, summed in fp64, equal the reference; the partial count is the taps launchers'
+    partition over one CTA per SM, or 1 (one atomically accumulated partial)."""
     buf, n, ref, S = wgrad_case(k, layer, B, "int", gen_for("wgrad", layer, B))
     exact_ok(S, layer)
-    (C, _, taps, _, gw), windows = WGRAD[layer]
-    assert n == wgrad_k_tiles(B * gw * gw, windows, C, k.sms)[0]
+    gw = WGRAD[layer][4]
+    assert n == (taps_schedule(B * gw * gw, k.sms)[0] if layer in TAPS_WGRAD else 1), (layer, B, n)
     check_partials(k, buf, n, ref, "%s wgrad B=%d" % (layer, B))
+
+
+@gpu
+@pytest.mark.parametrize("layer", ["conv1", "conv2", "conv3", "odd96"])
+def test_wgrad_dispatch_gaussian(k, layer):
+    """Batch 512 with Gaussian bf16 operands through nature_tc.wgrad_partials: the summed partials within 1e-5 normwise of
+    float64."""
+    case = "wgrad_" + layer
+    buf, n, ref, _ = wgrad_case(k, layer, 512, "gauss", gen_for("gauss", case))
+    check_partials(k, buf, n, ref, case, kind="gauss")
 
 
 # ================================================================================================= 5. K1: conv1 from the uint8 ring
@@ -526,15 +536,14 @@ def test_k1_from_ring_exact(k, B, n_step, which):
 
 
 # ================================================================================================= 6. Gaussian operands
-GAUSS = ["fwd_conv1", "fwd_conv2", "fwd_conv3", "dgrad_conv3", "dgrad_conv2", "dgrad_fc4", "wgrad_conv1", "wgrad_conv2",
-         "wgrad_conv3", "wgrad_odd96", "k1"]
+GAUSS = ["fwd_conv1", "fwd_conv2", "fwd_conv3", "dgrad_conv3", "dgrad_conv2", "dgrad_fc4", "k1"]
 
 
 @gpu
 @pytest.mark.parametrize("case", GAUSS)
 def test_gaussian_operands(k, case):
     """Batch 512 with Gaussian bf16 operands: |got - ref| <= 2^-8 |ref| + K 2^-23 sum|a*b| per element on forward and dgrad
-    outputs, 1e-5 normwise on the summed weight-gradient partials."""
+    outputs, 1e-5 normwise on K1's summed weight-gradient partials (the other weight gradients: test_wgrad_dispatch_gaussian)."""
     B = 512
     gen = gen_for("gauss", case)
     kind, layer = case.split("_", 1) if "_" in case else (case, None)
@@ -552,9 +561,6 @@ def test_gaussian_operands(k, case):
         written = place(torch.ones_like(c.S), c.out_map, c.ref.shape, 0.0, G, V, sub_c) > 0
         assert_bf16_bounded(c.out[written], c.ref[written], S[written], c.K, case)
         assert bool((c.out[~written] == SENT).all()), case
-    elif kind == "wgrad":
-        buf, n, ref, _ = wgrad_case(k, layer, B, "gauss", gen)
-        check_partials(k, buf, n, ref, case, kind="gauss")
     else:
         lib = k.lib
         rf, x0 = k1_case(k, B, 1, 0, "gauss", gen)
@@ -596,7 +602,7 @@ def test_tap_addressing_fallback_exact(k):
             assert_bf16_equal(c.out, c.ref, "%s dgrad, tap addressing" % layer)
             assert torch.equal(c.db.double(), c.db_ref), layer
         for layer in ("conv1", "conv2", "conv3"):
-            (C, n, taps, tx, gw), _ = WGRAD[layer]
+            C, n, taps, tx, gw = WGRAD[layer]
             gen = gen_for("tap-wgrad", layer)
             X = draw(gen, (B * gw * gw, C), "int", 0, 7)
             Gr = draw(gen, (B * gw * gw, n), "int", -1, 1)
@@ -755,10 +761,12 @@ def test_batches_reach_the_schedules(k):
         assert any(wg1 >= 2 for _, wg1 in sched), (name, sched)
         assert any(per > MAX_STAGES for per, _ in sched), (name, sched)
     assert gemm_k_tiles(2048, 3136, 512, 128, sms) > MAX_STAGES, "gemm<128,4,EXT> fc4 dgrad"
-    for name, ((C, _, _, _, gw), windows) in WGRAD.items():
-        assert any(wgrad_k_tiles(B * gw * gw, windows, C, sms)[1] > MAX_STAGES for B in (512, 2048)), name
-        assert wgrad_k_tiles(512 * gw * gw, windows, C, sms)[1] > MAX_STAGES, name + ": the bench batch wraps the ring"
-    assert wgrad_k_tiles(512 * 441, 2, 64, sms)[1] > 4, "K1 wgrad (four operand stages)"
+    for name in TAPS_WGRAD:
+        gw = WGRAD[name][4]
+        assert any(taps_schedule(B * gw * gw, sms)[1] > MAX_STAGES for B in (512, 2048)), name
+        bench_ctas = sms if name == "conv1" else k.tc.SIDE_CTAS     # conv2 / conv3 run on the side branch's CTAs
+        assert taps_schedule(512 * gw * gw, bench_ctas)[1] > MAX_STAGES, name + ": the bench batch wraps the ring"
+    assert taps_schedule(512 * 441, sms)[1] > 4, "K1 wgrad (four operand stages)"
 
 
 # ================================================================================================= 10. CPU: the reference itself
